@@ -725,8 +725,10 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
         // starts (prefetch window included) only after ring k has finished
         // (only when one thread per lane does not fit a CTA: measured, a dedicated thread per lane is faster)
         // Two thread layouts of the same schedule.  "Latency": one thread per lane whenever that fits a CTA (measured:
-        // fastest for a single scan).  "Throughput": the smallest M, so that the CTA is small and two or three scans
-        // share an SM (measured: +4 % on batches).  GG_SPIRAL_M raises the throughput layout's M (0: same as latency).
+        // fastest for a single scan).  "Throughput": a CTA with M lane threads per side, GG_SPIRAL_M (multiple of 32;
+        // 0, the default: same as latency; 32: the smallest M, so that two or three scans share an SM).  On an H100 SXM
+        // three small CTAs per SM run a level about 5x slower than one large CTA alone (DESIGN.md section 3.3), so batches
+        // run one thread per lane as well.
         int M = 32, phases = 1, M_thr = 32, phases_thr = 1;
         if (sk.ok) {
             const int kGap = 2 * 8 + 4;  // 2 * PF_FAR of k_spiral_skew + slack
@@ -747,7 +749,7 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
             };
             M = (4 * sk.KP + 64 <= 1024) ? sk.KP : smallest_fitting(32);
             phases = (sk.KP + M - 1) / M;
-            int m0 = 32;
+            int m0 = 0;
             if (const char* e = getenv("GG_SPIRAL_M")) m0 = atoi(e) / 32 * 32;
             M_thr = m0 <= 0 ? M : smallest_fitting(std::max(32, m0));
             phases_thr = (sk.KP + M_thr - 1) / M_thr;
