@@ -81,6 +81,8 @@ def load(build_if_missing=True):
         "gg_num_slots": (i, [vp]),
         "gg_set_config": (i, [vp, C.POINTER(Config)]),
         "gg_get_config": (i, [vp, C.POINTER(Config)]),
+        "gg_set_slot_config": (i, [vp, i, C.POINTER(Config)]),
+        "gg_get_slot_config": (i, [vp, i, C.POINTER(Config)]),
         "gg_init_map": (i, [vp, i, d, d, d]),
         "gg_update_pose": (i, [vp, i, d, d, vp, C.POINTER(i)]),
         "gg_update_pose_batch": (i, [vp, i, vp, vp, vp, vp]),
@@ -126,6 +128,9 @@ def load(build_if_missing=True):
         "gg_host_expected_points": (i, [d, C.c_float, vp]),
         "gg_host_spiral_schedule": (i, [i, vp, i, vp, i, C.POINTER(i), C.POINTER(i)]),
         "gg_host_move_map": (i, [d, vp, d, d, vp]),
+        "gg_host_geometry_constants": (i, [d, C.c_float, C.c_uint, vp]),
+        "gg_host_config_constants": (i, [C.POINTER(Config), vp]),
+        "gg_host_config_registry": (i, [i, i, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -174,6 +179,45 @@ def host_move_map(res, pos_xy, new_xy):
     return bool(moved), pos, (int(shift[0]), int(shift[1]))
 
 
+GEOMETRY_CONSTANTS = ("N", "N2", "full_layers", "res_f", "res", "rres", "len", "half", "res_sq")
+CONFIG_CONSTANTS = ("max_ring", "pc_var_thresh_f", "min_outlier_conf", "outlier_tol", "gp_thresh", "df_sq", "mdf_sq", "mdf10_sq",
+                    "psc_sq", "occ_factor", "occ_factor2", "dec_factor", "lab_fac", "lab_thres", "lab_obs", "decay_floor_ok")
+
+
+def default_config():
+    cfg = Config()
+    load().gg_default_config(C.byref(cfg))
+    return cfg
+
+
+def host_geometry_constants(dimension_m, resolution, full_layers=False):
+    """{name: value} of the geometry constants the kernels get (gg::Const)."""
+    out = np.zeros(len(GEOMETRY_CONSTANTS), np.float64)
+    load().gg_host_geometry_constants(float(dimension_m), np.float32(resolution), GG_FLAG_FULL_LAYERS if full_layers else 0, _ptr(out))
+    return dict(zip(GEOMETRY_CONSTANTS, out.tolist()))
+
+
+def host_config_constants(cfg):
+    """{name: value} of the constants derived from one configuration (gg::CfgConst)."""
+    out = np.zeros(len(CONFIG_CONSTANTS), np.float64)
+    load().gg_host_config_constants(C.byref(cfg), _ptr(out))
+    return dict(zip(CONFIG_CONSTANTS, out.tolist()))
+
+
+def host_config_registry(n_slots, ops):
+    """Replays ops = [(slot or None for the whole handle, Config)] on the configuration-variant bookkeeping of a new
+    handle; (("invalidate", v), None) marks variant v as holding unknown device data (a failed build).  Returns (per op: (variant id, built, live variants, variant ids) as int array [n_ops, 4], final variant
+    of every slot)."""
+    n = len(ops)
+    slots = np.array([-1 if s is None else (-2 - s[1] if isinstance(s, tuple) else s) for s, _ in ops], np.int32)
+    cfgs = (Config * max(1, n))(*[c if c is not None else default_config() for _, c in ops])
+    out = np.zeros(4 * n + n_slots, np.int32)
+    rc = load().gg_host_config_registry(int(n_slots), n, _ptr(slots), C.cast(cfgs, C.c_void_p), _ptr(out))
+    if rc != 0:
+        raise GroundGridError(rc, "gg_host_config_registry: bad argument")
+    return out[:4 * n].reshape(n, 4), out[4 * n:]
+
+
 # ---- device handle ------------------------------------------------------------------------
 class GroundGridB200:
     """One handle = `n_slots` independent GroundGrid maps on one GPU (see the C header)."""
@@ -203,14 +247,27 @@ class GroundGridB200:
             pass
 
     # -- config / state
-    def set_config(self, **kw):
-        cfg = Config()
-        _check(self._l.gg_get_config(self._h, C.byref(cfg)))
+    def set_config(self, slot=None, **kw):
+        """Changes the given fields.  slot=None: the handle-wide configuration (every slot's, gg_set_config);
+        an integer: that slot's own configuration only (gg_set_slot_config)."""
+        cfg = self.get_config(slot)
         for k, v in kw.items():
             if not hasattr(cfg, k):
                 raise KeyError(k)
             setattr(cfg, k, v)
-        _check(self._l.gg_set_config(self._h, C.byref(cfg)))
+        if slot is None:
+            _check(self._l.gg_set_config(self._h, C.byref(cfg)))
+        else:
+            _check(self._l.gg_set_slot_config(self._h, int(slot), C.byref(cfg)))
+
+    def get_config(self, slot=None):
+        """The handle-wide configuration (slot=None) or the one a slot runs with."""
+        cfg = Config()
+        if slot is None:
+            _check(self._l.gg_get_config(self._h, C.byref(cfg)))
+        else:
+            _check(self._l.gg_get_slot_config(self._h, int(slot), C.byref(cfg)))
+        return cfg
 
     def init_map(self, x, y, z, slot=0):
         _check(self._l.gg_init_map(self._h, slot, x, y, z))

@@ -290,7 +290,10 @@ struct gg_handle_s {
     unsigned flags = 0;
     double dimension_m = 0.0;
     float resolution = 0.f;
-    gg_config cfg{};
+    gg_config cfg{};                   // what gg_set_config last set (gg_get_config)
+    std::vector<gg_config> slot_cfg;   // per slot: what gg_set_slot_config / gg_set_config last set
+    gg::ConfigRegistry variants;       // slot -> configuration variant (shared by slots with identical constants)
+    std::vector<float4*> variant_tab;  // per variant id: detect table of its constants (N2 entries)
     gg::View view{};
     std::vector<SlotState> slots;
     cudaStream_t streams[kStreams] = {};
@@ -337,7 +340,6 @@ struct gg_handle_s {
     cudaStream_t copy_in[10] = {}, copy_out = nullptr;  // [0, n_copy_in): packed clouds, then 2 for raw clouds;  // H2D / D2H of gg_filter_cloud_batch, never behind kernels
     int n_copy_in = 4;                                   // GG_COPY_STREAMS
     int main_help = 1;                                   // GG_MAIN_HELP
-    float4* detect_tab = nullptr;  // per-cell constants of the patch detection, rebuilt by gg_set_config
     CUtensorMap layer_map{};        // TMA descriptor of the layer arena (k_detect_tma); valid iff have_layer_map
     bool have_layer_map = false;
     bool inputs_busy = false;  // asynchronous work that reads or writes the slots' input buffers may be in flight
@@ -435,9 +437,34 @@ int ring_release(gg_handle h, int pos, cudaStream_t st) {
 int stream_index(gg_handle h, int slot) { return (int)((long long)slot * h->n_streams / h->n_slots); }
 cudaStream_t stream_of(gg_handle h, int slot) { return h->streams[stream_index(h, slot)]; }
 
+// Device buffer of variant id `id` (allocated once, kept for reuse by later variants).
+int ensure_variant_buffer(gg_handle h, int id) {
+    int rc;
+    while ((int)h->variant_tab.size() <= id) {
+        float4* p = nullptr;
+        if ((rc = dev_alloc(h, &p, (size_t)h->view.k.N2))) return rc;
+        h->variant_tab.push_back(p);
+    }
+    return GG_OK;
+}
+
+// Device data of variant `id` (its detect table) from its constants on `st`, then a wait on `st`, so that every stream
+// may use the variant afterwards.  Only called for a variant no enqueued work reads.
+int build_variant(gg_handle h, int id, cudaStream_t st) {
+    int rc;
+    if ((rc = ensure_variant_buffer(h, id))) return rc;
+    h->launches += gg::launch_build_detect_table(h->view, h->variants.constants(id), h->variant_tab[id], st);
+    GG_CUDA(cudaGetLastError());
+    GG_CUDA(cudaStreamSynchronize(st));
+    return GG_OK;
+}
+
 void fill_params(gg_handle h, const gg_scan_desc& d, gg::SlotParams& p, const gg_point* src, const float* packed = nullptr) {
     const SlotState& s = h->slots[d.slot];
     std::memset(&p, 0, sizeof(p));
+    const int var = h->variants.variant_of(d.slot);
+    p.cfg = h->variants.constants(var);
+    p.detect_tab = h->variant_tab[var];
     p.px = s.px;
     p.py = s.py;
     p.ox = d.origin[0];
@@ -619,8 +646,14 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     h->resolution = resolution;
     gg_default_config(&h->cfg);
     h->slots.resize(n_slots);
+    h->slot_cfg.assign((size_t)n_slots, h->cfg);
+    {
+        gg::CfgConst kc;
+        gg::derive_config(h->cfg, kc);
+        h->variants.reset(n_slots, kc);
+    }
     gg::View& v = h->view;
-    gg::derive_constants(h->cfg, dimension_m, resolution, flags, v.k);
+    gg::derive_geometry(dimension_m, resolution, flags, v.k);
     if (v.k.N != n) {
         const int n_geo = v.k.N;
         delete h;
@@ -654,8 +687,6 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     float* expected = nullptr;
     GG_TRY(dev_alloc(h, &expected, N2));
     v.expected = expected;
-    GG_TRY(dev_alloc(h, &h->detect_tab, N2));
-    v.detect_tab = h->detect_tab;
     GG_TRY(dev_alloc(h, &v.points, S * P));
     GG_TRY(dev_alloc(h, &v.zw, S * P));
     GG_TRY(dev_alloc(h, &v.zsorted, S * P));
@@ -889,9 +920,7 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     GG_TRY(dev_alloc(h, &h->d_ring, (size_t)kRing * S));
     for (int i = 0; i < kRing; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->ring_ev[i], cudaEventDisableTiming));
     for (int i = 0; i < kStreams; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->stagger_ev[i], cudaEventDisableTiming));
-    h->launches += gg::launch_build_detect_table(v, h->detect_tab, h->streams[0]);
-    GG_CUDA_TRY(cudaGetLastError());
-    GG_CUDA_TRY(cudaStreamSynchronize(h->streams[0]));
+    GG_TRY(build_variant(h, 0, h->streams[0]));
 #undef GG_TRY
 #undef GG_CUDA_TRY
     *out = h;
@@ -948,16 +977,59 @@ int gg_set_config(gg_handle h, const gg_config* cfg) {
     int rc = gg_synchronize(h);  // kernels in flight keep the tables of the old configuration
     if (rc) return rc;
     h->cfg = *cfg;
-    gg::derive_constants(h->cfg, h->dimension_m, h->resolution, h->flags, h->view.k);  // by-value kernel argument: applies to the next launch
-    h->launches += gg::launch_build_detect_table(h->view, h->detect_tab, h->streams[0]);
-    GG_CUDA(cudaGetLastError());
-    GG_CUDA(cudaStreamSynchronize(h->streams[0]));
-    return GG_OK;
+    h->slot_cfg.assign((size_t)h->n_slots, *cfg);
+    gg::CfgConst kc;
+    gg::derive_config(*cfg, kc);
+    h->variants.reset(h->n_slots, kc);   // every slot on variant 0; nothing reads the others any more
+    return build_variant(h, 0, h->streams[0]);
 }
 
 int gg_get_config(gg_handle h, gg_config* cfg) {
     if (!h || !cfg) return fail(GG_E_ARG, "null argument");
     *cfg = h->cfg;
+    return GG_OK;
+}
+
+int gg_set_slot_config(gg_handle h, int slot, const gg_config* cfg) {
+    int rc = check_slot(h, slot);
+    if (rc) return rc;
+    if (!cfg) return fail(GG_E_ARG, "null argument");
+    GG_CUDA(cudaSetDevice(h->device));
+    // Every kernel that reads the slot's variant runs on the slot's stream: once that stream is idle, the old variant
+    // is read by nobody if the slot was its last user (and may be rebuilt for the new constants below).  Other stream
+    // groups keep running on their own variants, which assign() never touches while a slot uses them.
+    cudaStream_t st = stream_of(h, slot);
+    GG_CUDA(cudaStreamSynchronize(st));
+    gg::CfgConst kc;
+    gg::derive_config(*cfg, kc);
+    const gg::ConfigRegistry before = h->variants;
+    bool build = false;
+    const int id = h->variants.assign(slot, kc, &build);
+    if (build) {
+        // On failure the slot keeps its old configuration.  A new id gets its buffer before anything is written, so a
+        // failed allocation changes nothing.
+        if ((rc = ensure_variant_buffer(h, id))) {
+            h->variants = before;
+            return rc;
+        }
+        if ((rc = build_variant(h, id, st))) {
+            // A launch error leaves the table untouched; an unused id whose table may have been partly rewritten no
+            // longer holds the data of its old constants.  (A fault inside the kernel leaves the CUDA context failing
+            // every later call, the slot's own old variant included.)
+            h->variants = before;
+            if (id < before.ids() && before.refs(id) == 0) h->variants.invalidate(id);
+            return rc;
+        }
+    }
+    h->slot_cfg[slot] = *cfg;
+    return GG_OK;
+}
+
+int gg_get_slot_config(gg_handle h, int slot, gg_config* cfg) {
+    int rc = check_slot(h, slot);
+    if (rc) return rc;
+    if (!cfg) return fail(GG_E_ARG, "null argument");
+    *cfg = h->slot_cfg[slot];
     return GG_OK;
 }
 
@@ -1211,7 +1283,7 @@ int gg_interpolate_cell(gg_handle h, int slot, int x, int y) {
     const int N = h->view.k.N;
     if (x < 1 || y < 1 || x >= N - 1 || y >= N - 1) return fail(GG_E_ARG, "cell (%d, %d) has no 3x3 neighbourhood", x, y);
     GG_CUDA(cudaSetDevice(h->device));
-    h->launches += gg::launch_interpolate_cell(h->view, slot, x, y, stream_of(h, slot));
+    h->launches += gg::launch_interpolate_cell(h->view, h->variants.constants(h->variants.variant_of(slot)), slot, x, y, stream_of(h, slot));
     GG_CUDA(cudaGetLastError());
     return GG_OK;
 }
@@ -1223,7 +1295,7 @@ int gg_detect_ground_patch(gg_handle h, int slot, int patch_size, int i, int j) 
     const int N = h->view.k.N, H = patch_size / 2;
     if (i < H || j < H || i >= N - H || j >= N - H) return fail(GG_E_ARG, "cell (%d, %d) has no %dx%d neighbourhood", i, j, patch_size, patch_size);
     GG_CUDA(cudaSetDevice(h->device));
-    h->launches += gg::launch_detect_cell(h->view, slot, patch_size, i, j, stream_of(h, slot));
+    h->launches += gg::launch_detect_cell(h->view, h->variants.constants(h->variants.variant_of(slot)), slot, patch_size, i, j, stream_of(h, slot));
     GG_CUDA(cudaGetLastError());
     return GG_OK;
 }

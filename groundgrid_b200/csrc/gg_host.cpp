@@ -36,22 +36,27 @@ void build_expected_points(int n, std::vector<float>& table) {
         }
 }
 
-// grid_map::GridMap::setGeometry + the constants the kernels need; squares are written as
+// grid_map::GridMap::setGeometry and the geometry constants the kernels need; squares are written as
 // x * x, which is what the reference's compiler emits for std::pow(x, 2.0).
-void derive_constants(const gg_config& c, double dimension_m, float resolution, unsigned flags, Const& k) {
+void derive_geometry(double dimension_m, float resolution, unsigned flags, Const& k) {
     const double res = (double)resolution;
     const int n = (int)std::round((double)(float)dimension_m / res);
     k.N = n;
     k.N2 = n * n;
-    k.max_ring = c.max_ring;
     k.full_layers = (flags & GG_FLAG_FULL_LAYERS) ? 1 : 0;
-    k.pc_var_thresh_f = (float)c.point_count_cell_variance_threshold;
     k.res_f = (float)res;
     k.res = res;
     k.rres = 1.0 / res;
     k.len = (double)n * res;
     k.half = 0.5 * k.len;
     k.res_sq = (double)k.res_f * (double)k.res_f;
+}
+
+// The constants of one configuration (GroundSegmentation::setConfig, GroundGrid::setConfig).
+void derive_config(const gg_config& c, CfgConst& k) {
+    std::memset(&k, 0, sizeof(k));
+    k.max_ring = c.max_ring;
+    k.pc_var_thresh_f = (float)c.point_count_cell_variance_threshold;
     k.min_outlier_conf = c.min_outlier_detection_ground_confidence;
     k.outlier_tol = c.outlier_tolerance;
     k.gp_thresh = c.ground_patch_detection_minimum_point_count_threshold;
@@ -74,6 +79,44 @@ void derive_constants(const gg_config& c, double dimension_m, float resolution, 
         const double dec = o - o / k.dec_factor;
         k.decay_floor_ok = (k.dec_factor >= 1.0 && dec < 0.000999) ? 1 : 0;
     }
+}
+
+void ConfigRegistry::reset(int n_slots, const CfgConst& k) {
+    for (Variant& v : vars_) v.refs = 0;
+    if (vars_.empty()) vars_.push_back(Variant{});
+    vars_[0].k = k;
+    vars_[0].refs = n_slots;
+    slot_var_.assign((size_t)n_slots, 0);
+}
+
+int ConfigRegistry::assign(int slot, const CfgConst& k, bool* build) {
+    *build = false;
+    const int old = slot_var_[slot];
+    if (std::memcmp(&vars_[old].k, &k, sizeof(k)) == 0) return old;
+    --vars_[old].refs;
+    // a variant with these constants, used or not (an unused one still holds intact device data)
+    int id = -1;
+    for (int i = 0; i < (int)vars_.size() && id < 0; ++i)
+        if (std::memcmp(&vars_[i].k, &k, sizeof(k)) == 0) id = i;
+    if (id < 0) {
+        for (int i = 0; i < (int)vars_.size() && id < 0; ++i)
+            if (vars_[i].refs == 0) id = i;
+        if (id < 0) {
+            id = (int)vars_.size();
+            vars_.push_back(Variant{});
+        }
+        vars_[id].k = k;
+        *build = true;
+    }
+    ++vars_[id].refs;
+    slot_var_[slot] = id;
+    return id;
+}
+
+int ConfigRegistry::live() const {
+    int n = 0;
+    for (const Variant& v : vars_) n += v.refs > 0;
+    return n;
 }
 
 // grid_map::GridMap::move (getIndexShiftFromPositionShift / getPositionShiftFromIndexShift):
@@ -784,5 +827,61 @@ int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* 
 int gg_host_move_map(double res, double* pos_xy, double nx, double ny, int* shift_ij) {
     gg::move_map(res, pos_xy[0], pos_xy[1], nx, ny, shift_ij[0], shift_ij[1]);
     return (shift_ij[0] != 0 || shift_ij[1] != 0) ? 1 : 0;
+}
+
+// out[9]: N, N2, full_layers, res_f, res, rres, len, half, res_sq
+int gg_host_geometry_constants(double dimension_m, float resolution, unsigned flags, double* out) {
+    gg::Const k;
+    gg::derive_geometry(dimension_m, resolution, flags, k);
+    const double v[9] = {(double)k.N, (double)k.N2, (double)k.full_layers, (double)k.res_f, k.res, k.rres, k.len, k.half, k.res_sq};
+    std::memcpy(out, v, sizeof(v));
+    return 0;
+}
+
+// out[16]: the fields of gg::CfgConst in declaration order (reserved left out)
+int gg_host_config_constants(const gg_config* cfg, double* out) {
+    gg::CfgConst k;
+    gg::derive_config(*cfg, k);
+    const double v[16] = {(double)k.max_ring, (double)k.pc_var_thresh_f, k.min_outlier_conf, k.outlier_tol, k.gp_thresh, k.df_sq, k.mdf_sq,
+                          k.mdf10_sq, k.psc_sq, k.occ_factor, k.occ_factor2, k.dec_factor, k.lab_fac, k.lab_thres, k.lab_obs,
+                          (double)k.decay_floor_ok};
+    std::memcpy(out, v, sizeof(v));
+    return 0;
+}
+
+// Replays configuration changes on a registry of n_slots slots that starts like a new handle (every slot on the
+// default configuration).  Operation i sets op_cfg[i] on slot op_slot[i], or on the whole handle if op_slot[i] == -1;
+// op_slot[i] = -2 - v marks variant v as holding unknown data (a failed build; op_cfg[i] is ignored).
+// out: per operation (variant id of the slot or 0, 1 if the variant had to be built, live variants, variant ids),
+// then the final variant of every slot.
+int gg_host_config_registry(int n_slots, int n_ops, const int* op_slot, const gg_config* op_cfg, int* out) {
+    if (n_slots <= 0 || n_ops < 0 || (n_ops && (!op_slot || !op_cfg)) || !out) return GG_E_ARG;
+    gg::ConfigRegistry reg;
+    gg_config c0;
+    gg_default_config(&c0);
+    gg::CfgConst k;
+    gg::derive_config(c0, k);
+    reg.reset(n_slots, k);
+    for (int i = 0; i < n_ops; ++i) {
+        if (op_slot[i] >= n_slots || (op_slot[i] <= -2 && -2 - op_slot[i] >= reg.ids())) return GG_E_ARG;
+        gg::derive_config(op_cfg[i], k);
+        int id = 0;
+        bool build = true;
+        if (op_slot[i] <= -2) {
+            id = -2 - op_slot[i];
+            build = false;
+            reg.invalidate(id);
+        } else if (op_slot[i] < 0)
+            reg.reset(n_slots, k);
+        else
+            id = reg.assign(op_slot[i], k, &build);
+        int* o = out + 4 * (size_t)i;
+        o[0] = id;
+        o[1] = build ? 1 : 0;
+        o[2] = reg.live();
+        o[3] = reg.ids();
+    }
+    for (int s = 0; s < n_slots; ++s) out[4 * (size_t)n_ops + s] = reg.variant_of(s);
+    return 0;
 }
 }

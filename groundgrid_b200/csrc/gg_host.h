@@ -8,7 +8,38 @@
 namespace gg {
 int cells_per_side(double dimension_m, float resolution);
 void build_expected_points(int n, std::vector<float>& table);
-void derive_constants(const gg_config& c, double dimension_m, float resolution, unsigned flags, Const& k);
+void derive_geometry(double dimension_m, float resolution, unsigned flags, Const& k);
+void derive_config(const gg_config& c, CfgConst& k);
+
+// Configuration variants of a handle.  Slots whose derived constants are identical share one variant (one
+// constants record and one detect table on the device), so device memory grows with the number of distinct
+// configurations in use, not with the number of slots.  Host bookkeeping only: the caller owns one device buffer
+// per variant id and (re)builds it when assign() says so.  A variant no slot uses keeps its id and its buffer and is
+// taken again by the next new configuration.
+class ConfigRegistry {
+  public:
+    // every slot on variant 0 with constants k; every other variant becomes unused
+    void reset(int n_slots, const CfgConst& k);
+    // Points `slot` at the variant of `k` and returns its id; *build = true if that variant's device data must be
+    // built first (a new id, or an unused one that held other constants).
+    int assign(int slot, const CfgConst& k, bool* build);
+    // Marks an unused variant's device data as unknown (a build of it failed half way): no constants match it any
+    // more, so the next configuration that takes the id builds it again.
+    void invalidate(int id) { vars_[id].k.reserved = 1; }   // derive_config leaves reserved at 0
+    int variant_of(int slot) const { return slot_var_[slot]; }
+    const CfgConst& constants(int id) const { return vars_[id].k; }
+    int refs(int id) const { return vars_[id].refs; }
+    int live() const;                                 // variants at least one slot uses
+    int ids() const { return (int)vars_.size(); }     // variant ids handed out so far (= device buffers)
+
+  private:
+    struct Variant {
+        CfgConst k;
+        int refs;
+    };
+    std::vector<Variant> vars_;
+    std::vector<int> slot_var_;
+};
 void move_map(double res, double& px, double& py, double nx, double ny, int& shift_i, int& shift_j);
 void build_spiral_schedule(int n, std::vector<int>& level_start, std::vector<uint32_t>& visits);
 // cached: plain stores (destination meant to stay in the last-level cache until the DMA engine reads it)
@@ -62,6 +93,9 @@ int gg_host_expected_points(double dimension_m, float resolution, float* dst);
 int gg_host_spiral_schedule(int n, int* level_start, int level_cap, uint32_t* visits, int visit_cap, int* n_levels, int* n_visits);
 int gg_host_spiral_records(int n, float resolution, int dist, uint32_t* recs, int rec_cap_words, int* max_recent);
 int gg_host_move_map(double res, double* pos_xy, double nx, double ny, int* shift_ij);
+int gg_host_geometry_constants(double dimension_m, float resolution, unsigned flags, double* out);
+int gg_host_config_constants(const gg_config* cfg, double* out);
+int gg_host_config_registry(int n_slots, int n_ops, const int* op_slot, const gg_config* op_cfg, int* out);
 int gg_host_pack_cloud(const gg_point* src, size_t n, unsigned char* dst);
 int gg_host_pack_cloud_cached(const gg_point* src, size_t n, unsigned char* dst);
 int gg_host_packer_selftest(int threads, int n_jobs, size_t n_points, int ring_slots, int rounds, int lag);

@@ -39,28 +39,40 @@ enum PointClass : unsigned {
     PC_OUTLIER = 5,         // below-ground outlier: always labelled ground (:270,185-189)
 };
 
-// Constants derived once per set_config on the host, with the reference's own expressions
-// (so the fp64 values are what the reference's compiler computes).
+// Geometry constants of a handle (grid_map::GridMap::setGeometry), derived once in gg_create on the host.
 struct Const {
     int N, N2;
-    int max_ring;
     int full_layers;
-    float pc_var_thresh_f;  // (float) point_count_cell_variance_threshold (float >= int compare, :374)
     float res_f;            // (float) map.getResolution()
     double res;             // map.getResolution()  == (double) res_f
     double rres;            // 1 / res (only to skip IEEE divisions whose integer part is not in doubt)
     double len, half;       // N * res, 0.5 * len
     double res_sq;          // res * res  (std::pow(resolution, 2.0), :332,356,463)
+};
+
+// Constants derived from one configuration on the host, with the reference's own expressions (so the fp64 values
+// are what the reference's compiler computes).  One record per configuration variant (gg_host.h:ConfigRegistry); it
+// travels by value in the SlotParams of every scan.  No padding: records are compared bytewise.
+struct CfgConst {
+    int max_ring;
+    float pc_var_thresh_f;  // (float) point_count_cell_variance_threshold (float >= int compare, :374)
     double min_outlier_conf, outlier_tol;
     double gp_thresh;       // ground_patch_detection_minimum_point_count_threshold
     double df_sq, mdf_sq, mdf10_sq, psc_sq;
     double occ_factor, occ_factor2, dec_factor;
     double lab_fac, lab_thres, lab_obs;
     int decay_floor_ok;     // decay of a confidence <= 0.001f gives 0.001f again (checked on the host for dec_factor)
+    int reserved;           // zero
 };
+static_assert(sizeof(CfgConst) == 120, "CfgConst has no padding");
 
 // Per-scan, per-slot parameters (changes every scan / pose update).
 struct SlotParams {
+    // configuration variant of the slot (set by every launch that reads it; zero otherwise): its constants by value
+    // (a pointer would add a dependent load to the start of every block) and its detect table, [N2] per-cell constants
+    // of the patch detection (gg_kernels.cu:k_build_detect_table), built once and immutable while a slot uses it
+    CfgConst cfg;
+    const float4* detect_tab;
     double px, py;        // map centre position
     double t20, t21, t22, t23;  // row 2 of T_base_from_map (seed of exposed cells)
     float ox, oy, oz;     // cloud origin
@@ -116,7 +128,6 @@ struct View {
     float* layers;        // [n_slots][n_layers][N2]
     int n_layers;
     const float* expected;  // [N2] expectedPoints table (GroundSegmentation.cpp:40-46)
-    const float4* detect_tab;  // [N2] per-cell constants of the patch detection (gg_kernels.cu:k_build_detect_table)
     gg_point* points;     // [n_slots][pcap]
     unsigned char* packed;  // [n_slots][14 * pcap] packed clouds (allocated on first use)
     uint2* zw;            // [n_slots][pcap] per input point: (z bits, position in the cell's segment | run-head flag << 31)
@@ -173,7 +184,7 @@ struct Profiler {
 // ---- launchers (gg_kernels.cu); every function enqueues on `st` and returns the number of
 // kernel launches it issued (for gg_kernel_launches()). -----------------------------------
 int launch_init_map(const View& v, int slot, float z, cudaStream_t st);
-int launch_build_detect_table(const View& v, float4* tab, cudaStream_t st);
+int launch_build_detect_table(const View& v, const CfgConst& c, float4* tab, cudaStream_t st);
 int launch_roll(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof);
 // layer_map: TMA descriptor of the handle's layer arena as a 3-D tensor (i, j, slot * n_layers + layer), box
 // 40 x 12 x 1 (k_detect_tma); null -> the patch detection stages its tile with plain loads (N % 4 != 0)
@@ -183,8 +194,8 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
 // single phases / single cells (the reference's public per-phase methods)
 int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map);
 int launch_spiral_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof);
-int launch_interpolate_cell(const View& v, int slot, int x, int y, cudaStream_t st);
-int launch_detect_cell(const View& v, int slot, int S, int i, int j, cudaStream_t st);
+int launch_interpolate_cell(const View& v, const CfgConst& c, int slot, int x, int y, cudaStream_t st);
+int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, cudaStream_t st);
 int launch_output(const View& v, const SlotParams* batch, int count, int max_points, bool want_cloud, cudaStream_t st,
                   Profiler* prof);
 // "next" rows of SURVEY.md section 8(f)

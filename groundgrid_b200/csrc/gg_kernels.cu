@@ -233,6 +233,7 @@ __global__ void __launch_bounds__(256) k_roll_commit(View v, const SlotParams* _
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t rasterize_point(const View& v, const SlotParams& sp, int i, float& zout) {
     const Const& k = v.k;
+    const CfgConst& kc = sp.cfg;
     const int N = k.N;
     const size_t base = (size_t)sp.slot * v.pcap;
 
@@ -271,7 +272,7 @@ __device__ __forceinline__ uint32_t rasterize_point(const View& v, const SlotPar
         const int cell = g0 + g1 * N;
         const bool border = (N <= g0 + 3) || (N <= g1 + 3);  // :167
         if (k.full_layers) atomicAdd(v.raw_i + (size_t)sp.slot * k.N2 + cell, 1);  // pointsRaw, :234
-        if (ring > k.max_ring || sqdist < 12.0f) {  // :237
+        if (ring > kc.max_ring || sqdist < 12.0f) {  // :237
             code = ((border ? PC_IGNORED_BORDER : PC_IGNORED) << 24) | (uint32_t)cell;
         } else {
             const float* G = v.layer(sp.slot, L_GROUND);
@@ -301,8 +302,8 @@ __device__ __forceinline__ uint32_t rasterize_point(const View& v, const SlotPar
 #pragma unroll
                         for (int q = 0; q < 9; ++q) e[q] = C[(r0 + q % 3) + (c0 + q / 3) * N];
                         const float bs = tree9(e);
-                        if ((double)bs > k.min_outlier_conf && C[ix + iy * N] > 0.01f &&
-                            (double)G[ix + iy * N] >= __dadd_rn((double)__fadd_rn(sz, oz), k.outlier_tol)) {
+                        if ((double)bs > kc.min_outlier_conf && C[ix + iy * N] > 0.01f &&
+                            (double)G[ix + iy * N] >= __dadd_rn((double)__fadd_rn(sz, oz), kc.outlier_tol)) {
                             outlier = true;
                             break;
                         }
@@ -738,18 +739,19 @@ constexpr int DT_W = DT_X + 2 * DT_H;   // 36
 constexpr int DT_R = DT_Y + 2 * DT_H;   // 12
 
 // confidence decay of interpolate_cell (:464): std::max(c - c / decrease_factor, 0.001) in fp64
-__device__ __forceinline__ float decay_confidence(const Const& k, float occ) {
+__device__ __forceinline__ float decay_confidence(const CfgConst& kc, float occ) {
     // Confidences sit at the 0.001 floor in most of the map; from there (and below) the result is the floor
-    // again (host-checked for the configured factor, Const::decay_floor_ok), which skips the fp64 division.
-    if (k.decay_floor_ok && occ <= 0.001f) return 0.001f;
+    // again (host-checked for the configured factor, CfgConst::decay_floor_ok), which skips the fp64 division.
+    if (kc.decay_floor_ok && occ <= 0.001f) return 0.001f;
     const double o = (double)occ;
-    const double dec = __dsub_rn(o, __ddiv_rn(o, k.dec_factor));
+    const double dec = __dsub_rn(o, __ddiv_rn(o, kc.dec_factor));
     return (float)((dec < 0.001) ? 0.001 : dec);
 }
 
 // Fused into k_detect: every cell is copied to its home slot(s) as soon as its final G, C are known.
 __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams& sp, int cell, int x, int y, float g, float c, bool far) {
     const Const& k = v.k;
+    const CfgConst& kc = sp.cfg;
     const int4 home = __ldg(reinterpret_cast<const int4*>(v.skew.cell_home) + cell);
     if (home.x < 0) return;
     const int cidx = k.N / 2 - 1;
@@ -758,7 +760,7 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
         c = 1.0f;
     }
     // :463: beyond minDistSquared (`far`, from the per-cell table) the visit stores the decayed confidence (:464)
-    const float d1 = far ? decay_confidence(k, c) : -1.0f;
+    const float d1 = far ? decay_confidence(kc, c) : -1.0f;
     float2* SK = v.skew.sk + (size_t)sp.slot * v.skew.slots;
     float* SD = v.skew.sd + (size_t)sp.slot * v.skew.slots;
     const float2 gc = make_float2(g, c);
@@ -766,19 +768,19 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
     SD[home.x] = d1;
     if (home.y >= 0) {
         SK[home.y] = gc;
-        SD[home.y] = far ? decay_confidence(k, d1) : -1.0f;  // second visit of a ring corner
+        SD[home.y] = far ? decay_confidence(kc, d1) : -1.0f;  // second visit of a ring corner
     }
     if (home.z >= 0) SK[home.z] = gc;
     if (home.w >= 0) SK[home.w] = gc;
 }
 
 // Per-cell quantities of detect_ground_patches that depend only on the grid and the configuration, computed
-// once (gg_create / gg_set_config) with the very operations of the per-scan code they replace:
+// once per configuration variant (gg_capi.cu:build_variant) with the very operations of the per-scan code they replace:
 //   x: max(3, floor(threshold * S * expectedPoints))  (:364; integer valued, exact in float, capped at 2^24)
 //   y: variance threshold (:369)      z: expectedPoints      w: flags
 constexpr int DTF_S5 = 1, DTF_FAR = 2, DTF_INNER = 4;
 
-__global__ void k_build_detect_table(View v, float4* __restrict__ tab) {
+__global__ void k_build_detect_table(View v, const CfgConst kc, float4* __restrict__ tab) {
     const Const& k = v.k;
     const int N = k.N;
     const int cell = blockIdx.x * blockDim.x + threadIdx.x;
@@ -788,7 +790,7 @@ __global__ void k_build_detect_table(View v, float4* __restrict__ tab) {
     const float sqdist = (float)__dmul_rn(__dadd_rn(__dmul_rn(di, di), __dmul_rn(dj, dj)), k.res_sq);  // :332,356
     const float e = v.expected[cell];
     int flags = 0;
-    if (!((double)sqdist <= k.psc_sq)) flags |= DTF_S5;
+    if (!((double)sqdist <= kc.psc_sq)) flags |= DTF_S5;
     // union of the four sections, :325-328: first index in [2, 2 * (N / 2) - 2) (the upper half starts at N / 2 and has
     // N / 2 - 2 entries: one row short of N - 2 when N is odd), second index in [2, N - 2)
     if (i >= 2 && i < 2 * (N / 2) - 2 && j >= 2 && j < N - 2) flags |= DTF_INNER;
@@ -796,12 +798,12 @@ __global__ void k_build_detect_table(View v, float4* __restrict__ tab) {
     const float fx = __fsub_rn((float)i, (float)cidx), fy = __fsub_rn((float)j, (float)cidx);
     if (__dmul_rn(__dadd_rn(__dmul_rn((double)fx, (double)fx), __dmul_rn((double)fy, (double)fy)), k.res_sq) > 12.0) flags |= DTF_FAR;  // :463
     const double S = (flags & DTF_S5) ? 5.0 : 3.0;
-    double need = floor(__dmul_rn(__dmul_rn(k.gp_thresh, S), (double)e));
+    double need = floor(__dmul_rn(__dmul_rn(kc.gp_thresh, S), (double)e));
     need = (need < 3.0) ? 3.0 : need;                 // NaN -> NaN: the comparison below stays false, as in the reference
     if (need > 16777216.0) need = 16777216.0;         // patch sums are counts far below 2^24
-    const double a = __dmul_rn((double)sqdist, k.df_sq);
-    const double m = (a < k.mdf_sq) ? k.mdf_sq : a;
-    const float vt = (float)((k.mdf10_sq < m) ? k.mdf10_sq : m);
+    const double a = __dmul_rn((double)sqdist, kc.df_sq);
+    const double m = (a < kc.mdf_sq) ? kc.mdf_sq : a;
+    const float vt = (float)((kc.mdf10_sq < m) ? kc.mdf10_sq : m);
     tab[cell] = make_float4((float)need, vt, e, __int_as_float(flags));
 }
 
@@ -809,7 +811,7 @@ __global__ void k_build_detect_table(View v, float4* __restrict__ tab) {
 // sPV / sPM hold the products count * variance and count * minHeight of every tile entry (the very fmul the
 // reference's cwiseProduct performs, done once per entry instead of once per window position)
 template <int S>
-__device__ __forceinline__ bool detect_patch(const Const& k, const float (*sP)[DT_W], const float (*sPV)[DT_W], const float (*sPM)[DT_W],
+__device__ __forceinline__ bool detect_patch(const CfgConst& kc, const float (*sP)[DT_W], const float (*sPV)[DT_W], const float (*sPM)[DT_W],
                                              const float (*sM)[DT_W], int li, int lj, float variance, float need, float vt, float e, float& g,
                                              float& c) {
     constexpr int H = S / 2;
@@ -826,7 +828,7 @@ __device__ __forceinline__ bool detect_patch(const Const& k, const float (*sP)[D
         const float t = sM[c0 + q / S][r0 + q % S];
         localmin = (t < localmin) ? t : localmin;
     }
-    const float maxVar = (sP[lj][li] >= k.pc_var_thresh_f)
+    const float maxVar = (sP[lj][li] >= kc.pc_var_thresh_f)
                              ? variance
                              : __fdiv_rn(TreeSum<0, S * S>::run([&](int q) { return sPV[c0 + q / S][r0 + q % S]; }), psum);
     const float groundlevel = __fdiv_rn(TreeSum<0, S * S>::run([&](int q) { return sPM[c0 + q / S][r0 + q % S]; }), psum);
@@ -834,16 +836,16 @@ __device__ __forceinline__ bool detect_patch(const Const& k, const float (*sP)[D
     const float groundDiff = (gd < 1.0f) ? 1.0f : gd;  // std::max(gd, 1.0f)
 
     // do not update known high confidence estimations upward, :379
-    if ((double)oc > 0.5 && (double)groundlevel >= __dadd_rn((double)og, k.outlier_tol)) return false;
+    if ((double)oc > 0.5 && (double)groundlevel >= __dadd_rn((double)og, kc.outlier_tol)) return false;
 
     if ((double)vt > __dmul_rn((double)maxVar, (double)maxVar) && maxVar > 0.0f &&
-        (double)psum > __dmul_rn((double)__fmul_rn(__fmul_rn(groundDiff, e), (float)S), k.gp_thresh)) {
-        const double ncd = __ddiv_rn((double)psum, k.occ_factor);
+        (double)psum > __dmul_rn((double)__fmul_rn(__fmul_rn(groundDiff, e), (float)S), kc.gp_thresh)) {
+        const double ncd = __ddiv_rn((double)psum, kc.occ_factor);
         const float nc = (float)((1.0 < ncd) ? 1.0 : ncd);  // std::min(ncd, 1.0)
         const float num = __fadd_rn(__fmul_rn(groundlevel, nc), __fmul_rn(__fmul_rn(oc, og), 2.0f));
         const float den = __fadd_rn(nc, __fmul_rn(oc, 2.0f));
         g = __fdiv_rn(num, den);
-        const double cd = __ddiv_rn(__dadd_rn(__ddiv_rn((double)psum, k.occ_factor2), (double)oc), 2.0);
+        const double cd = __ddiv_rn(__dadd_rn(__ddiv_rn((double)psum, kc.occ_factor2), (double)oc), 2.0);
         c = (float)((1.0 < cd) ? 1.0 : cd);
         return true;
     }
@@ -861,6 +863,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_ldg(View v, c
     __shared__ float sP[DT_R][DT_W], sPV[DT_R][DT_W], sPM[DT_R][DT_W], sM[DT_R][DT_W];
     const SlotParams& sp = batch[blockIdx.z];
     const Const& k = v.k;
+    const CfgConst& kc = sp.cfg;
     const int N = k.N;
     const int i0 = blockIdx.x * DT_X, j0 = blockIdx.y * DT_Y;
     // one 64-bit base per scan, 32-bit offsets below it (all layers of a slot span far less than 2^31 floats)
@@ -895,7 +898,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_ldg(View v, c
         g = L0[L_GROUND * N2 + cell];
         c = L0[L_GROUNDPATCH * N2 + cell];
         variance = V[cell];
-        tb = __ldg(v.detect_tab + cell);
+        tb = __ldg(sp.detect_tab + cell);
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -913,8 +916,8 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_ldg(View v, c
     const int flags = __float_as_int(tb.w);
     if (flags & DTF_INNER) {
         const int li = threadIdx.x + DT_H, lj = threadIdx.y + DT_H;
-        const bool changed = (flags & DTF_S5) ? detect_patch<5>(k, sP, sPV, sPM, sM, li, lj, variance, tb.x, tb.y, tb.z, g, c)
-                                              : detect_patch<3>(k, sP, sPV, sPM, sM, li, lj, variance, tb.x, tb.y, tb.z, g, c);
+        const bool changed = (flags & DTF_S5) ? detect_patch<5>(kc, sP, sPV, sPM, sM, li, lj, variance, tb.x, tb.y, tb.z, g, c)
+                                              : detect_patch<3>(kc, sP, sPV, sPM, sM, li, lj, variance, tb.x, tb.y, tb.z, g, c);
         if (changed) {
             L0[L_GROUND * N2 + cell] = g;
             L0[L_GROUNDPATCH * N2 + cell] = c;
@@ -927,10 +930,10 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_ldg(View v, c
         // confidence of a cell only changes at its own visit(s), so decay(C) after patch
         // detection is exactly what the (first) visit will store; ring corners (i == j) are
         // visited twice and need the second decay as well.
-        const float d1 = decay_confidence(k, c);
+        const float d1 = decay_confidence(kc, c);
         float* D1 = v.roll_scratch + (size_t)sp.slot * 2 * k.N2;
         D1[cell] = d1;
-        if (i == j) D1[k.N2 + cell] = decay_confidence(k, d1);
+        if (i == j) D1[k.N2 + cell] = decay_confidence(kc, d1);
     }
 }
 
@@ -1019,28 +1022,28 @@ __device__ __forceinline__ float tree9s(const float (*Q)[DT_WT], const float (*P
 
 // the decision part of detect_ground_patch<S> (:364-394) on the window quantities; returns true when (g, c) changed
 template <int S>
-__device__ __forceinline__ bool detect_decide(const Const& k, float psum, float localmin, float sumPV, float sumPM, float centerP, float variance, float vt,
+__device__ __forceinline__ bool detect_decide(const CfgConst& kc, float psum, float localmin, float sumPV, float sumPM, float centerP, float variance, float vt,
                                               float e, float& g, float& c) {
     const float oc = c, og = g;
-    const float maxVar = (centerP >= k.pc_var_thresh_f) ? variance : __fdiv_rn(sumPV, psum);
+    const float maxVar = (centerP >= kc.pc_var_thresh_f) ? variance : __fdiv_rn(sumPV, psum);
     const float groundlevel = __fdiv_rn(sumPM, psum);
     const float gd = __fmul_rn(__fsub_rn(groundlevel, og), __fmul_rn(2.0f, oc));
     const float groundDiff = (gd < 1.0f) ? 1.0f : gd;  // std::max(gd, 1.0f)
     // do not update known high confidence estimations upward, :379
-    if ((double)oc > 0.5 && (double)groundlevel >= __dadd_rn((double)og, k.outlier_tol)) return false;
+    if ((double)oc > 0.5 && (double)groundlevel >= __dadd_rn((double)og, kc.outlier_tol)) return false;
     if ((double)vt > __dmul_rn((double)maxVar, (double)maxVar) && maxVar > 0.0f &&
-        (double)psum > __dmul_rn((double)__fmul_rn(__fmul_rn(groundDiff, e), (float)S), k.gp_thresh)) {
+        (double)psum > __dmul_rn((double)__fmul_rn(__fmul_rn(groundDiff, e), (float)S), kc.gp_thresh)) {
         // std::min(psum / factor, 1.0): a quotient of at least one needs no division (psum >= factor > 0 <=> quotient >= 1)
         float nc = 1.0f;
-        if (!(k.occ_factor > 0.0 && (double)psum >= k.occ_factor)) {
-            const double ncd = __ddiv_rn((double)psum, k.occ_factor);
+        if (!(kc.occ_factor > 0.0 && (double)psum >= kc.occ_factor)) {
+            const double ncd = __ddiv_rn((double)psum, kc.occ_factor);
             nc = (float)((1.0 < ncd) ? 1.0 : ncd);
         }
         const float num = __fadd_rn(__fmul_rn(groundlevel, nc), __fmul_rn(__fmul_rn(oc, og), 2.0f));
         const float den = __fadd_rn(nc, __fmul_rn(oc, 2.0f));
         g = __fdiv_rn(num, den);
         // std::min((psum / (factor * 2.0f) + oc) / 2.0, 1.0): halving is exact (x * 0.5)
-        const double cd = __dmul_rn(__dadd_rn(__ddiv_rn((double)psum, k.occ_factor2), (double)oc), 0.5);
+        const double cd = __dmul_rn(__dadd_rn(__ddiv_rn((double)psum, kc.occ_factor2), (double)oc), 0.5);
         c = (float)((1.0 < cd) ? 1.0 : cd);
         return true;
     }
@@ -1063,6 +1066,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_tma(View v, c
     __shared__ __align__(8) uint64_t s_bar[2];
     const SlotParams& sp = batch[blockIdx.z];
     const Const& k = v.k;
+    const CfgConst& kc = sp.cfg;
     const int N = k.N, N2 = k.N2;
     const int i0 = blockIdx.x * DT_X;
     const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * DT_X + tx;
@@ -1101,7 +1105,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_tma(View v, c
         if (live) {
             g = L0[L_GROUND * N2 + cell];
             c = L0[L_GROUNDPATCH * N2 + cell];
-            tb = __ldg(v.detect_tab + cell);
+            tb = __ldg(sp.detect_tab + cell);
         }
         const int flags = __float_as_int(tb.w);
         mbar_wait(&s_bar[kk & 1], (uint32_t)((kk >> 1) & 1));
@@ -1176,7 +1180,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_tma(View v, c
                         const float t = s.N5[c0 + q][r0];
                         localmin = (t < localmin) ? t : localmin;
                     }
-                    changed = detect_decide<5>(k, psum, localmin, tree25(s.QV, s.PV2, s.TV, r0, c0), tree25(s.QM, s.PM2, s.TM, r0, c0), centerP, variance,
+                    changed = detect_decide<5>(kc, psum, localmin, tree25(s.QV, s.PV2, s.TV, r0, c0), tree25(s.QM, s.PM2, s.TM, r0, c0), centerP, variance,
                                                tb.y, tb.z, g, c);
                 } else {
                     const int r0 = li - 1, c0 = lj - 1;
@@ -1186,7 +1190,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_tma(View v, c
                         const float t = s.N3[c0 + q][r0];
                         localmin = (t < localmin) ? t : localmin;
                     }
-                    changed = detect_decide<3>(k, psum, localmin, tree9s(s.QV, s.PV2, r0, c0), tree9s(s.QM, s.PM2, r0, c0), centerP, variance, tb.y, tb.z, g, c);
+                    changed = detect_decide<3>(kc, psum, localmin, tree9s(s.QV, s.PV2, r0, c0), tree9s(s.QM, s.PM2, r0, c0), centerP, variance, tb.y, tb.z, g, c);
                 }
             }
         }
@@ -1198,18 +1202,18 @@ __global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_tma(View v, c
             if (v.skew.sk) {
                 skew_store_cell(v, sp, cell, i, j, g, c, (flags & DTF_FAR) != 0);
             } else if (v.spiral_recs) {
-                const float d1 = decay_confidence(k, c);
+                const float d1 = decay_confidence(kc, c);
                 float* D1 = v.roll_scratch + (size_t)sp.slot * 2 * k.N2;
                 D1[cell] = d1;
-                if (i == j) D1[k.N2 + cell] = decay_confidence(k, d1);
+                if (i == j) D1[k.N2 + cell] = decay_confidence(kc, d1);
             }
         }
         __syncthreads();   // the derived arrays and this stage are free again
     }
 }
 
-int launch_build_detect_table(const View& v, float4* tab, cudaStream_t st) {
-    k_build_detect_table<<<(v.k.N2 + 255) / 256, 256, 0, st>>>(v, tab);
+int launch_build_detect_table(const View& v, const CfgConst& c, float4* tab, cudaStream_t st) {
+    k_build_detect_table<<<(v.k.N2 + 255) / 256, 256, 0, st>>>(v, c, tab);
     return 1;
 }
 
@@ -1224,6 +1228,7 @@ constexpr int SPIRAL_THREADS = 512;
 __global__ void __launch_bounds__(SPIRAL_THREADS) k_spiral(View v, const SlotParams* __restrict__ batch) {
     const SlotParams& sp = batch[blockIdx.x];
     const Const& k = v.k;
+    const CfgConst& kc = sp.cfg;
     const int N = k.N;
     float* G = v.layer(sp.slot, L_GROUND);
     float* C = v.layer(sp.slot, L_GROUNDPATCH);
@@ -1255,7 +1260,7 @@ __global__ void __launch_bounds__(SPIRAL_THREADS) k_spiral(View v, const SlotPar
             const double d2 = __dmul_rn(__dadd_rn(__dmul_rn((double)fx, (double)fx), __dmul_rn((double)fy, (double)fy)), k.res_sq);
             if (d2 > 12.0) {  // :463
                 const double o = (double)occ;
-                const double dec = __dsub_rn(o, __ddiv_rn(o, k.dec_factor));
+                const double dec = __dsub_rn(o, __ddiv_rn(o, kc.dec_factor));
                 C[x + y * N] = (float)((dec < 0.001) ? 0.001 : dec);  // std::max(dec, 0.001)
             }
         }
@@ -1782,9 +1787,10 @@ __global__ void __launch_bounds__(256) k_label(View v, const SlotParams* __restr
         } else if (cls == PC_KEPT || cls == PC_IGNORED) {
             const double groundheight = (double)gh[u];
             // std::max(std::min((f * dist) / variance * thres, thres), obs_thres) with C++ min/max semantics
-            const double a = __dmul_rn(__ddiv_rn(__dmul_rn(k.lab_fac, (double)dist[u]), (double)var[u]), k.lab_thres);
-            double t = (k.lab_thres < a) ? k.lab_thres : a;
-            t = (t < k.lab_obs) ? k.lab_obs : t;
+            const double lab_fac = sp.cfg.lab_fac, lab_thres = sp.cfg.lab_thres, lab_obs = sp.cfg.lab_obs;
+            const double a = __dmul_rn(__ddiv_rn(__dmul_rn(lab_fac, (double)dist[u]), (double)var[u]), lab_thres);
+            double t = (lab_thres < a) ? lab_thres : a;
+            t = (t < lab_obs) ? lab_obs : t;
             if (__dadd_rn(t, groundheight) < (double)z[u]) {
                 label = GG_LABEL_NONGROUND;
                 atomicAdd(OBS + cell, 1.0f);  // small exact integers: order free
@@ -2147,7 +2153,7 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
 // interpolate_cell -- for callers that drive the phases themselves.  Same arithmetic as the pipeline kernels.
 // ------------------------------------------------------------------------------------------
 // GroundSegmentation::interpolate_cell (:445-465) for one cell, in place
-__global__ void k_interpolate_cell(View v, int slot, int x, int y) {
+__global__ void k_interpolate_cell(View v, const CfgConst kc, int slot, int x, int y) {
     const Const& k = v.k;
     const int N = k.N;
     float* G = v.layer(slot, L_GROUND);
@@ -2169,14 +2175,14 @@ __global__ void k_interpolate_cell(View v, int slot, int x, int y) {
     const double d2 = __dmul_rn(__dadd_rn(__dmul_rn((double)fx, (double)fx), __dmul_rn((double)fy, (double)fy)), k.res_sq);
     if (d2 > 12.0) {  // :463
         const double o = (double)occ;
-        const double dec = __dsub_rn(o, __ddiv_rn(o, k.dec_factor));
+        const double dec = __dsub_rn(o, __ddiv_rn(o, kc.dec_factor));
         C[x + y * N] = (float)((dec < 0.001) ? 0.001 : dec);  // std::max(dec, 0.001)
     }
 }
 
 // GroundSegmentation::detect_ground_patch<S> (:343-395) for one cell, reading the layers directly
 template <int S>
-__global__ void k_detect_cell(View v, int slot, int i, int j) {
+__global__ void k_detect_cell(View v, const CfgConst kc, int slot, int i, int j) {
     const Const& k = v.k;
     const int N = k.N, H = S / 2;
     const float* P = v.layer(slot, L_COUNT);
@@ -2190,12 +2196,12 @@ __global__ void k_detect_cell(View v, int slot, int i, int j) {
     const float sqdist = (float)__dmul_rn(__dadd_rn(__dmul_rn(di, di), __dmul_rn(dj, dj)), k.res_sq);  // :356
     const float e = v.expected[cell];
     const float psum = TreeSum<0, S * S>::run([&](int q) { return at(P, q); });
-    double need = floor(__dmul_rn(__dmul_rn(k.gp_thresh, (double)S), (double)e));
+    double need = floor(__dmul_rn(__dmul_rn(kc.gp_thresh, (double)S), (double)e));
     need = (need < 3.0) ? 3.0 : need;
     if ((double)psum < need) return;  // :364
-    const double a = __dmul_rn((double)sqdist, k.df_sq);
-    const double m = (a < k.mdf_sq) ? k.mdf_sq : a;
-    const float vt = (float)((k.mdf10_sq < m) ? k.mdf10_sq : m);  // :369
+    const double a = __dmul_rn((double)sqdist, kc.df_sq);
+    const double m = (a < kc.mdf_sq) ? kc.mdf_sq : a;
+    const float vt = (float)((kc.mdf10_sq < m) ? kc.mdf10_sq : m);  // :369
     float localmin = at(M, 0);
     for (int q = 1; q < S * S; ++q) {
         const float t = at(M, q);
@@ -2204,7 +2210,7 @@ __global__ void k_detect_cell(View v, int slot, int i, int j) {
     const float sumPV = TreeSum<0, S * S>::run([&](int q) { return __fmul_rn(at(P, q), at(V, q)); });
     const float sumPM = TreeSum<0, S * S>::run([&](int q) { return __fmul_rn(at(P, q), at(M, q)); });
     float g = G[cell], c = C[cell];
-    if (detect_decide<S>(k, psum, localmin, sumPV, sumPM, P[cell], V[cell], vt, e, g, c)) {
+    if (detect_decide<S>(kc, psum, localmin, sumPV, sumPM, P[cell], V[cell], vt, e, g, c)) {
         G[cell] = g;
         C[cell] = c;
     }
@@ -2225,16 +2231,16 @@ int launch_spiral_only(const View& v, const SlotParams* batch, int count, cudaSt
     return 1;
 }
 
-int launch_interpolate_cell(const View& v, int slot, int x, int y, cudaStream_t st) {
-    k_interpolate_cell<<<1, 1, 0, st>>>(v, slot, x, y);
+int launch_interpolate_cell(const View& v, const CfgConst& c, int slot, int x, int y, cudaStream_t st) {
+    k_interpolate_cell<<<1, 1, 0, st>>>(v, c, slot, x, y);
     return 1;
 }
 
-int launch_detect_cell(const View& v, int slot, int S, int i, int j, cudaStream_t st) {
+int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, cudaStream_t st) {
     if (S == 3)
-        k_detect_cell<3><<<1, 1, 0, st>>>(v, slot, i, j);
+        k_detect_cell<3><<<1, 1, 0, st>>>(v, c, slot, i, j);
     else
-        k_detect_cell<5><<<1, 1, 0, st>>>(v, slot, i, j);
+        k_detect_cell<5><<<1, 1, 0, st>>>(v, c, slot, i, j);
     return 1;
 }
 

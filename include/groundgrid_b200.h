@@ -19,8 +19,10 @@
  *   - layers: N x N float, column-major like Eigen::MatrixXf: element (i, j) at i + j*N,
  *     row index i grows toward -x, column index j toward -y (grid_map convention).
  *   - one handle owns `n_slots` independent maps ("slots"); slot s is what one
- *     GroundGrid + GroundSegmentation pair owns in the reference.  n_slots == 1 is the
- *     plain drop-in; n_slots > 1 is the batched throughput mode (independent scans).
+ *     GroundGrid + GroundSegmentation pair owns in the reference: its map and its
+ *     configuration (gg_set_slot_config).  n_slots == 1 is the plain drop-in; n_slots > 1 is
+ *     the batched throughput mode (independent scans, e.g. of sensors with different
+ *     settings, in one launch).
  */
 #ifndef GROUNDGRID_B200_H
 #define GROUNDGRID_B200_H
@@ -110,6 +112,22 @@ int gg_num_slots(gg_handle h);
  * (src/GroundGrid.cpp:48, src/GroundSegmentation.cpp:468-471; GroundGridNodelet.cpp:299-302). */
 int gg_set_config(gg_handle h, const gg_config* cfg);
 int gg_get_config(gg_handle h, gg_config* cfg);
+/* gg_set_config is handle-wide: it waits for all work of the handle, then sets every slot's configuration
+ * (replacing per-slot settings); gg_get_config returns what it last set (the defaults until then). */
+
+/* GroundSegmentation::setConfig / GroundGrid::setConfig of the pair that owns slot `slot`
+ * (src/GroundSegmentation.cpp:468-471, src/GroundGrid.cpp:48, GroundGridNodelet.cpp:299-302).
+ * A slot starts with the handle-wide configuration and keeps its own through gg_init_map, rolls and
+ * configuration changes of other slots.  The new configuration applies from the slot's next launch on
+ * (every path: gg_filter_cloud[_batch[_begin]], gg_run_scans[_device], the per-phase entries).
+ * gg_set_slot_config waits only for the work already enqueued on the slot's stream group; other groups keep
+ * running with their own configurations.  (That stream may itself wait on work of other groups -- with GG_STAGGER
+ * set, or after gg_fork_streams / gg_join_streams -- and such work is then waited for as well.)  A
+ * gg_filter_cloud_batch_begin batch that contains the slot must be waited for (gg_filter_cloud_batch_wait or
+ * gg_synchronize) first.  Slots with identical settings share one copy of the derived device data.  thread_count is accepted and unused.  GG_E_ARG: null handle or config,
+ * slot out of range; values are not validated (like gg_set_config). */
+int gg_set_slot_config(gg_handle h, int slot, const gg_config* cfg);
+int gg_get_slot_config(gg_handle h, int slot, gg_config* cfg);
 
 /* Replaces GroundGrid::initGroundGrid (src/GroundGrid.cpp:50-80): map centred on (x, y),
  * ground = z, groundpatch = 1e-7, points = 0, min = 100, max = -100. */
@@ -149,7 +167,7 @@ int gg_filter_cloud(gg_handle h, int slot, const gg_point* points, size_t n, con
  * cross the bus; whenever the packers fall behind the bus (fewer than two packed clouds queued for
  * copying), the calling thread sends scans from the back of the batch, which no packer has reached
  * yet, as plain 32-byte records.  GG_HOST_PACK=1 packs every scan, GG_HOST_PACK=0 none.  Results
- * are identical in all modes. */
+ * are identical in all modes.  Every scan runs with its slot's configuration (gg_set_slot_config). */
 int gg_filter_cloud_batch(gg_handle h, int count, const gg_scan_desc* scans, const gg_point* const* points,
                           uint8_t* const* labels_out);
 
