@@ -12,6 +12,8 @@ from .synth import POINT_DTYPE
 
 GG_FLAG_FULL_LAYERS = 1
 LABEL_ABSENT, LABEL_GROUND, LABEL_NONGROUND = 0, 49, 99
+SELECT_GROUND, SELECT_NONGROUND = 1, 2
+SELECT = {None: 0, "ground": SELECT_GROUND, "nonground": SELECT_NONGROUND, "all": SELECT_GROUND | SELECT_NONGROUND}
 
 
 class GroundGridError(RuntimeError):
@@ -50,6 +52,35 @@ class ScanDesc(C.Structure):
         ("_pad", C.c_float),
         ("base_z", C.c_double),
     ]
+
+
+# numpy image of an array of gg_scan_desc (ScanDesc)
+SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "n_points", "origin", "base_z"], "formats": [np.int32, np.uint64, (np.float32, 3), np.float64],
+                            "offsets": [0, 8, 16, 32], "itemsize": C.sizeof(ScanDesc)})
+
+
+class DeviceOutputs:
+    """What GroundGridB200.run_scans_to_device returns: per-scan views into flat CUDA tensors.
+      labels[k] : uint8 [n_k], the labels of every input point (None unless asked for)
+      cloud[k]  : float32 [n_k, 8], the selected output points as 32-byte records, intensity 49 / 99 (None without select)
+      index[k]  : int32 [n_k], input index of each selected point (None unless asked for)
+      counts    : int32 [count] on the device, selected points of each scan (None without select)
+    Only the first counts[k] entries of cloud[k] / index[k] are written.  They are complete in the order of `stream`."""
+
+    def __init__(self, labels, cloud, index, counts, stream):
+        self.labels, self.cloud, self.index, self.counts, self.stream = labels, cloud, index, counts, stream
+
+    def trimmed(self):
+        """(cloud, index) with every view cut to its count: one host synchronisation (counts.tolist()) per batch."""
+        import torch
+
+        with torch.cuda.stream(self.stream):
+            n = self.counts.tolist()
+
+        def cut(views):
+            return None if views is None else [v[:k] for v, k in zip(views, n)]
+
+        return cut(self.cloud), cut(self.index)
 
 
 _lib = None
@@ -97,6 +128,7 @@ def load(build_if_missing=True):
         "gg_download_labels": (i, [vp, i, vp, sz]),
         "gg_synchronize": (i, [vp]),
         "gg_run_scans_device": (i, [vp, i, vp, vp, i]),
+        "gg_run_scans_to_device": (i, [vp, i, vp, vp, vp, C.c_uint, vp, vp]),
         "gg_upload_cloud_msg": (i, [vp, i, vp, sz, i, vp, vp]),
         "gg_terrain_image": (i, [vp, i, vp]),
         "gg_layer_image_u8": (i, [vp, i, C.c_char_p, vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
@@ -385,6 +417,73 @@ class GroundGridB200:
         """dev_ptrs: device addresses (ints) of the per-scan clouds (32-byte records)."""
         pp = (C.c_void_p * len(descs))(*dev_ptrs)
         _check(self._l.gg_run_scans_device(self._h, len(descs), descs, pp, stop_after))
+
+    def run_scans_to_device_ptrs(self, descs, dev_ptrs, out_ptrs, select, counts_ptr, stream_ptr):
+        """gg_run_scans_to_device with raw device addresses.  descs: ScanDesc array or SCAN_DESC_DTYPE array;
+        out_ptrs: uint64 [count, 3] (labels, index, cloud; 0 = none) or None; select: GG_SELECT_* bits;
+        counts_ptr / stream_ptr: ints or None (stream None = the legacy default stream)."""
+        count = len(descs)
+        d = _ptr(descs) if isinstance(descs, np.ndarray) else descs
+        pp = np.ascontiguousarray(np.array(dev_ptrs, dtype=np.uint64).reshape(count))
+        op = None if out_ptrs is None else np.ascontiguousarray(out_ptrs, dtype=np.uint64).reshape(count, 3)
+        _check(self._l.gg_run_scans_to_device(self._h, count, d, _ptr(pp), _ptr(op), int(select), counts_ptr, stream_ptr))
+
+    def run_scans_to_device(self, clouds, slots, origins, base_z, labels=True, select="nonground", index=False, stream=None):
+        """One scan per slot on caller-owned CUDA tensors, results left in new CUDA tensors (gg_run_scans_to_device).
+          clouds : contiguous CUDA tensors of 32-byte point records (e.g. float32 [n, 8] or uint8 [n * 32]), 16-byte aligned
+          origins: [count][3] sensor positions in the map frame; base_z: one value or one per scan
+          select : labels of the output cloud to return: "nonground" (the obstacle points), "ground", "all" (what get_output
+                   returns) or None (no cloud)
+          index  : also return the input index of each returned point
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream); the outputs are allocated on it.
+        The call returns without waiting for the device.  Work enqueued on `stream` afterwards sees complete outputs, and
+        the inputs may be freed right after the call when they were allocated on `stream` (other streams' inputs are
+        marked in use on `stream`).  Returns DeviceOutputs."""
+        import torch
+
+        if select not in SELECT:
+            raise ValueError(f"select must be one of {list(SELECT)}")
+        sel = SELECT[select]
+        if index and not sel:
+            raise ValueError("index needs a select")
+        dev = torch.device("cuda", self.device)
+        current = torch.cuda.current_stream(dev)
+        stream = current if stream is None else stream
+        count = len(clouds)
+        n = []
+        for c in clouds:
+            nbytes = c.numel() * c.element_size()
+            if c.device != dev or not c.is_contiguous() or nbytes % 32:
+                raise ValueError(f"clouds must be contiguous tensors of 32-byte records on {dev}")
+            n.append(nbytes // 32)
+        base_z = np.broadcast_to(np.asarray(base_z, np.float64), (count,))
+        descs = np.zeros(count, SCAN_DESC_DTYPE)
+        descs["slot"] = np.asarray(slots, np.int32)
+        descs["n_points"] = n
+        descs["origin"] = np.asarray(origins, np.float32).reshape(count, 3)
+        descs["base_z"] = base_z
+        offs = np.zeros(count, np.uint64)
+        offs[1:] = np.cumsum(n[:-1], dtype=np.uint64)
+        total = int(sum(n))
+        with torch.cuda.stream(stream):
+            lab = torch.empty(total, dtype=torch.uint8, device=dev) if labels else None
+            cld = torch.empty((total, 8), dtype=torch.float32, device=dev) if sel else None
+            idx = torch.empty(total, dtype=torch.int32, device=dev) if index else None
+            counts = torch.empty(count, dtype=torch.int32, device=dev) if sel else None
+        ptrs = np.zeros((count, 3), np.uint64)
+        for col, t, size in ((0, lab, 1), (1, idx, 4), (2, cld, 32)):
+            if t is not None and total:
+                ptrs[:, col] = np.uint64(t.data_ptr()) + offs * np.uint64(size)
+        if stream != current:
+            for c in clouds:
+                c.record_stream(stream)
+        self.run_scans_to_device_ptrs(descs, [c.data_ptr() for c in clouds], ptrs, sel,
+                                      counts.data_ptr() if counts is not None else None, stream.cuda_stream or None)
+
+        def views(t):
+            return None if t is None else list(torch.split(t, n))
+
+        return DeviceOutputs(views(lab), views(cld), views(idx), counts, stream)
 
     # -- steps next to the path (SURVEY section 8f)
     def upload_cloud_msg(self, raw, n_points, point_step, field_offsets, T_map_from_frame=None, slot=0):

@@ -302,7 +302,11 @@ struct gg_handle_s {
     // parameter staging ring: pinned host copy + device copy per entry
     gg::SlotParams* h_ring = nullptr;
     gg::SlotParams* d_ring = nullptr;
+    gg::OutDest* h_dest = nullptr;   // output destinations of the entry's scans, same shape as h_ring / d_ring
+    gg::OutDest* d_dest = nullptr;
     cudaEvent_t ring_ev[kRing] = {};
+    cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
+    cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
     bool ring_used[kRing] = {};
     int ring_pos = 0;
     uint64_t launches = 0;
@@ -423,6 +427,14 @@ int ring_commit(gg_handle h, int pos, int count, cudaStream_t st) {
     return GG_OK;
 }
 
+// Output destinations of a staging entry (the array parallel to its SlotParams) and their copy to the device.
+gg::OutDest* ring_dests(gg_handle h, int pos) { return h->h_dest + (size_t)pos * h->n_slots; }
+gg::OutDest* ring_dests_dev(gg_handle h, int pos) { return h->d_dest + (size_t)pos * h->n_slots; }
+int ring_commit_dests(gg_handle h, int pos, int count, cudaStream_t st) {
+    GG_CUDA(cudaMemcpyAsync(ring_dests_dev(h, pos), ring_dests(h, pos), (size_t)count * sizeof(gg::OutDest), cudaMemcpyHostToDevice, st));
+    return GG_OK;
+}
+
 // The entry may be reused once the kernels that read it have finished (they may run on any of
 // the handle's streams, so the event is recorded AFTER the launches, not after the copy).
 int ring_release(gg_handle h, int pos, cudaStream_t st) {
@@ -477,9 +489,18 @@ void fill_params(gg_handle h, const gg_scan_desc& d, gg::SlotParams& p, const gg
     p.packed = packed;
 }
 
-// enqueue the kernels of `count` scans, each group of slots on its own stream
+// Caller-owned destinations of gg_run_scans_to_device (validated by it) and the caller's stream.
+struct CallerOutputs {
+    const gg_scan_outputs* outs;  // [count] or null
+    unsigned select;
+    int32_t* counts;              // [count] or null
+    cudaStream_t stream;
+};
+
+// enqueue the kernels of `count` scans, each group of slots on its own stream; with `caller`, each group also writes
+// its scans' outputs and is ordered after / before the caller's stream
 int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int stop_after, const gg_point* const* dev_points = nullptr,
-                      const float* const* packed_ptrs = nullptr, uint8_t* labels_base = nullptr) {
+                      const float* const* packed_ptrs = nullptr, uint8_t* labels_base = nullptr, const CallerOutputs* caller = nullptr) {
     if (count <= 0) return GG_OK;
     if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
     int rc;
@@ -494,15 +515,31 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
     }
     gg::View view = h->view;
     if (labels_base) view.labels = labels_base;
+    // count + scan passes when counts are wanted; the write pass when any scan wants labels, index or cloud
+    const bool compact = caller && caller->counts && caller->select;
+    if (caller) GG_CUDA(cudaEventRecord(h->caller_in, caller->stream));
     for (int g = 0; g < h->n_streams; ++g) {
         gg::SlotParams *hp = nullptr, *dp = nullptr;
         int pos = 0, m = 0, max_points = 0;
+        bool write = false;
         for (int i = 0; i < count; ++i) {
             const gg_scan_desc& d = scans[i];
             if (stream_index(h, d.slot) != g) continue;
             if (m == 0 && (rc = ring_acquire(h, &hp, &dp, &pos))) return rc;
             const float* packed = packed_ptrs ? packed_ptrs[i] : nullptr;
             fill_params(h, d, hp[m], dev_points ? dev_points[i] : nullptr, packed);
+            if (caller) {
+                gg::OutDest& od = ring_dests(h, pos)[m];
+                std::memset(&od, 0, sizeof(od));
+                if (caller->outs) {
+                    od.labels = caller->outs[i].labels;
+                    od.index = caller->outs[i].index;
+                    od.cloud = caller->outs[i].cloud;
+                }
+                od.count = compact ? caller->counts + i : nullptr;
+                od.select = caller->select;
+                write = write || od.labels || od.index || od.cloud;
+            }
             ++m;
             max_points = std::max(max_points, (int)d.n_points);
             SlotState& s = h->slots[d.slot];
@@ -516,6 +553,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         if (m == 0) continue;
         cudaStream_t st = h->streams[g];
         if ((rc = ring_commit(h, pos, m, st))) return rc;
+        if ((compact || write) && (rc = ring_commit_dests(h, pos, m, st))) return rc;
         // Staggered stream pairs: the spiral is latency bound (a CTA per scan, a few warps per SM), every other kernel
         // fills the machine.  Stream 2k + 1 starts its scans when stream 2k has reached its spiral, so in steady state the
         // spirals of one half of the batch run underneath the bulk kernels of the other half instead of all at once.
@@ -529,9 +567,18 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
                 h->stagger_armed[g - 1] = false;
             }
         }
+        if (caller) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
         h->launches += gg::launch_scan_pipeline(view, dp, m, max_points, stop_after, st, h->prof, h->have_layer_map ? &h->layer_map : nullptr, after_detect);
         GG_CUDA(cudaGetLastError());
+        if (compact || write) {
+            h->launches += gg::launch_output(view, dp, ring_dests_dev(h, pos), m, max_points, compact, write, st, h->prof);
+            GG_CUDA(cudaGetLastError());
+        }
         if ((rc = ring_release(h, pos, st))) return rc;
+        if (caller) {
+            GG_CUDA(cudaEventRecord(h->caller_out[g], st));
+            GG_CUDA(cudaStreamWaitEvent(caller->stream, h->caller_out[g], 0));
+        }
     }
     return GG_OK;
 }
@@ -585,8 +632,14 @@ int run_output_on(gg_handle h, int slot, bool want_cloud, cudaStream_t st) {
     hp[0].slot = slot;
     hp[0].n_points = (int)s.n_points;
     hp[0].src = s.src ? s.src : h->view.points + (size_t)slot * h->pcap;
+    gg::OutDest& od = ring_dests(h, pos)[0];
+    std::memset(&od, 0, sizeof(od));
+    od.index = h->view.out_index + (size_t)slot * h->pcap;
+    od.cloud = want_cloud ? h->view.out_cloud + (size_t)slot * h->pcap : nullptr;
+    od.select = GG_SELECT_GROUND | GG_SELECT_NONGROUND;
     if ((rc = ring_commit(h, pos, 1, st))) return rc;
-    h->launches += gg::launch_output(h->view, dp, 1, (int)s.n_points, want_cloud, st, h->prof);
+    if ((rc = ring_commit_dests(h, pos, 1, st))) return rc;
+    h->launches += gg::launch_output(h->view, dp, ring_dests_dev(h, pos), 1, (int)s.n_points, true, true, st, h->prof);
     GG_CUDA(cudaGetLastError());
     if ((rc = ring_release(h, pos, st))) return rc;
     s.output_valid = true;
@@ -918,8 +971,12 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     }
     GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_ring), sizeof(gg::SlotParams) * kRing * S, cudaHostAllocDefault));
     GG_TRY(dev_alloc(h, &h->d_ring, (size_t)kRing * S));
+    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_dest), sizeof(gg::OutDest) * kRing * S, cudaHostAllocDefault));
+    GG_TRY(dev_alloc(h, &h->d_dest, (size_t)kRing * S));
     for (int i = 0; i < kRing; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->ring_ev[i], cudaEventDisableTiming));
     for (int i = 0; i < kStreams; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->stagger_ev[i], cudaEventDisableTiming));
+    GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_in, cudaEventDisableTiming));
+    for (int i = 0; i < kStreams; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_out[i], cudaEventDisableTiming));
     GG_TRY(build_variant(h, 0, h->streams[0]));
 #undef GG_TRY
 #undef GG_CUDA_TRY
@@ -937,8 +994,11 @@ int gg_destroy(gg_handle h) {
         if (h->d_raw[g]) cudaFree(h->d_raw[g]);
     if (h->h_stage) cudaFreeHost(h->h_stage);
     for (cudaEvent_t e : h->slot_ev) cudaEventDestroy(e);
-    for (int i = 0; i < kStreams; ++i)
+    for (int i = 0; i < kStreams; ++i) {
         if (h->stagger_ev[i]) cudaEventDestroy(h->stagger_ev[i]);
+        if (h->caller_out[i]) cudaEventDestroy(h->caller_out[i]);
+    }
+    if (h->caller_in) cudaEventDestroy(h->caller_in);
     for (int e = 0; e < 2; ++e)
         if (h->batch_done[e]) cudaEventDestroy(h->batch_done[e]);
     for (int e = 0; e < 8; ++e)
@@ -949,6 +1009,7 @@ int gg_destroy(gg_handle h) {
     if (h->copy_out) cudaStreamDestroy(h->copy_out);
     for (void* p : h->dev_allocs) cudaFree(p);
     if (h->h_ring) cudaFreeHost(h->h_ring);
+    if (h->h_dest) cudaFreeHost(h->h_dest);
     for (int i = 0; i < kRing; ++i)
         if (h->ring_ev[i]) cudaEventDestroy(h->ring_ev[i]);
     if (h->own_streams)
@@ -1144,6 +1205,42 @@ int gg_run_scans_device(gg_handle h, int count, const gg_scan_desc* scans, const
         if (!dev_points[i] && scans[i].n_points) return fail(GG_E_ARG, "scan %d: null device cloud", i);
     GG_CUDA(cudaSetDevice(h->device));
     return run_scans_grouped(h, count, scans, stop_after, dev_points);
+}
+
+namespace {
+bool ranges_overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+    const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+    return a && b && a_bytes && b_bytes && x < y + b_bytes && y < x + a_bytes;
+}
+}  // namespace
+
+int gg_run_scans_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_point* const* dev_points, const gg_scan_outputs* outs,
+                           unsigned select, int32_t* dev_counts, void* stream) {
+    if (!h || !scans || !dev_points) return fail(GG_E_ARG, "null argument");
+    if (select & ~(GG_SELECT_GROUND | GG_SELECT_NONGROUND)) return fail(GG_E_ARG, "unknown select bits 0x%x", select);
+    if (reinterpret_cast<uintptr_t>(dev_counts) % alignof(int32_t)) return fail(GG_E_ARG, "dev_counts is not 4-byte aligned");
+    h->inputs_busy = true;
+    for (int i = 0; i < count; ++i) {
+        const size_t n = scans[i].n_points;
+        const gg_point* in = dev_points[i];
+        if (!in && n) return fail(GG_E_ARG, "scan %d: null device cloud", i);
+        if (ranges_overlap(dev_counts ? dev_counts + i : nullptr, sizeof(int32_t), in, n * sizeof(gg_point)))
+            return fail(GG_E_ARG, "scan %d: dev_counts overlaps the input cloud", i);
+        if (!outs) continue;
+        const gg_scan_outputs& o = outs[i];
+        if (o.index || o.cloud) {
+            if (!select) return fail(GG_E_ARG, "scan %d: index / cloud requested with select 0", i);
+            if (!dev_counts) return fail(GG_E_ARG, "scan %d: index / cloud requested without dev_counts", i);
+        }
+        if (reinterpret_cast<uintptr_t>(o.index) % 4) return fail(GG_E_ARG, "scan %d: index is not 4-byte aligned", i);
+        if (reinterpret_cast<uintptr_t>(o.cloud) % 16) return fail(GG_E_ARG, "scan %d: cloud is not 16-byte aligned", i);
+        if (ranges_overlap(o.labels, n, in, n * sizeof(gg_point)) || ranges_overlap(o.index, n * sizeof(uint32_t), in, n * sizeof(gg_point)) ||
+            ranges_overlap(o.cloud, n * sizeof(gg_point), in, n * sizeof(gg_point)))
+            return fail(GG_E_ARG, "scan %d: an output overlaps the input cloud", i);
+    }
+    GG_CUDA(cudaSetDevice(h->device));
+    const CallerOutputs caller{outs, select, dev_counts, static_cast<cudaStream_t>(stream)};
+    return run_scans_grouped(h, count, scans, 0, dev_points, nullptr, nullptr, &caller);
 }
 
 // ---- "next" rows of SURVEY.md section 8(f) --------------------------------------------------

@@ -86,6 +86,18 @@ struct SlotParams {
     const float* packed;
 };
 
+// Per-scan destinations of the output kernels (launch_output).  They sit in the staging entry next to the scans'
+// SlotParams, in a parallel array with the same index: the handle's own buffers for gg_get_output, the caller's for
+// gg_run_scans_to_device.
+struct OutDest {
+    uint8_t* labels;   // [n_points] copy of the scan's labels; null: none
+    uint32_t* index;   // input index of each selected output point; null: none
+    gg_point* cloud;   // the selected output points (intensity = label); null: none
+    int* count;        // receives the number of selected points; null: none
+    unsigned select;   // GG_SELECT_* bits: labels that enter index / cloud / count
+    int reserved;      // zero
+};
+
 // Device side of the skewed-layout spiral (gg_host.h:SkewTables); null sk -> not used.
 constexpr int SKEW_XCH_ASYNC = 4;    // depth of the exchange ring of the barrier-free spiral variants (the barrier variant needs 2); the
                                      // synchronisation table is built for exactly this depth (gg_capi.cu -> build_skew_sync)
@@ -196,8 +208,11 @@ int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaSt
 int launch_spiral_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof);
 int launch_interpolate_cell(const View& v, const CfgConst& c, int slot, int x, int y, cudaStream_t st);
 int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, cudaStream_t st);
-int launch_output(const View& v, const SlotParams* batch, int count, int max_points, bool want_cloud, cudaStream_t st,
-                  Profiler* prof);
+// The output cloud of `count` completed scans, compacted into dests[k] (dests[k] goes with batch[k]).
+// compact: count + scan passes (needed for index / cloud / count); write: the write pass (needed for index / cloud /
+// labels).  A batch that wants only labels needs only the write pass.
+int launch_output(const View& v, const SlotParams* batch, const OutDest* dests, int count, int max_points, bool compact, bool write,
+                  cudaStream_t st, Profiler* prof);
 // "next" rows of SURVEY.md section 8(f)
 struct UnpackDesc {   // f1: PointCloud2 payload -> PointXYZIR records in the map frame
     const unsigned char* raw;  // device copy of msg.data

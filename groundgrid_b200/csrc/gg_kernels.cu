@@ -1810,10 +1810,20 @@ __device__ __forceinline__ int out_class(uint32_t code) {
     return cls == PC_KEPT ? 0 : (cls == PC_IGNORED ? 1 : (cls == PC_OUTLIER ? 2 : -1));
 }
 
-__global__ void __launch_bounds__(OUT_TILE) k_out_count(View v, const SlotParams* __restrict__ batch, int nblk) {
+// out_class of input point i of a scan, or -1 when its label is not in `select` (GG_SELECT_*; outliers are ground)
+__device__ __forceinline__ int out_class_selected(const View& v, size_t base, int i, int n, unsigned select) {
+    if (i >= n) return -1;
+    const int c = out_class(v.code[base + i]);
+    if (c < 0 || select == (GG_SELECT_GROUND | GG_SELECT_NONGROUND)) return c;
+    const unsigned bit = (v.labels[base + i] == GG_LABEL_NONGROUND) ? GG_SELECT_NONGROUND : GG_SELECT_GROUND;
+    return (select & bit) ? c : -1;
+}
+
+__global__ void __launch_bounds__(OUT_TILE) k_out_count(View v, const SlotParams* __restrict__ batch, const OutDest* __restrict__ dests,
+                                                        int nblk) {
     const SlotParams& sp = batch[blockIdx.y];
     const int i = blockIdx.x * OUT_TILE + threadIdx.x;
-    const int c = (i < sp.n_points) ? out_class(v.code[(size_t)sp.slot * v.pcap + i]) : -1;
+    const int c = out_class_selected(v, (size_t)sp.slot * v.pcap, i, sp.n_points, dests[blockIdx.y].select);
     int* counts = v.out_counts + (size_t)sp.slot * (3 * v.out_blocks + 1);
     const int n0 = __syncthreads_count(c == 0);
     const int n1 = __syncthreads_count(c == 1);
@@ -1825,20 +1835,26 @@ __global__ void __launch_bounds__(OUT_TILE) k_out_count(View v, const SlotParams
     }
 }
 
-__global__ void __launch_bounds__(1024) k_out_scan(View v, const SlotParams* __restrict__ batch, int nblk) {
+__global__ void __launch_bounds__(1024) k_out_scan(View v, const SlotParams* __restrict__ batch, const OutDest* __restrict__ dests, int nblk) {
     const SlotParams& sp = batch[blockIdx.x];
     int* counts = v.out_counts + (size_t)sp.slot * (3 * v.out_blocks + 1);
     const int total = block_exclusive_scan_1024(counts, counts, 3 * nblk);
-    if (threadIdx.x == 0) counts[3 * v.out_blocks] = total;
+    if (threadIdx.x == 0) {
+        counts[3 * v.out_blocks] = total;
+        if (int* dc = dests[blockIdx.x].count) *dc = total;
+    }
 }
 
-template <bool CLOUD>
-__global__ void __launch_bounds__(OUT_TILE) k_out_write(View v, const SlotParams* __restrict__ batch, int nblk) {
+__global__ void __launch_bounds__(OUT_TILE) k_out_write(View v, const SlotParams* __restrict__ batch, const OutDest* __restrict__ dests,
+                                                        int nblk) {
     __shared__ int s_w[3][32];
     const SlotParams& sp = batch[blockIdx.y];
+    const OutDest d = dests[blockIdx.y];
     const size_t base = (size_t)sp.slot * v.pcap;
     const int i = blockIdx.x * OUT_TILE + threadIdx.x;
-    const int c = (i < sp.n_points) ? out_class(v.code[base + i]) : -1;
+    if (d.labels && i < sp.n_points) d.labels[i] = v.labels[base + i];
+    if (!d.index && !d.cloud) return;  // the same for the whole block
+    const int c = out_class_selected(v, base, i, sp.n_points, d.select);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t lt_mask = (1u << lane) - 1u;
     int rank_in_warp = 0;
@@ -1858,12 +1874,12 @@ __global__ void __launch_bounds__(OUT_TILE) k_out_write(View v, const SlotParams
     if (c < 0) return;
     const int* counts = v.out_counts + (size_t)sp.slot * (3 * v.out_blocks + 1);
     const int pos = counts[c * nblk + blockIdx.x] + s_w[c][warp] + rank_in_warp;
-    v.out_index[base + pos] = (uint32_t)i;
-    if (CLOUD) {
+    if (d.index) d.index[pos] = (uint32_t)i;
+    if (d.cloud) {
         const uint4* rec = reinterpret_cast<const uint4*>(sp.src + i);
         uint4 a = rec[0], b = rec[1];
         b.x = __float_as_uint((float)v.labels[base + i]);  // intensity = 49 / 99 (:175,180,188)
-        uint4* dst = reinterpret_cast<uint4*>(v.out_cloud + base + pos);
+        uint4* dst = reinterpret_cast<uint4*>(d.cloud + pos);
         dst[0] = a;
         dst[1] = b;
     }
@@ -2244,16 +2260,20 @@ int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i,
     return 1;
 }
 
-int launch_output(const View& v, const SlotParams* batch, int count, int max_points, bool want_cloud, cudaStream_t st,
-                  Profiler* prof) {
+int launch_output(const View& v, const SlotParams* batch, const OutDest* dests, int count, int max_points, bool compact, bool write,
+                  cudaStream_t st, Profiler* prof) {
     const int nblk = max(1, cdiv(max_points, OUT_TILE));
-    GG_LAUNCH(K_OUT_COUNT, k_out_count<<<dim3(nblk, count), OUT_TILE, 0, st>>>(v, batch, nblk));
-    GG_LAUNCH(K_OUT_SCAN, k_out_scan<<<count, 1024, 0, st>>>(v, batch, nblk));
-    if (want_cloud)
-        GG_LAUNCH(K_OUT_WRITE, k_out_write<true><<<dim3(nblk, count), OUT_TILE, 0, st>>>(v, batch, nblk));
-    else
-        GG_LAUNCH(K_OUT_WRITE, k_out_write<false><<<dim3(nblk, count), OUT_TILE, 0, st>>>(v, batch, nblk));
-    return 3;
+    int launches = 0;
+    if (compact) {
+        GG_LAUNCH(K_OUT_COUNT, k_out_count<<<dim3(nblk, count), OUT_TILE, 0, st>>>(v, batch, dests, nblk));
+        GG_LAUNCH(K_OUT_SCAN, k_out_scan<<<count, 1024, 0, st>>>(v, batch, dests, nblk));
+        launches += 2;
+    }
+    if (write) {
+        GG_LAUNCH(K_OUT_WRITE, k_out_write<<<dim3(nblk, count), OUT_TILE, 0, st>>>(v, batch, dests, nblk));
+        ++launches;
+    }
+    return launches;
 }
 
 int launch_unpack(const UnpackDesc& d, cudaStream_t st, Profiler* prof) {

@@ -218,6 +218,38 @@ int gg_interpolate_cell(gg_handle h, int slot, int x, int y);
  * must stay valid until the work is complete (and until gg_get_output, if that is used). */
 int gg_run_scans_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_point* const* dev_points, int stop_after);
 
+/* Caller-owned DEVICE destinations of one scan of gg_run_scans_to_device (on the handle's device; each may be NULL).
+ * Each needs room for the scan's n_points entries. */
+typedef struct gg_scan_outputs {
+    uint8_t* labels;   /* per input point: 0 absent / 49 ground / 99 non-ground (the bytes gg_download_labels returns) */
+    uint32_t* index;   /* input index of each selected output point, in the reference's output order (4-byte aligned) */
+    gg_point* cloud;   /* the selected output points as records, intensity = 49 / 99, like gg_get_output (16-byte aligned) */
+} gg_scan_outputs;
+
+#define GG_SELECT_GROUND 1u     /* output points labelled 49 (outliers are always ground) */
+#define GG_SELECT_NONGROUND 2u  /* output points labelled 99; both bits = the whole output cloud of filter_cloud */
+
+/* gg_run_scans_device(.., stop_after = 0) with the results written into caller-owned device memory, ordered on the
+ * caller's stream.  The slots' state afterwards is the same as after gg_run_scans_device (layers, gg_get_output,
+ * gg_download_labels, gg_eval_accumulate), and so is the lifetime rule for dev_points.
+ *   outs       : `count` entries (NULL: no outputs).  index / cloud of scan k receive the reference's output cloud
+ *                (kept, then ignored, then outlier points, input order within each class) restricted to the labels in
+ *                `select`: GG_SELECT_GROUND | GG_SELECT_NONGROUND gives exactly what gg_get_output gives,
+ *                GG_SELECT_NONGROUND the obstacle cloud (kept and ignored points labelled 99, in that order).
+ *   dev_counts : device int32[count]; dev_counts[k] = number of selected points of scan k, nothing is written past it.
+ *                Required when any index or cloud is given; written whenever it is given and select != 0.
+ *   stream     : cudaStream_t; NULL is the legacy default stream (not "unordered").  The call's device work starts
+ *                after everything already enqueued on `stream`, and everything enqueued on `stream` after the call
+ *                starts after all outputs are written (one event each way per stream group with scans in the batch).
+ *                So with a stream-ordered allocator the caller may free the inputs or reuse the outputs' memory on
+ *                `stream` right after the call.  The call does not wait on the host for device work, except for the
+ *                flow control of the parameter staging ring (as every launching call).
+ * GG_E_ARG, with nothing enqueued: what gg_run_scans_device rejects (GG_E_STATE for a map not initialised); index or
+ * cloud with select 0; unknown select bits; index or cloud without dev_counts; index not 4-byte or cloud not 16-byte
+ * aligned; an output range of a scan (its labels, index, cloud or dev_counts entry) that overlaps its own input cloud. */
+int gg_run_scans_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_point* const* dev_points,
+                           const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream);
+
 /* ---- steps next to the path (SURVEY.md section 8f) -------------------------------------------
  * gg_upload_cloud_msg replaces pcl::fromROSMsg + the per-point tf2::doTransform loop of
  * GroundGridNodelet::points_callback (src/GroundGridNodelet.cpp:119-120,148-184): the raw
