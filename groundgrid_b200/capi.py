@@ -147,6 +147,8 @@ def load(build_if_missing=True):
         "gg_get_layer": (i, [vp, i, C.c_char_p, vp]),
         "gg_set_layer": (i, [vp, i, C.c_char_p, vp]),
         "gg_layer_device_ptr": (i, [vp, i, C.c_char_p, C.POINTER(vp)]),
+        "gg_get_layers_to_device": (i, [vp, i, vp, i, vp, vp, vp]),
+        "gg_set_layers_from_device": (i, [vp, i, vp, i, vp, vp, vp]),
         "gg_stream": (vp, [vp]),
         "gg_num_streams": (i, [vp]),
         "gg_host_pack_threads": (i, [vp]),
@@ -340,6 +342,67 @@ class GroundGridB200:
         p = C.c_void_p()
         _check(self._l.gg_layer_device_ptr(self._h, slot, name.encode(), C.byref(p)))
         return p.value
+
+    @staticmethod
+    def _layer_batch_args(slots, names):
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        nm = None if names is None else (C.c_char_p * max(1, len(names)))(*[None if n is None else n.encode() for n in names])
+        return sl, (0 if names is None else len(names)), nm
+
+    def get_layers_to_device_ptrs(self, slots, names, dst_ptr, stream_ptr):
+        """gg_get_layers_to_device with raw device addresses: dst_ptr float32 [count][n_names][N*N] (each plane
+        column-major), stream_ptr an int or None (None = the legacy default stream)."""
+        sl, n, nm = self._layer_batch_args(slots, names)
+        _check(self._l.gg_get_layers_to_device(self._h, len(sl), _ptr(sl), n, nm, dst_ptr, stream_ptr))
+
+    def set_layers_from_device_ptrs(self, slots, names, src_ptr, stream_ptr):
+        """gg_set_layers_from_device with raw device addresses (the layout of get_layers_to_device_ptrs)."""
+        sl, n, nm = self._layer_batch_args(slots, names)
+        _check(self._l.gg_set_layers_from_device(self._h, len(sl), _ptr(sl), n, nm, src_ptr, stream_ptr))
+
+    def _layer_stream(self, stream):
+        import torch
+
+        dev = torch.device("cuda", self.device)
+        current = torch.cuda.current_stream(dev)
+        return torch, dev, current, (current if stream is None else stream)
+
+    def get_layers_to_device(self, slots, names=("ground", "groundpatch"), out=None, stream=None):
+        """Layers `names` of `slots` as one float32 CUDA tensor [count, n_names, N, N] indexed [k, l, i, j] like layer()
+        (gg_get_layers_to_device).  Each plane is column-major: the tensor is a transpose(-1, -2) view of a contiguous
+        buffer.  It is allocated on `stream` (a torch.cuda.Stream; default: the current stream), or `out` (same shape
+        and storage order) is filled.  The call returns without waiting for the device; work enqueued on `stream`
+        afterwards sees the layers as of the slots' last enqueued scan or roll."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        shape = (len(slots), len(names), self.n, self.n)
+        if out is None:
+            with torch.cuda.stream(stream):
+                out = torch.empty(shape, dtype=torch.float32, device=dev).transpose(-1, -2)
+        else:
+            if tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != dev or not out.transpose(-1, -2).is_contiguous():
+                raise ValueError(f"out must be a float32 tensor {shape} on {dev} whose planes are column-major (a transpose(-1, -2) "
+                                 "view of a contiguous tensor)")
+            if stream != current:
+                out.record_stream(stream)
+        self.get_layers_to_device_ptrs(slots, names, out.data_ptr(), stream.cuda_stream or None)
+        return out
+
+    def set_layers_from_device(self, slots, names, src, stream=None):
+        """Writes src [count, n_names, N, N] (indexed [k, l, i, j] like get_layers_to_device returns it) into layers
+        `names` of `slots` (gg_set_layers_from_device), ordered on `stream` (default: the current stream).  A tensor
+        that is not float32 on this device with column-major planes is first copied into that layout on `stream`.
+        `src` may be freed right after the call (a tensor of another stream is marked in use on `stream`)."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        shape = (len(slots), len(names), self.n, self.n)
+        if tuple(src.shape) != shape:
+            raise ValueError(f"src must have shape {shape}")
+        buf = src.transpose(-1, -2)
+        if buf.dtype != torch.float32 or buf.device != dev or not buf.is_contiguous():
+            with torch.cuda.stream(stream):
+                buf = buf.to(device=dev, dtype=torch.float32).contiguous()
+        elif stream != current:
+            buf.record_stream(stream)
+        self.set_layers_from_device_ptrs(slots, names, buf.data_ptr(), stream.cuda_stream or None)
 
     @property
     def stream(self):

@@ -1485,7 +1485,7 @@ const char* gg_profile_kernel_name(int id) {
     static const char* names[gg::K_NUM] = {"k_rasterize",   "k_cell_tiles",    "k_cell_place",    "k_scatter",
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
-                                           "k_terrain_image", "k_eval_counts"};
+                                           "k_terrain_image", "k_eval_counts", "k_layer_copy"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2005,6 +2005,99 @@ int gg_layer_device_ptr(gg_handle h, int slot, const char* name, void** dptr) {
     if ((rc = layer_index(h, slot, name, &idx))) return rc;
     *dptr = h->view.layer(slot, idx);
     return GG_OK;
+}
+
+namespace {
+// The layer "points" names for `slot` (layer_index without the name lookup).
+int points_layer(gg_handle h, int slot) {
+    int idx = 0;
+    layer_index(h, slot, "points", &idx);
+    return idx;
+}
+
+// gg_get_layers_to_device (import = false) / gg_set_layers_from_device (import = true).  Everything is validated
+// before anything is enqueued; then one k_layer_copy per stream group with slots in the batch, after everything
+// already enqueued on the caller's stream and on the group's stream, and before whatever the caller enqueues next.
+int layer_transfer(gg_handle h, int count, const int* slots, int n_names, const char* const* names, float* buf, bool import, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0 || n_names < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0 || n_names == 0) return GG_OK;
+    if (!slots || !names || !buf) return fail(GG_E_ARG, "null argument");
+    if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
+    if (n_names > gg::L_NUM) return fail(GG_E_ARG, "%d layer names, at most %d", n_names, (int)gg::L_NUM);
+    if (reinterpret_cast<uintptr_t>(buf) % alignof(float)) return fail(GG_E_ARG, "buffer is not 4-byte aligned");
+    const gg::View& v = h->view;
+    const size_t plane = (size_t)v.k.N2 * sizeof(float);
+    if (ranges_overlap(buf, (size_t)count * n_names * plane, v.layers, (size_t)h->n_slots * v.n_layers * plane))
+        return fail(GG_E_ARG, "buffer overlaps the handle's layers");
+    int rc;
+    std::vector<unsigned char>& seen = h->seen_scratch;
+    seen.assign((size_t)h->n_slots, 0);
+    for (int i = 0; i < count; ++i) {
+        if ((rc = check_slot(h, slots[i]))) return rc;
+        if (seen[slots[i]]++) return fail(GG_E_ARG, "slot %d appears twice in one batch", slots[i]);
+        if (!h->slots[slots[i]].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slots[i]);
+    }
+    gg::LayerList list{};
+    list.n = n_names;
+    int points_at = -1;  // position of "points" among the names
+    for (int l = 0; l < n_names; ++l) {
+        const char* name = names[l];
+        if (!name) return fail(GG_E_ARG, "null layer name");
+        for (int m = 0; m < l; ++m)
+            if (std::strcmp(names[m], name) == 0) return fail(GG_E_ARG, "layer '%s' appears twice", name);
+        if (std::strcmp(name, "expectedPoints") == 0) return fail(GG_E_LAYER, "'expectedPoints' is a table of the handle, not a layer of a slot");
+        if (std::strcmp(name, "points") == 0) {
+            list.idx[l] = gg::LAYER_POINTS;
+            points_at = l;
+        } else if ((rc = layer_index(h, slots[0], name, &list.idx[l]))) {
+            return rc;
+        }
+    }
+    // an import must not write one layer of a slot twice ("points" is also "obstacles" or "count")
+    if (import && points_at >= 0)
+        for (int i = 0; i < count; ++i) {
+            const int p = points_layer(h, slots[i]);
+            for (int l = 0; l < n_names; ++l)
+                if (list.idx[l] == p)
+                    return fail(GG_E_ARG, "slot %d: '%s' and 'points' are the same layer", slots[i], names[l]);
+        }
+    GG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t caller = static_cast<cudaStream_t>(stream);
+    GG_CUDA(cudaEventRecord(h->caller_in, caller));
+    for (int g = 0; g < h->n_streams; ++g) {
+        gg::SlotParams *hp = nullptr, *dp = nullptr;
+        int pos = 0, m = 0;
+        for (int i = 0; i < count; ++i) {
+            if (stream_index(h, slots[i]) != g) continue;
+            if (m == 0 && (rc = ring_acquire(h, &hp, &dp, &pos))) return rc;
+            gg::SlotParams& p = hp[m++];
+            std::memset(&p, 0, sizeof(p));
+            p.slot = slots[i];
+            p.n_points = i;
+            p.shift_i = points_layer(h, slots[i]);
+        }
+        if (m == 0) continue;
+        cudaStream_t st = h->streams[g];
+        if ((rc = ring_commit(h, pos, m, st))) return rc;
+        GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
+        h->launches += gg::launch_layer_copy(v, dp, m, list, buf, import, st, h->prof);
+        GG_CUDA(cudaGetLastError());
+        if ((rc = ring_release(h, pos, st))) return rc;
+        GG_CUDA(cudaEventRecord(h->caller_out[g], st));
+        GG_CUDA(cudaStreamWaitEvent(caller, h->caller_out[g], 0));
+    }
+    return GG_OK;
+}
+}  // namespace
+
+int gg_get_layers_to_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, float* dst, void* stream) {
+    return layer_transfer(h, count, slots, n_names, names, dst, false, stream);
+}
+
+int gg_set_layers_from_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, const float* src,
+                              void* stream) {
+    return layer_transfer(h, count, slots, n_names, names, const_cast<float*>(src), true, stream);
 }
 
 }  // extern "C"

@@ -182,7 +182,7 @@ constexpr int OUT_TILE = 1024;
 // kernels of the pipeline, as reported by the profiling hooks (gg_profile_read)
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
-    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_NUM
+    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_NUM
 };
 
 // Optional per-kernel CUDA-event timing (bench.py's roofline needs the dominant kernel's own
@@ -213,6 +213,19 @@ int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i,
 // labels).  A batch that wants only labels needs only the write pass.
 int launch_output(const View& v, const SlotParams* batch, const OutDest* dests, int count, int max_points, bool compact, bool write,
                   cudaStream_t st, Profiler* prof);
+// Layers named in one gg_get_layers_to_device / gg_set_layers_from_device call, resolved once and passed by value.
+// LAYER_POINTS stands for "points", whose layer depends on the slot (it travels with each scan, see launch_layer_copy).
+constexpr int LAYER_POINTS = -1;
+struct LayerList {
+    int idx[L_NUM];  // [n] layer index (Layer) or LAYER_POINTS
+    int n;
+};
+// Copies `count` slots' layers between the arena and the caller's buffer buf[k][l][N2] (plane l of scan k at
+// (k * names.n + l) * N2), exporting (import = false: arena -> buf) or importing (import = true: buf -> arena).  Per
+// scan the staging entry carries batch[s].slot = the slot, batch[s].n_points = its position k in the call and
+// batch[s].shift_i = the layer "points" names for it; every other field is zero.  buf must not overlap the arena.
+int launch_layer_copy(const View& v, const SlotParams* batch, int count, const LayerList& names, float* buf, bool import, cudaStream_t st,
+                      Profiler* prof);
 // "next" rows of SURVEY.md section 8(f)
 struct UnpackDesc {   // f1: PointCloud2 payload -> PointXYZIR records in the map frame
     const unsigned char* raw;  // device copy of msg.data

@@ -1886,6 +1886,37 @@ __global__ void __launch_bounds__(OUT_TILE) k_out_write(View v, const SlotParams
 }
 
 // ------------------------------------------------------------------------------------------
+// Batched layer transfer (gg_get_layers_to_device / gg_set_layers_from_device): block (x, s, l) copies LC_ILP * 256
+// cells of plane l of scan s between the arena (View::layer) and the caller's buffer, coalesced over the cells.
+// N2 may be odd, so the copy stays scalar (4-byte aligned buffers).
+// ------------------------------------------------------------------------------------------
+constexpr int LC_THREADS = 256;
+constexpr int LC_ILP = 4;
+
+template <bool IMPORT>
+__global__ void __launch_bounds__(LC_THREADS) k_layer_copy(View v, const SlotParams* __restrict__ batch, LayerList names, float* __restrict__ buf) {
+    const SlotParams& sp = batch[blockIdx.y];
+    const int l = blockIdx.z;
+    const int idx = names.idx[l];
+    float* lay = v.layer(sp.slot, idx == LAYER_POINTS ? sp.shift_i : idx);
+    float* ext = buf + ((size_t)sp.n_points * names.n + l) * v.k.N2;
+    const float* __restrict__ src = IMPORT ? ext : lay;
+    float* __restrict__ dst = IMPORT ? lay : ext;
+    const int i0 = blockIdx.x * (LC_THREADS * LC_ILP) + threadIdx.x;
+    float r[LC_ILP];
+#pragma unroll
+    for (int q = 0; q < LC_ILP; ++q) {
+        const int i = i0 + q * LC_THREADS;
+        if (i < v.k.N2) r[q] = src[i];
+    }
+#pragma unroll
+    for (int q = 0; q < LC_ILP; ++q) {
+        const int i = i0 + q * LC_THREADS;
+        if (i < v.k.N2) dst[i] = r[q];
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // "next" rows (SURVEY.md section 8f)
 // ------------------------------------------------------------------------------------------
 // f1: pcl::fromROSMsg (field-offset driven unpack, GroundGridNodelet.cpp:119-120) + the per-point
@@ -2274,6 +2305,16 @@ int launch_output(const View& v, const SlotParams* batch, const OutDest* dests, 
         ++launches;
     }
     return launches;
+}
+
+int launch_layer_copy(const View& v, const SlotParams* batch, int count, const LayerList& names, float* buf, bool import, cudaStream_t st,
+                      Profiler* prof) {
+    const dim3 grid(cdiv(v.k.N2, LC_THREADS * LC_ILP), count, names.n);
+    if (import)
+        GG_LAUNCH(K_LAYER_COPY, k_layer_copy<true><<<grid, LC_THREADS, 0, st>>>(v, batch, names, buf));
+    else
+        GG_LAUNCH(K_LAYER_COPY, k_layer_copy<false><<<grid, LC_THREADS, 0, st>>>(v, batch, names, buf));
+    return 1;
 }
 
 int launch_unpack(const UnpackDesc& d, cudaStream_t st, Profiler* prof) {

@@ -301,6 +301,34 @@ int gg_set_layer(gg_handle h, int slot, const char* name, const float* src);
 int gg_layer_device_ptr(gg_handle h, int slot, const char* name, void** dptr);
 int gg_set_map_position(gg_handle h, int slot, double x, double y);
 
+/* Layers of `count` distinct slots copied into (get) or out of (set) ONE caller-owned device buffer, ordered on the
+ * caller's stream: the batched, device-side form of gg_get_layer / gg_set_layer.
+ *   slots      : `count` distinct slots, each with an initialised map
+ *   names      : `n_names` (<= 12) distinct layer names, resolved as gg_get_layer resolves them ("points" per slot:
+ *                the kept-point count after a scan stopped before labelling, else the non-ground count)
+ *   dst / src  : float[count][n_names][N*N] on the handle's device, 4-byte aligned; the plane of scan k and name l
+ *                starts at (k * n_names + l) * N*N and is column-major like gg_get_layer (cell (i, j) at i + j*N)
+ *   stream     : cudaStream_t; NULL is the legacy default stream.  The same contract as gg_run_scans_to_device: the copy
+ *                starts after everything already enqueued on `stream` and on the stream group of every slot in the
+ *                batch (so it reads / overwrites the state after the slot's last enqueued scan or roll), and work
+ *                enqueued on `stream` after the call sees it complete.  Only the stream groups with slots in the batch
+ *                take part; nothing waits on the host except the flow control of the parameter staging ring.  A
+ *                stream-ordered allocator may therefore free `src` or reuse `dst` on `stream` right after the call.
+ * Later scans of a slot read what gg_set_layers_from_device wrote.  Moving a stream to another slot, handle or GPU:
+ * gg_init_map at the old slot's map position, gg_set_slot_config with its configuration, then import "ground" and
+ * "groundpatch" (the only layers a scan reads from the previous one): the slot then continues bit-identically.
+ * count == 0 or n_names == 0 enqueues nothing and returns GG_OK.  Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle; null slots / names / buffer; count > n_slots; a slot out of range or repeated; a name
+ *              repeated; n_names > 12; a buffer not 4-byte aligned or overlapping the handle's layers (e.g. a
+ *              gg_layer_device_ptr address); on import, "points" together with the layer it names for a slot
+ *   GG_E_LAYER an unknown name, a GG_FLAG_FULL_LAYERS layer without the flag, "expectedPoints" (not a slot layer)
+ *   GG_E_STATE a slot whose map is not initialised
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_get_layers_to_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, float* dst, void* stream);
+int gg_set_layers_from_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, const float* src,
+                              void* stream);
+
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
  * touches a slot is enqueued on its stream.  gg_stream() is the primary stream;
