@@ -54,6 +54,22 @@ class ScanDesc(C.Structure):
     ]
 
 
+class CloudMsg(C.Structure):
+    """gg_cloud_msg: one PointCloud2 payload in device memory (data), T_map_from_frame a host pointer or None."""
+
+    _fields_ = [
+        ("data", C.c_void_p),
+        ("point_step", C.c_int),
+        ("field_offsets", C.c_int * 5),
+        ("T_map_from_frame", C.c_void_p),
+    ]
+
+
+# numpy image of an array of gg_cloud_msg (CloudMsg)
+CLOUD_MSG_DTYPE = np.dtype({"names": ["data", "point_step", "field_offsets", "T_map_from_frame"],
+                            "formats": [np.uint64, np.int32, (np.int32, 5), np.uint64], "offsets": [0, 8, 12, 32],
+                            "itemsize": C.sizeof(CloudMsg)})
+
 # numpy image of an array of gg_scan_desc (ScanDesc)
 SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "n_points", "origin", "base_z"], "formats": [np.int32, np.uint64, (np.float32, 3), np.float64],
                             "offsets": [0, 8, 16, 32], "itemsize": C.sizeof(ScanDesc)})
@@ -130,6 +146,7 @@ def load(build_if_missing=True):
         "gg_run_scans_device": (i, [vp, i, vp, vp, i]),
         "gg_run_scans_to_device": (i, [vp, i, vp, vp, vp, C.c_uint, vp, vp]),
         "gg_upload_cloud_msg": (i, [vp, i, vp, sz, i, vp, vp]),
+        "gg_run_cloud_msgs_to_device": (i, [vp, i, vp, vp, vp, C.c_uint, vp, vp]),
         "gg_terrain_image": (i, [vp, i, vp]),
         "gg_layer_image_u8": (i, [vp, i, C.c_char_p, vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
         "gg_get_point_classes": (i, [vp, i, vp, sz]),
@@ -502,6 +519,74 @@ class GroundGridB200:
         The call returns without waiting for the device.  Work enqueued on `stream` afterwards sees complete outputs, and
         the inputs may be freed right after the call when they were allocated on `stream` (other streams' inputs are
         marked in use on `stream`).  Returns DeviceOutputs."""
+        torch, dev, stream, sel = self._device_call(select, index, stream)
+        n = []
+        for c in clouds:
+            nbytes = c.numel() * c.element_size()
+            if c.device != dev or not c.is_contiguous() or nbytes % 32:
+                raise ValueError(f"clouds must be contiguous tensors of 32-byte records on {dev}")
+            n.append(nbytes // 32)
+        descs = self._device_descs(slots, n, origins, base_z)
+        out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, clouds)
+        self.run_scans_to_device_ptrs(descs, [c.data_ptr() for c in clouds], ptrs, sel,
+                                      out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
+        return out
+
+    def run_cloud_msgs_to_device_ptrs(self, descs, data_ptrs, point_step, field_offsets, T, out_ptrs, select, counts_ptr, stream_ptr):
+        """gg_run_cloud_msgs_to_device with raw device addresses.  data_ptrs: one device address (int, 0 = NULL) per scan;
+        point_step / field_offsets: one value / one 5-tuple, or one per scan; T: None, an array [count, 3, 4] or a list
+        with None entries (None: the payload is in the map frame); the rest as in run_scans_to_device_ptrs."""
+        count = len(descs)
+        d = _ptr(descs) if isinstance(descs, np.ndarray) else descs
+        msgs = np.zeros(max(1, count), CLOUD_MSG_DTYPE)
+        msgs["data"][:count] = np.asarray(data_ptrs, np.uint64).reshape(count)
+        msgs["point_step"][:count] = point_step
+        msgs["field_offsets"][:count] = np.asarray(field_offsets, np.int32).reshape(-1, 5)
+        if isinstance(T, np.ndarray):                  # read during the call only
+            Tarr = np.ascontiguousarray(T, np.float64).reshape(count, 12)
+            msgs["T_map_from_frame"][:count] = Tarr.ctypes.data + 96 * np.arange(count, dtype=np.uint64)
+        elif T is not None:
+            if len(T) != count:
+                raise ValueError("T needs one entry per scan")
+            Tarr = np.zeros((count, 12), np.float64)
+            for k, t in enumerate(T):
+                if t is not None:
+                    Tarr[k] = np.asarray(t, np.float64).reshape(12)
+                    msgs["T_map_from_frame"][k] = Tarr.ctypes.data + 96 * k
+        op = None if out_ptrs is None else np.ascontiguousarray(out_ptrs, dtype=np.uint64).reshape(count, 3)
+        _check(self._l.gg_run_cloud_msgs_to_device(self._h, count, d, _ptr(msgs), _ptr(op), int(select), counts_ptr, stream_ptr))
+
+    def run_cloud_msgs_to_device(self, payloads, point_step, field_offsets, T, slots, origins, base_z, labels=True, select="nonground",
+                                 index=False, stream=None):
+        """One sensor_msgs/PointCloud2 payload per slot, in caller-owned CUDA memory, unpacked and transformed to the map frame
+        on the device and then run like run_scans_to_device (gg_run_cloud_msgs_to_device).
+          payloads      : contiguous CUDA tensors of any dtype whose byte size is a multiple of the scan's point_step
+                          (e.g. float32 [n, 4] with step 16, or uint8 [n, 18])
+          point_step    : bytes per point, one value or one per scan
+          field_offsets : byte offsets of x, y, z, intensity, ring (-1 absent), one 5-tuple or one per scan
+          T             : None (every payload in the map frame), an array [count, 3, 4] of lookupTransform("map", frame_id), or
+                          a list with None entries
+        origins, base_z, labels, select, index and stream as in run_scans_to_device.  Each payload may be freed right
+        after the call when it was allocated on `stream` (other streams' payloads are marked in use on `stream`).
+        Returns DeviceOutputs."""
+        torch, dev, stream, sel = self._device_call(select, index, stream)
+        count = len(payloads)
+        steps = np.broadcast_to(np.asarray(point_step, np.int64), (count,))
+        n = []
+        for c, step in zip(payloads, steps):
+            nbytes = c.numel() * c.element_size()
+            if c.device != dev or not c.is_contiguous() or step <= 0 or nbytes % step:
+                raise ValueError(f"payloads must be contiguous tensors on {dev} whose byte size is a multiple of point_step")
+            n.append(int(nbytes // step))
+        descs = self._device_descs(slots, n, origins, base_z)
+        out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, payloads)
+        self.run_cloud_msgs_to_device_ptrs(descs, [c.data_ptr() for c in payloads], steps, field_offsets, T, ptrs, sel,
+                                           out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
+        return out
+
+    # shared by run_scans_to_device / run_cloud_msgs_to_device
+    def _device_call(self, select, index, stream):
+        """(torch, device, stream, select bits); stream defaults to the current stream."""
         import torch
 
         if select not in SELECT:
@@ -510,21 +595,24 @@ class GroundGridB200:
         if index and not sel:
             raise ValueError("index needs a select")
         dev = torch.device("cuda", self.device)
-        current = torch.cuda.current_stream(dev)
-        stream = current if stream is None else stream
-        count = len(clouds)
-        n = []
-        for c in clouds:
-            nbytes = c.numel() * c.element_size()
-            if c.device != dev or not c.is_contiguous() or nbytes % 32:
-                raise ValueError(f"clouds must be contiguous tensors of 32-byte records on {dev}")
-            n.append(nbytes // 32)
-        base_z = np.broadcast_to(np.asarray(base_z, np.float64), (count,))
+        return torch, dev, (torch.cuda.current_stream(dev) if stream is None else stream), sel
+
+    @staticmethod
+    def _device_descs(slots, n, origins, base_z):
+        count = len(n)
         descs = np.zeros(count, SCAN_DESC_DTYPE)
         descs["slot"] = np.asarray(slots, np.int32)
         descs["n_points"] = n
         descs["origin"] = np.asarray(origins, np.float32).reshape(count, 3)
-        descs["base_z"] = base_z
+        descs["base_z"] = np.broadcast_to(np.asarray(base_z, np.float64), (count,))
+        return descs
+
+    @staticmethod
+    def _device_outputs(torch, dev, stream, n, labels, sel, index, inputs):
+        """Flat output tensors allocated on `stream` for scans of n[k] points, as DeviceOutputs, and their per-scan addresses
+        uint64 [count, 3] (labels, index, cloud).  Inputs of another stream than the current one are marked in use on
+        `stream`."""
+        count = len(n)
         offs = np.zeros(count, np.uint64)
         offs[1:] = np.cumsum(n[:-1], dtype=np.uint64)
         total = int(sum(n))
@@ -537,16 +625,14 @@ class GroundGridB200:
         for col, t, size in ((0, lab, 1), (1, idx, 4), (2, cld, 32)):
             if t is not None and total:
                 ptrs[:, col] = np.uint64(t.data_ptr()) + offs * np.uint64(size)
-        if stream != current:
-            for c in clouds:
+        if stream != torch.cuda.current_stream(dev):
+            for c in inputs:
                 c.record_stream(stream)
-        self.run_scans_to_device_ptrs(descs, [c.data_ptr() for c in clouds], ptrs, sel,
-                                      counts.data_ptr() if counts is not None else None, stream.cuda_stream or None)
 
         def views(t):
             return None if t is None else list(torch.split(t, n))
 
-        return DeviceOutputs(views(lab), views(cld), views(idx), counts, stream)
+        return DeviceOutputs(views(lab), views(cld), views(idx), counts, stream), ptrs
 
     # -- steps next to the path (SURVEY section 8f)
     def upload_cloud_msg(self, raw, n_points, point_step, field_offsets, T_map_from_frame=None, slot=0):

@@ -304,6 +304,8 @@ struct gg_handle_s {
     gg::SlotParams* d_ring = nullptr;
     gg::OutDest* h_dest = nullptr;   // output destinations of the entry's scans, same shape as h_ring / d_ring
     gg::OutDest* d_dest = nullptr;
+    gg::UnpackDesc* h_unpack = nullptr;  // PointCloud2 payloads of the entry's scans, same shape as h_ring / d_ring
+    gg::UnpackDesc* d_unpack = nullptr;
     cudaEvent_t ring_ev[kRing] = {};
     cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
     cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
@@ -435,6 +437,34 @@ int ring_commit_dests(gg_handle h, int pos, int count, cudaStream_t st) {
     return GG_OK;
 }
 
+// PointCloud2 payloads of a staging entry (the other array parallel to its SlotParams) and their copy to the device.
+gg::UnpackDesc* ring_unpack(gg_handle h, int pos) { return h->h_unpack + (size_t)pos * h->n_slots; }
+gg::UnpackDesc* ring_unpack_dev(gg_handle h, int pos) { return h->d_unpack + (size_t)pos * h->n_slots; }
+int ring_commit_unpack(gg_handle h, int pos, int count, cudaStream_t st) {
+    GG_CUDA(cudaMemcpyAsync(ring_unpack_dev(h, pos), ring_unpack(h, pos), (size_t)count * sizeof(gg::UnpackDesc), cudaMemcpyHostToDevice, st));
+    return GG_OK;
+}
+
+// Unpack descriptor of one payload whose layout has been validated (check_cloud_msg).
+void fill_unpack(gg::UnpackDesc& d, const void* data, int point_step, const int field_offsets[5], const double* T_map_from_frame) {
+    std::memset(&d, 0, sizeof(d));
+    d.raw = static_cast<const unsigned char*>(data);
+    d.point_step = point_step;
+    for (int f = 0; f < 5; ++f) d.off[f] = field_offsets[f];
+    d.transform = T_map_from_frame ? 1 : 0;
+    if (T_map_from_frame) std::memcpy(d.T, T_map_from_frame, sizeof(d.T));
+}
+
+// The layout rules of a PointCloud2 payload: x, y, z present, every present field inside point_step.
+int check_cloud_msg(const void* data, size_t n_points, int point_step, const int field_offsets[5]) {
+    if ((n_points && !data) || !field_offsets || point_step < 12) return fail(GG_E_ARG, "bad PointCloud2 layout");
+    for (int f = 0; f < 5; ++f) {
+        const int width = f == 4 ? 2 : 4;
+        if ((f < 3 && field_offsets[f] < 0) || field_offsets[f] + width > point_step) return fail(GG_E_ARG, "field %d does not fit point_step", f);
+    }
+    return GG_OK;
+}
+
 // The entry may be reused once the kernels that read it have finished (they may run on any of
 // the handle's streams, so the event is recorded AFTER the launches, not after the copy).
 int ring_release(gg_handle h, int pos, cudaStream_t st) {
@@ -489,16 +519,19 @@ void fill_params(gg_handle h, const gg_scan_desc& d, gg::SlotParams& p, const gg
     p.packed = packed;
 }
 
-// Caller-owned destinations of gg_run_scans_to_device (validated by it) and the caller's stream.
+// Caller-owned destinations of gg_run_scans_to_device / gg_run_cloud_msgs_to_device (validated by them) and the
+// caller's stream.
 struct CallerOutputs {
     const gg_scan_outputs* outs;  // [count] or null
     unsigned select;
     int32_t* counts;              // [count] or null
     cudaStream_t stream;
+    const gg_cloud_msg* msgs;     // [count] or null: payloads unpacked into the slots' own buffers before the scans
 };
 
 // enqueue the kernels of `count` scans, each group of slots on its own stream; with `caller`, each group also writes
-// its scans' outputs and is ordered after / before the caller's stream
+// its scans' outputs and is ordered after / before the caller's stream (and, with caller->msgs, first unpacks its
+// scans' payloads)
 int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int stop_after, const gg_point* const* dev_points = nullptr,
                       const float* const* packed_ptrs = nullptr, uint8_t* labels_base = nullptr, const CallerOutputs* caller = nullptr) {
     if (count <= 0) return GG_OK;
@@ -539,6 +572,10 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
                 od.count = compact ? caller->counts + i : nullptr;
                 od.select = caller->select;
                 write = write || od.labels || od.index || od.cloud;
+                if (caller->msgs) {
+                    const gg_cloud_msg& msg = caller->msgs[i];
+                    fill_unpack(ring_unpack(h, pos)[m], msg.data, msg.point_step, msg.field_offsets, msg.T_map_from_frame);
+                }
             }
             ++m;
             max_points = std::max(max_points, (int)d.n_points);
@@ -554,6 +591,8 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         cudaStream_t st = h->streams[g];
         if ((rc = ring_commit(h, pos, m, st))) return rc;
         if ((compact || write) && (rc = ring_commit_dests(h, pos, m, st))) return rc;
+        const bool unpack = caller && caller->msgs;
+        if (unpack && (rc = ring_commit_unpack(h, pos, m, st))) return rc;
         // Staggered stream pairs: the spiral is latency bound (a CTA per scan, a few warps per SM), every other kernel
         // fills the machine.  Stream 2k + 1 starts its scans when stream 2k has reached its spiral, so in steady state the
         // spirals of one half of the batch run underneath the bulk kernels of the other half instead of all at once.
@@ -568,6 +607,10 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
             }
         }
         if (caller) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
+        if (unpack) {  // after the wait: the payloads may be produced on the caller's stream
+            h->launches += gg::launch_unpack(view, dp, ring_unpack_dev(h, pos), m, max_points, st, h->prof);
+            GG_CUDA(cudaGetLastError());
+        }
         h->launches += gg::launch_scan_pipeline(view, dp, m, max_points, stop_after, st, h->prof, h->have_layer_map ? &h->layer_map : nullptr, after_detect);
         GG_CUDA(cudaGetLastError());
         if (compact || write) {
@@ -973,6 +1016,8 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     GG_TRY(dev_alloc(h, &h->d_ring, (size_t)kRing * S));
     GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_dest), sizeof(gg::OutDest) * kRing * S, cudaHostAllocDefault));
     GG_TRY(dev_alloc(h, &h->d_dest, (size_t)kRing * S));
+    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_unpack), sizeof(gg::UnpackDesc) * kRing * S, cudaHostAllocDefault));
+    GG_TRY(dev_alloc(h, &h->d_unpack, (size_t)kRing * S));
     for (int i = 0; i < kRing; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->ring_ev[i], cudaEventDisableTiming));
     for (int i = 0; i < kStreams; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->stagger_ev[i], cudaEventDisableTiming));
     GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_in, cudaEventDisableTiming));
@@ -1010,6 +1055,7 @@ int gg_destroy(gg_handle h) {
     for (void* p : h->dev_allocs) cudaFree(p);
     if (h->h_ring) cudaFreeHost(h->h_ring);
     if (h->h_dest) cudaFreeHost(h->h_dest);
+    if (h->h_unpack) cudaFreeHost(h->h_unpack);
     for (int i = 0; i < kRing; ++i)
         if (h->ring_ev[i]) cudaEventDestroy(h->ring_ev[i]);
     if (h->own_streams)
@@ -1249,11 +1295,7 @@ int gg_upload_cloud_msg(gg_handle h, int slot, const void* data, size_t n_points
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (n_points > h->pcap) return fail(GG_E_ARG, "%zu points exceed capacity %zu", n_points, h->pcap);
-    if ((n_points && !data) || !field_offsets || point_step < 12) return fail(GG_E_ARG, "bad PointCloud2 layout");
-    for (int f = 0; f < 5; ++f) {
-        const int width = f == 4 ? 2 : 4;
-        if ((f < 3 && field_offsets[f] < 0) || field_offsets[f] + width > point_step) return fail(GG_E_ARG, "field %d does not fit point_step", f);
-    }
+    if ((rc = check_cloud_msg(data, n_points, point_step, field_offsets))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     h->inputs_busy = true;
     cudaStream_t st = stream_of(h, slot);
@@ -1268,19 +1310,47 @@ int gg_upload_cloud_msg(gg_handle h, int slot, const void* data, size_t n_points
         h->d_raw_cap[sg] = bytes;
     }
     if (bytes) GG_CUDA(cudaMemcpyAsync(h->d_raw[sg], data, bytes, cudaMemcpyHostToDevice, st));
-    gg::UnpackDesc d;
-    std::memset(&d, 0, sizeof(d));
-    d.raw = h->d_raw[sg];
-    d.dst = h->view.points + (size_t)slot * h->pcap;
-    d.n = (int)n_points;
-    d.point_step = point_step;
-    for (int f = 0; f < 5; ++f) d.off[f] = field_offsets[f];
-    d.transform = T_map_from_frame ? 1 : 0;
-    if (T_map_from_frame) std::memcpy(d.T, T_map_from_frame, sizeof(d.T));
-    h->launches += gg::launch_unpack(d, st, h->prof);
+    // a one-scan batch of the unpack kernel of gg_run_cloud_msgs_to_device
+    gg::SlotParams *hp = nullptr, *dp = nullptr;
+    int pos = 0;
+    if ((rc = ring_acquire(h, &hp, &dp, &pos))) return rc;
+    std::memset(&hp[0], 0, sizeof(gg::SlotParams));
+    hp[0].slot = slot;
+    hp[0].n_points = (int)n_points;
+    fill_unpack(ring_unpack(h, pos)[0], h->d_raw[sg], point_step, field_offsets, T_map_from_frame);
+    if ((rc = ring_commit(h, pos, 1, st))) return rc;
+    if ((rc = ring_commit_unpack(h, pos, 1, st))) return rc;
+    h->launches += gg::launch_unpack(h->view, dp, ring_unpack_dev(h, pos), 1, (int)n_points, st, h->prof);
     GG_CUDA(cudaGetLastError());
+    if ((rc = ring_release(h, pos, st))) return rc;
     h->slots[slot].n_points = n_points;
     return GG_OK;
+}
+
+int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_cloud_msg* msgs, const gg_scan_outputs* outs,
+                                unsigned select, int32_t* dev_counts, void* stream) {
+    if (!h || !scans || !msgs) return fail(GG_E_ARG, "null argument");
+    if (select & ~(GG_SELECT_GROUND | GG_SELECT_NONGROUND)) return fail(GG_E_ARG, "unknown select bits 0x%x", select);
+    if (reinterpret_cast<uintptr_t>(dev_counts) % alignof(int32_t)) return fail(GG_E_ARG, "dev_counts is not 4-byte aligned");
+    int rc;
+    for (int i = 0; i < count; ++i) {
+        const gg_cloud_msg& m = msgs[i];
+        if ((rc = check_cloud_msg(m.data, scans[i].n_points, m.point_step, m.field_offsets))) return fail(rc, "scan %d: %s", i, g_last_error.c_str());
+        // outputs may overlap the scan's own payload: the output kernels read the slot's buffer, and the payload has
+        // been consumed by the unpack kernel that runs before them on the same stream
+        if (!outs) continue;
+        const gg_scan_outputs& o = outs[i];
+        if (o.index || o.cloud) {
+            if (!select) return fail(GG_E_ARG, "scan %d: index / cloud requested with select 0", i);
+            if (!dev_counts) return fail(GG_E_ARG, "scan %d: index / cloud requested without dev_counts", i);
+        }
+        if (reinterpret_cast<uintptr_t>(o.index) % 4) return fail(GG_E_ARG, "scan %d: index is not 4-byte aligned", i);
+        if (reinterpret_cast<uintptr_t>(o.cloud) % 16) return fail(GG_E_ARG, "scan %d: cloud is not 16-byte aligned", i);
+    }
+    h->inputs_busy = true;
+    GG_CUDA(cudaSetDevice(h->device));
+    const CallerOutputs caller{outs, select, dev_counts, static_cast<cudaStream_t>(stream), msgs};
+    return run_scans_grouped(h, count, scans, 0, nullptr, nullptr, nullptr, &caller);
 }
 
 int gg_terrain_image(gg_handle h, int slot, float* dst) {

@@ -227,15 +227,19 @@ struct LayerList {
 int launch_layer_copy(const View& v, const SlotParams* batch, int count, const LayerList& names, float* buf, bool import, cudaStream_t st,
                       Profiler* prof);
 // "next" rows of SURVEY.md section 8(f)
-struct UnpackDesc {   // f1: PointCloud2 payload -> PointXYZIR records in the map frame
-    const unsigned char* raw;  // device copy of msg.data
-    gg_point* dst;
-    int n, point_step;
+// f1: one PointCloud2 payload of a batch (gg_upload_cloud_msg, gg_run_cloud_msgs_to_device).  It sits in the staging
+// entry next to the scans' SlotParams, in a parallel array with the same index (like OutDest).
+struct UnpackDesc {
+    const unsigned char* raw;  // msg.data on the device (the handle's staging copy or the caller's buffer)
+    int point_step;
     int off[5];                // byte offsets of x, y, z, intensity, ring (-1: field absent)
     int transform;             // 0: frame_id == "map", copy only
+    int reserved;              // zero
     double T[12];              // row-major 3x4 [R|t] of lookupTransform("map", frame_id)
 };
-int launch_unpack(const UnpackDesc& d, cudaStream_t st, Profiler* prof);
+// PointCloud2 payloads -> PointXYZIR records in the map frame, for `count` scans: descs[k] (batch[k].n_points records)
+// lands in the slot's own cloud buffer, v.points + batch[k].slot * pcap.
+int launch_unpack(const View& v, const SlotParams* batch, const UnpackDesc* descs, int count, int max_points, cudaStream_t st, Profiler* prof);
 int launch_terrain_image(const View& v, int slot, float* dst, cudaStream_t st, Profiler* prof);
 // mm: 2 floats (ordered-int keys of min / max), preset by the caller to the keys of +inf / -inf; dst: N * N bytes, row-major (i, j)
 int launch_layer_image_u8(const View& v, const float* layer, float* mm, unsigned char* dst, cudaStream_t st);

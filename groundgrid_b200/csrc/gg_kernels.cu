@@ -1920,10 +1920,14 @@ __global__ void __launch_bounds__(LC_THREADS) k_layer_copy(View v, const SlotPar
 // "next" rows (SURVEY.md section 8f)
 // ------------------------------------------------------------------------------------------
 // f1: pcl::fromROSMsg (field-offset driven unpack, GroundGridNodelet.cpp:119-120) + the per-point
-// tf2::doTransform into the map frame in fp64, stored as float (:166-181).
-__global__ void __launch_bounds__(256) k_unpack_transform(UnpackDesc d) {
+// tf2::doTransform into the map frame in fp64, stored as float (:166-181).  Block (x, s) unpacks 256 points of scan s
+// into its slot's cloud buffer.  The loads are byte-wise: payloads may be unaligned and fields sit at any offset (the
+// KITTI player's 18-byte points).
+__global__ void __launch_bounds__(256) k_unpack_transform(View v, const SlotParams* __restrict__ batch, const UnpackDesc* __restrict__ descs) {
     const int i = blockIdx.x * 256 + threadIdx.x;
-    if (i >= d.n) return;
+    const SlotParams& sp = batch[blockIdx.y];
+    if (i >= sp.n_points) return;
+    const UnpackDesc& d = descs[blockIdx.y];
     const unsigned char* p = d.raw + (size_t)i * d.point_step;
     auto rd32 = [&](int off) -> uint32_t {
         if (off < 0) return 0u;
@@ -1934,12 +1938,13 @@ __global__ void __launch_bounds__(256) k_unpack_transform(UnpackDesc d) {
     const uint32_t ring = d.off[4] < 0 ? 0u : ((uint32_t)p[d.off[4]] | ((uint32_t)p[d.off[4] + 1] << 8));
     if (d.transform) {
         const double dx = (double)x, dy = (double)y, dz = (double)z;
+        const double* T = d.T;
         // tf2::Transform * Vector3: row.dot(v) (left to right) + origin
-        x = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(d.T[0], dx), __dmul_rn(d.T[1], dy)), __dmul_rn(d.T[2], dz)), d.T[3]);
-        y = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(d.T[4], dx), __dmul_rn(d.T[5], dy)), __dmul_rn(d.T[6], dz)), d.T[7]);
-        z = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(d.T[8], dx), __dmul_rn(d.T[9], dy)), __dmul_rn(d.T[10], dz)), d.T[11]);
+        x = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], dx), __dmul_rn(T[1], dy)), __dmul_rn(T[2], dz)), T[3]);
+        y = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], dx), __dmul_rn(T[5], dy)), __dmul_rn(T[6], dz)), T[7]);
+        z = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], dx), __dmul_rn(T[9], dy)), __dmul_rn(T[10], dz)), T[11]);
     }
-    uint4* dst = reinterpret_cast<uint4*>(d.dst + i);
+    uint4* dst = reinterpret_cast<uint4*>(v.points + (size_t)sp.slot * v.pcap + i);
     dst[0] = make_uint4(__float_as_uint(x), __float_as_uint(y), __float_as_uint(z), 0u);
     dst[1] = make_uint4(inten, ring, 0u, 0u);
 }
@@ -2317,8 +2322,8 @@ int launch_layer_copy(const View& v, const SlotParams* batch, int count, const L
     return 1;
 }
 
-int launch_unpack(const UnpackDesc& d, cudaStream_t st, Profiler* prof) {
-    GG_LAUNCH(K_UNPACK, k_unpack_transform<<<max(1, cdiv(d.n, 256)), 256, 0, st>>>(d));
+int launch_unpack(const View& v, const SlotParams* batch, const UnpackDesc* descs, int count, int max_points, cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_UNPACK, k_unpack_transform<<<dim3(max(1, cdiv(max_points, 256)), count), 256, 0, st>>>(v, batch, descs));
     return 1;
 }
 

@@ -267,6 +267,39 @@ int gg_run_scans_to_device(gg_handle h, int count, const gg_scan_desc* scans, co
  * non-ground, accumulated over the scans it was called for (1024 ids). */
 int gg_upload_cloud_msg(gg_handle h, int slot, const void* data, size_t n_points, int point_step, const int field_offsets[5],
                         const double T_map_from_frame[12]);
+
+/* One sensor_msgs/PointCloud2 payload in DEVICE memory (on the handle's device).  The field rules are those of
+ * gg_upload_cloud_msg: x, y, z, intensity float32 and ring uint16 at field_offsets, -1 = absent (x, y, z required). */
+typedef struct gg_cloud_msg {
+    const void* data;                /* n_points * point_step bytes, no alignment required */
+    int point_step;
+    int field_offsets[5];            /* x, y, z, intensity, ring */
+    const double* T_map_from_frame;  /* HOST pointer, row-major 3x4 of lookupTransform("map", frame_id); NULL: frame_id == "map" */
+} gg_cloud_msg;
+
+/* The whole of GroundGridNodelet::points_callback after the lookups (src/GroundGridNodelet.cpp:119-120,148-184: pcl::fromROSMsg,
+ * the per-point tf2::doTransform, filter_cloud) for a batch of payloads already in device memory.  For every scan k:
+ *   1. msgs[k] (scans[k].n_points records) is unpacked into the slot's OWN cloud buffer and, when T_map_from_frame is
+ *      given, transformed to the map frame in fp64 (the result per point is bit-identical to gg_upload_cloud_msg of the
+ *      same bytes);
+ *   2. then what gg_run_scans_to_device does follows on that buffer: outs, select, dev_counts and the stream contract
+ *      are the same (NULL stream = the legacy default stream; the work starts after everything already enqueued on
+ *      `stream`, work enqueued on `stream` afterwards sees the outputs complete; no host wait except the flow control of
+ *      the parameter staging ring).
+ * scans[k].origin is still the caller's: the reference takes it from a separate lookup, map <- velodyne (:131,139-146).
+ * Consequences:
+ *   - each payload is consumed by the first kernel of its slot's stream group, so a stream-ordered allocator may free
+ *     it, or reuse its memory, on `stream` right after the call;
+ *   - an output of scan k may overlap scan k's own payload (the output kernels read the slot's buffer, not the payload);
+ *     buffers of different scans must not overlap;
+ *   - T_map_from_frame is read during the call and may be reused when it returns;
+ *   - the slots' state afterwards is what gg_upload_cloud_msg of the same bytes + gg_run_scans leaves: layers,
+ *     gg_download_labels, gg_eval_accumulate, and gg_get_output without the payload having to stay alive.
+ * count == 0 returns GG_OK and enqueues nothing.  GG_E_ARG, with nothing enqueued: what gg_run_scans_to_device rejects
+ * except its input-overlap rule (GG_E_STATE for a map not initialised); null msgs; per message the layout rules of
+ * gg_upload_cloud_msg: null data with n_points > 0, point_step < 12, x, y or z absent, a field outside point_step. */
+int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_cloud_msg* msgs,
+                                const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream);
 int gg_terrain_image(gg_handle h, int slot, float* dst);
 /* The other branch of publish_grid_map_layer (src/GroundGridNodelet.cpp:238-245): the single-channel 8-bit image that
  * grid_map::GridMapCvConverter::toImage<unsigned char, 1>(map, layer, CV_8UC1, img) produces and cv::applyColorMap then
