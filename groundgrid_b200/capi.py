@@ -166,6 +166,8 @@ def load(build_if_missing=True):
         "gg_layer_device_ptr": (i, [vp, i, C.c_char_p, C.POINTER(vp)]),
         "gg_get_layers_to_device": (i, [vp, i, vp, i, vp, vp, vp]),
         "gg_set_layers_from_device": (i, [vp, i, vp, i, vp, vp, vp]),
+        "gg_layer_images_to_device": (i, [vp, i, vp, i, vp, vp, vp, vp]),
+        "gg_terrain_images_to_device": (i, [vp, i, vp, vp, vp]),
         "gg_stream": (vp, [vp]),
         "gg_num_streams": (i, [vp]),
         "gg_host_pack_threads": (i, [vp]),
@@ -420,6 +422,51 @@ class GroundGridB200:
         elif stream != current:
             buf.record_stream(stream)
         self.set_layers_from_device_ptrs(slots, names, buf.data_ptr(), stream.cuda_stream or None)
+
+    def layer_images_to_device_ptrs(self, slots, names, dst_ptr, range_ptr, stream_ptr):
+        """gg_layer_images_to_device with raw device addresses: dst_ptr uint8 [count][n_names][N][N] (row-major planes),
+        range_ptr float32 [count][n_names][2] or None, stream_ptr an int or None (None = the legacy default stream)."""
+        sl, n, nm = self._layer_batch_args(slots, names)
+        _check(self._l.gg_layer_images_to_device(self._h, len(sl), _ptr(sl), n, nm, dst_ptr, range_ptr, stream_ptr))
+
+    def terrain_images_to_device_ptrs(self, slots, dst_ptr, stream_ptr):
+        """gg_terrain_images_to_device with raw device addresses: dst_ptr float32 [count][N][N][3]."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        _check(self._l.gg_terrain_images_to_device(self._h, len(sl), _ptr(sl), dst_ptr, stream_ptr))
+
+    @staticmethod
+    def _stream_out(torch, dev, current, stream, out, shape, dtype, what):
+        """`out` checked (contiguous `dtype` `shape` on `dev`) and marked in use on `stream`, or a new tensor allocated on `stream`."""
+        if out is None:
+            with torch.cuda.stream(stream):
+                return torch.empty(shape, dtype=dtype, device=dev)
+        if tuple(out.shape) != shape or out.dtype != dtype or out.device != dev or not out.is_contiguous():
+            raise ValueError(f"{what} must be a contiguous {dtype} tensor {shape} on {dev}")
+        if stream != current:
+            out.record_stream(stream)
+        return out
+
+    def layer_images_to_device(self, slots, names=("ground", "groundpatch"), out=None, ranges=None, stream=None):
+        """The 8-bit images gg_layer_image_u8 gives for layers `names` of `slots` (gg_layer_images_to_device):
+        (uint8 CUDA tensor [count, n_names, N, N] indexed [k, l, i, j] like the cv::Mat, C-contiguous;
+        float32 [count, n_names, 2] = lower, upper).  Allocated on `stream` (a torch.cuda.Stream; default: the current
+        stream), or `out` / `ranges` are filled.  The call returns without waiting for the device; work enqueued on
+        `stream` afterwards sees the images of the slots' layers as of their last enqueued scan or roll."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        shape = (len(slots), len(names), self.n, self.n)
+        out = self._stream_out(torch, dev, current, stream, out, shape, torch.uint8, "out")
+        ranges = self._stream_out(torch, dev, current, stream, ranges, shape[:2] + (2,), torch.float32, "ranges")
+        self.layer_images_to_device_ptrs(slots, names, out.data_ptr(), ranges.data_ptr(), stream.cuda_stream or None)
+        return out, ranges
+
+    def terrain_images_to_device(self, slots, out=None, stream=None):
+        """The terrain images gg_terrain_image gives for `slots` (gg_terrain_images_to_device): float32 CUDA tensor
+        [count, N, N, 3], C-contiguous, allocated on `stream` (default: the current stream) or filled into `out`.
+        Needs the full layers."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        out = self._stream_out(torch, dev, current, stream, out, (len(slots), self.n, self.n, 3), torch.float32, "out")
+        self.terrain_images_to_device_ptrs(slots, out.data_ptr(), stream.cuda_stream or None)
+        return out
 
     @property
     def stream(self):

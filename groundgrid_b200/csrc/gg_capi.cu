@@ -12,6 +12,8 @@
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -325,7 +327,8 @@ struct gg_handle_s {
     size_t d_raw_cap[kStreams] = {};
     float* d_image = nullptr;        // f3: terrain image staging (N * N * 3)
     unsigned char* d_image_u8 = nullptr;  // f3: 8-bit layer image staging (N * N)
-    float* d_minmax = nullptr;       //     and its min / max keys
+    float* d_minmax = nullptr;       //     and its lower / upper
+    int2* d_img_part = nullptr;      // f3: per-block ranges of the layer images, [n_slots][L_NUM][cdiv(N2, IMG_RANGE_CELLS)]
     unsigned long long* d_eval = nullptr;  // f4: [EVAL_LABELS][2] tallies
     HostPacker* packer = nullptr;    // created on the first packed batch call
     // gg_filter_cloud_batch[_begin] alternates between two sets of input / label buffers ("parity"), so the
@@ -1353,6 +1356,131 @@ int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scan
     return run_scans_grouped(h, count, scans, 0, nullptr, nullptr, nullptr, &caller);
 }
 
+namespace {
+// The layer "points" names for `slot` (layer_index without the name lookup).
+int points_layer(gg_handle h, int slot) {
+    int idx = 0;
+    layer_index(h, slot, "points", &idx);
+    return idx;
+}
+
+// A caller-owned device buffer of a batched slot call.
+struct CallerBuf {
+    const void* p;
+    size_t bytes;
+    size_t align;
+    bool required;     // false: may be null
+    const char* what;
+};
+
+// The validation shared by the batched calls on a set of slots and layer names (gg_get_layers_to_device,
+// gg_set_layers_from_device, gg_layer_images_to_device, gg_terrain_images_to_device), in this order: the handle, the
+// counts (count == 0 or n_names == 0 is a valid call with nothing to do: GG_OK, and the caller enqueues nothing), null
+// arguments, count <= n_slots, at most L_NUM names, each buffer (aligned, outside the layer arena, disjoint from the
+// other buffers), `count` distinct slots with initialised maps, `n_names` distinct names resolved as gg_get_layer
+// resolves them ("points" per slot, as LAYER_POINTS at *points_at; "expectedPoints" is not a layer of a slot).
+int check_slot_batch(gg_handle h, int count, const int* slots, int n_names, const char* const* names, std::initializer_list<CallerBuf> bufs,
+                     gg::LayerList* list, int* points_at) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0 || n_names < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0 || n_names == 0) return GG_OK;
+    if (!slots || !names) return fail(GG_E_ARG, "null argument");
+    for (const CallerBuf& b : bufs)
+        if (b.required && !b.p) return fail(GG_E_ARG, "null argument");
+    if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
+    if (n_names > gg::L_NUM) return fail(GG_E_ARG, "%d layer names, at most %d", n_names, (int)gg::L_NUM);
+    const gg::View& v = h->view;
+    const size_t arena = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    for (const CallerBuf& b : bufs) {
+        if (!b.p) continue;
+        if (reinterpret_cast<uintptr_t>(b.p) % b.align) return fail(GG_E_ARG, "%s is not %zu-byte aligned", b.what, b.align);
+        if (ranges_overlap(b.p, b.bytes, v.layers, arena)) return fail(GG_E_ARG, "%s overlaps the handle's layers", b.what);
+        for (const CallerBuf& o : bufs)
+            if (&o < &b && o.p && ranges_overlap(b.p, b.bytes, o.p, o.bytes)) return fail(GG_E_ARG, "%s overlaps %s", b.what, o.what);
+    }
+    int rc;
+    std::vector<unsigned char>& seen = h->seen_scratch;
+    seen.assign((size_t)h->n_slots, 0);
+    for (int i = 0; i < count; ++i) {
+        if ((rc = check_slot(h, slots[i]))) return rc;
+        if (seen[slots[i]]++) return fail(GG_E_ARG, "slot %d appears twice in one batch", slots[i]);
+        if (!h->slots[slots[i]].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slots[i]);
+    }
+    list->n = n_names;
+    for (int l = 0; l < n_names; ++l) {
+        const char* name = names[l];
+        if (!name) return fail(GG_E_ARG, "null layer name");
+        for (int m = 0; m < l; ++m)
+            if (std::strcmp(names[m], name) == 0) return fail(GG_E_ARG, "layer '%s' appears twice", name);
+        if (std::strcmp(name, "expectedPoints") == 0) return fail(GG_E_LAYER, "'expectedPoints' is a table of the handle, not a layer of a slot");
+        if (std::strcmp(name, "points") == 0) {
+            list->idx[l] = gg::LAYER_POINTS;
+            *points_at = l;
+        } else if ((rc = layer_index(h, slots[0], name, &list->idx[l]))) {
+            return rc;
+        }
+    }
+    return GG_OK;
+}
+
+// The stream pattern of the batched slot calls: per stream group with slots in the batch, one staging entry (per scan
+// p.slot, p.n_points = its position in the call, p.shift_i = the layer "points" names for the slot) and
+// launch(device entry, scans, group stream), after everything already enqueued on `stream` and on the group's stream;
+// `stream` then waits for the group.  No host wait but the flow control of the staging ring.
+int enqueue_slot_batch(gg_handle h, int count, const int* slots, void* stream,
+                       const std::function<int(const gg::SlotParams*, int, cudaStream_t)>& launch) {
+    int rc;
+    GG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t caller = static_cast<cudaStream_t>(stream);
+    GG_CUDA(cudaEventRecord(h->caller_in, caller));
+    for (int g = 0; g < h->n_streams; ++g) {
+        gg::SlotParams *hp = nullptr, *dp = nullptr;
+        int pos = 0, m = 0;
+        for (int i = 0; i < count; ++i) {
+            if (stream_index(h, slots[i]) != g) continue;
+            if (m == 0 && (rc = ring_acquire(h, &hp, &dp, &pos))) return rc;
+            gg::SlotParams& p = hp[m++];
+            std::memset(&p, 0, sizeof(p));
+            p.slot = slots[i];
+            p.n_points = i;
+            p.shift_i = points_layer(h, slots[i]);
+        }
+        if (m == 0) continue;
+        cudaStream_t st = h->streams[g];
+        if ((rc = ring_commit(h, pos, m, st))) return rc;
+        GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
+        h->launches += launch(dp, m, st);
+        GG_CUDA(cudaGetLastError());
+        if ((rc = ring_release(h, pos, st))) return rc;
+        GG_CUDA(cudaEventRecord(h->caller_out[g], st));
+        GG_CUDA(cudaStreamWaitEvent(caller, h->caller_out[g], 0));
+    }
+    return GG_OK;
+}
+
+// Per-block range scratch of the layer images (launch_layer_images), allocated on first use.
+int ensure_image_partials(gg_handle h) {
+    if (h->d_img_part) return GG_OK;
+    GG_CUDA(cudaSetDevice(h->device));
+    const size_t n = (size_t)h->n_slots * gg::L_NUM * ((h->view.k.N2 + gg::IMG_RANGE_CELLS - 1) / gg::IMG_RANGE_CELLS);
+    return dev_alloc(h, &h->d_img_part, n);
+}
+
+int layer_images(gg_handle h, int count, const int* slots, const gg::LayerList& list, uint8_t* dst, float* dev_range, void* stream) {
+    return enqueue_slot_batch(h, count, slots, stream, [&](const gg::SlotParams* dp, int m, cudaStream_t st) {
+        return gg::launch_layer_images(h->view, dp, m, list, h->d_img_part, dst, dev_range, st, h->prof);
+    });
+}
+
+int terrain_images(gg_handle h, int count, const int* slots, float* dst, void* stream) {
+    return enqueue_slot_batch(h, count, slots, stream, [&](const gg::SlotParams* dp, int m, cudaStream_t st) {
+        return gg::launch_terrain_images(h->view, dp, m, dst, st, h->prof);
+    });
+}
+}  // namespace
+
+// f3: the per-slot calls are one-scan batches of the kernels of gg_terrain_images_to_device / gg_layer_images_to_device
+// on the slot's own stream, followed by a pageable copy and a synchronise.
 int gg_terrain_image(gg_handle h, int slot, float* dst) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
@@ -1362,8 +1490,7 @@ int gg_terrain_image(gg_handle h, int slot, float* dst) {
     const size_t n = (size_t)h->view.k.N2 * 3;
     if (!h->d_image && (rc = dev_alloc(h, &h->d_image, n))) return rc;
     cudaStream_t st = stream_of(h, slot);
-    h->launches += gg::launch_terrain_image(h->view, slot, h->d_image, st, h->prof);
-    GG_CUDA(cudaGetLastError());
+    if ((rc = terrain_images(h, 1, &slot, h->d_image, st))) return rc;
     GG_CUDA(cudaMemcpyAsync(dst, h->d_image, n * sizeof(float), cudaMemcpyDeviceToHost, st));
     GG_CUDA(cudaStreamSynchronize(st));
     return GG_OK;
@@ -1374,27 +1501,50 @@ int gg_layer_image_u8(gg_handle h, int slot, const char* name, uint8_t* dst, flo
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (!name || !dst) return fail(GG_E_ARG, "null argument");
-    int l = 0;
-    if ((rc = layer_index(h, slot, name, &l))) return rc;
+    gg::LayerList list{};
+    list.n = 1;
+    if ((rc = layer_index(h, slot, name, &list.idx[0]))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     const size_t n = (size_t)h->view.k.N2;
     if (!h->d_image_u8) {
         if ((rc = dev_alloc(h, &h->d_image_u8, n))) return rc;
         if ((rc = dev_alloc(h, &h->d_minmax, 2))) return rc;
     }
+    if ((rc = ensure_image_partials(h))) return rc;
     cudaStream_t st = stream_of(h, slot);
-    const int init[2] = {0x7f800000, (int)(0xff800000u ^ 0x7fffffffu)};   // ordered keys of +inf / -inf
-    GG_CUDA(cudaMemcpyAsync(h->d_minmax, init, sizeof(init), cudaMemcpyHostToDevice, st));
-    h->launches += gg::launch_layer_image_u8(h->view, h->view.layer(slot, l), h->d_minmax, h->d_image_u8, st);
-    GG_CUDA(cudaGetLastError());
-    int keys[2];
+    if ((rc = layer_images(h, 1, &slot, list, h->d_image_u8, h->d_minmax, st))) return rc;
+    float range[2];
     GG_CUDA(cudaMemcpyAsync(dst, h->d_image_u8, n, cudaMemcpyDeviceToHost, st));
-    GG_CUDA(cudaMemcpyAsync(keys, h->d_minmax, sizeof(keys), cudaMemcpyDeviceToHost, st));
+    GG_CUDA(cudaMemcpyAsync(range, h->d_minmax, sizeof(range), cudaMemcpyDeviceToHost, st));
     GG_CUDA(cudaStreamSynchronize(st));
-    auto unkey = [](int k) { const int b = k >= 0 ? k : (k ^ 0x7fffffff); float f; std::memcpy(&f, &b, 4); return f; };
-    if (lower) *lower = unkey(keys[0]);
-    if (upper) *upper = unkey(keys[1]);
+    if (lower) *lower = range[0];
+    if (upper) *upper = range[1];
     return GG_OK;
+}
+
+int gg_layer_images_to_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, uint8_t* dst, float* dev_range,
+                              void* stream) {
+    gg::LayerList list{};
+    int points_at = -1, rc;
+    const size_t planes = (size_t)count * n_names, plane = h ? (size_t)h->view.k.N2 : 0;
+    if ((rc = check_slot_batch(h, count, slots, n_names, names,
+                               {{dst, planes * plane, 1, true, "dst"}, {dev_range, planes * 2 * sizeof(float), alignof(float), false, "dev_range"}},
+                               &list, &points_at)) ||
+        count == 0 || n_names == 0)
+        return rc;
+    if ((rc = ensure_image_partials(h))) return rc;
+    return layer_images(h, count, slots, list, dst, dev_range, stream);
+}
+
+int gg_terrain_images_to_device(gg_handle h, int count, const int* slots, float* dst, void* stream) {
+    // the terrain image reads "pointsRaw": resolving that name rejects a handle without the full layers (GG_E_LAYER)
+    static const char* const raw[1] = {"pointsRaw"};
+    gg::LayerList list{};
+    int points_at = -1, rc;
+    const size_t bytes = h ? (size_t)count * h->view.k.N2 * 3 * sizeof(float) : 0;
+    if ((rc = check_slot_batch(h, count, slots, 1, raw, {{dst, bytes, alignof(float), true, "dst"}}, &list, &points_at)) || count == 0)
+        return rc;
+    return terrain_images(h, count, slots, dst, stream);
 }
 
 // ---- single phases (GroundSegmentation.h:56-62 of the reference) ------------------------------
@@ -1555,7 +1705,7 @@ const char* gg_profile_kernel_name(int id) {
     static const char* names[gg::K_NUM] = {"k_rasterize",   "k_cell_tiles",    "k_cell_place",    "k_scatter",
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
-                                           "k_terrain_image", "k_eval_counts", "k_layer_copy"};
+                                           "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2078,52 +2228,15 @@ int gg_layer_device_ptr(gg_handle h, int slot, const char* name, void** dptr) {
 }
 
 namespace {
-// The layer "points" names for `slot` (layer_index without the name lookup).
-int points_layer(gg_handle h, int slot) {
-    int idx = 0;
-    layer_index(h, slot, "points", &idx);
-    return idx;
-}
-
-// gg_get_layers_to_device (import = false) / gg_set_layers_from_device (import = true).  Everything is validated
-// before anything is enqueued; then one k_layer_copy per stream group with slots in the batch, after everything
-// already enqueued on the caller's stream and on the group's stream, and before whatever the caller enqueues next.
+// gg_get_layers_to_device (import = false) / gg_set_layers_from_device (import = true): one k_layer_copy per stream
+// group with slots in the batch.
 int layer_transfer(gg_handle h, int count, const int* slots, int n_names, const char* const* names, float* buf, bool import, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0 || n_names < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0 || n_names == 0) return GG_OK;
-    if (!slots || !names || !buf) return fail(GG_E_ARG, "null argument");
-    if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
-    if (n_names > gg::L_NUM) return fail(GG_E_ARG, "%d layer names, at most %d", n_names, (int)gg::L_NUM);
-    if (reinterpret_cast<uintptr_t>(buf) % alignof(float)) return fail(GG_E_ARG, "buffer is not 4-byte aligned");
-    const gg::View& v = h->view;
-    const size_t plane = (size_t)v.k.N2 * sizeof(float);
-    if (ranges_overlap(buf, (size_t)count * n_names * plane, v.layers, (size_t)h->n_slots * v.n_layers * plane))
-        return fail(GG_E_ARG, "buffer overlaps the handle's layers");
-    int rc;
-    std::vector<unsigned char>& seen = h->seen_scratch;
-    seen.assign((size_t)h->n_slots, 0);
-    for (int i = 0; i < count; ++i) {
-        if ((rc = check_slot(h, slots[i]))) return rc;
-        if (seen[slots[i]]++) return fail(GG_E_ARG, "slot %d appears twice in one batch", slots[i]);
-        if (!h->slots[slots[i]].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slots[i]);
-    }
     gg::LayerList list{};
-    list.n = n_names;
-    int points_at = -1;  // position of "points" among the names
-    for (int l = 0; l < n_names; ++l) {
-        const char* name = names[l];
-        if (!name) return fail(GG_E_ARG, "null layer name");
-        for (int m = 0; m < l; ++m)
-            if (std::strcmp(names[m], name) == 0) return fail(GG_E_ARG, "layer '%s' appears twice", name);
-        if (std::strcmp(name, "expectedPoints") == 0) return fail(GG_E_LAYER, "'expectedPoints' is a table of the handle, not a layer of a slot");
-        if (std::strcmp(name, "points") == 0) {
-            list.idx[l] = gg::LAYER_POINTS;
-            points_at = l;
-        } else if ((rc = layer_index(h, slots[0], name, &list.idx[l]))) {
-            return rc;
-        }
-    }
+    int points_at = -1, rc;
+    const size_t bytes = h ? (size_t)count * n_names * h->view.k.N2 * sizeof(float) : 0;
+    if ((rc = check_slot_batch(h, count, slots, n_names, names, {{buf, bytes, alignof(float), true, "buffer"}}, &list, &points_at)) ||
+        count == 0 || n_names == 0)
+        return rc;
     // an import must not write one layer of a slot twice ("points" is also "obstacles" or "count")
     if (import && points_at >= 0)
         for (int i = 0; i < count; ++i) {
@@ -2132,32 +2245,9 @@ int layer_transfer(gg_handle h, int count, const int* slots, int n_names, const 
                 if (list.idx[l] == p)
                     return fail(GG_E_ARG, "slot %d: '%s' and 'points' are the same layer", slots[i], names[l]);
         }
-    GG_CUDA(cudaSetDevice(h->device));
-    cudaStream_t caller = static_cast<cudaStream_t>(stream);
-    GG_CUDA(cudaEventRecord(h->caller_in, caller));
-    for (int g = 0; g < h->n_streams; ++g) {
-        gg::SlotParams *hp = nullptr, *dp = nullptr;
-        int pos = 0, m = 0;
-        for (int i = 0; i < count; ++i) {
-            if (stream_index(h, slots[i]) != g) continue;
-            if (m == 0 && (rc = ring_acquire(h, &hp, &dp, &pos))) return rc;
-            gg::SlotParams& p = hp[m++];
-            std::memset(&p, 0, sizeof(p));
-            p.slot = slots[i];
-            p.n_points = i;
-            p.shift_i = points_layer(h, slots[i]);
-        }
-        if (m == 0) continue;
-        cudaStream_t st = h->streams[g];
-        if ((rc = ring_commit(h, pos, m, st))) return rc;
-        GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
-        h->launches += gg::launch_layer_copy(v, dp, m, list, buf, import, st, h->prof);
-        GG_CUDA(cudaGetLastError());
-        if ((rc = ring_release(h, pos, st))) return rc;
-        GG_CUDA(cudaEventRecord(h->caller_out[g], st));
-        GG_CUDA(cudaStreamWaitEvent(caller, h->caller_out[g], 0));
-    }
-    return GG_OK;
+    return enqueue_slot_batch(h, count, slots, stream, [&](const gg::SlotParams* dp, int m, cudaStream_t st) {
+        return gg::launch_layer_copy(h->view, dp, m, list, buf, import, st, h->prof);
+    });
 }
 }  // namespace
 

@@ -182,7 +182,7 @@ constexpr int OUT_TILE = 1024;
 // kernels of the pipeline, as reported by the profiling hooks (gg_profile_read)
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
-    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_NUM
+    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_NUM
 };
 
 // Optional per-kernel CUDA-event timing (bench.py's roofline needs the dominant kernel's own
@@ -240,9 +240,16 @@ struct UnpackDesc {
 // PointCloud2 payloads -> PointXYZIR records in the map frame, for `count` scans: descs[k] (batch[k].n_points records)
 // lands in the slot's own cloud buffer, v.points + batch[k].slot * pcap.
 int launch_unpack(const View& v, const SlotParams* batch, const UnpackDesc* descs, int count, int max_points, cudaStream_t st, Profiler* prof);
-int launch_terrain_image(const View& v, int slot, float* dst, cudaStream_t st, Profiler* prof);
-// mm: 2 floats (ordered-int keys of min / max), preset by the caller to the keys of +inf / -inf; dst: N * N bytes, row-major (i, j)
-int launch_layer_image_u8(const View& v, const float* layer, float* mm, unsigned char* dst, cudaStream_t st);
+// f3: the images of publish_grid_map_layer for `count` scans, with the staging entry of launch_layer_copy (batch[s].slot,
+// batch[s].n_points = position k in the call, batch[s].shift_i = the layer "points" names for it).
+// launch_layer_images: plane l of scan k -> dst[(k * names.n + l) * N2] as N * N bytes, row-major (i, j); range (may be
+// null) [k][l][2] = lower, upper.  partial: [n_slots][L_NUM][cdiv(N2, IMG_RANGE_CELLS)] scratch of the per-block
+// ranges, indexed by slot (two calls that share a slot are ordered on the slot's stream).
+constexpr int IMG_RANGE_CELLS = 4096;
+int launch_layer_images(const View& v, const SlotParams* batch, int count, const LayerList& names, int2* partial, unsigned char* dst, float* range,
+                        cudaStream_t st, Profiler* prof);
+// launch_terrain_images: the terrain image of scan k -> dst[k][N][N][3] (needs the full layers)
+int launch_terrain_images(const View& v, const SlotParams* batch, int count, float* dst, cudaStream_t st, Profiler* prof);
 int launch_eval(const View& v, const SlotParams* batch, unsigned long long* counts, cudaStream_t st, Profiler* prof);
 constexpr int EVAL_LABELS = 1024;  // ring values (SemanticKITTI label ids <= 259) x {ground, non-ground}
 

@@ -307,6 +307,29 @@ int gg_terrain_image(gg_handle h, int slot, float* dst);
  * non-finite cells 0.  dst: N*N bytes, row-major (i, j) like the cv::Mat; lower / upper (may be NULL) receive the range.
  * The colour table itself (cv::COLORMAP_TWILIGHT, 256 BGR triples) is OpenCV data: the caller applies it. */
 int gg_layer_image_u8(gg_handle h, int slot, const char* name, uint8_t* dst, float* lower, float* upper);
+
+/* The images of publish_grid_map_layer (src/GroundGridNodelet.cpp:216-228,234-291) for `count` distinct slots, written
+ * into caller-owned device memory and ordered on the caller's stream: the batched, device-side form of
+ * gg_layer_image_u8 / gg_terrain_image.
+ *   slots      : `count` distinct slots, each with an initialised map
+ *   names      : `n_names` (<= 12) distinct layer names, resolved as in gg_get_layers_to_device ("points" per slot)
+ *   dst        : gg_layer_images_to_device: uint8[count][n_names][N][N], the image of scan k and name l at
+ *                (k * n_names + l) * N*N, row-major like the cv::Mat of gg_layer_image_u8 (pixel (i, j) at i*N + j);
+ *                gg_terrain_images_to_device: float[count][N][N][3] (4-byte aligned), each image that of gg_terrain_image
+ *   dev_range  : NULL or float[count][n_names][2] (4-byte aligned): lower, upper of each image
+ *   stream     : cudaStream_t; NULL is the legacy default stream.  The contract of gg_get_layers_to_device: the work
+ *                starts after everything already enqueued on `stream` and on the stream group of every slot in the
+ *                batch, work enqueued on `stream` afterwards sees the images complete, and nothing waits on the host
+ *                except the flow control of the parameter staging ring.
+ * Pixels and ranges are bit-identical to gg_layer_image_u8 / gg_terrain_image of the same slot and name at the same
+ * point of the slot's stream (ordered min / max: -0 below +0; 0 for a non-finite cell; 0 everywhere for a plane that is
+ * constant or has no finite cell).
+ * count == 0 or n_names == 0 enqueues nothing and returns GG_OK.  Rejected with nothing enqueued: what
+ * gg_get_layers_to_device rejects, and (GG_E_ARG) a misaligned dev_range, dst or dev_range overlapping the handle's
+ * layers or each other.  gg_terrain_images_to_device without GG_FLAG_FULL_LAYERS: GG_E_LAYER. */
+int gg_layer_images_to_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, uint8_t* dst,
+                              float* dev_range, void* stream);
+int gg_terrain_images_to_device(gg_handle h, int count, const int* slots, float* dst, void* stream);
 int gg_eval_accumulate(gg_handle h, int slot);
 int gg_eval_read(gg_handle h, uint64_t* counts, int reset);
 
