@@ -156,6 +156,7 @@ def load(build_if_missing=True):
         "gg_interpolate_cell": (i, [vp, i, i, i]),
         "gg_eval_accumulate": (i, [vp, i]),
         "gg_eval_read": (i, [vp, vp, i]),
+        "gg_eval_counts_to_device": (i, [vp, i, vp, vp, vp]),
         "gg_profile_enable": (i, [vp, i]),
         "gg_profile_read": (i, [vp, vp, vp, i]),
         "gg_profile_kernel_count": (i, []),
@@ -727,6 +728,28 @@ class GroundGridB200:
         counts = np.zeros((1024, 2), np.uint64)
         _check(self._l.gg_eval_read(self._h, _ptr(counts), 1 if reset else 0))
         return counts
+
+    def eval_counts_to_device_ptrs(self, slots, dst_ptr, stream_ptr):
+        """gg_eval_counts_to_device with raw device addresses: dst_ptr uint64 [count][1024][2] (8-byte aligned), to which
+        the tallies are added; stream_ptr an int or None (None = the legacy default stream)."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        _check(self._l.gg_eval_counts_to_device(self._h, len(sl), _ptr(sl), dst_ptr, stream_ptr))
+
+    def eval_counts_to_device(self, slots, out=None, stream=None):
+        """The tallies eval_accumulate adds, for the last completed scan of each of `slots`, one tally per slot
+        (gg_eval_counts_to_device): int64 CUDA tensor [count, 1024, 2] ([k, id, 0] ground, [k, id, 1] non-ground; the
+        bits of the uint64 counts).  Without `out` a zeroed tensor is allocated on `stream` (a torch.cuda.Stream;
+        default: the current stream); with `out` the tallies are added to it, so one tensor keeps running sums over a
+        sequence.  The call returns without waiting for the device; work enqueued on `stream` afterwards sees them."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        shape = (len(slots), 1024, 2)
+        if out is None:
+            with torch.cuda.stream(stream):
+                out = torch.zeros(shape, dtype=torch.int64, device=dev)
+        else:
+            out = self._stream_out(torch, dev, current, stream, out, shape, torch.int64, "out")
+        self.eval_counts_to_device_ptrs(slots, out.data_ptr(), stream.cuda_stream or None)
+        return out
 
     def profile_enable(self, on=True):
         _check(self._l.gg_profile_enable(self._h, 1 if on else 0))

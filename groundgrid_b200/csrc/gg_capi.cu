@@ -1379,16 +1379,18 @@ struct CallerBuf {
 // arguments, count <= n_slots, at most L_NUM names, each buffer (aligned, outside the layer arena, disjoint from the
 // other buffers), `count` distinct slots with initialised maps, `n_names` distinct names resolved as gg_get_layer
 // resolves them ("points" per slot, as LAYER_POINTS at *points_at; "expectedPoints" is not a layer of a slot).
+// A call without layer names (gg_eval_counts_to_device) passes list == nullptr: n_names and names are then ignored.
 int check_slot_batch(gg_handle h, int count, const int* slots, int n_names, const char* const* names, std::initializer_list<CallerBuf> bufs,
                      gg::LayerList* list, int* points_at) {
+    const bool named = list != nullptr;
     if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0 || n_names < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0 || n_names == 0) return GG_OK;
-    if (!slots || !names) return fail(GG_E_ARG, "null argument");
+    if (count < 0 || (named && n_names < 0)) return fail(GG_E_ARG, "negative count");
+    if (count == 0 || (named && n_names == 0)) return GG_OK;
+    if (!slots || (named && !names)) return fail(GG_E_ARG, "null argument");
     for (const CallerBuf& b : bufs)
         if (b.required && !b.p) return fail(GG_E_ARG, "null argument");
     if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
-    if (n_names > gg::L_NUM) return fail(GG_E_ARG, "%d layer names, at most %d", n_names, (int)gg::L_NUM);
+    if (named && n_names > gg::L_NUM) return fail(GG_E_ARG, "%d layer names, at most %d", n_names, (int)gg::L_NUM);
     const gg::View& v = h->view;
     const size_t arena = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
     for (const CallerBuf& b : bufs) {
@@ -1406,6 +1408,7 @@ int check_slot_batch(gg_handle h, int count, const int* slots, int n_names, cons
         if (seen[slots[i]]++) return fail(GG_E_ARG, "slot %d appears twice in one batch", slots[i]);
         if (!h->slots[slots[i]].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slots[i]);
     }
+    if (!named) return GG_OK;
     list->n = n_names;
     for (int l = 0; l < n_names; ++l) {
         const char* name = names[l];
@@ -1427,8 +1430,10 @@ int check_slot_batch(gg_handle h, int count, const int* slots, int n_names, cons
 // p.slot, p.n_points = its position in the call, p.shift_i = the layer "points" names for the slot) and
 // launch(device entry, scans, group stream), after everything already enqueued on `stream` and on the group's stream;
 // `stream` then waits for the group.  No host wait but the flow control of the staging ring.
+// last_scan: the entries describe the slot's last scan instead (launch_eval): p.n_points = its point count, p.src /
+// p.packed = where its records are (as the scan saw them), and the position in the call moves to p.shift_j.
 int enqueue_slot_batch(gg_handle h, int count, const int* slots, void* stream,
-                       const std::function<int(const gg::SlotParams*, int, cudaStream_t)>& launch) {
+                       const std::function<int(const gg::SlotParams*, int, cudaStream_t)>& launch, bool last_scan = false) {
     int rc;
     GG_CUDA(cudaSetDevice(h->device));
     cudaStream_t caller = static_cast<cudaStream_t>(stream);
@@ -1444,6 +1449,13 @@ int enqueue_slot_batch(gg_handle h, int count, const int* slots, void* stream,
             p.slot = slots[i];
             p.n_points = i;
             p.shift_i = points_layer(h, slots[i]);
+            if (last_scan) {
+                const SlotState& s = h->slots[slots[i]];
+                p.n_points = (int)s.n_points;
+                p.shift_j = i;
+                p.src = s.src ? s.src : h->view.points + (size_t)slots[i] * h->pcap;
+                p.packed = s.packed_input;
+            }
         }
         if (m == 0) continue;
         cudaStream_t st = h->streams[g];
@@ -1476,6 +1488,21 @@ int terrain_images(gg_handle h, int count, const int* slots, float* dst, void* s
     return enqueue_slot_batch(h, count, slots, stream, [&](const gg::SlotParams* dp, int m, cudaStream_t st) {
         return gg::launch_terrain_images(h->view, dp, m, dst, st, h->prof);
     });
+}
+
+// f4: the rule of every evaluation call (the scan's labels are complete)
+int check_completed_scan(gg_handle h, int slot) {
+    const SlotState& s = h->slots[slot];
+    if (!s.ran || s.last_stop != 0) return fail(GG_E_STATE, "slot %d: no completed scan", slot);
+    return GG_OK;
+}
+
+int eval_counts(gg_handle h, int count, const int* slots, unsigned long long* dst, void* stream) {
+    int max_points = 0;
+    for (int i = 0; i < count; ++i) max_points = std::max(max_points, (int)h->slots[slots[i]].n_points);
+    return enqueue_slot_batch(
+        h, count, slots, stream,
+        [&](const gg::SlotParams* dp, int m, cudaStream_t st) { return gg::launch_eval(h->view, dp, m, max_points, dst, st, h->prof); }, true);
 }
 }  // namespace
 
@@ -1630,29 +1657,29 @@ int gg_get_point_classes(gg_handle h, int slot, uint32_t* codes, size_t n) {
     return GG_OK;
 }
 
+// f4: a one-scan batch of gg_eval_counts_to_device into the handle's tally, on the slot's own stream
 int gg_eval_accumulate(gg_handle h, int slot) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
-    SlotState& s = h->slots[slot];
-    if (!s.ran || s.last_stop != 0) return fail(GG_E_STATE, "slot %d: no completed scan", slot);
+    if ((rc = check_completed_scan(h, slot))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     if (!h->d_eval) {
         if ((rc = dev_alloc(h, &h->d_eval, (size_t)gg::EVAL_LABELS * 2))) return rc;
         GG_CUDA(cudaMemset(h->d_eval, 0, sizeof(unsigned long long) * gg::EVAL_LABELS * 2));
     }
-    cudaStream_t st = stream_of(h, slot);
-    gg::SlotParams *hp = nullptr, *dp = nullptr;
-    int pos = 0;
-    if ((rc = ring_acquire(h, &hp, &dp, &pos))) return rc;
-    std::memset(&hp[0], 0, sizeof(gg::SlotParams));
-    hp[0].slot = slot;
-    hp[0].n_points = (int)s.n_points;
-    hp[0].src = s.src ? s.src : h->view.points + (size_t)slot * h->pcap;
-    hp[0].packed = s.packed_input;
-    if ((rc = ring_commit(h, pos, 1, st))) return rc;
-    h->launches += gg::launch_eval(h->view, dp, h->d_eval, st, h->prof);
-    GG_CUDA(cudaGetLastError());
-    return ring_release(h, pos, st);
+    return eval_counts(h, 1, &slot, h->d_eval, stream_of(h, slot));
+}
+
+int gg_eval_counts_to_device(gg_handle h, int count, const int* slots, uint64_t* dev_counts, void* stream) {
+    static_assert(sizeof(uint64_t) == sizeof(unsigned long long), "64-bit tallies");
+    int rc;
+    const size_t bytes = count > 0 ? (size_t)count * gg::EVAL_LABELS * 2 * sizeof(uint64_t) : 0;
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr, {{dev_counts, bytes, alignof(uint64_t), true, "dev_counts"}}, nullptr, nullptr)) ||
+        count == 0)
+        return rc;
+    for (int i = 0; i < count; ++i)
+        if ((rc = check_completed_scan(h, slots[i]))) return rc;
+    return eval_counts(h, count, slots, reinterpret_cast<unsigned long long*>(dev_counts), stream);
 }
 
 int gg_eval_read(gg_handle h, uint64_t* counts, int reset) {

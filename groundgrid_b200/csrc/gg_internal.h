@@ -250,7 +250,10 @@ int launch_layer_images(const View& v, const SlotParams* batch, int count, const
                         cudaStream_t st, Profiler* prof);
 // launch_terrain_images: the terrain image of scan k -> dst[k][N][N][3] (needs the full layers)
 int launch_terrain_images(const View& v, const SlotParams* batch, int count, float* dst, cudaStream_t st, Profiler* prof);
-int launch_eval(const View& v, const SlotParams* batch, unsigned long long* counts, cudaStream_t st, Profiler* prof);
-constexpr int EVAL_LABELS = 1024;  // ring values (SemanticKITTI label ids <= 259) x {ground, non-ground}
+// f4: the evaluation tallies of the last completed scan of `count` slots, added into counts[k][EVAL_LABELS][2] (k =
+// batch[s].shift_j, the scan's position in the call).  batch[s].n_points / src / packed describe the scan's input;
+// max_points: the largest n_points of the batch.
+int launch_eval(const View& v, const SlotParams* batch, int count, int max_points, unsigned long long* counts, cudaStream_t st, Profiler* prof);
+constexpr int EVAL_LABELS = GG_EVAL_IDS;  // ring values (SemanticKITTI label ids <= 259) x {ground, non-ground}
 
 }  // namespace gg

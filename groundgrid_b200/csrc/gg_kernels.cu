@@ -27,8 +27,6 @@
 #include "gg_internal.h"
 
 namespace gg {
-// grid-stride kernels: one CTA per SM of an H100 SXM
-constexpr int GRID_STRIDE_BLOCKS = 132;
 
 // ------------------------------------------------------------------------------------------
 // small helpers
@@ -2118,28 +2116,51 @@ __global__ void __launch_bounds__(IMG_TILE * IMG_ROWS) k_terrain_image(View v, c
     }
 }
 
-// f4: the tallies of scripts/eval_groundpoint_classifier.py:95-118 for one segmented cloud: per
+// f4: the tallies of scripts/eval_groundpoint_classifier.py:95-118 for a batch of segmented clouds: per
 // ground-truth label id (carried in `ring`, scripts/kitti_data_publisher.py:122-132) the number of
-// points predicted non-ground (intensity 99) and ground (49).
-__global__ void __launch_bounds__(256) k_eval_counts(View v, const SlotParams* __restrict__ batch, unsigned long long* __restrict__ counts) {
+// points predicted ground (49, bin 2 * id) and non-ground (99, bin 2 * id + 1); absent points and ids
+// >= EVAL_LABELS are not counted.  Blocks (x, scan): block x tallies points [x, x + 1) * EVAL_TILE of
+// scan batch[scan] in a shared histogram, then adds each non-zero bin into the scan's tally at
+// counts + batch[scan].shift_j * 2 * EVAL_LABELS with one 64-bit atomic.  Most points of a scene fall
+// into a few ids (road, building, vegetation): the lanes of a warp that hit one bin add once
+// (__match_any_sync, as k_rasterize does for its runs).  Per point: the label byte and the ring
+// (uint16 of the packed cloud, else the second 16 bytes of the 32-byte record).
+constexpr int EVAL_THREADS = 256, EVAL_ILP = 4, EVAL_ROUNDS = 8;
+constexpr int EVAL_TILE = EVAL_THREADS * EVAL_ILP * EVAL_ROUNDS;   // points per block
+__global__ void __launch_bounds__(EVAL_THREADS) k_eval_counts(View v, const SlotParams* __restrict__ batch, unsigned long long* __restrict__ counts) {
+    const SlotParams& sp = batch[blockIdx.y];
+    const int n = sp.n_points, tile0 = blockIdx.x * EVAL_TILE;
+    if (tile0 >= n) return;   // the grid covers the largest scan of the batch
     __shared__ unsigned int s_cnt[EVAL_LABELS * 2];
-    for (int t = threadIdx.x; t < EVAL_LABELS * 2; t += 256) s_cnt[t] = 0u;
+    for (int t = threadIdx.x; t < EVAL_LABELS * 2; t += EVAL_THREADS) s_cnt[t] = 0u;
     __syncthreads();
-    const SlotParams& sp = batch[0];
-    const size_t base = (size_t)sp.slot * v.pcap;
-    for (int i = blockIdx.x * 256 + threadIdx.x; i < sp.n_points; i += gridDim.x * 256) {
-        const unsigned label = v.labels[base + i];
-        if (label == GG_LABEL_ABSENT) continue;
-        unsigned ring;
-        if (sp.packed)
-            ring = reinterpret_cast<const unsigned short*>(sp.packed + 3 * ((sp.n_points + 7) & ~7))[i];
-        else
-            ring = reinterpret_cast<const uint4*>(sp.src + i)[1].y & 0xffffu;
-        if (ring < EVAL_LABELS) atomicAdd(&s_cnt[ring * 2 + (label == GG_LABEL_NONGROUND ? 1 : 0)], 1u);
+    const uint8_t* labels = v.labels + (size_t)sp.slot * v.pcap;
+    const unsigned short* rings = sp.packed ? reinterpret_cast<const unsigned short*>(sp.packed + 3 * ((n + 7) & ~7)) : nullptr;
+    const int end = min(n, tile0 + EVAL_TILE), lane = threadIdx.x & 31;
+    constexpr unsigned NO_BIN = 0xffffffffu;
+    for (int r0 = tile0; r0 < end; r0 += EVAL_THREADS * EVAL_ILP) {   // uniform over the block: whole warps reach the match
+        unsigned bin[EVAL_ILP];
+#pragma unroll
+        for (int u = 0; u < EVAL_ILP; ++u) {
+            const int i = r0 + u * EVAL_THREADS + threadIdx.x;
+            bin[u] = NO_BIN;
+            if (i < end) {
+                const unsigned label = labels[i];
+                const unsigned ring = rings ? rings[i] : reinterpret_cast<const uint4*>(sp.src + i)[1].y & 0xffffu;
+                if (label != GG_LABEL_ABSENT && ring < EVAL_LABELS) bin[u] = ring * 2 + (label == GG_LABEL_NONGROUND ? 1 : 0);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < EVAL_ILP; ++u) {
+            // lanes without a point to count get a private pseudo key (never equal to a bin)
+            const unsigned peers = __match_any_sync(0xffffffffu, bin[u] != NO_BIN ? bin[u] : (0x80000000u | (unsigned)lane));
+            if (bin[u] != NO_BIN && lane == __ffs(peers) - 1) atomicAdd(&s_cnt[bin[u]], (unsigned)__popc(peers));
+        }
     }
     __syncthreads();
-    for (int t = threadIdx.x; t < EVAL_LABELS * 2; t += 256)
-        if (s_cnt[t]) atomicAdd(&counts[t], (unsigned long long)s_cnt[t]);
+    unsigned long long* dst = counts + (size_t)sp.shift_j * (EVAL_LABELS * 2);
+    for (int t = threadIdx.x; t < EVAL_LABELS * 2; t += EVAL_THREADS)
+        if (s_cnt[t]) atomicAdd(&dst[t], (unsigned long long)s_cnt[t]);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2439,8 +2460,8 @@ int launch_terrain_images(const View& v, const SlotParams* batch, int count, flo
     return 1;
 }
 
-int launch_eval(const View& v, const SlotParams* batch, unsigned long long* counts, cudaStream_t st, Profiler* prof) {
-    GG_LAUNCH(K_EVAL, k_eval_counts<<<GRID_STRIDE_BLOCKS, 256, 0, st>>>(v, batch, counts));
+int launch_eval(const View& v, const SlotParams* batch, int count, int max_points, unsigned long long* counts, cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_EVAL, k_eval_counts<<<dim3(max(1, cdiv(max_points, EVAL_TILE)), count), EVAL_THREADS, 0, st>>>(v, batch, counts));
     return 1;
 }
 

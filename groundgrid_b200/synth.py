@@ -60,8 +60,13 @@ def make_scene(seed=1234, n_boxes=24, rmin=5.0, rmax=50.0, stream_len=0.0, undul
     return Scene(boxes, undulation)
 
 
+# SemanticKITTI ids of the surfaces (semantic-kitti.yaml): what lidar_scan(..., labels=True) reports per point
+LABEL_ROAD, LABEL_CAR, LABEL_BUILDING = 40, 10, 50
+
+
 def _cast(scene, origins, dirs, ego_xy):
-    """Nearest hit distance along each ray (float64)."""
+    """Nearest hit distance along each ray (float64) and the SemanticKITTI id (uint16) of the surface hit: road for
+    the ground, car for a box, building for the enclosure wall."""
     ox, oy, oz = origins[:, 0], origins[:, 1], origins[:, 2]
     dx, dy, dz = dirs[:, 0], dirs[:, 1], dirs[:, 2]
     big = 1.0e9
@@ -82,6 +87,7 @@ def _cast(scene, origins, dirs, ego_xy):
                 t = np.where((t > 0) & np.isfinite(t), t, big)
                 t_w = np.minimum(t_w, t)
         t_best = np.minimum(t_g, t_w)
+        ids = np.where(t_g <= t_w, LABEL_ROAD, LABEL_BUILDING).astype(np.uint16)
         # boxes: slab test
         for b in scene.boxes:
             inv = [1.0 / dx, 1.0 / dy, 1.0 / dz]
@@ -95,32 +101,36 @@ def _cast(scene, origins, dirs, ego_xy):
             t1 = (b[5] - oz) * inv[2]
             tmin, tmax = np.maximum(tmin, np.minimum(t0, t1)), np.minimum(tmax, np.maximum(t0, t1))
             hit = (tmax >= tmin) & (tmin > 0)
-            t_best = np.where(hit & (tmin < t_best), tmin, t_best)
-    return t_best
+            closer = hit & (tmin < t_best)
+            t_best = np.where(closer, tmin, t_best)
+            ids[closer] = LABEL_CAR
+    return t_best, ids
 
 
 def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8), az_steps=2048,
                dropout=0.085, seed=1234, sensors=((0.0, 0.0, SENSOR_HEIGHT, 0.0),), range_noise=0.02,
-               frame="map"):
+               frame="map", labels=False):
     """One revolution of each sensor, concatenated sensor-major, ring-major then azimuth.
 
     sensors: (dx, dy, z, yaw_offset_deg) mounting poses in the ego frame.
     Returns (points[POINT_DTYPE], origin[3] float32) with points in the map frame
-    (or in the ego/base frame when frame == "base").
+    (or in the ego/base frame when frame == "base").  With labels=True also a uint16 array of the
+    SemanticKITTI id of the surface each point's ray hit (LABEL_ROAD, LABEL_CAR, LABEL_BUILDING); the
+    points and origin are the same bytes as without it.  The evaluation flow puts the ids into "ring".
     """
     rng = np.random.default_rng(seed)
     ego_xy = (float(ego_xy[0]), float(ego_xy[1]))
     elev = np.deg2rad(np.linspace(elev_deg[0], elev_deg[1], beams))[::-1]  # ring 0 = lowest beam
     az = np.arange(az_steps) * (2.0 * math.pi / az_steps)
     ce, se = np.cos(elev)[:, None], np.sin(elev)[:, None]
-    clouds = []
+    clouds, ids = [], []
     for (sx, sy, sz, syaw) in sensors:
         a = az[None, :] + yaw + math.radians(syaw)
         d = np.stack([ce * np.cos(a), ce * np.sin(a), np.broadcast_to(se, (beams, az_steps))], axis=-1).reshape(-1, 3)
         cy_, sy_ = math.cos(yaw), math.sin(yaw)
         o = np.array([ego_xy[0] + cy_ * sx - sy_ * sy, ego_xy[1] + sy_ * sx + cy_ * sy, sz])
         origins = np.broadcast_to(o, d.shape)
-        t = _cast(scene, origins, d, ego_xy)
+        t, hit_id = _cast(scene, origins, d, ego_xy)
         t = t + rng.normal(0.0, range_noise, size=t.shape)
         p = origins + t[:, None] * d
         keep = rng.uniform(size=t.shape) >= dropout
@@ -137,6 +147,7 @@ def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8
         pts["intensity"] = inten[keep].astype(np.float32)
         pts["ring"] = ring[keep]
         clouds.append(pts)
+        ids.append(hit_id[keep])
     if len(clouds) > 1:
         # np.concatenate drops the padding of the record dtype: fill a 32-byte-record array field by field instead
         cloud = np.zeros(sum(len(c) for c in clouds), POINT_DTYPE)
@@ -148,6 +159,8 @@ def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8
     else:
         cloud = clouds[0]
     origin = np.array([ego_xy[0], ego_xy[1], SENSOR_HEIGHT], np.float32)
+    if labels:
+        return cloud, origin, np.concatenate(ids)
     return cloud, origin
 
 

@@ -330,8 +330,42 @@ int gg_layer_image_u8(gg_handle h, int slot, const char* name, uint8_t* dst, flo
 int gg_layer_images_to_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, uint8_t* dst,
                               float* dev_range, void* stream);
 int gg_terrain_images_to_device(gg_handle h, int count, const int* slots, float* dst, void* stream);
+/* Evaluation tallies (scripts/eval_groundpoint_classifier.py:95-118): the ground-truth SemanticKITTI id of each point
+ * travels in `ring` (scripts/kitti_data_publisher.py:117-150); per id, the points predicted ground (49) and non-ground
+ * (99).  Absent points (label 0) and ids >= GG_EVAL_IDS are not counted.  gg_eval_accumulate adds the last completed
+ * scan of `slot` into one tally of the handle, uint64[GG_EVAL_IDS][2]; gg_eval_read synchronises the handle and copies
+ * it out (reset != 0: then zeroes it). */
+#define GG_EVAL_IDS 1024
 int gg_eval_accumulate(gg_handle h, int slot);
 int gg_eval_read(gg_handle h, uint64_t* counts, int reset);
+
+/* The tallies of gg_eval_accumulate for `count` distinct slots, each added into its own tally in caller-owned device
+ * memory and ordered on the caller's stream: the batched, device-side form of gg_eval_accumulate + gg_eval_read.
+ *   slots      : `count` distinct slots, each with a completed scan (not stopped early)
+ *   dev_counts : uint64[count][GG_EVAL_IDS][2] on the handle's device, 8-byte aligned.  The tallies of the last scan of
+ *                slots[k] are ADDED to dev_counts[k][id][c], c = 0 for points predicted ground, 1 for non-ground: zero
+ *                the buffer once and it keeps running sums per slot over a whole sequence.
+ *   stream     : cudaStream_t; NULL is the legacy default stream.  The contract of gg_get_layers_to_device: the work
+ *                starts after everything already enqueued on `stream` and on the stream group of every slot in the
+ *                batch, work enqueued on `stream` afterwards sees the tallies complete, and nothing waits on the host
+ *                except the flow control of the parameter staging ring.
+ * The ground truth is read where the scan took its input from:
+ *   - gg_filter_cloud, gg_upload_points / gg_upload_cloud_msg + gg_run_scans, gg_run_cloud_msgs_to_device: the slot's
+ *     own buffer (a gg_run_cloud_msgs_to_device payload may already be freed);
+ *   - gg_filter_cloud_batch: the handle's staging of that batch;
+ *   - gg_run_scans_device / gg_run_scans_to_device: the CALLER's cloud, which must still hold the scan's records when
+ *     the tallies run (e.g. freed on `stream` only after this call).
+ * The tallies are bit-identical to gg_eval_accumulate + gg_eval_read of the same slots at the same point of the slots'
+ * streams.  Because `ring` carries the label, a configuration with max_ring below the largest id of interest drops
+ * those points from the map (the reference does the same under its KITTI player), but they are still tallied.
+ * count == 0 enqueues nothing and returns GG_OK.  Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle, slots or dev_counts; count > n_slots; a slot out of range or repeated; dev_counts not
+ *              8-byte aligned or overlapping the handle's layers
+ *   GG_E_STATE a slot whose map is not initialised, or with no completed scan (none since gg_init_map, or the last
+ *              one stopped early)
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_eval_counts_to_device(gg_handle h, int count, const int* slots, uint64_t* dev_counts, void* stream);
 
 /* Per-kernel CUDA-event timing on the launching stream (bench.py roofline).  While enabled every
  * kernel launch is bracketed by an event pair; gg_profile_read synchronises and returns the
