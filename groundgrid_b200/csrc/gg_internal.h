@@ -84,6 +84,10 @@ struct SlotParams {
     // packed cloud (host-side packing of the batched host-buffer path): x | y | z as float[n_pad]
     // followed by ring as uint16[n_pad], n_pad = n_points rounded up to 8; null -> `src` is used
     const float* packed;
+    // batched calls on a list of slots: the scan's position in the call (where its part of the caller's buffer starts)
+    // and the layer "points" names for the slot (LAYER_POINTS); appended, so the fields above keep their offsets
+    int pos;
+    int points_layer;
 };
 
 // Per-scan destinations of the output kernels (launch_output).  They sit in the staging entry next to the scans'
@@ -200,9 +204,8 @@ int launch_build_detect_table(const View& v, const CfgConst& c, float4* tab, cud
 int launch_roll(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof);
 // layer_map: TMA descriptor of the handle's layer arena as a 3-D tensor (i, j, slot * n_layers + layer), box
 // 40 x 12 x 1 (k_detect_tma); null -> the patch detection stages its tile with plain loads (N % 4 != 0)
-// after_detect (may be null): recorded on st right before the spiral kernel
 int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int max_points, int stop_after, cudaStream_t st,
-                         Profiler* prof, const CUtensorMap* layer_map, cudaEvent_t after_detect);
+                         Profiler* prof, const CUtensorMap* layer_map);
 // single phases / single cells (the reference's public per-phase methods)
 int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map);
 int launch_spiral_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof);
@@ -222,8 +225,8 @@ struct LayerList {
 };
 // Copies `count` slots' layers between the arena and the caller's buffer buf[k][l][N2] (plane l of scan k at
 // (k * names.n + l) * N2), exporting (import = false: arena -> buf) or importing (import = true: buf -> arena).  Per
-// scan the staging entry carries batch[s].slot = the slot, batch[s].n_points = its position k in the call and
-// batch[s].shift_i = the layer "points" names for it; every other field is zero.  buf must not overlap the arena.
+// scan the staging entry carries batch[s].slot, batch[s].pos = its position k in the call and batch[s].points_layer;
+// every other field is zero.  buf must not overlap the arena.
 int launch_layer_copy(const View& v, const SlotParams* batch, int count, const LayerList& names, float* buf, bool import, cudaStream_t st,
                       Profiler* prof);
 // "next" rows of SURVEY.md section 8(f)
@@ -241,7 +244,7 @@ struct UnpackDesc {
 // lands in the slot's own cloud buffer, v.points + batch[k].slot * pcap.
 int launch_unpack(const View& v, const SlotParams* batch, const UnpackDesc* descs, int count, int max_points, cudaStream_t st, Profiler* prof);
 // f3: the images of publish_grid_map_layer for `count` scans, with the staging entry of launch_layer_copy (batch[s].slot,
-// batch[s].n_points = position k in the call, batch[s].shift_i = the layer "points" names for it).
+// batch[s].pos = position k in the call, batch[s].points_layer).
 // launch_layer_images: plane l of scan k -> dst[(k * names.n + l) * N2] as N * N bytes, row-major (i, j); range (may be
 // null) [k][l][2] = lower, upper.  partial: [n_slots][L_NUM][cdiv(N2, IMG_RANGE_CELLS)] scratch of the per-block
 // ranges, indexed by slot (two calls that share a slot are ordered on the slot's stream).
@@ -251,7 +254,7 @@ int launch_layer_images(const View& v, const SlotParams* batch, int count, const
 // launch_terrain_images: the terrain image of scan k -> dst[k][N][N][3] (needs the full layers)
 int launch_terrain_images(const View& v, const SlotParams* batch, int count, float* dst, cudaStream_t st, Profiler* prof);
 // f4: the evaluation tallies of the last completed scan of `count` slots, added into counts[k][EVAL_LABELS][2] (k =
-// batch[s].shift_j, the scan's position in the call).  batch[s].n_points / src / packed describe the scan's input;
+// batch[s].pos, the scan's position in the call).  batch[s].n_points / src / packed describe the scan's input;
 // max_points: the largest n_points of the batch.
 int launch_eval(const View& v, const SlotParams* batch, int count, int max_points, unsigned long long* counts, cudaStream_t st, Profiler* prof);
 constexpr int EVAL_LABELS = GG_EVAL_IDS;  // ring values (SemanticKITTI label ids <= 259) x {ground, non-ground}

@@ -1896,8 +1896,8 @@ __global__ void __launch_bounds__(LC_THREADS) k_layer_copy(View v, const SlotPar
     const SlotParams& sp = batch[blockIdx.y];
     const int l = blockIdx.z;
     const int idx = names.idx[l];
-    float* lay = v.layer(sp.slot, idx == LAYER_POINTS ? sp.shift_i : idx);
-    float* ext = buf + ((size_t)sp.n_points * names.n + l) * v.k.N2;
+    float* lay = v.layer(sp.slot, idx == LAYER_POINTS ? sp.points_layer : idx);
+    float* ext = buf + ((size_t)sp.pos * names.n + l) * v.k.N2;
     const float* __restrict__ src = IMPORT ? ext : lay;
     float* __restrict__ dst = IMPORT ? lay : ext;
     const int i0 = blockIdx.x * (LC_THREADS * LC_ILP) + threadIdx.x;
@@ -1950,8 +1950,8 @@ __global__ void __launch_bounds__(256) k_unpack_transform(View v, const SlotPara
 // f3: the images of GroundGridNodelet::publish_grid_map_layer (:234-291) for a batch of scans.  Both are the transpose
 // of the column-major layers (cv::Mat row = index(0), col = index(1)): block (t, s[, l]) owns an IMG_TILE x IMG_TILE tile
 // of the image, reads it along i (coalesced in the layer), and writes it along j (coalesced in the image) through
-// shared memory.  Per scan the staging entry carries batch[s].slot, batch[s].n_points = its position k in the call and
-// batch[s].shift_i = the layer "points" names for it (as launch_layer_copy).
+// shared memory.  Per scan the staging entry carries batch[s].slot, batch[s].pos = its position k in the call and
+// batch[s].points_layer (as launch_layer_copy).
 constexpr int IMG_TILE = 32;
 constexpr int IMG_ROWS = 8;   // blockDim (IMG_TILE, IMG_ROWS): every thread handles IMG_TILE / IMG_ROWS rows of a tile
 constexpr int IR_THREADS = 256;
@@ -1965,7 +1965,7 @@ __device__ __forceinline__ bool finite_f(float x) { return fabsf(x) <= FLT_MAX; 
 
 __device__ __forceinline__ const float* __restrict__ image_plane(const View& v, const SlotParams& sp, const LayerList& names, int l) {
     const int idx = names.idx[l];
-    return v.layer(sp.slot, idx == LAYER_POINTS ? sp.shift_i : idx);
+    return v.layer(sp.slot, idx == LAYER_POINTS ? sp.points_layer : idx);
 }
 
 // The 8-bit image grid_map::GridMapCvConverter::toImage<unsigned char, 1>(map, layer, CV_8UC1, img) hands to
@@ -2036,7 +2036,7 @@ __global__ void __launch_bounds__(IMG_TILE * IMG_ROWS) k_layer_image(View v, con
             s_range[0] = order_unkey(lo);
             s_range[1] = order_unkey(hi);
             if (range && blockIdx.x == 0) {
-                float* out = range + ((size_t)sp.n_points * names.n + l) * 2;
+                float* out = range + ((size_t)sp.pos * names.n + l) * 2;
                 out[0] = s_range[0];
                 out[1] = s_range[1];
             }
@@ -2054,7 +2054,7 @@ __global__ void __launch_bounds__(IMG_TILE * IMG_ROWS) k_layer_image(View v, con
         tile[ty + r * IMG_ROWS][tx] = px;
     }
     __syncthreads();
-    unsigned char* __restrict__ img = dst + ((size_t)sp.n_points * names.n + l) * v.k.N2;
+    unsigned char* __restrict__ img = dst + ((size_t)sp.pos * names.n + l) * v.k.N2;
 #pragma unroll
     for (int r = 0; r < IMG_TILE / IMG_ROWS; ++r) {
         const int i = i0 + ty + r * IMG_ROWS, j = j0 + tx;
@@ -2091,7 +2091,7 @@ __global__ void __launch_bounds__(IMG_TILE * IMG_ROWS) k_terrain_image(View v, c
     for (int r = 0; r < IMG_TILE / IMG_ROWS; ++r) {
         const int ii = ty + r * IMG_ROWS, i = i0 + ii;
         if (i >= N) break;
-        float* __restrict__ row = dst + ((size_t)sp.n_points * v.k.N2 + (size_t)i * N + j0) * 3;
+        float* __restrict__ row = dst + ((size_t)sp.pos * v.k.N2 + (size_t)i * N + j0) * 3;
 #pragma unroll
         for (int q = 0; q < 3; ++q) {
             const int f = tx + q * IMG_TILE;
@@ -2121,7 +2121,7 @@ __global__ void __launch_bounds__(IMG_TILE * IMG_ROWS) k_terrain_image(View v, c
 // points predicted ground (49, bin 2 * id) and non-ground (99, bin 2 * id + 1); absent points and ids
 // >= EVAL_LABELS are not counted.  Blocks (x, scan): block x tallies points [x, x + 1) * EVAL_TILE of
 // scan batch[scan] in a shared histogram, then adds each non-zero bin into the scan's tally at
-// counts + batch[scan].shift_j * 2 * EVAL_LABELS with one 64-bit atomic.  Most points of a scene fall
+// counts + batch[scan].pos * 2 * EVAL_LABELS with one 64-bit atomic.  Most points of a scene fall
 // into a few ids (road, building, vegetation): the lanes of a warp that hit one bin add once
 // (__match_any_sync, as k_rasterize does for its runs).  Per point: the label byte and the ring
 // (uint16 of the packed cloud, else the second 16 bytes of the 32-byte record).
@@ -2158,7 +2158,7 @@ __global__ void __launch_bounds__(EVAL_THREADS) k_eval_counts(View v, const Slot
         }
     }
     __syncthreads();
-    unsigned long long* dst = counts + (size_t)sp.shift_j * (EVAL_LABELS * 2);
+    unsigned long long* dst = counts + (size_t)sp.pos * (EVAL_LABELS * 2);
     for (int t = threadIdx.x; t < EVAL_LABELS * 2; t += EVAL_THREADS)
         if (s_cnt[t]) atomicAdd(&dst[t], (unsigned long long)s_cnt[t]);
 }
@@ -2219,7 +2219,7 @@ int launch_roll(const View& v, const SlotParams* batch, int count, cudaStream_t 
 }
 
 int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int max_points, int stop_after, cudaStream_t st,
-                         Profiler* prof, const CUtensorMap* layer_map, cudaEvent_t after_detect) {
+                         Profiler* prof, const CUtensorMap* layer_map) {
     int launches = 0;
     const int nb = max(1, cdiv(max_points, RASTER_TILE));
 
@@ -2253,7 +2253,6 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
     else
         GG_LAUNCH(K_DETECT, k_detect_ldg<4><<<dgrid, dim3(DT_X, DT_Y), 0, st>>>(v, batch));
     ++launches;
-    if (after_detect) cudaEventRecord(after_detect, st);   // the spiral (few warps per SM, latency bound) starts here: see gg_capi.cu
     if (stop_after == 2) return launches;
 
     if (v.skew.sk) {

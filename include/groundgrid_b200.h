@@ -121,8 +121,8 @@ int gg_get_config(gg_handle h, gg_config* cfg);
  * configuration changes of other slots.  The new configuration applies from the slot's next launch on
  * (every path: gg_filter_cloud[_batch[_begin]], gg_run_scans[_device], the per-phase entries).
  * gg_set_slot_config waits only for the work already enqueued on the slot's stream group; other groups keep
- * running with their own configurations.  (That stream may itself wait on work of other groups -- with GG_STAGGER
- * set, or after gg_fork_streams / gg_join_streams -- and such work is then waited for as well.)  A
+ * running with their own configurations.  (That stream may itself wait on work of other groups -- after
+ * gg_fork_streams / gg_join_streams -- and such work is then waited for as well.)  A
  * gg_filter_cloud_batch_begin batch that contains the slot must be waited for (gg_filter_cloud_batch_wait or
  * gg_synchronize) first.  Slots with identical settings share one copy of the derived device data.  thread_count is accepted and unused.  GG_E_ARG: null handle or config,
  * slot out of range; values are not validated (like gg_set_config). */
