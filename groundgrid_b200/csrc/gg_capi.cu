@@ -373,6 +373,17 @@ int dev_alloc(gg_handle h, T** p, size_t count) {
     return GG_OK;
 }
 
+// a new device copy of src, with room for `pad` more elements (kernels that run ahead may read up to them)
+template <typename T>
+int dev_upload(gg_handle h, const T** p, const std::vector<T>& src, size_t pad = 0) {
+    T* d = nullptr;
+    int rc = dev_alloc(h, &d, src.size() + pad);
+    if (rc) return rc;
+    GG_CUDA(cudaMemcpy(d, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
+    *p = d;
+    return GG_OK;
+}
+
 int check_slot(gg_handle h, int slot) {
     if (!h) return fail(GG_E_ARG, "null handle");
     if (slot < 0 || slot >= h->n_slots) return fail(GG_E_ARG, "slot %d out of range [0, %d)", slot, h->n_slots);
@@ -654,12 +665,10 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
 // TMA descriptor of the layer arena seen as a 3-D fp32 tensor (i fastest, j, plane = slot * n_layers + layer), box
 // 40 x 12 x 1 = the halo tile of k_detect_tma (the box starts at i0 - 4: TMA wants a 16-byte aligned innermost start).  cuTensorMapEncodeTiled is a driver-API call; it is resolved through the
 // runtime (cudaGetDriverEntryPoint) so that the library needs no link-time libcuda.  Row pitch must be a multiple of
-// 16 bytes: maps with N % 4 != 0 keep the plain-load kernel.  GG_DETECT_TMA=0 forces that kernel too.
+// 16 bytes: maps with N % 4 != 0 keep the plain-load kernel.
 bool encode_layer_map(gg_handle h) {
     const gg::View& v = h->view;
     if (v.k.N % 4 != 0) return false;
-    if (const char* e = getenv("GG_DETECT_TMA"))
-        if (atoi(e) == 0) return false;
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
     void* fn = nullptr;
@@ -873,186 +882,55 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     GG_CUDA_TRY(cudaMemset(v.cnt64, 0, S * N2 * sizeof(unsigned long long)));
     if (flags & GG_FLAG_FULL_LAYERS) GG_CUDA_TRY(cudaMemset(v.raw_i, 0, S * N2 * sizeof(int)));
 
-    // expectedPoints table (host libm, like the reference) and the spiral wavefront schedule
+    // expectedPoints table (host libm, like the reference) and the tables of the spiral path (gg_host.cpp:plan_spiral)
     {
         std::vector<float> table;
         gg::build_expected_points(n, table);
         GG_CUDA_TRY(cudaMemcpy(expected, table.data(), N2 * sizeof(float), cudaMemcpyHostToDevice));
-        std::vector<int> ls;
-        std::vector<uint32_t> vs;
-        gg::build_spiral_schedule(n, ls, vs);
-        int* d_ls = nullptr;
-        uint32_t* d_vs = nullptr;
-        GG_TRY(dev_alloc(h, &d_ls, ls.size()));
-        GG_TRY(dev_alloc(h, &d_vs, vs.size() + 1));
-        GG_CUDA_TRY(cudaMemcpy(d_ls, ls.data(), ls.size() * sizeof(int), cudaMemcpyHostToDevice));
-        GG_CUDA_TRY(cudaMemcpy(d_vs, vs.data(), vs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        v.level_start = d_ls;
-        v.visits = d_vs;
-        v.levels = (int)ls.size() - 1;
+        gg::SpiralPlan plan;
+        gg::plan_spiral(n, v.k.res_sq, plan);
+        GG_TRY(dev_upload(h, &v.level_start, plan.level_start));
+        GG_TRY(dev_upload(h, &v.visits, plan.visits, 1));
+        v.levels = (int)plan.level_start.size() - 1;
         h->sched_levels = v.levels;
-        h->sched_visits = (int)vs.size();
-        for (size_t l = 0; l + 1 < ls.size(); ++l) h->sched_max = std::max(h->sched_max, ls[l + 1] - ls[l]);
-        // records of the pipelined spiral kernel (GG_SPIRAL_DIST=0 selects the plain wavefront kernel)
+        h->sched_visits = (int)plan.visits.size();
+        h->sched_max = plan.max_per_level;
+        v.spiral_threads = plan.threads;
         v.spiral_recs = nullptr;
-        v.spiral_dist = 0;
-        v.spiral_threads = h->sched_max <= 512 ? 512 : 1024;
-        int dist = 2;
-        if (const char* e = getenv("GG_SPIRAL_DIST")) dist = atoi(e);
-        std::vector<uint32_t> rc;
-        int max_recent = 0;
-        if (dist >= 1 && dist <= 3 && h->sched_max <= 1024 && gg::build_spiral_records(n, v.k.res_sq, ls, vs, dist, rc, max_recent)) {
-            uint32_t* d_rc = nullptr;
-            GG_TRY(dev_alloc(h, &d_rc, rc.size() + 4));
-            GG_CUDA_TRY(cudaMemcpy(d_rc, rc.data(), rc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-            v.spiral_recs = reinterpret_cast<const uint4*>(d_rc);
-            v.spiral_dist = dist;
-        }
-        // skewed-layout spiral (GG_SPIRAL_SKEW=0 keeps the pipelined kernel)
         std::memset(&v.skew, 0, sizeof(v.skew));
-        int want_skew = 1;
-        if (const char* e = getenv("GG_SPIRAL_SKEW")) want_skew = atoi(e);
-        gg::SkewTables sk;
-        if (want_skew) gg::build_spiral_skew(n, ls, vs, sk);
-        // time-sharing of lane threads: the smallest M (multiple of 32) such that ring k + M of a side
-        // starts (prefetch window included) only after ring k has finished
-        // (only when one thread per lane does not fit a CTA: measured, a dedicated thread per lane is faster)
-        // Two thread layouts of the same schedule.  "Latency": one thread per lane whenever that fits a CTA (measured:
-        // fastest for a single scan).  "Throughput": a CTA with M lane threads per side, GG_SPIRAL_M (multiple of 32;
-        // 0, the default: same as latency; 32: the smallest M, so that two or three scans share an SM).  On an H100 SXM
-        // three small CTAs per SM run a level about 5x slower than one large CTA alone (DESIGN.md section 3.3), so batches
-        // run one thread per lane as well.
-        int M = 32, phases = 1, M_thr = 32, phases_thr = 1;
-        if (sk.ok) {
-            const int kGap = 2 * 8 + 4;  // 2 * PF_FAR of k_spiral_skew + slack
-            auto smallest_fitting = [&](int m0) {
-                int m = m0;
-                for (; m < sk.KP; m += 32) {
-                    bool fits = true;
-                    for (int sd = 0; sd < 4 && fits; ++sd)
-                        for (int c0 = 0; c0 + m < sk.KP && fits; ++c0) {
-                            const int a = sd * sk.KP + c0, b2 = a + m;
-                            if (sk.lane_begin[a] < sk.lane_end[a] && sk.lane_begin[b2] < sk.lane_end[b2] &&
-                                sk.lane_end[a] + kGap > sk.lane_begin[b2])
-                                fits = false;
-                        }
-                    if (fits) break;
-                }
-                return std::min(m, sk.KP);
-            };
-            M = (4 * sk.KP + 64 <= 1024) ? sk.KP : smallest_fitting(32);
-            phases = (sk.KP + M - 1) / M;
-            int m0 = 0;
-            if (const char* e = getenv("GG_SPIRAL_M")) m0 = atoi(e) / 32 * 32;
-            M_thr = m0 <= 0 ? M : smallest_fitting(std::max(32, m0));
-            phases_thr = (sk.KP + M_thr - 1) / M_thr;
-            // one CTA: lane threads + the two irregular warps (one thread per (visit, neighbour))
-            if (4 * M + 64 > 1024 || 4 * M_thr + 64 > 1024 || sk.max_irr_per_level * 9 > 64) sk.ok = false;
-        }
-        if (sk.ok) {
-            // re-layout of the irregular records: one dense block per level (see SkewView)
-            const int irr_max = std::max(1, sk.max_irr_per_level);
-            const int irr_words = ((irr_max * 22 + 3) / 4) * 4;
-            std::vector<uint32_t> blocks((size_t)(sk.levels + 4) * irr_words, 0xffffffffu);
-            for (int l = 0; l < sk.levels; ++l)
-                for (int r = sk.irr_level_start[l]; r < sk.irr_level_start[l + 1]; ++r) {
-                    const uint32_t* w = &sk.irr_recs[(size_t)r * 16];
-                    const int vv = r - sk.irr_level_start[l];
-                    uint32_t* blk = &blocks[(size_t)l * irr_words];
-                    for (int q = 0; q < 9; ++q) {
-                        blk[(vv * 9 + q) * 2] = w[1 + q];
-                        blk[(vv * 9 + q) * 2 + 1] = 0xffffffffu;
-                    }
-                    const uint32_t ents[4] = {w[10] & 0xffffu, w[10] >> 16, w[11] & 0xffffu, w[11] >> 16};
-                    for (uint32_t e : ents)
-                        if (e != 0xffffu) blk[(vv * 9 + (e >> 12)) * 2 + 1] = e & 4095u;
-                    uint32_t* hd = blk + irr_max * 18 + vv * 4;
-                    hd[0] = w[0];
-                    hd[1] = w[12];
-                    hd[2] = w[13];
-                    hd[3] = w[14];
-                }
-            // [phase][side * M + m] tables of a layout
-            auto upload_phases = [&](int m_, int phases_, const int** d_b, const int** d_e, const int** d_c) -> int {
-                std::vector<int> ph_b((size_t)phases_ * 4 * m_, 0), ph_e((size_t)phases_ * 4 * m_, 0), ph_c((size_t)phases_ * 4 * m_, 0);
-                for (int ph = 0; ph < phases_; ++ph)
-                    for (int sd = 0; sd < 4; ++sd)
-                        for (int m = 0; m < m_; ++m) {
-                            const int col = ph * m_ + m;
-                            if (col >= sk.KP) continue;
-                            const size_t dst = ((size_t)ph * 4 + sd) * m_ + m;
-                            ph_b[dst] = sk.lane_begin[sd * sk.KP + col];
-                            ph_e[dst] = sk.lane_end[sd * sk.KP + col];
-                            ph_c[dst] = sk.lane_cell0[sd * sk.KP + col];
-                        }
-                int *d_lb = nullptr, *d_le = nullptr, *d_lc = nullptr;
-                int rc2;
-                if ((rc2 = dev_alloc(h, &d_lb, ph_b.size())) || (rc2 = dev_alloc(h, &d_le, ph_e.size())) || (rc2 = dev_alloc(h, &d_lc, ph_c.size())))
-                    return rc2;
-                if (cudaMemcpy(d_lb, ph_b.data(), ph_b.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess ||
-                    cudaMemcpy(d_le, ph_e.data(), ph_e.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess ||
-                    cudaMemcpy(d_lc, ph_c.data(), ph_c.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess)
-                    return fail(GG_E_CUDA, "upload of the spiral phase tables failed");
-                *d_b = d_lb;
-                *d_e = d_le;
-                *d_c = d_lc;
-                return GG_OK;
-            };
-            GG_TRY(upload_phases(M, phases, &v.skew.ph_begin, &v.skew.ph_end, &v.skew.ph_cell0));
-            GG_TRY(upload_phases(M_thr, phases_thr, &v.skew.thr_ph_begin, &v.skew.thr_ph_end, &v.skew.thr_ph_cell0));
-            int* d_home = nullptr;
-            uint32_t* d_irr = nullptr;
-            GG_TRY(dev_alloc(h, &d_home, sk.cell_home.size()));
-            GG_TRY(dev_alloc(h, &d_irr, blocks.size() + 16));
-            GG_CUDA_TRY(cudaMemcpy(d_home, sk.cell_home.data(), sk.cell_home.size() * sizeof(int), cudaMemcpyHostToDevice));
-            GG_CUDA_TRY(cudaMemcpy(d_irr, blocks.data(), blocks.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        if (plan.kind == gg::SPIRAL_PIPE) {
+            const uint32_t* d_rc = nullptr;
+            GG_TRY(dev_upload(h, &d_rc, plan.recs, 4));
+            v.spiral_recs = reinterpret_cast<const uint4*>(d_rc);
+        } else if (plan.kind == gg::SPIRAL_SKEW) {
+            const gg::SkewTables& sk = plan.skew;
+            gg::SkewView& w = v.skew;
+            GG_TRY(dev_upload(h, &w.ph_begin, plan.ph_begin));
+            GG_TRY(dev_upload(h, &w.ph_end, plan.ph_end));
+            GG_TRY(dev_upload(h, &w.ph_cell0, plan.ph_cell0));
+            GG_TRY(dev_upload(h, &w.cell_home, sk.cell_home));
+            const uint32_t* d_irr = nullptr;
+            GG_TRY(dev_upload(h, &d_irr, plan.irr_blocks, 16));
             float2* d_sk = nullptr;
             float* d_sd = nullptr;
             GG_TRY(dev_alloc(h, &d_sk, S * sk.slots));
             GG_TRY(dev_alloc(h, &d_sd, S * sk.slots));
             GG_CUDA_TRY(cudaMemset(d_sk, 0, S * sk.slots * sizeof(float2)));
             GG_CUDA_TRY(cudaMemset(d_sd, 0, S * sk.slots * sizeof(float)));
-            v.skew.sk = d_sk;
-            v.skew.sd = d_sd;
-            v.skew.slots = sk.slots;
-            v.skew.cell_home = d_home;
-            v.skew.M = M;
-            v.skew.phases = phases;
-            v.skew.thr_M = M_thr;
-            v.skew.thr_phases = phases_thr;
-            // barrier-free synchronisation of the spiral kernel: opt-in (GG_SPIRAL_ASYNC=1).  The release fence of every
-            // publish also waits for the warp's loads of the next level, which the CTA barrier per level lets stay in flight.
-            int want_async = 0;
-            if (const char* e = getenv("GG_SPIRAL_ASYNC")) want_async = atoi(e);
-            auto upload_req = [&](int m_, const uint16_t** d_req) -> int {
-                *d_req = nullptr;
-                std::vector<uint16_t> rq;
-                int n_agents = 0;
-                if (!want_async || !gg::build_skew_sync(sk, m_, gg::SKEW_XCH_ASYNC, rq, n_agents)) return GG_OK;
-                uint16_t* d = nullptr;
-                int rc2;
-                if ((rc2 = dev_alloc(h, &d, rq.size()))) return rc2;
-                if (cudaMemcpy(d, rq.data(), rq.size() * sizeof(uint16_t), cudaMemcpyHostToDevice) != cudaSuccess)
-                    return fail(GG_E_CUDA, "upload of the spiral synchronisation table failed");
-                *d_req = d;
-                return GG_OK;
-            };
-            v.skew.sync_sleep = 20;
-            if (const char* e = getenv("GG_SPIRAL_SLEEP")) v.skew.sync_sleep = std::max(0, atoi(e));
-            GG_TRY(upload_req(M, &v.skew.req));
-            if (M_thr == M)
-                v.skew.thr_req = v.skew.req;
-            else
-                GG_TRY(upload_req(M_thr, &v.skew.thr_req));
-            v.skew.irr_blocks = reinterpret_cast<const uint4*>(d_irr);
-            v.skew.irr_max = irr_max;
-            v.skew.irr_chunks = irr_words / 4;
-            v.skew.KP = sk.KP;
-            v.skew.rows = sk.rows;
-            v.skew.row0 = sk.row0;
-            v.skew.lanes = sk.lanes;
-            v.skew.levels = sk.levels;
-            std::memcpy(v.skew.pattern, sk.pattern, sizeof(sk.pattern));
+            w.sk = d_sk;
+            w.sd = d_sd;
+            w.slots = sk.slots;
+            w.M = plan.M;
+            w.phases = plan.phases;
+            w.irr_blocks = reinterpret_cast<const uint4*>(d_irr);
+            w.irr_max = plan.irr_max;
+            w.irr_chunks = plan.irr_chunks;
+            w.KP = sk.KP;
+            w.rows = sk.rows;
+            w.row0 = sk.row0;
+            w.lanes = sk.lanes;
+            w.levels = sk.levels;
+            std::memcpy(w.pattern, sk.pattern, sizeof(sk.pattern));
         }
     }
 

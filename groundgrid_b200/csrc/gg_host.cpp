@@ -414,22 +414,6 @@ void build_spiral_skew(int n, const std::vector<int>& level_start, const std::ve
             mirror = (hown[0] == own) ? hown[1] : hown[0];
             if (hown[2] >= 0) return;
         }
-        {
-            SkewTables::Access a;
-            a.level = v.level;
-            a.lane = lane;
-            a.own = own;
-            a.mirror = mirror;
-            a.cell = (int)cell;
-            a.regular = regular;
-            for (int q = 0; q < 9; ++q) {
-                a.nb[q] = nb[q];
-                a.recent_lane[q] = -1;
-            }
-            for (int e = 0; e < 4; ++e)
-                if (rec[e] != 0xffffu) a.recent_lane[rec[e] >> 12] = (int)(rec[e] & 4095u);
-            t.acc.push_back(a);
-        }
         if (regular) {
             ++t.n_regular;
             if (reg_first[lane] < 0) {
@@ -476,99 +460,90 @@ void build_spiral_skew(int n, const std::vector<int>& level_start, const std::ve
     t.ok = true;
 }
 
-bool build_skew_sync(const SkewTables& t, int M, int xch_depth, std::vector<uint16_t>& req, int& n_agents) {
-    req.clear();
-    n_agents = 0;
-    if (!t.ok || M < 32 || (M % 32) != 0 || xch_depth < 2 || (xch_depth & (xch_depth - 1))) return false;
-    const int lane_agents = 4 * M / 32;
-    if (lane_agents + 1 > 32 || t.levels >= 65535) return false;
-    n_agents = lane_agents + 1;
-    const int IRR = lane_agents, L = t.levels;
-    req.assign((size_t)n_agents * L * 32, 0);
-    bool ok = true;
-    auto agent_of = [&](const SkewTables::Access& a) {
-        if (!a.regular) return IRR;
-        const int side = a.lane / t.KP, col = a.lane % t.KP;
-        return (side * M + col % M) / 32;
-    };
-    // "before agent a starts level lvl, agent b has completed level done" (progress[b] >= done + 1)
-    auto need = [&](int a, int lvl, int b, int done) {
-        if (a == b || b < 0) return;
-        if (lvl < 0) lvl = 0;
-        if (done + 1 > lvl) {   // only levels that a barrier would have separated as well
-            if (getenv("GG_SYNC_DEBUG")) fprintf(stderr, "sync: agent %d level %d needs agent %d done %d\n", a, lvl, b, done);
-            ok = false;
+// The path choice, in order of preference:
+//   1. skew, when build_spiral_skew covers the geometry and one CTA holds the layout.  One lane thread per lane when that
+//      fits (measured fastest, for single scans and batches alike, DESIGN.md section 3.3); otherwise lane threads are
+//      time-shared: the smallest M (multiple of 32) such that ring k + M of a side starts (prefetch window included)
+//      only after ring k has finished.
+//   2. pipe, when every level has at most 1024 visits and build_spiral_records succeeds.
+//   3. plain k_spiral.
+void plan_spiral(int n, double res_sq, SpiralPlan& p) {
+    p = SpiralPlan();
+    build_spiral_schedule(n, p.level_start, p.visits);
+    for (size_t l = 0; l + 1 < p.level_start.size(); ++l) p.max_per_level = std::max(p.max_per_level, p.level_start[l + 1] - p.level_start[l]);
+
+    SkewTables& sk = p.skew;
+    build_spiral_skew(n, p.level_start, p.visits, sk);
+    if (sk.ok) {
+        int M = sk.KP;
+        if (4 * sk.KP + SKEW_IRR_THREADS > 1024) {
+            const int kGap = 2 * 8 + 4;  // 2 * PF_FAR of k_spiral_skew + slack
+            for (M = 32; M < sk.KP; M += 32) {
+                bool fits = true;
+                for (int sd = 0; sd < 4 && fits; ++sd)
+                    for (int c0 = 0; c0 + M < sk.KP && fits; ++c0) {
+                        const int a = sd * sk.KP + c0, b2 = a + M;
+                        if (sk.lane_begin[a] < sk.lane_end[a] && sk.lane_begin[b2] < sk.lane_end[b2] && sk.lane_end[a] + kGap > sk.lane_begin[b2])
+                            fits = false;
+                    }
+                if (fits) break;
+            }
+            M = std::min(M, sk.KP);
+        }
+        // one CTA: lane threads + the two irregular warps (one thread per (visit, neighbour))
+        if (4 * M + SKEW_IRR_THREADS <= 1024 && sk.max_irr_per_level * 9 <= SKEW_IRR_THREADS) {
+            p.kind = SPIRAL_SKEW;
+            p.M = M;
+            p.phases = (sk.KP + M - 1) / M;
+            p.threads = 4 * M + SKEW_IRR_THREADS;
+            // [phase][side * M + m] tables of the lane threads
+            const size_t cols = (size_t)p.phases * 4 * M;
+            p.ph_begin.assign(cols, 0);
+            p.ph_end.assign(cols, 0);
+            p.ph_cell0.assign(cols, 0);
+            for (int ph = 0; ph < p.phases; ++ph)
+                for (int sd = 0; sd < 4; ++sd)
+                    for (int m = 0; m < M; ++m) {
+                        const int col = ph * M + m;
+                        if (col >= sk.KP) continue;
+                        const size_t dst = ((size_t)ph * 4 + sd) * M + m;
+                        p.ph_begin[dst] = sk.lane_begin[sd * sk.KP + col];
+                        p.ph_end[dst] = sk.lane_end[sd * sk.KP + col];
+                        p.ph_cell0[dst] = sk.lane_cell0[sd * sk.KP + col];
+                    }
+            // re-layout of the irregular records: one dense block per level (see SkewView)
+            p.irr_max = std::max(1, sk.max_irr_per_level);
+            const int irr_words = ((p.irr_max * 22 + 3) / 4) * 4;
+            p.irr_chunks = irr_words / 4;
+            p.irr_blocks.assign((size_t)(sk.levels + 4) * irr_words, 0xffffffffu);
+            for (int l = 0; l < sk.levels; ++l)
+                for (int r = sk.irr_level_start[l]; r < sk.irr_level_start[l + 1]; ++r) {
+                    const uint32_t* w = &sk.irr_recs[(size_t)r * 16];
+                    const int vv = r - sk.irr_level_start[l];
+                    uint32_t* blk = &p.irr_blocks[(size_t)l * irr_words];
+                    for (int q = 0; q < 9; ++q) {
+                        blk[(vv * 9 + q) * 2] = w[1 + q];
+                        blk[(vv * 9 + q) * 2 + 1] = 0xffffffffu;
+                    }
+                    const uint32_t ents[4] = {w[10] & 0xffffu, w[10] >> 16, w[11] & 0xffffu, w[11] >> 16};
+                    for (uint32_t e : ents)
+                        if (e != 0xffffu) blk[(vv * 9 + (e >> 12)) * 2 + 1] = e & 4095u;
+                    uint32_t* hd = blk + p.irr_max * 18 + vv * 4;
+                    hd[0] = w[0];
+                    hd[1] = w[12];
+                    hd[2] = w[13];
+                    hd[3] = w[14];
+                }
             return;
         }
-        uint16_t& r = req[((size_t)a * L + lvl) * 32 + b];
-        r = std::max<uint16_t>(r, (uint16_t)(done + 1));
-    };
-    struct Loc {
-        int w_agent = -1, w_level = -1;
-        std::vector<std::pair<int, int>> reads;   // (agent, level at which the value has been consumed) since the last write
-    };
-    // The skewed copy and the normal layers: one location per slot / cell, and the sequential order of the visits IS the
-    // order of any two conflicting accesses.  The exchange ring is different: entry (lane, level % depth) is storage
-    // shared by the values (lane, level), (lane, level + depth), ... -- each value is written once (at its level) and read
-    // at the next level; its conflicts are worked out per value after the pass.
-    const size_t n_cells = (size_t)t.n * t.n;
-    std::vector<Loc> loc(t.slots + n_cells);
-    auto SK = [&](int slot) -> Loc& { return loc[(size_t)slot]; };
-    auto CELL = [&](int cell) -> Loc& { return loc[t.slots + (size_t)cell]; };
-    auto read = [&](Loc& x, int a, int load_level, int done_level) {
-        need(a, load_level, x.w_agent, x.w_level);
-        x.reads.push_back({a, done_level});
-    };
-    auto write = [&](Loc& x, int a, int level) {
-        for (const auto& r : x.reads) need(a, level, r.first, r.second);
-        need(a, level, x.w_agent, x.w_level);
-        x.reads.clear();
-        x.w_agent = a;
-        x.w_level = level;
-    };
-    struct XVal {
-        int level, writer;
-        std::vector<int> readers;
-    };
-    std::vector<std::vector<XVal>> xch((size_t)t.lanes);   // per lane, in increasing level (a lane's visits are sequential)
-    for (const SkewTables::Access& v : t.acc) {
-        const int a = agent_of(v), l = v.level;
-        for (int q = 0; q < 9; ++q) {
-            if (v.recent_lane[q] >= 0) {
-                // the value the producer lane published at level l - 1 (visits of inner rings come earlier in the sequence
-                // but may sit at later levels, so it need not be the lane's latest entry)
-                std::vector<XVal>& xs = xch[(size_t)v.recent_lane[q]];
-                size_t i = xs.size();
-                while (i > 0 && xs[i - 1].level > l - 1) --i;
-                if (i == 0 || xs[i - 1].level != l - 1) {
-                    if (getenv("GG_SYNC_DEBUG")) fprintf(stderr, "sync: exchange value (%d, %d) missing\n", v.recent_lane[q], l - 1);
-                    ok = false;
-                    continue;
-                }
-                need(a, l, xs[i - 1].writer, l - 1);
-                xs[i - 1].readers.push_back(a);
-            } else {
-                if (v.nb[q] < 0 || (size_t)v.nb[q] >= t.slots) return false;
-                read(SK(v.nb[q]), a, l - 1, l);
-            }
-        }
-        write(SK(v.own), a, l);
-        if (v.mirror >= 0) write(SK(v.mirror), a, l);
-        write(CELL(v.cell), a, l);
-        std::vector<XVal>& own = xch[(size_t)v.lane];
-        if (!own.empty() && own.back().level >= l) ok = false;
-        own.push_back({l, a, {}});
     }
-    // storage reuse of the exchange ring: value (lane, l2) overwrites the last earlier value with l1 = l2 (mod depth)
-    for (const std::vector<XVal>& xs : xch)
-        for (size_t i = 0; i < xs.size(); ++i)
-            for (size_t j = i; j-- > 0;) {
-                if ((xs[i].level - xs[j].level) % xch_depth != 0) continue;
-                need(xs[i].writer, xs[i].level, xs[j].writer, xs[j].level);
-                for (int r : xs[j].readers) need(xs[i].writer, xs[i].level, r, xs[j].level + 1);
-                break;
-            }
-    return ok;
+    int max_recent = 0;
+    if (p.max_per_level <= 1024 && build_spiral_records(n, res_sq, p.level_start, p.visits, SPIRAL_PIPE_DIST, p.recs, max_recent)) {
+        p.kind = SPIRAL_PIPE;
+        p.threads = p.max_per_level <= 512 ? 512 : 1024;
+        return;
+    }
+    p.threads = SPIRAL_THREADS;
 }
 
 // ---- host-side cloud packing (gg_filter_cloud_batch) -------------------------------------
@@ -789,19 +764,13 @@ int gg_host_spiral_records(int n, float resolution, int dist, uint32_t* recs, in
     return ok ? 1 : 0;
 }
 
-// synchronisation table of the barrier-free spiral kernel for a thread layout (see build_skew_sync); returns 1 if it exists
-int gg_host_spiral_skew_sync(int n, int M, int xch_depth, uint16_t* req, int req_cap, int* n_agents) {
-    std::vector<int> ls;
-    std::vector<uint32_t> vs;
-    gg::build_spiral_schedule(n, ls, vs);
-    gg::SkewTables t;
-    gg::build_spiral_skew(n, ls, vs, t);
-    std::vector<uint16_t> r;
-    int na = 0;
-    const bool ok = gg::build_skew_sync(t, M, xch_depth, r, na);
-    if (n_agents) *n_agents = na;
-    if (ok && req && req_cap >= (int)r.size()) std::memcpy(req, r.data(), r.size() * sizeof(uint16_t));
-    return ok ? 1 : 0;
+// out[4]: the spiral path of a map (see plan_spiral): kind (gg::SpiralKind), CTA threads, M, phases
+int gg_host_spiral_plan(int n, float resolution, int* out) {
+    gg::SpiralPlan p;
+    gg::plan_spiral(n, (double)resolution * (double)resolution, p);
+    const int v[4] = {(int)p.kind, p.threads, p.M, p.phases};
+    std::memcpy(out, v, sizeof(v));
+    return 0;
 }
 
 // header: ok, K, KP, rows, levels, row0, lanes, n_irregular, max_irr_per_level, n_regular

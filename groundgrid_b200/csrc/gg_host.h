@@ -62,28 +62,30 @@ struct SkewTables {
     std::vector<uint32_t> irr_recs;      // 16 words per irregular visit: own, nb[9], recents01, recents23, mirror, lane, cell, pad
     int max_irr_per_level = 0;
     size_t n_regular = 0, n_irregular = 0;
-    // every visit in SEQUENTIAL order with the memory it touches in k_spiral_skew (input of build_skew_sync)
-    struct Access {
-        int level, lane;          // lane = side * KP + ring + 1 (also the visit's exchange-buffer entry)
-        int own, mirror, cell;    // slots written (mirror: -1 or the second home of a ring corner), cell of the normal layers
-        int nb[9];                // slots read
-        int recent_lane[9];       // >= 0: neighbour q was written one level ago and arrives through the exchange buffer entry of this lane
-        bool regular;             // executed by its lane thread (else by the irregular warps)
-    };
-    std::vector<Access> acc;
 };
-// Point-to-point synchronisation of k_spiral_skew<.., ASYNC>: the CTA-wide barrier per level is replaced by progress
-// counters, one per AGENT (a warp of lane threads, or the two irregular warps together).  req[(agent * levels + l) * 32 + b]
-// = progress agent b must have reached (= number of levels it has completed) before `agent` may start level l.
-// Derived from the exact read / write sets of every visit (RAW, WAR and WAW on the skewed copy, the normal layers and
-// the exchange ring of depth xch_depth), with the kernel's timing: the slots of a visit at level l are loaded during
-// level l - 1, neighbours written at level l - 1 are read from the exchange ring during level l, stores happen at level l.
-// M = lane threads per side (thread layout).  Returns false if some dependence cannot be expressed (then the barrier
-// kernel is used).
-bool build_skew_sync(const SkewTables& t, int M, int xch_depth, std::vector<uint16_t>& req, int& n_agents);
 void build_spiral_skew(int n, const std::vector<int>& level_start, const std::vector<uint32_t>& visits, SkewTables& t);
 bool build_spiral_records(int n, double res_sq, const std::vector<int>& level_start, const std::vector<uint32_t>& visits,
                           int dist, std::vector<uint32_t>& recs, int& max_recent);
+
+// The spiral kernel a map of n cells per side runs, and the host tables it reads (gg_create uploads them):
+//   SPIRAL_SKEW   k_spiral_skew<threads>: the skewed layout fits one CTA (4 * M lane threads + SKEW_IRR_THREADS)
+//   SPIRAL_PIPE   k_spiral_pipe<threads, SPIRAL_PIPE_DIST>: at most 1024 visits per level and records that fit
+//   SPIRAL_PLAIN  k_spiral: anything else
+enum SpiralKind : int { SPIRAL_PLAIN = 0, SPIRAL_PIPE = 1, SPIRAL_SKEW = 2 };
+struct SpiralPlan {
+    SpiralKind kind = SPIRAL_PLAIN;
+    int threads = 0;                     // CTA threads of the spiral launch
+    int M = 0, phases = 0;               // skew: lane threads per side, rings each lane thread walks one after the other
+    std::vector<int> level_start;        // the wavefront schedule (every kind; k_spiral reads it directly)
+    std::vector<uint32_t> visits;
+    int max_per_level = 0;
+    std::vector<uint32_t> recs;          // pipe: build_spiral_records at SPIRAL_PIPE_DIST
+    SkewTables skew;                     // skew: the layout (sizes, pattern, cell homes)
+    std::vector<int> ph_begin, ph_end, ph_cell0;   // skew: [phase][side * M + m] (SkewView)
+    std::vector<uint32_t> irr_blocks;    // skew: the irregular visits, one block of irr_chunks uint4 per level (+ 4 padding levels)
+    int irr_max = 0, irr_chunks = 0;
+};
+void plan_spiral(int n, double res_sq, SpiralPlan& p);
 }  // namespace gg
 
 extern "C" {
@@ -99,6 +101,6 @@ int gg_host_config_registry(int n_slots, int n_ops, const int* op_slot, const gg
 int gg_host_pack_cloud(const gg_point* src, size_t n, unsigned char* dst);
 int gg_host_pack_cloud_cached(const gg_point* src, size_t n, unsigned char* dst);
 int gg_host_packer_selftest(int threads, int n_jobs, size_t n_points, int ring_slots, int rounds, int lag);
-int gg_host_spiral_skew_sync(int n, int M, int xch_depth, uint16_t* req, int req_cap, int* n_agents);
+int gg_host_spiral_plan(int n, float resolution, int* out);
 int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* lane_end, int* cell_home, int* irr_level_start, uint32_t* irr_recs, int irr_cap_words);
 }

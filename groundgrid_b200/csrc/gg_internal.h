@@ -102,9 +102,13 @@ struct OutDest {
     int reserved;      // zero
 };
 
+// Spiral kernels (the path is chosen by gg_host.cpp:plan_spiral)
+constexpr int SPIRAL_THREADS = 512;   // CTA threads of the plain k_spiral
+constexpr int SPIRAL_PIPE_DIST = 2;   // prefetch distance (levels) of k_spiral_pipe, and of the records built for it
+constexpr int SKEW_IRR_THREADS = 64;  // threads of k_spiral_skew that run the irregular visits (after the 4 * M lane threads)
+constexpr int SKEW_XCH_DEPTH = 2;     // levels in the exchange ring of k_spiral_skew: a value written at level l is read at l + 1
+
 // Device side of the skewed-layout spiral (gg_host.h:SkewTables); null sk -> not used.
-constexpr int SKEW_XCH_ASYNC = 4;    // depth of the exchange ring of the barrier-free spiral variants (the barrier variant needs 2); the
-                                     // synchronisation table is built for exactly this depth (gg_capi.cu -> build_skew_sync)
 struct SkewView {
     float2* sk;             // [n_slots][slots] (G, C) in (side, level, ring) order
     float* sd;              // [n_slots][slots] decayed confidence the visit will store, -1: confidence unchanged
@@ -117,17 +121,6 @@ struct SkewView {
     const int* ph_end;
     const int* ph_cell0;    // cell (x + y * N) of the first regular visit
     int M, phases;
-    // second layout of the same tables with the smallest possible M (small CTAs: several scans per SM); the
-    // launcher swaps it in for batches, the first one serves single scans (lowest latency)
-    const int* thr_ph_begin;
-    const int* thr_ph_end;
-    const int* thr_ph_cell0;
-    int thr_M, thr_phases;
-    // point-to-point synchronisation tables of the two layouts (gg_host.cpp:build_skew_sync), nullptr: CTA barrier per level
-    //   [agent][level][32] progress agent b must have reached before `agent` starts the level
-    const uint16_t* req;
-    const uint16_t* thr_req;
-    int sync_sleep;         // ns a waiting warp sleeps between two looks at the progress counters (0: spin)
     // irregular visits, one fixed-size block per level (irr_chunks x uint4):
     //   words [ (v * 9 + q) * 2 + {0, 1} ] = slot of neighbour q of visit v, producer lane if it was
     //                                        written one level ago (else 0xffffffff)
@@ -172,8 +165,7 @@ struct View {
     int levels;
     // pipelined spiral (k_spiral_pipe): 16-byte records, see gg_host.cpp:build_spiral_records
     const uint4* spiral_recs; // null -> plain k_spiral
-    int spiral_dist;          // prefetch distance the records were built for (1..3)
-    int spiral_threads;       // 512 or 1024 (>= max visits per level)
+    int spiral_threads;       // CTA threads of the spiral launch (gg_host.h:SpiralPlan::threads)
     SkewView skew;            // skew.sk != null -> k_skew + k_spiral_skew + k_unskew replace k_spiral_pipe
 
     __host__ __device__ float* layer(int slot, int l) const { return layers + ((size_t)slot * n_layers + l) * k.N2; }

@@ -333,8 +333,7 @@ constexpr uint32_t RUN_LOW26 = (1u << 26) - 1u;
 // cell, high word: runs of the cell); lane order inside the run is input order.  Runs of one cell never interleave
 // (different warps own disjoint index ranges), so input order inside a cell = runs sorted by run id -- which
 // k_cell_stats restores from the (few) directory entries without any sort pass over the points.
-template <int MIN_BLOCKS>
-__global__ void __launch_bounds__(RASTER_THREADS, MIN_BLOCKS) k_rasterize(View v, const SlotParams* __restrict__ batch) {
+__global__ void __launch_bounds__(RASTER_THREADS, 5) k_rasterize(View v, const SlotParams* __restrict__ batch) {
     const SlotParams& sp = batch[blockIdx.y];
     const int n = sp.n_points;
     const int tile0 = blockIdx.x * RASTER_TILE;
@@ -856,8 +855,7 @@ __device__ __forceinline__ bool detect_patch(const CfgConst& kc, const float (*s
     return false;
 }
 
-template <int MIN_BLOCKS>
-__global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_ldg(View v, const SlotParams* __restrict__ batch) {
+__global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const SlotParams* __restrict__ batch) {
     __shared__ float sP[DT_R][DT_W], sPV[DT_R][DT_W], sPM[DT_R][DT_W], sM[DT_R][DT_W];
     const SlotParams& sp = batch[blockIdx.z];
     const Const& k = v.k;
@@ -1058,8 +1056,7 @@ __device__ __forceinline__ bool detect_decide(const CfgConst& kc, float psum, fl
 // (two stages of raw tiles, one mbarrier each, phase parity flips every second use).
 constexpr int DT_TILES = 4;
 
-template <int MIN_BLOCKS>
-__global__ void __launch_bounds__(DT_X* DT_Y, MIN_BLOCKS) k_detect_tma(View v, const SlotParams* __restrict__ batch, const __grid_constant__ CUtensorMap tmap) {
+__global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const SlotParams* __restrict__ batch, const __grid_constant__ CUtensorMap tmap) {
     __shared__ DetectTile s;
     __shared__ __align__(8) uint64_t s_bar[2];
     const SlotParams& sp = batch[blockIdx.z];
@@ -1221,8 +1218,6 @@ int launch_build_detect_table(const View& v, const CfgConst& c, float4* tab, cud
 // sweep, GroundSegmentation.cpp:413-440) guarantees that visits of one level touch disjoint
 // data, so executing levels in order reproduces the sequential result bit for bit.
 // ------------------------------------------------------------------------------------------
-constexpr int SPIRAL_THREADS = 512;
-
 __global__ void __launch_bounds__(SPIRAL_THREADS) k_spiral(View v, const SlotParams* __restrict__ batch) {
     const SlotParams& sp = batch[blockIdx.x];
     const Const& k = v.k;
@@ -1436,42 +1431,17 @@ __device__ __forceinline__ float2 spiral_visit(const float2* nb, float d) {
 // cycles apart), not by memory.  So both roles keep their per-level code short: lane threads are
 // compiled per side (compile-time neighbour index of the lane's previous cell, running pointers),
 // and the irregular visits are spread over 64 threads (one thread per (visit, neighbour) gathers,
-// one thread per visit computes) instead of unrolled in one thread.
-constexpr int SKEW_IRR_THREADS = 64;
+// one thread per visit computes; SKEW_IRR_THREADS in all) instead of unrolled in one thread.
 constexpr int SKEW_RING = 16;      // levels of irregular-visit blocks kept in shared memory
 constexpr int SKEW_STAGE_LEAD = 10;  // a block is staged this many levels before its visits run
 
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 
-// ---- point-to-point synchronisation (ASYNC variants) ---------------------------------------
-// Instead of one CTA barrier per level every AGENT (a warp of lane threads; the two irregular warps together) publishes
-// the number of levels it has completed in shared memory and, before a level, waits until the agents it depends on have
-// reached the progress the host table asks for (gg_host.cpp:build_skew_sync: exact RAW / WAR / WAW sets of the level's
-// visits).  Neighbouring rings trail each other by three levels, so most requirements leave a level of slack: a warp
-// that is late (a cache miss, a lost issue slot) no longer stalls the whole CTA.  Lane b of a warp watches agent b.
-__device__ __forceinline__ void skew_publish(int* s_prog, int agent, int completed, int lane) {
-    __syncwarp();
-    if (lane == 0) asm volatile("st.release.cta.shared.u32 [%0], %1;" ::"r"(smem_u32(s_prog + agent)), "r"(completed) : "memory");
-}
-__device__ __forceinline__ void skew_wait(const int* s_prog, int need, int lane, int sleep_ns) {
-    const uint32_t addr = smem_u32(s_prog + lane);
-    for (;;) {
-        int p;
-        asm volatile("ld.acquire.cta.shared.u32 %0, [%1];" : "=r"(p) : "r"(addr) : "memory");
-        if (__all_sync(0xffffffffu, p >= need)) break;
-        if (sleep_ns) __nanosleep(sleep_ns);
-    }
-}
-
-template <int SIDE, bool ASYNC>
-__device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams& sp, float2* s_xch, int* s_prog) {
+template <int SIDE>
+__device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams& sp, float2* s_xch) {
     const SkewView& w = v.skew;
-    constexpr int XM = (ASYNC ? SKEW_XCH_ASYNC : 2) - 1;   // exchange ring: entry of level l is [l & XM]
-    const int lane_id = threadIdx.x & 31;
-    const int agent = threadIdx.x >> 5;
-    const uint16_t* __restrict__ req = ASYNC ? w.req + (size_t)agent * w.levels * 32 + lane_id : nullptr;
-    int need_nxt = ASYNC ? (int)__ldg(req) : 0;   // requirement of the next level this warp executes, loaded one level ahead
+    constexpr int XM = SKEW_XCH_DEPTH - 1;   // exchange ring: entry of level l is [l & XM]
     constexpr int PQ = SIDE == 0 ? 1 : (SIDE == 1 ? 3 : (SIDE == 2 ? 7 : 5));  // neighbour index of the lane's previous cell
     constexpr int PF_FAR = 8, PF_NEAR = 2;
     const int L = w.levels, KP = w.KP, lanes = w.lanes, M = w.M;
@@ -1532,11 +1502,6 @@ __device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams
 #define GG_LANE_LEVEL(l_, CUR, CURD, NXT, NXTD)                                                      \
     {                                                                                               \
         const int l__ = (l_);                                                                       \
-        if (ASYNC) {                                                                                \
-            const int need__ = need_nxt;                                                            \
-            if (l__ + 1 < L) need_nxt = (int)__ldg(req + (size_t)(l__ + 1) * 32);                   \
-            skew_wait(s_prog, need__, lane_id, w.sync_sleep);                                                     \
-        }                                                                                           \
         if (l__ + PF_FAR >= lb && l__ + PF_FAR < le) {                                              \
             prefetch_l2(SK + (base0 + (l__ + PF_FAR) * KP + off_new));                              \
             prefetch_l2(SD + (base0 + (l__ + PF_FAR) * KP));                                        \
@@ -1558,10 +1523,7 @@ __device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams
             Gn[cell0 + l__ * cstep] = r__.x;                                                        \
             if (CURD >= 0.0f) Cn[cell0 + l__ * cstep] = r__.y;                                      \
         }                                                                                           \
-        if (ASYNC)                                                                                  \
-            skew_publish(s_prog, agent, l__ + 1, lane_id);                                          \
-        else                                                                                        \
-            __syncthreads();                                                                        \
+        __syncthreads();                                                                            \
     }
     for (int l = 0; l < L; l += 2) {
         // done with this ring: move on to ring + M (it starts well after this one ended)
@@ -1576,13 +1538,8 @@ __device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams
         // a warp (32 consecutive rings of one side) has work only in a window of levels; outside of it
         // the per-level cost must be the barrier alone (the level time is set by instruction issue)
         if (l < w_first || l >= w_last) {
-            if (ASYNC) {   // nothing to do and nothing to wait for: the warp has "completed" both levels
-                skew_publish(s_prog, agent, min(l + 2, L), lane_id);
-                if (l + 2 < L) need_nxt = (int)__ldg(req + (size_t)(l + 2) * 32);
-            } else {
-                __syncthreads();
-                if (l + 1 < L) __syncthreads();
-            }
+            __syncthreads();
+            if (l + 1 < L) __syncthreads();
             continue;
         }
         GG_LANE_LEVEL(l, A, dA, B, dB)
@@ -1593,15 +1550,10 @@ __device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams
 
 __device__ __forceinline__ void skew_named_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(SKEW_IRR_THREADS) : "memory"); }
 
-template <bool ASYNC>
-__device__ __forceinline__ void skew_irregular_thread(const View& v, const SlotParams& sp, float2* s_xch, uint4* s_ring, float2* s_nb, float* s_dd, int* s_prog) {
+__device__ __forceinline__ void skew_irregular_thread(const View& v, const SlotParams& sp, float2* s_xch, uint4* s_ring, float2* s_nb, float* s_dd) {
     const SkewView& w = v.skew;
     const int ti = threadIdx.x - 4 * w.M;  // 0 .. 63
-    constexpr int XM = (ASYNC ? SKEW_XCH_ASYNC : 2) - 1;
-    const int lane_id = threadIdx.x & 31;
-    const int agent = 4 * w.M / 32;        // both warps form one agent
-    const uint16_t* __restrict__ req = ASYNC ? w.req + (size_t)agent * w.levels * 32 + lane_id : nullptr;
-    int need_nxt = ASYNC ? (int)__ldg(req) : 0;
+    constexpr int XM = SKEW_XCH_DEPTH - 1;
     const int L = w.levels, lanes = w.lanes;
     const int chunks = w.irr_chunks, irr_max = w.irr_max;
     float2* __restrict__ SK = w.sk + (size_t)sp.slot * w.slots;
@@ -1640,11 +1592,6 @@ __device__ __forceinline__ void skew_irregular_thread(const View& v, const SlotP
         }
     }
     for (int l = 0; l < L; ++l) {
-        if (ASYNC) {
-            const int need = need_nxt;
-            if (l + 1 < L) need_nxt = (int)__ldg(req + (size_t)(l + 1) * 32);
-            skew_wait(s_prog, need, lane_id, w.sync_sleep);
-        }
         // (1) block of level l + LEAD (loaded during the previous level) -> ring; start loading the next one
         if (stager) {
             s_ring[((l + SKEW_STAGE_LEAD) % SKEW_RING) * chunks + ti] = stage;
@@ -1695,44 +1642,33 @@ __device__ __forceinline__ void skew_irregular_thread(const View& v, const SlotP
                 if (s_dd[ti] >= 0.0f) Cn[hd[3]] = r.y;
             }
         }
-        if (ASYNC) {
-            skew_named_barrier();   // both warps are done with the level (and with s_nb / s_dd)
-            if (ti == 0) asm volatile("st.release.cta.shared.u32 [%0], %1;" ::"r"(smem_u32(s_prog + agent)), "r"(l + 1) : "memory");
-        } else {
-            __syncthreads();
-        }
+        __syncthreads();
     }
 }
 
-template <int MAXT, int MIN_CTAS = 1, bool ASYNC = false>
+template <int MAXT, int MIN_CTAS = 1>
 __global__ void __launch_bounds__(MAXT, MIN_CTAS) k_spiral_skew(View v, const SlotParams* __restrict__ batch) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     const SkewView& w = v.skew;
-    // [ring: SKEW_RING levels x irr_chunks uint4][xch: depth x lanes float2][nb: irr_max*9 float2][dd: irr_max float][progress: 32 int]
+    // [ring: SKEW_RING levels x irr_chunks uint4][xch: SKEW_XCH_DEPTH x lanes float2][nb: irr_max*9 float2][dd: irr_max float]
     uint4* s_ring = reinterpret_cast<uint4*>(s_raw);
     float2* s_xch = reinterpret_cast<float2*>(s_ring + SKEW_RING * w.irr_chunks);
-    float2* s_nb = s_xch + (ASYNC ? SKEW_XCH_ASYNC : 2) * w.lanes;
+    float2* s_nb = s_xch + SKEW_XCH_DEPTH * w.lanes;
     float* s_dd = reinterpret_cast<float*>(s_nb + w.irr_max * 9);
-    int* s_prog = reinterpret_cast<int*>(s_dd + w.irr_max);
     const SlotParams& sp = batch[blockIdx.x];
     const int tid = threadIdx.x;
-    if (ASYNC) {
-        // agents that do not exist count as finished (their table entries are 0 anyway)
-        if (tid < 32) s_prog[tid] = tid <= 4 * w.M / 32 ? 0 : 0x7fffffff;
-        __syncthreads();
-    }
     if (tid < 4 * w.M) {
         const int side = tid / w.M;  // warp-uniform: M is a multiple of 32
         if (side == 0)
-            skew_lane_thread<0, ASYNC>(v, sp, s_xch, s_prog);
+            skew_lane_thread<0>(v, sp, s_xch);
         else if (side == 1)
-            skew_lane_thread<1, ASYNC>(v, sp, s_xch, s_prog);
+            skew_lane_thread<1>(v, sp, s_xch);
         else if (side == 2)
-            skew_lane_thread<2, ASYNC>(v, sp, s_xch, s_prog);
+            skew_lane_thread<2>(v, sp, s_xch);
         else
-            skew_lane_thread<3, ASYNC>(v, sp, s_xch, s_prog);
+            skew_lane_thread<3>(v, sp, s_xch);
     } else {
-        skew_irregular_thread<ASYNC>(v, sp, s_xch, s_ring, s_nb, s_dd, s_prog);
+        skew_irregular_thread(v, sp, s_xch, s_ring, s_nb, s_dd);
     }
 }
 
@@ -2218,16 +2154,20 @@ int launch_roll(const View& v, const SlotParams* batch, int count, cudaStream_t 
     return 2;
 }
 
+// patch detection: the TMA-staged tile when the arena has a descriptor (it needs a 16-byte row pitch: N % 4 == 0), else plain loads
+static void enqueue_detect(const View& v, const SlotParams* batch, int count, cudaStream_t st, const CUtensorMap* layer_map) {
+    if (layer_map)
+        k_detect_tma<<<dim3(cdiv(v.k.N, DT_X), cdiv(cdiv(v.k.N, DT_Y), DT_TILES), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch, *layer_map);
+    else
+        k_detect_ldg<<<dim3(cdiv(v.k.N, DT_X), cdiv(v.k.N, DT_Y), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch);
+}
+
 int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int max_points, int stop_after, cudaStream_t st,
                          Profiler* prof, const CUtensorMap* layer_map) {
     int launches = 0;
     const int nb = max(1, cdiv(max_points, RASTER_TILE));
 
-    static const int raster_occ = getenv("GG_RASTER_OCC") ? atoi(getenv("GG_RASTER_OCC")) : 5;
-    if (raster_occ >= 5)
-        GG_LAUNCH(K_RASTERIZE, k_rasterize<5><<<dim3(nb, count), RASTER_THREADS, 0, st>>>(v, batch));
-    else
-        GG_LAUNCH(K_RASTERIZE, k_rasterize<4><<<dim3(nb, count), RASTER_THREADS, 0, st>>>(v, batch));
+    GG_LAUNCH(K_RASTERIZE, k_rasterize<<<dim3(nb, count), RASTER_THREADS, 0, st>>>(v, batch));
     GG_LAUNCH(K_CELL_TILES, k_cell_tiles<<<dim3(v.cell_tiles, count), CT_THREADS, 0, st>>>(v, batch));
     GG_LAUNCH(K_CELL_PLACE, k_cell_place<<<dim3(v.cell_tiles, count), CT_THREADS, 0, st>>>(v, batch));
     GG_LAUNCH(K_SCATTER, k_scatter<<<dim3(max(1, cdiv(max_points, 256 * SCATTER_ILP)), count), 256, 0, st>>>(v, batch));
@@ -2240,50 +2180,21 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
     ++launches;
     if (stop_after == 1) return launches;
 
-    static const int detect_occ = getenv("GG_DETECT_OCC") ? atoi(getenv("GG_DETECT_OCC")) : 5;
-    const dim3 dgrid(cdiv(v.k.N, DT_X), cdiv(v.k.N, DT_Y), count);
-    const dim3 tgrid(cdiv(v.k.N, DT_X), cdiv(cdiv(v.k.N, DT_Y), DT_TILES), count);
-    if (layer_map) {   // TMA-staged tile (needs a 16-byte row pitch: N % 4 == 0)
-        if (detect_occ >= 5)
-            GG_LAUNCH(K_DETECT, k_detect_tma<5><<<tgrid, dim3(DT_X, DT_Y), 0, st>>>(v, batch, *layer_map));
-        else
-            GG_LAUNCH(K_DETECT, k_detect_tma<4><<<tgrid, dim3(DT_X, DT_Y), 0, st>>>(v, batch, *layer_map));
-    } else if (detect_occ >= 5)
-        GG_LAUNCH(K_DETECT, k_detect_ldg<5><<<dgrid, dim3(DT_X, DT_Y), 0, st>>>(v, batch));
-    else
-        GG_LAUNCH(K_DETECT, k_detect_ldg<4><<<dgrid, dim3(DT_X, DT_Y), 0, st>>>(v, batch));
+    GG_LAUNCH(K_DETECT, enqueue_detect(v, batch, count, st, layer_map));
     ++launches;
     if (stop_after == 2) return launches;
 
+    const int threads = v.spiral_threads;
     if (v.skew.sk) {
-        // batches run the small-CTA layout (two or three scans share an SM and leave room for the other streams'
-        // kernels); a few scans alone get one thread per lane.  GG_SPIRAL_SHARE_MIN: smallest batch that shares.
-        static const int share_min = getenv("GG_SPIRAL_SHARE_MIN") ? atoi(getenv("GG_SPIRAL_SHARE_MIN")) : 9;
-        View vs = v;
-        if (count >= share_min) {
-            vs.skew.M = v.skew.thr_M;
-            vs.skew.phases = v.skew.thr_phases;
-            vs.skew.ph_begin = v.skew.thr_ph_begin;
-            vs.skew.ph_end = v.skew.thr_ph_end;
-            vs.skew.ph_cell0 = v.skew.thr_ph_cell0;
-            vs.skew.req = v.skew.thr_req;
-        }
-        const bool async = vs.skew.req != nullptr;   // point-to-point synchronisation table of this thread layout
-        const int threads = 4 * vs.skew.M + SKEW_IRR_THREADS;
-        const size_t shm = (size_t)SKEW_RING * v.skew.irr_chunks * sizeof(uint4) + (size_t)(async ? SKEW_XCH_ASYNC : 2) * v.skew.lanes * sizeof(float2) +
-                           (size_t)v.skew.irr_max * 9 * sizeof(float2) + (size_t)v.skew.irr_max * sizeof(float) + 32 * sizeof(int) + 16;
+        const size_t shm = (size_t)SKEW_RING * v.skew.irr_chunks * sizeof(uint4) + (size_t)SKEW_XCH_DEPTH * v.skew.lanes * sizeof(float2) +
+                           (size_t)v.skew.irr_max * 9 * sizeof(float2) + (size_t)v.skew.irr_max * sizeof(float) + 16;
 #define GG_SKEW_LAUNCH(T, C)                                                                                                     \
     {                                                                                                                            \
-        if (shm > 48 * 1024) {   /* large maps: opt in to more dynamic shared memory */                                         \
-            cudaFuncSetAttribute(k_spiral_skew<T, C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);             \
-            cudaFuncSetAttribute(k_spiral_skew<T, C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);              \
-        }                                                                                                                        \
-        if (async)                                                                                                               \
-            GG_LAUNCH(K_SPIRAL, (k_spiral_skew<T, C, true><<<count, threads, shm, st>>>(vs, batch)));                            \
-        else                                                                                                                     \
-            GG_LAUNCH(K_SPIRAL, (k_spiral_skew<T, C, false><<<count, threads, shm, st>>>(vs, batch)));                           \
+        if (shm > 48 * 1024)   /* large maps: opt in to more dynamic shared memory */                                           \
+            cudaFuncSetAttribute(k_spiral_skew<T, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);                    \
+        GG_LAUNCH(K_SPIRAL, (k_spiral_skew<T, C><<<count, threads, shm, st>>>(v, batch)));                                       \
     }
-        if (threads <= 320)       // time-shared lane threads (GG_SPIRAL_M): several scans share an SM
+        if (threads <= 320)       // small maps: several scans share an SM
             GG_SKEW_LAUNCH(320, 3)
         else if (threads <= 448)
             GG_SKEW_LAUNCH(448, 2)
@@ -2293,19 +2204,17 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
             GG_SKEW_LAUNCH(1024, 1)
 #undef GG_SKEW_LAUNCH
     } else if (v.spiral_recs) {
-        const size_t shm = (size_t)((v.levels + 4) & ~3) * sizeof(int) + (size_t)(v.spiral_dist + 1) * v.spiral_threads * sizeof(float2);
-#define GG_SPIRAL_CASE(T, D)                                                                      \
-    if (v.spiral_threads == T && v.spiral_dist == D) {                                            \
-        if (shm > 48 * 1024) cudaFuncSetAttribute(k_spiral_pipe<T, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm); \
-        GG_LAUNCH(K_SPIRAL, k_spiral_pipe<T, D><<<count, T, shm, st>>>(v, batch));                \
+        const size_t shm = (size_t)((v.levels + 4) & ~3) * sizeof(int) + (size_t)(SPIRAL_PIPE_DIST + 1) * threads * sizeof(float2);
+#define GG_PIPE_LAUNCH(T)                                                                                                        \
+    {                                                                                                                            \
+        if (shm > 48 * 1024) cudaFuncSetAttribute(k_spiral_pipe<T, SPIRAL_PIPE_DIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm); \
+        GG_LAUNCH(K_SPIRAL, (k_spiral_pipe<T, SPIRAL_PIPE_DIST><<<count, T, shm, st>>>(v, batch)));                             \
     }
-        GG_SPIRAL_CASE(512, 1)
-        GG_SPIRAL_CASE(512, 2)
-        GG_SPIRAL_CASE(512, 3)
-        GG_SPIRAL_CASE(1024, 1)
-        GG_SPIRAL_CASE(1024, 2)
-        GG_SPIRAL_CASE(1024, 3)
-#undef GG_SPIRAL_CASE
+        if (threads == 512)
+            GG_PIPE_LAUNCH(512)
+        else
+            GG_PIPE_LAUNCH(1024)
+#undef GG_PIPE_LAUNCH
     } else {
         GG_LAUNCH(K_SPIRAL, k_spiral<<<count, SPIRAL_THREADS, 0, st>>>(v, batch));
     }
@@ -2387,11 +2296,7 @@ __global__ void k_detect_cell(View v, const CfgConst kc, int slot, int i, int j)
 }
 
 int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map) {
-    const dim3 dgrid(cdiv(v.k.N, DT_X), cdiv(v.k.N, DT_Y), count);
-    if (layer_map)
-        GG_LAUNCH(K_DETECT, k_detect_tma<4><<<dim3(cdiv(v.k.N, DT_X), cdiv(cdiv(v.k.N, DT_Y), DT_TILES), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch, *layer_map));
-    else
-        GG_LAUNCH(K_DETECT, k_detect_ldg<4><<<dgrid, dim3(DT_X, DT_Y), 0, st>>>(v, batch));
+    GG_LAUNCH(K_DETECT, enqueue_detect(v, batch, count, st, layer_map));
     return 1;
 }
 

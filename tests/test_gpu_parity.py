@@ -394,9 +394,9 @@ def test_batched_slots_match_single_and_are_deterministic():
 
 
 @pytest.mark.parametrize("dim,res", [(33.0, 0.33), (99.0, 0.33), (120.0, 0.33)])
-def test_batch_of_ten_uses_the_shared_sm_spiral_layout(dim, res):
-    """Launches of >= 9 scans run the spiral with time-shared lane threads (small CTAs, several scans per SM);
-    fewer scans get one thread per lane.  Both must reproduce the sequential sweep bit for bit."""
+def test_batch_of_ten_twice_matches_the_oracle(dim, res):
+    """Ten slots in one batched call, run twice: every slot's labels after each call, and its ground / groundpatch
+    after the second, equal the oracle's."""
     import torch
 
     B = 10
@@ -423,34 +423,27 @@ def test_batch_of_ten_uses_the_shared_sm_spiral_layout(dim, res):
     g.close()
 
 
-@pytest.mark.parametrize("dim,res", [(33.0, 0.33), (99.0, 0.33), (81.2, 0.4)])
-def test_spiral_point_to_point_sync_variant(monkeypatch, dim, res):
-    """GG_SPIRAL_ASYNC=1: k_spiral_skew without the CTA barrier per level (progress counters per warp, requirement table
-    from gg_host.cpp:build_skew_sync).  Both thread layouts (one scan alone, a batch of ten) against the oracle."""
-    import torch
-
-    monkeypatch.setenv("GG_SPIRAL_ASYNC", "1")
-    B = 10
-    g = capi.GroundGridB200(dim, res, n_slots=B, max_points=131072, full_layers=False)
-    scans = [synth.scan_64(synth.make_scene(seed=810 + b), ego_xy=(0.05 * b, 0.0), seed=810 + b) for b in range(B)]
-    hp = [torch.from_numpy(np.ascontiguousarray(p).view(np.uint8).copy()).pin_memory() for p, _ in scans]
-    hl = [torch.zeros(len(p), dtype=torch.uint8).pin_memory() for p, _ in scans]
-    for b in range(B):
-        g.init_map(0.05 * b, 0.0, 0.0, slot=b)
-    first = g.filter_cloud(scans[0][0], scans[0][1], 0.0, slot=0)      # one scan alone: one thread per lane
-    descs = g.make_descs(list(range(B)), [len(p) for p, _ in scans], [o for _, o in scans], [0.0] * B)
-    g.filter_cloud_batch_ptrs(descs, [t.data_ptr() for t in hp], [t.data_ptr() for t in hl])   # batch: time-shared lane threads
-    for b in range(B):
-        o = Oracle(dim, res)
-        o.init_map(0.05 * b, 0.0, 0.0)
-        if b == 0:   # slot 0 saw its cloud twice: alone, then in the batch
-            want, _, _ = o.filter_cloud(scans[0][0], scans[0][1], 0.0, threads=1)
-            assert np.array_equal(first, want)
-        want, _, _ = o.filter_cloud(scans[b][0], scans[b][1], 0.0, threads=1)
-        assert np.array_equal(hl[b].numpy(), want), f"slot {b}"
-        for name in ("ground", "groundpatch"):
-            r = diff_report(name, g.layer(name, slot=b), o.layer(name))
-            assert r is None, f"slot {b}: {r}"
+@pytest.mark.parametrize("dim,res,n", [(3.3, 0.33, 10), (120.0, 0.1, 1200), (160.0, 0.1, 1600)])
+def test_pipelined_and_plain_spiral_paths(dim, res, n):
+    """The map sizes whose spiral does not run the skewed layout: N = 10 (k_spiral_pipe<512>, plain-load patch
+    detection), N = 1200 (k_spiral_pipe<1024>, TMA patch detection) and N = 1600 (plain k_spiral: levels of more than
+    1024 visits).  A 64-beam scan, a roll, a second scan; labels and the spiral's layers against the oracle."""
+    g, o = make_pair(dim, res)
+    assert g.n == o.n == n
+    scene = synth.make_scene(seed=n)
+    for k in range(2):
+        ex, ey = 0.7 * k, -0.4 * k
+        pts, org = synth.scan_64(scene, ego_xy=(ex, ey), seed=n + k)
+        if k == 0:
+            g.init_map(ex, ey, 0.0)
+            o.init_map(ex, ey, 0.0)
+        else:
+            T = synth.base_from_map(ex, ey, 0.0, base_z=0.0, pitch=0.005)
+            assert int(g.update_pose(ex, ey, T)) == o.update(ex, ey, T) == 1
+        labels = g.filter_cloud(pts, org, 0.0)
+        want, _, _ = o.filter_cloud(pts, org, 0.0, threads=1)
+        assert np.array_equal(labels, want), f"N {n} scan {k}: {(labels != want).sum()} labels differ"
+        assert_layers_equal(g, o, ("ground", "groundpatch"), f"N {n} scan {k}")
     g.close()
 
 

@@ -397,162 +397,23 @@ def test_skewed_spiral_tables_emulation(dim, res):
     assert np.array_equal(o.layer("groundpatch"), Cf.reshape(n, n, order="F"))
 
 
-def host_spiral_skew_sync(n, M, depth, levels):
+# Parent-build values: the choice gg_create made before it moved into plan_spiral (skew tables, records, and the
+# smallest time-shared M, replayed from the gg_host_spiral_skew / gg_host_spiral_records exports).
+@pytest.mark.parametrize("n,kind,threads,M,phases", [(10, "pipe", 512, 0, 0), (16, "skew", 192, 32, 1), (100, "skew", 320, 64, 1),
+                                                    (300, "skew", 704, 160, 1), (364, "skew", 832, 192, 1), (600, "skew", 576, 128, 3),
+                                                    (1200, "pipe", 1024, 0, 0), (1600, "plain", 512, 0, 0)])
+def test_spiral_plan_picks_the_path_of_each_map_size(n, kind, threads, M, phases):
+    """gg_host_spiral_plan: the skewed layout while one CTA holds it (one lane thread per lane, time-shared rings from
+    N ~ 500), the pipelined kernel where the skew tables do not fit (small maps, N = 1200), the plain wavefront where a
+    level has more than 1024 visits."""
     import ctypes as C
 
-    L = capi.load()
-    fn = L.gg_host_spiral_skew_sync
+    fn = capi.load().gg_host_spiral_plan
     fn.restype = C.c_int
-    fn.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
-    na = C.c_int(0)
-    if not fn(n, M, depth, None, 0, C.byref(na)):
-        return None, 0
-    req = np.zeros(na.value * levels * 32, np.uint16)
-    assert fn(n, M, depth, req.ctypes.data, req.size, C.byref(na)) == 1
-    return req.reshape(na.value, levels, 32), na.value
-
-
-@pytest.mark.parametrize("dim,res,M,policy", [(13.2, 0.33, 32, "random"), (33.0, 0.33, 32, "ahead"), (33.0, 0.33, 64, "random"),
-                                              (99.0, 0.33, 64, "ahead"), (99.0, 0.33, 64, "random"), (99.0, 0.33, 160, "ahead"),
-                                              (30.5, 0.5, 32, "random"), (120.0, 0.33, 64, "behind"), (81.2, 0.4, 96, "random")])
-def test_skewed_spiral_point_to_point_sync_emulation(dim, res, M, policy):
-    """The barrier-free variant of k_spiral_skew on the CPU: every agent (a warp of lane threads / the irregular warps)
-    runs its levels on its own, held back only by the progress requirements of gg_host_spiral_skew_sync; memory is
-    touched exactly when the kernel touches it (slots of level l + 1 loaded during level l, previous-level values from
-    the exchange ring of depth 4, stores at the end of the level).  Agents are scheduled adversarially (the one that is
-    furthest ahead / behind first, or at random).  Must equal the oracle's sequential sweep bit for bit."""
-    DEPTH = 4
-    o = Oracle(dim, res)
-    n = o.n
-    t = host_spiral_skew(n)
-    assert t is not None
-    KP, rows, row0, lanes, L = t["KP"], t["rows"], t["row0"], t["lanes"], t["levels"]
-    M = min(M, KP)
-    req, n_agents = host_spiral_skew_sync(n, M, DEPTH, L)
-    assert req is not None and n_agents == 4 * M // 32 + 1
-    IRR = n_agents - 1
-    prev_q = np.array([1, 3, 7, 5])
-    rng = np.random.default_rng(23)
-    o.init_map(0.0, 0.0, 0.0)
-    G = rng.uniform(-1, 1, (n, n)).astype(np.float32)
-    C = (rng.uniform(0, 1, (n, n)) ** 4).astype(np.float32)
-    o.set_layer("ground", G)
-    o.set_layer("groundpatch", C)
-    o.spiral(0.3)
-    c = n // 2 - 1
-    Gf, Cf = G.reshape(-1, order="F").copy(), C.reshape(-1, order="F").copy()
-    Gf[c + c * n] = f32(0.3)
-    Cf[c + c * n] = 1.0
-    o64 = Cf.astype(np.float64)
-    D1 = np.maximum(o64 - o64 / 5.0, 0.001).astype(np.float32)
-    d64 = D1.astype(np.float64)
-    D2 = np.maximum(d64 - d64 / 5.0, 0.001).astype(np.float32)
-    ii, jj = np.meshgrid(np.arange(n), np.arange(n), indexing="ij")
-    fx = (ii.astype(np.float32) - f32(c)).astype(np.float64)
-    fy = (jj.astype(np.float32) - f32(c)).astype(np.float64)
-    far = ((fx * fx + fy * fy) * np.float64(f32(res)) ** 2 > 12.0).reshape(-1, order="F")
-    nslots = 4 * rows * KP
-    SKg, SKc, SD = np.zeros(nslots, np.float32), np.zeros(nslots, np.float32), np.full(nslots, -1.0, np.float32)
-    home = t["home"]
-    for h in range(4):
-        m = home[:, h] >= 0
-        SKg[home[m, h]] = Gf[m]
-        SKc[home[m, h]] = Cf[m]
-        if h < 2:
-            SD[home[m, h]] = np.where(far[m], (D1 if h == 0 else D2)[m], f32(-1.0))
-    lane = np.arange(lanes)
-    side, kcol = lane // KP, lane % KP
-    agent_of_lane = (side * M + kcol % M) // 32
-    xg, xc = np.zeros((DEPTH, lanes), np.float32), np.zeros((DEPTH, lanes), np.float32)
-    irr, ils = t["irr"], t["irr_level_start"]
-    lb, le = t["lane_begin"], t["lane_end"]
-    lanes_of = [lane[(agent_of_lane == a) & (lb < le)] for a in range(IRR)]
-
-    def tree(v):
-        return ((v[:, 0] + v[:, 1]) + (v[:, 2] + v[:, 3])) + ((v[:, 4] + v[:, 5]) + (v[:, 6] + (v[:, 7] + v[:, 8])))
-
-    def visit(gg, cc, dd):
-        s = tree(cc) + FLT_MIN
-        avg = tree(cc * gg) / s
-        occ = cc[:, 4]
-        newg = (f32(1.0) - occ) * avg + occ * gg[:, 4]
-        return newg.astype(np.float32), np.where(dd >= 0, dd, occ).astype(np.float32)
-
-    def fetch(a, lvl):   # the loads agent a issues for its visits of level lvl
-        if lvl >= L:
-            return None
-        if a == IRR:
-            r = irr[ils[lvl]:ils[lvl + 1]]
-            if not len(r):
-                return None
-            iidx = r[:, 1:10].astype(np.int64)
-            return (r, SKg[iidx].copy(), SKc[iidx].copy(), SD[r[:, 0].astype(np.int64)].copy())
-        la = lanes_of[a]
-        rl = la[(lb[la] <= lvl) & (lvl < le[la])]
-        if not len(rl):
-            return None
-        own = (side[rl] * rows + lvl + row0) * KP + kcol[rl]
-        idx = own[:, None] + t["pattern"][side[rl]]
-        return (rl, own, SKg[idx].copy(), SKc[idx].copy(), SD[own].copy())
-
-    pending = [fetch(a, 0) for a in range(n_agents)]   # prologue of the kernel
-
-    def run(a, lvl):
-        cur = pending[a]
-        pending[a] = fetch(a, lvl + 1)        # issued before this level's stores
-        if cur is None:
-            return
-        pb = (lvl - 1) % DEPTH
-        if a == IRR:
-            r, igg, icc, idd = cur
-            for w in (10, 11):
-                for sh in (0, 16):
-                    e = (r[:, w] >> sh) & 0xFFFF
-                    m = e != 0xFFFF
-                    q = np.where(m, e >> 12, 0).astype(np.int64)
-                    pl = (e & 4095).astype(np.int64)
-                    igg[m, q[m]] = xg[pb, pl[m]]
-                    icc[m, q[m]] = xc[pb, pl[m]]
-            ing, inc = visit(igg, icc, idd)
-            io = r[:, 0].astype(np.int64)
-            SKg[io], SKc[io] = ing, inc
-            mir = r[:, 12].astype(np.int32)
-            mm = mir >= 0
-            SKg[mir[mm]], SKc[mir[mm]] = ing[mm], inc[mm]
-            il = r[:, 13].astype(np.int64)
-            xg[lvl % DEPTH, il], xc[lvl % DEPTH, il] = ing, inc
-        else:
-            rl, own, gg, cc, dd = cur
-            pq = prev_q[side[rl]]
-            gg[np.arange(len(rl)), pq] = xg[pb, rl]
-            cc[np.arange(len(rl)), pq] = xc[pb, rl]
-            ng, nc = visit(gg, cc, dd)
-            SKg[own], SKc[own] = ng, nc
-            xg[lvl % DEPTH, rl], xc[lvl % DEPTH, rl] = ng, nc
-
-    progress = np.zeros(32, np.int64)
-    progress[n_agents:] = L
-    sched = np.random.default_rng(5)
-    max_skew = 0
-    while np.any(progress[:n_agents] < L):
-        runnable = [a for a in range(n_agents) if progress[a] < L and np.all(progress >= req[a, progress[a]])]
-        assert runnable, "deadlock"
-        if policy == "random":
-            a = runnable[sched.integers(len(runnable))]
-        elif policy == "ahead":
-            a = max(runnable, key=lambda b: progress[b])
-        else:
-            a = min(runnable, key=lambda b: progress[b])
-        run(a, int(progress[a]))
-        progress[a] += 1
-        act = progress[:n_agents]
-        max_skew = max(max_skew, int(act.max() - act.min()))
-    m = home[:, 0] >= 0
-    Gf[m], Cf[m] = SKg[home[m, 0]], SKc[home[m, 0]]
-    assert np.array_equal(o.layer("ground"), Gf.reshape(n, n, order="F"))
-    assert np.array_equal(o.layer("groundpatch"), Cf.reshape(n, n, order="F"))
-    if policy == "ahead" and n >= 100:
-        assert max_skew >= 2   # the point of the exercise: agents really do run apart
+    fn.argtypes = [C.c_int, C.c_float, C.c_void_p]
+    out = np.zeros(4, np.int32)
+    assert fn(n, 0.33, out.ctypes.data) == 0
+    assert (["plain", "pipe", "skew"][out[0]], int(out[1]), int(out[2]), int(out[3])) == (kind, threads, M, phases)
 
 
 @pytest.mark.parametrize("threads,n_jobs,n_points,ring,rounds,lag", [(4, 40, 20000, 8, 4, 3), (3, 17, 50001, 4, 3, 1),
