@@ -70,6 +70,71 @@ CLOUD_MSG_DTYPE = np.dtype({"names": ["data", "point_step", "field_offsets", "T_
                             "formats": [np.uint64, np.int32, (np.int32, 5), np.uint64], "offsets": [0, 8, 12, 32],
                             "itemsize": C.sizeof(CloudMsg)})
 
+MAX_CLOUD_PARTS = 16   # GG_MAX_CLOUD_PARTS
+
+
+class CloudPart(C.Structure):
+    """gg_cloud_part: one sensor's payload of a merged scan and its point count."""
+
+    _fields_ = [("msg", CloudMsg), ("n_points", C.c_size_t)]
+
+
+# numpy image of an array of gg_cloud_part (CloudPart)
+CLOUD_PART_DTYPE = np.dtype({"names": ["data", "point_step", "field_offsets", "T_map_from_frame", "n_points"],
+                             "formats": [np.uint64, np.int32, (np.int32, 5), np.uint64, np.uint64],
+                             "offsets": [0, 8, 12, 32, C.sizeof(CloudMsg)], "itemsize": C.sizeof(CloudPart)})
+
+
+def _per_part(value, n_parts, item_ndim, name):
+    """`value` for every part, or nested [scan][part] -> a flat list over the parts.  An item has item_ndim dimensions
+    (None counts as an item: a part without T)."""
+    def is_item(v):
+        if v is None:
+            return True
+        try:
+            a = np.asarray(v)          # nested lists holding None or ragged ones are no item
+        except ValueError:
+            return False
+        return a.dtype != object and a.ndim == item_ndim
+
+    if is_item(value):
+        return [value] * int(sum(n_parts))
+    if len(value) != len(n_parts) or any(len(v) != m for v, m in zip(value, n_parts)):
+        raise ValueError(f"{name} must be one value or nested [scan][part] like the payloads")
+    flat = [v for scan in value for v in scan]
+    if not all(is_item(v) for v in flat):
+        raise ValueError(f"{name} must be one value or nested [scan][part] like the payloads")
+    return flat
+
+
+def cloud_parts(nbytes, data_ptrs, point_step, field_offsets, T):
+    """Flattens the nested arguments of merged scans into what gg_run_merged_cloud_msgs_to_device / gg_upload_cloud_msgs
+    take.  nbytes / data_ptrs: nested [scan][part] payload sizes in bytes and addresses; point_step, field_offsets
+    (5-tuple) and T (None or a 3x4 of lookupTransform("map", frame_id)) one value for every part or nested [scan][part].
+    Returns (n_parts int32 [count], parts CLOUD_PART_DTYPE [total], T array): the T pointers of `parts` point into the T
+    array, which must stay alive until the call."""
+    n_parts = np.array([len(s) for s in nbytes], np.int32)
+    if len(data_ptrs) != len(n_parts) or any(len(d) != m for d, m in zip(data_ptrs, n_parts)):
+        raise ValueError("data_ptrs must be nested [scan][part] like nbytes")
+    total = int(n_parts.sum())
+    steps = _per_part(point_step, n_parts, 0, "point_step")
+    offs = _per_part(field_offsets, n_parts, 1, "field_offsets")
+    Ts = _per_part(T, n_parts, 2, "T")
+    parts = np.zeros(max(1, total), CLOUD_PART_DTYPE)
+    Tarr = np.zeros((max(1, total), 12), np.float64)
+    for p, (nb, ptr, step, off, t) in enumerate(zip((b for s in nbytes for b in s), (d for s in data_ptrs for d in s), steps, offs, Ts)):
+        step = int(step)
+        if step <= 0 or int(nb) % step:
+            raise ValueError(f"part {p}: {nb} bytes is not a multiple of point_step {step}")
+        parts["data"][p] = int(ptr)
+        parts["point_step"][p] = step
+        parts["field_offsets"][p] = np.asarray(off, np.int32).reshape(5)
+        parts["n_points"][p] = int(nb) // step
+        if t is not None:
+            Tarr[p] = np.asarray(t, np.float64).reshape(12)
+            parts["T_map_from_frame"][p] = Tarr.ctypes.data + 96 * p
+    return n_parts, parts[:total], Tarr
+
 # numpy image of an array of gg_scan_desc (ScanDesc)
 SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "n_points", "origin", "base_z"], "formats": [np.int32, np.uint64, (np.float32, 3), np.float64],
                             "offsets": [0, 8, 16, 32], "itemsize": C.sizeof(ScanDesc)})
@@ -147,6 +212,8 @@ def load(build_if_missing=True):
         "gg_run_scans_to_device": (i, [vp, i, vp, vp, vp, C.c_uint, vp, vp]),
         "gg_upload_cloud_msg": (i, [vp, i, vp, sz, i, vp, vp]),
         "gg_run_cloud_msgs_to_device": (i, [vp, i, vp, vp, vp, C.c_uint, vp, vp]),
+        "gg_run_merged_cloud_msgs_to_device": (i, [vp, i, vp, vp, vp, vp, C.c_uint, vp, vp]),
+        "gg_upload_cloud_msgs": (i, [vp, i, i, vp]),
         "gg_terrain_image": (i, [vp, i, vp]),
         "gg_layer_image_u8": (i, [vp, i, C.c_char_p, vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
         "gg_get_point_classes": (i, [vp, i, vp, sz]),
@@ -632,7 +699,49 @@ class GroundGridB200:
                                            out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
         return out
 
-    # shared by run_scans_to_device / run_cloud_msgs_to_device
+    def run_merged_cloud_msgs_to_device_ptrs(self, descs, n_parts, parts, out_ptrs, select, counts_ptr, stream_ptr):
+        """gg_run_merged_cloud_msgs_to_device with raw device addresses.  n_parts: int32 [count]; parts: CLOUD_PART_DTYPE
+        array (see cloud_parts); the rest as in run_scans_to_device_ptrs."""
+        count = len(descs)
+        d = _ptr(descs) if isinstance(descs, np.ndarray) else descs
+        n_parts = np.ascontiguousarray(n_parts, np.int32)
+        parts = np.ascontiguousarray(parts, CLOUD_PART_DTYPE)
+        op = None if out_ptrs is None else np.ascontiguousarray(out_ptrs, dtype=np.uint64).reshape(count, 3)
+        _check(self._l.gg_run_merged_cloud_msgs_to_device(self._h, count, d, _ptr(n_parts), _ptr(parts), _ptr(op), int(select), counts_ptr,
+                                                          stream_ptr))
+
+    def run_merged_cloud_msgs_to_device(self, payloads, point_step, field_offsets, T, slots, origins, base_z, labels=True,
+                                        select="nonground", index=False, stream=None):
+        """Scans made of several sensor_msgs/PointCloud2 payloads each (a multi-LiDAR rig), in caller-owned CUDA memory:
+        every part is unpacked and transformed to the map frame on the device, the parts of a scan are concatenated in
+        order in the slot's buffer, and the merged scans then run like run_scans_to_device
+        (gg_run_merged_cloud_msgs_to_device).
+          payloads      : payloads[k] is the list of contiguous CUDA tensors of scan k (at most MAX_CLOUD_PARTS), any
+                          dtype whose byte size is a multiple of the part's point_step
+          point_step    : bytes per point, one value for every part or nested [k][p]
+          field_offsets : byte offsets of x, y, z, intensity, ring (-1 absent), one 5-tuple or nested [k][p]
+          T             : lookupTransform("map", frame_id) as a 3x4, one for every part or nested [k][p]; None: the part
+                          is already in the map frame
+        origins (one cloudOrigin per merged scan), base_z, labels, select, index and stream as in run_scans_to_device.
+        Each payload may be freed right after the call when it was allocated on `stream` (other streams' payloads are
+        marked in use on `stream`).  Returns DeviceOutputs."""
+        torch, dev, stream, sel = self._device_call(select, index, stream)
+        for scan in payloads:
+            for c in scan:
+                if c.device != dev or not c.is_contiguous():
+                    raise ValueError(f"payloads must be contiguous tensors on {dev}")
+        n_parts, parts, Tarr = cloud_parts([[c.numel() * c.element_size() for c in scan] for scan in payloads],
+                                           [[c.data_ptr() for c in scan] for scan in payloads], point_step, field_offsets, T)
+        first = np.cumsum(n_parts) - n_parts
+        n = [int(parts["n_points"][b:b + m].sum()) for b, m in zip(first, n_parts)]
+        descs = self._device_descs(slots, n, origins, base_z)
+        out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, [c for scan in payloads for c in scan])
+        self.run_merged_cloud_msgs_to_device_ptrs(descs, n_parts, parts, ptrs, sel, out.counts.data_ptr() if out.counts is not None else None,
+                                                  stream.cuda_stream or None)
+        del Tarr                   # the transforms `parts` points to: read during the call only
+        return out
+
+    # shared by run_scans_to_device / run_cloud_msgs_to_device / run_merged_cloud_msgs_to_device
     def _device_call(self, select, index, stream):
         """(torch, device, stream, select bits); stream defaults to the current stream."""
         import torch
@@ -690,6 +799,16 @@ class GroundGridB200:
         T = None if T_map_from_frame is None else np.ascontiguousarray(T_map_from_frame, np.float64).reshape(12)
         _check(self._l.gg_upload_cloud_msg(self._h, slot, _ptr(raw), int(n_points), int(point_step), _ptr(off), _ptr(T)))
         return raw
+
+    def upload_cloud_msgs(self, parts, slot=0):
+        """The payloads of one merged scan from host memory (gg_upload_cloud_msgs): parts = [(raw, point_step,
+        field_offsets, T_map_from_frame or None), ...], raw a uint8 array of the part's PointCloud2 payload.  The records
+        land in the slot's buffer back to back; follow with run_scans for the total point count.  Returns the payloads."""
+        raws = [np.ascontiguousarray(p[0], np.uint8) for p in parts]
+        n_parts, arr, Tarr = cloud_parts([[r.nbytes for r in raws]], [[r.ctypes.data for r in raws]], [[p[1] for p in parts]],
+                                         [[p[2] for p in parts]], [[p[3] for p in parts]])
+        _check(self._l.gg_upload_cloud_msgs(self._h, slot, int(n_parts[0]), _ptr(arr)))
+        return raws
 
     def terrain_image(self, slot=0):
         img = np.zeros((self.n, self.n, 3), np.float32)

@@ -315,6 +315,7 @@ struct gg_handle_s {
     uint64_t launches = 0;
     std::vector<void*> dev_allocs;
     std::vector<unsigned char> seen_scratch;  // duplicate-slot check of the batch calls (check_slots)
+    std::vector<int> part_base;               // gg_run_merged_cloud_msgs_to_device: index in `parts` of each scan's first part
     int sched_levels = 0, sched_visits = 0, sched_max = 0;
     bool out_cloud_ready = false;
     // f1: device copy of a PointCloud2 payload, one buffer per stream group (the copy and the unpack kernel of a slot
@@ -521,7 +522,8 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
 
 // Every launch of a batch goes through here.  Per stream group with scans in the batch, on the group's stream: one
 // staging entry, fill(i, entry) for each of the group's scans i (it fills record entry.m and returns whether the record
-// needs the device), the copy of the entry, launch(entry, stream) (returns the number of kernels it launched), and the
+// needs the device), the copy of the entry, launch(entry, stream) (returns the number of kernels it launched, or a
+// negative error code), and the
 // release of the entry.  A group whose records need nothing (a roll that moves no slot) only takes and releases its
 // entry.  With `fenced`, the groups start after everything enqueued on `caller` so far, and `caller` waits for them: no
 // host wait but the flow control of the staging ring.
@@ -544,7 +546,9 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
         if (work) {
             if ((rc = e.commit(st))) return rc;
             if (fenced) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
-            h->launches += launch(e, st);
+            const int n = launch(e, st);
+            if (n < 0) return n;
+            h->launches += n;
             GG_CUDA(cudaGetLastError());
         }
         if ((rc = e.release(h, st))) return rc;
@@ -604,11 +608,57 @@ struct CallerOutputs {
     int32_t* counts;              // [count] or null
     cudaStream_t stream;
     const gg_cloud_msg* msgs;     // [count] or null: payloads unpacked into the slots' own buffers before the scans
+    // or, for merged scans (validated by gg_run_merged_cloud_msgs_to_device), the n_parts[k] payloads of scan k at
+    // parts + part_base[k]
+    const int* n_parts = nullptr;
+    const gg_cloud_part* parts = nullptr;
+    const int* part_base = nullptr;
 };
 
+// A staging entry per part round is taken while the group's scan entry is held, so the rounds of one group never
+// wrap the ring onto it.
+static_assert(GG_MAX_CLOUD_PARTS < kRing, "the part rounds of a group must fit in the staging ring");
+
+// The part rounds of the merged scans in the scan entry `e` (e.hp[j].pos = the scan's position in the call), on the
+// group's stream `st`: round p is one launch of the unpack kernel over part p of every scan of the group that has a
+// non-empty one, each landing in its slot's buffer after the scan's parts before p.  Each round takes its own staging
+// entry.  Returns the number of launches, or a negative error code.
+int launch_part_rounds(gg_handle h, const Staging& e, const CallerOutputs& c, cudaStream_t st) {
+    int rounds = 0, n = 0, rc;
+    for (int j = 0; j < e.m; ++j) rounds = std::max(rounds, c.n_parts[e.hp[j].pos]);
+    for (int p = 0; p < rounds; ++p) {
+        Staging r;
+        for (int j = 0; j < e.m; ++j) {
+            const int k = e.hp[j].pos;
+            if (p >= c.n_parts[k]) continue;
+            const gg_cloud_part* part = c.parts + c.part_base[k];
+            if (part[p].n_points == 0) continue;
+            if (r.m == 0 && (rc = r.acquire(h))) return rc;
+            gg::SlotParams& sp = r.hp[r.m];
+            std::memset(&sp, 0, sizeof(sp));
+            sp.slot = e.hp[j].slot;
+            sp.n_points = (int)part[p].n_points;
+            const gg_cloud_msg& msg = part[p].msg;
+            fill_unpack(r.hunpack[r.m], msg.data, msg.point_step, msg.field_offsets, msg.T_map_from_frame);
+            size_t first = 0;
+            for (int q = 0; q < p; ++q) first += part[q].n_points;
+            r.hunpack[r.m].first = (int)first;
+            r.max_points = std::max(r.max_points, sp.n_points);
+            ++r.m;
+        }
+        if (r.m == 0) continue;
+        r.unpack = true;
+        if ((rc = r.commit(st))) return rc;
+        n += gg::launch_unpack(h->view, r.dp, r.dunpack, r.m, r.max_points, st, h->prof);
+        GG_CUDA(cudaGetLastError());
+        if ((rc = r.release(h, st))) return rc;
+    }
+    return n;
+}
+
 // enqueue the kernels of `count` scans, each group of slots on its own stream; with `caller`, each group also writes
-// its scans' outputs and is ordered after / before the caller's stream (and, with caller->msgs, first unpacks its
-// scans' payloads)
+// its scans' outputs and is ordered after / before the caller's stream (and, with caller->msgs or caller->parts, first
+// unpacks its scans' payloads)
 int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int stop_after, const gg_point* const* dev_points = nullptr,
                       const float* const* packed_ptrs = nullptr, uint8_t* labels_base = nullptr, const CallerOutputs* caller = nullptr) {
     if (count <= 0) return GG_OK;
@@ -641,6 +691,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
                 fill_unpack(e.hunpack[e.m], msg.data, msg.point_step, msg.field_offsets, msg.T_map_from_frame);
                 e.unpack = true;
             }
+            if (caller->parts) e.hp[e.m].pos = i;
         }
         SlotState& s = h->slots[d.slot];
         s.n_points = d.n_points;
@@ -655,6 +706,11 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         int n = 0;
         // after the wait on the caller's stream: the payloads may be produced there
         if (e.unpack) n += gg::launch_unpack(view, e.dp, e.dunpack, e.m, e.max_points, st, h->prof);
+        if (caller && caller->parts) {
+            const int r = launch_part_rounds(h, e, *caller, st);
+            if (r < 0) return r;
+            n += r;
+        }
         n += gg::launch_scan_pipeline(view, e.dp, e.m, e.max_points, stop_after, st, h->prof, h->have_layer_map ? &h->layer_map : nullptr);
         if (e.dests) n += gg::launch_output(view, e.dp, e.ddest, e.m, e.max_points, compact, write, st, h->prof);
         return n;
@@ -1224,17 +1280,17 @@ int gg_run_scans_to_device(gg_handle h, int count, const gg_scan_desc* scans, co
 }
 
 // ---- "next" rows of SURVEY.md section 8(f) --------------------------------------------------
-int gg_upload_cloud_msg(gg_handle h, int slot, const void* data, size_t n_points, int point_step, const int field_offsets[5],
-                        const double T_map_from_frame[12]) {
-    int rc = check_slot(h, slot);
-    if (rc) return rc;
-    if (n_points > h->pcap) return fail(GG_E_ARG, "%zu points exceed capacity %zu", n_points, h->pcap);
-    if ((rc = check_cloud_msg(data, n_points, point_step, field_offsets))) return rc;
+namespace {
+// gg_upload_cloud_msg[s] after validation: the host payloads are copied back to back into the slot's stream-group
+// buffer d_raw (grown to their total bytes), then each part is a one-scan batch of the unpack kernel of
+// gg_run_cloud_msgs_to_device, landing after the parts before it.
+int upload_parts(gg_handle h, int slot, int n_parts, const gg_cloud_part* parts) {
     GG_CUDA(cudaSetDevice(h->device));
     h->inputs_busy = true;
     cudaStream_t st = stream_of(h, slot);
-    const size_t bytes = n_points * (size_t)point_step;
     const int sg = stream_index(h, slot);
+    size_t bytes = 0, n_points = 0;
+    for (int p = 0; p < n_parts; ++p) bytes += parts[p].n_points * (size_t)parts[p].msg.point_step;
     if (bytes > h->d_raw_cap[sg]) {
         GG_CUDA(cudaStreamSynchronize(st));   // the only users of this buffer are on `st`
         if (h->d_raw[sg]) GG_CUDA(cudaFree(h->d_raw[sg]));
@@ -1243,20 +1299,56 @@ int gg_upload_cloud_msg(gg_handle h, int slot, const void* data, size_t n_points
         GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&h->d_raw[sg]), bytes + 256));
         h->d_raw_cap[sg] = bytes;
     }
-    if (bytes) GG_CUDA(cudaMemcpyAsync(h->d_raw[sg], data, bytes, cudaMemcpyHostToDevice, st));
-    // a one-scan batch of the unpack kernel of gg_run_cloud_msgs_to_device
-    auto fill = [&](int, Staging& e) {
-        std::memset(&e.hp[0], 0, sizeof(gg::SlotParams));
-        e.hp[0].slot = slot;
-        e.hp[0].n_points = (int)n_points;
-        fill_unpack(e.hunpack[0], h->d_raw[sg], point_step, field_offsets, T_map_from_frame);
-        e.unpack = true;
-        return true;
-    };
-    auto launch = [&](const Staging& e, cudaStream_t s) { return gg::launch_unpack(h->view, e.dp, e.dunpack, 1, e.max_points, s, h->prof); };
-    if ((rc = run_groups(h, 1, &slot, false, nullptr, fill, launch))) return rc;
+    int rc;
+    size_t at = 0;
+    for (int p = 0; p < n_parts; ++p) {
+        const gg_cloud_part& part = parts[p];
+        const size_t part_bytes = part.n_points * (size_t)part.msg.point_step;
+        if (part_bytes) GG_CUDA(cudaMemcpyAsync(h->d_raw[sg] + at, part.msg.data, part_bytes, cudaMemcpyHostToDevice, st));
+        auto fill = [&](int, Staging& e) {
+            std::memset(&e.hp[0], 0, sizeof(gg::SlotParams));
+            e.hp[0].slot = slot;
+            e.hp[0].n_points = (int)part.n_points;
+            fill_unpack(e.hunpack[0], h->d_raw[sg] + at, part.msg.point_step, part.msg.field_offsets, part.msg.T_map_from_frame);
+            e.hunpack[0].first = (int)n_points;
+            e.unpack = true;
+            return true;
+        };
+        auto launch = [&](const Staging& e, cudaStream_t s) { return gg::launch_unpack(h->view, e.dp, e.dunpack, 1, e.max_points, s, h->prof); };
+        if ((rc = run_groups(h, 1, &slot, false, nullptr, fill, launch))) return rc;
+        at += part_bytes;
+        n_points += part.n_points;
+    }
     h->slots[slot].n_points = n_points;
     return GG_OK;
+}
+}  // namespace
+
+int gg_upload_cloud_msg(gg_handle h, int slot, const void* data, size_t n_points, int point_step, const int field_offsets[5],
+                        const double T_map_from_frame[12]) {
+    int rc = check_slot(h, slot);
+    if (rc) return rc;
+    if (n_points > h->pcap) return fail(GG_E_ARG, "%zu points exceed capacity %zu", n_points, h->pcap);
+    if ((rc = check_cloud_msg(data, n_points, point_step, field_offsets))) return rc;
+    gg_cloud_part part{{data, point_step, {}, T_map_from_frame}, n_points};
+    std::memcpy(part.msg.field_offsets, field_offsets, sizeof(part.msg.field_offsets));
+    return upload_parts(h, slot, 1, &part);
+}
+
+int gg_upload_cloud_msgs(gg_handle h, int slot, int n_parts, const gg_cloud_part* parts) {
+    int rc = check_slot(h, slot);
+    if (rc) return rc;
+    if (n_parts < 0 || n_parts > GG_MAX_CLOUD_PARTS) return fail(GG_E_ARG, "%d parts, not in [0, %d]", n_parts, GG_MAX_CLOUD_PARTS);
+    if (n_parts && !parts) return fail(GG_E_ARG, "null parts");
+    size_t n_points = 0;
+    for (int p = 0; p < n_parts; ++p) {
+        const gg_cloud_part& part = parts[p];
+        if ((rc = check_cloud_msg(part.msg.data, part.n_points, part.msg.point_step, part.msg.field_offsets)))
+            return fail(rc, "part %d: %s", p, g_last_error.c_str());
+        if (part.n_points > h->pcap - n_points) return fail(GG_E_ARG, "part %d: the parts exceed capacity %zu", p, h->pcap);
+        n_points += part.n_points;
+    }
+    return upload_parts(h, slot, n_parts, parts);
 }
 
 int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_cloud_msg* msgs, const gg_scan_outputs* outs,
@@ -1274,6 +1366,42 @@ int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scan
     h->inputs_busy = true;
     GG_CUDA(cudaSetDevice(h->device));
     const CallerOutputs caller{outs, select, dev_counts, static_cast<cudaStream_t>(stream), msgs};
+    return run_scans_grouped(h, count, scans, 0, nullptr, nullptr, nullptr, &caller);
+}
+
+int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const int* n_parts, const gg_cloud_part* parts,
+                                       const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream) {
+    if (!h || !scans || (count > 0 && (!n_parts || !parts))) return fail(GG_E_ARG, "null argument");
+    int rc;
+    if ((rc = check_outputs(outs, -1, select, dev_counts))) return rc;
+    std::vector<int>& base = h->part_base;
+    base.assign((size_t)std::max(count, 0), 0);
+    int next = 0;
+    for (int i = 0; i < count; ++i) {
+        const int m = n_parts[i];
+        if (m < 0 || m > GG_MAX_CLOUD_PARTS) return fail(GG_E_ARG, "scan %d: %d parts, not in [0, %d]", i, m, GG_MAX_CLOUD_PARTS);
+        base[i] = next;
+        size_t n = 0;
+        for (int p = 0; p < m; ++p) {
+            const gg_cloud_part& part = parts[next + p];
+            if ((rc = check_cloud_msg(part.msg.data, part.n_points, part.msg.point_step, part.msg.field_offsets)))
+                return fail(rc, "scan %d part %d: %s", i, p, g_last_error.c_str());
+            if (part.n_points > scans[i].n_points - n)
+                return fail(GG_E_ARG, "scan %d: its parts hold more than its n_points %zu", i, scans[i].n_points);
+            n += part.n_points;
+        }
+        if (n != scans[i].n_points) return fail(GG_E_ARG, "scan %d: its parts hold %zu points, its n_points is %zu", i, n, scans[i].n_points);
+        next += m;
+        // as in gg_run_cloud_msgs_to_device, outputs may overlap the scan's own parts: every part is consumed before the
+        // scan's first kernel on the same stream
+        if ((rc = check_outputs(outs, i, select, dev_counts))) return rc;
+    }
+    h->inputs_busy = true;
+    GG_CUDA(cudaSetDevice(h->device));
+    CallerOutputs caller{outs, select, dev_counts, static_cast<cudaStream_t>(stream), nullptr};
+    caller.n_parts = n_parts;
+    caller.parts = parts;
+    caller.part_base = base.data();
     return run_scans_grouped(h, count, scans, 0, nullptr, nullptr, nullptr, &caller);
 }
 

@@ -222,18 +222,19 @@ struct LayerList {
 int launch_layer_copy(const View& v, const SlotParams* batch, int count, const LayerList& names, float* buf, bool import, cudaStream_t st,
                       Profiler* prof);
 // "next" rows of SURVEY.md section 8(f)
-// f1: one PointCloud2 payload of a batch (gg_upload_cloud_msg, gg_run_cloud_msgs_to_device).  It sits in the staging
-// entry next to the scans' SlotParams, in a parallel array with the same index (like OutDest).
+// f1: one PointCloud2 payload of a batch (gg_upload_cloud_msg[s], gg_run_cloud_msgs_to_device,
+// gg_run_merged_cloud_msgs_to_device).  It sits in the staging entry next to the scans' SlotParams, in a parallel array
+// with the same index (like OutDest).
 struct UnpackDesc {
     const unsigned char* raw;  // msg.data on the device (the handle's staging copy or the caller's buffer)
     int point_step;
     int off[5];                // byte offsets of x, y, z, intensity, ring (-1: field absent)
     int transform;             // 0: frame_id == "map", copy only
-    int reserved;              // zero
+    int first;                 // record of the slot's buffer where the payload's first point lands (one part of a merged scan)
     double T[12];              // row-major 3x4 [R|t] of lookupTransform("map", frame_id)
 };
-// PointCloud2 payloads -> PointXYZIR records in the map frame, for `count` scans: descs[k] (batch[k].n_points records)
-// lands in the slot's own cloud buffer, v.points + batch[k].slot * pcap.
+// PointCloud2 payloads -> PointXYZIR records in the map frame, for `count` payloads: descs[k] (batch[k].n_points records)
+// lands in the slot's own cloud buffer at v.points + batch[k].slot * pcap + descs[k].first.
 int launch_unpack(const View& v, const SlotParams* batch, const UnpackDesc* descs, int count, int max_points, cudaStream_t st, Profiler* prof);
 // f3: the images of publish_grid_map_layer for `count` scans, with the staging entry of launch_layer_copy (batch[s].slot,
 // batch[s].pos = position k in the call, batch[s].points_layer).

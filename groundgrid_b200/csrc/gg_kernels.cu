@@ -1854,9 +1854,9 @@ __global__ void __launch_bounds__(LC_THREADS) k_layer_copy(View v, const SlotPar
 // "next" rows (SURVEY.md section 8f)
 // ------------------------------------------------------------------------------------------
 // f1: pcl::fromROSMsg (field-offset driven unpack, GroundGridNodelet.cpp:119-120) + the per-point
-// tf2::doTransform into the map frame in fp64, stored as float (:166-181).  Block (x, s) unpacks 256 points of scan s
-// into its slot's cloud buffer.  The loads are byte-wise: payloads may be unaligned and fields sit at any offset (the
-// KITTI player's 18-byte points).
+// tf2::doTransform into the map frame in fp64, stored as float (:166-181).  Block (x, s) unpacks 256 points of payload s
+// into its slot's cloud buffer, from record descs[s].first on.  The loads are byte-wise: payloads may be unaligned and
+// fields sit at any offset (the KITTI player's 18-byte points).
 __global__ void __launch_bounds__(256) k_unpack_transform(View v, const SlotParams* __restrict__ batch, const UnpackDesc* __restrict__ descs) {
     const int i = blockIdx.x * 256 + threadIdx.x;
     const SlotParams& sp = batch[blockIdx.y];
@@ -1878,7 +1878,7 @@ __global__ void __launch_bounds__(256) k_unpack_transform(View v, const SlotPara
         y = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], dx), __dmul_rn(T[5], dy)), __dmul_rn(T[6], dz)), T[7]);
         z = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], dx), __dmul_rn(T[9], dy)), __dmul_rn(T[10], dz)), T[11]);
     }
-    uint4* dst = reinterpret_cast<uint4*>(v.points + (size_t)sp.slot * v.pcap + i);
+    uint4* dst = reinterpret_cast<uint4*>(v.points + (size_t)sp.slot * v.pcap + d.first + i);
     dst[0] = make_uint4(__float_as_uint(x), __float_as_uint(y), __float_as_uint(z), 0u);
     dst[1] = make_uint4(inten, ring, 0u, 0u);
 }

@@ -109,7 +109,7 @@ def _cast(scene, origins, dirs, ego_xy):
 
 def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8), az_steps=2048,
                dropout=0.085, seed=1234, sensors=((0.0, 0.0, SENSOR_HEIGHT, 0.0),), range_noise=0.02,
-               frame="map", labels=False):
+               frame="map", labels=False, split=False):
     """One revolution of each sensor, concatenated sensor-major, ring-major then azimuth.
 
     sensors: (dx, dy, z, yaw_offset_deg) mounting poses in the ego frame.
@@ -117,6 +117,8 @@ def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8
     (or in the ego/base frame when frame == "base").  With labels=True also a uint16 array of the
     SemanticKITTI id of the surface each point's ray hit (LABEL_ROAD, LABEL_CAR, LABEL_BUILDING); the
     points and origin are the same bytes as without it.  The evaluation flow puts the ids into "ring".
+    With split=True the points (and ids) are lists with one array per sensor, as a multi-sensor rig delivers
+    them; concatenated, they are the same bytes as without split.
     """
     rng = np.random.default_rng(seed)
     ego_xy = (float(ego_xy[0]), float(ego_xy[1]))
@@ -148,7 +150,9 @@ def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8
         pts["ring"] = ring[keep]
         clouds.append(pts)
         ids.append(hit_id[keep])
-    if len(clouds) > 1:
+    if split:
+        cloud = clouds
+    elif len(clouds) > 1:
         # np.concatenate drops the padding of the record dtype: fill a 32-byte-record array field by field instead
         cloud = np.zeros(sum(len(c) for c in clouds), POINT_DTYPE)
         at = 0
@@ -160,7 +164,7 @@ def lidar_scan(scene, ego_xy=(0.0, 0.0), yaw=0.0, beams=64, elev_deg=(2.0, -24.8
         cloud = clouds[0]
     origin = np.array([ego_xy[0], ego_xy[1], SENSOR_HEIGHT], np.float32)
     if labels:
-        return cloud, origin, np.concatenate(ids)
+        return cloud, origin, ids if split else np.concatenate(ids)
     return cloud, origin
 
 

@@ -300,6 +300,46 @@ typedef struct gg_cloud_msg {
  * gg_upload_cloud_msg: null data with n_points > 0, point_step < 12, x, y or z absent, a field outside point_step. */
 int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_cloud_msg* msgs,
                                 const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream);
+
+/* ---- a multi-LiDAR rig: several sensor payloads per scan ----
+ * One scan of a rig with several sensors arrives as one PointCloud2 payload per sensor, each in its own frame.  The
+ * reference sees such a rig as one cloud merged upstream in the map frame: every sensor's points go through
+ * tf2::doTransform in fp64, are stored as float and are concatenated, and filter_cloud runs on the merged cloud with one
+ * cloudOrigin.  These calls do that merge on the device, into the slot's own cloud buffer. */
+#define GG_MAX_CLOUD_PARTS 16
+
+/* One sensor's payload of a merged scan: the layout and frame rules of gg_cloud_msg, and its own point count.
+ * msg.data is DEVICE memory for gg_run_merged_cloud_msgs_to_device and HOST memory for gg_upload_cloud_msgs;
+ * msg.T_map_from_frame is a HOST pointer in both (NULL: the part is already in the map frame). */
+typedef struct gg_cloud_part {
+    gg_cloud_msg msg;
+    size_t n_points;
+} gg_cloud_part;
+
+/* gg_run_cloud_msgs_to_device for scans made of several payloads.  Scan k owns the next n_parts[k] entries of `parts`,
+ * taken in order (0 <= n_parts[k] <= GG_MAX_CLOUD_PARTS).  Part p of scan k is unpacked and, when it has a
+ * T_map_from_frame, transformed into the slot's own cloud buffer from record sum(n_points of the scan's parts before p)
+ * on; per point the result is bit-identical to gg_upload_cloud_msg of the same bytes.  scans[k].n_points must equal the
+ * sum of its parts' n_points, and the scan then runs on the whole buffer exactly as in gg_run_cloud_msgs_to_device:
+ * outs, select, dev_counts, the stream contract (the work, including every part's unpack, starts after everything
+ * already enqueued on `stream`; no host wait except the flow control of the parameter staging ring), payloads that may
+ * be freed on `stream` right after the call, outputs that may overlap their own scan's parts, and the slots' state
+ * afterwards (layers, gg_get_output, gg_eval_counts_to_device / gg_eval_accumulate read the slot's buffer).
+ * scans[k].origin is the single cloudOrigin of the merged scan.  A scan with no parts and n_points == 0 is empty.
+ * count == 0 returns GG_OK and enqueues nothing.  GG_E_ARG, with nothing enqueued: what gg_run_cloud_msgs_to_device
+ * rejects (GG_E_STATE for a map not initialised); null n_parts or parts with count > 0; n_parts[k] < 0 or
+ * > GG_MAX_CLOUD_PARTS; scans[k].n_points other than the sum of its parts' n_points; per part the layout rules of
+ * gg_upload_cloud_msg (the error text names the scan and the part). */
+int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const int* n_parts,
+                                       const gg_cloud_part* parts, const gg_scan_outputs* outs, unsigned select,
+                                       int32_t* dev_counts, void* stream);
+
+/* The host-memory form, as gg_upload_cloud_msg is for gg_run_cloud_msgs_to_device: the n_parts payloads in HOST memory
+ * are copied to the device, unpacked and transformed into the slot's cloud buffer back to back (part p from record
+ * sum(n_points of the parts before p) on).  Follow with gg_run_scans for n_points = the sum of the parts' n_points.
+ * GG_E_ARG: slot out of range, n_parts < 0 or > GG_MAX_CLOUD_PARTS, null parts with n_parts > 0, more points than the
+ * capacity, a part breaking the layout rules of gg_upload_cloud_msg (the error text names the part). */
+int gg_upload_cloud_msgs(gg_handle h, int slot, int n_parts, const gg_cloud_part* parts);
 int gg_terrain_image(gg_handle h, int slot, float* dst);
 /* The other branch of publish_grid_map_layer (src/GroundGridNodelet.cpp:238-245): the single-channel 8-bit image that
  * grid_map::GridMapCvConverter::toImage<unsigned char, 1>(map, layer, CV_8UC1, img) produces and cv::applyColorMap then
