@@ -135,6 +135,28 @@ def cloud_parts(nbytes, data_ptrs, point_step, field_offsets, T):
             parts["T_map_from_frame"][p] = Tarr.ctypes.data + 96 * p
     return n_parts, parts[:total], Tarr
 
+class Positions(C.Structure):
+    """gg_positions: one set of query positions of a slot (device memory) and where its results go."""
+
+    _fields_ = [
+        ("data", C.c_void_p),
+        ("n", C.c_size_t),
+        ("point_step", C.c_int),
+        ("off_x", C.c_int),
+        ("off_y", C.c_int),
+        ("dst", C.c_void_p),
+        ("cell", C.c_void_p),
+    ]
+
+
+# numpy image of an array of gg_positions (Positions)
+POSITIONS_DTYPE = np.dtype({"names": ["data", "n", "point_step", "off_x", "off_y", "dst", "cell"],
+                            "formats": [np.uint64, np.uint64, np.int32, np.int32, np.int32, np.uint64, np.uint64],
+                            "offsets": [Positions.data.offset, Positions.n.offset, Positions.point_step.offset, Positions.off_x.offset,
+                                        Positions.off_y.offset, Positions.dst.offset, Positions.cell.offset],
+                            "itemsize": C.sizeof(Positions)})
+SAMPLE_MODES = {"nearest": 0, "linear": 1}   # GG_SAMPLE_NEAREST, GG_SAMPLE_LINEAR
+
 # numpy image of an array of gg_scan_desc (ScanDesc)
 SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "n_points", "origin", "base_z"], "formats": [np.int32, np.uint64, (np.float32, 3), np.float64],
                             "offsets": [0, 8, 16, 32], "itemsize": C.sizeof(ScanDesc)})
@@ -234,6 +256,7 @@ def load(build_if_missing=True):
         "gg_layer_device_ptr": (i, [vp, i, C.c_char_p, C.POINTER(vp)]),
         "gg_get_layers_to_device": (i, [vp, i, vp, i, vp, vp, vp]),
         "gg_set_layers_from_device": (i, [vp, i, vp, i, vp, vp, vp]),
+        "gg_sample_layers_to_device": (i, [vp, i, vp, vp, i, vp, i, vp]),
         "gg_layer_images_to_device": (i, [vp, i, vp, i, vp, vp, vp, vp]),
         "gg_terrain_images_to_device": (i, [vp, i, vp, vp, vp]),
         "gg_stream": (vp, [vp]),
@@ -490,6 +513,65 @@ class GroundGridB200:
         elif stream != current:
             buf.record_stream(stream)
         self.set_layers_from_device_ptrs(slots, names, buf.data_ptr(), stream.cuda_stream or None)
+
+    def sample_layers_to_device_ptrs(self, slots, queries, names, mode, stream_ptr):
+        """gg_sample_layers_to_device with raw device addresses: queries a POSITIONS_DTYPE array, one set per slot;
+        mode "nearest" / "linear" (or GG_SAMPLE_*); stream_ptr an int or None (None = the legacy default stream)."""
+        sl, n, nm = self._layer_batch_args(slots, names)
+        q = None if queries is None else np.ascontiguousarray(queries, POSITIONS_DTYPE)
+        m = SAMPLE_MODES[mode] if isinstance(mode, str) else int(mode)
+        _check(self._l.gg_sample_layers_to_device(self._h, len(sl), _ptr(sl), _ptr(q), n, nm, m, stream_ptr))
+
+    def sample_layers_to_device(self, slots, positions, names=("ground", "groundpatch"), mode="nearest", cells=False, out=None, stream=None):
+        """Values of layers `names` of `slots` at map-frame positions (gg_sample_layers_to_device).
+          positions : one CUDA tensor per slot: float32 [n, >= 2] with x, y in columns 0 and 1 and unit column stride
+                      (e.g. [n, 2], or the float32 [n, 8] view of 32-byte point records); the row stride is the record step
+          mode      : "nearest" (the cell's value) or "linear" (the header's bilinear definition)
+          cells     : also return each query's cell i + j * N (-1 outside the map)
+          out       : None, or one contiguous float32 [n_names, n] tensor per slot to fill
+          stream    : torch.cuda.Stream the work is ordered on (default: the current stream); outputs are allocated on it.
+        Returns a list of float32 [n_names, n] tensors (value of name l at query q at [l, q]; NaN outside the map), and
+        with cells=True also a list of int32 [n] tensors.  The call returns without waiting for the device; the positions
+        may be freed right after it when they were allocated on `stream` (others are marked in use on `stream`)."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        if len(positions) != len(slots):
+            raise ValueError("positions needs one tensor per slot")
+        if mode not in SAMPLE_MODES:
+            raise ValueError(f"mode must be one of {list(SAMPLE_MODES)}")
+        L = len(names)
+        q = np.zeros(max(1, len(slots)), POSITIONS_DTYPE)
+        ns = []
+        for k, p in enumerate(positions):
+            if p.dtype != torch.float32 or p.device != dev or p.dim() != 2 or p.shape[1] < 2 or (p.shape[0] > 1 and p.stride(1) != 1):
+                raise ValueError(f"positions[{k}] must be a float32 tensor [n, >= 2] on {dev} with unit column stride")
+            n = int(p.shape[0])
+            step = 4 * (p.stride(0) if n > 1 else max(2, p.shape[1]))
+            if n > 1 and p.stride(0) < 2:
+                raise ValueError(f"positions[{k}]: a row stride of {p.stride(0)} elements is no record layout")
+            ns.append(n)
+            q["data"][k], q["n"][k], q["point_step"][k], q["off_x"][k], q["off_y"][k] = p.data_ptr() if n else 0, n, step, 0, 4
+        total = sum(ns)
+        if out is None:
+            with torch.cuda.stream(stream):
+                flat = torch.empty(L * total, dtype=torch.float32, device=dev)
+            out = [t.view(L, n) for t, n in zip(torch.split(flat, [L * n for n in ns]), ns)]
+        else:
+            if len(out) != len(slots):
+                raise ValueError("out needs one tensor per slot")
+            out = [self._stream_out(torch, dev, current, stream, o, (L, n), torch.float32, f"out[{k}]") for k, (o, n) in enumerate(zip(out, ns))]
+        cell = None
+        if cells:
+            with torch.cuda.stream(stream):
+                cell = list(torch.split(torch.empty(total, dtype=torch.int32, device=dev), ns))
+        for k, n in enumerate(ns):
+            if n:
+                q["dst"][k] = out[k].data_ptr()
+                q["cell"][k] = cell[k].data_ptr() if cells else 0
+        if stream != current:
+            for p in positions:
+                p.record_stream(stream)
+        self.sample_layers_to_device_ptrs(slots, q[:len(slots)], names, mode, stream.cuda_stream or None)
+        return (out, cell) if cells else out
 
     def layer_images_to_device_ptrs(self, slots, names, dst_ptr, range_ptr, stream_ptr):
         """gg_layer_images_to_device with raw device addresses: dst_ptr uint8 [count][n_names][N][N] (row-major planes),

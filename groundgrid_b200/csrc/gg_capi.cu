@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -282,6 +283,13 @@ struct SlotState {
     const float* packed_input = nullptr;  // last scan came through the packed host path (no 32-byte records on the device)
 };
 
+// A caller's device byte range [begin, end) of one query set: its positions (input) or one of its outputs.
+struct ByteRange {
+    uintptr_t begin, end;
+    int set;
+    bool output;
+};
+
 }  // namespace
 
 struct gg_handle_s {
@@ -307,6 +315,8 @@ struct gg_handle_s {
     gg::OutDest* d_dest = nullptr;
     gg::UnpackDesc* h_unpack = nullptr;  // PointCloud2 payloads of the entry's scans, same shape as h_ring / d_ring
     gg::UnpackDesc* d_unpack = nullptr;
+    gg::QueryDesc* h_query = nullptr;    // terrain lookups: query sets of the entry's slots, same shape as h_ring / d_ring
+    gg::QueryDesc* d_query = nullptr;
     cudaEvent_t ring_ev[kRing] = {};
     cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
     cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
@@ -316,6 +326,7 @@ struct gg_handle_s {
     std::vector<void*> dev_allocs;
     std::vector<unsigned char> seen_scratch;  // duplicate-slot check of the batch calls (check_slots)
     std::vector<int> part_base;               // gg_run_merged_cloud_msgs_to_device: index in `parts` of each scan's first part
+    std::vector<ByteRange> range_scratch;     // gg_sample_layers_to_device: the overlap check of the sets' ranges
     int sched_levels = 0, sched_visits = 0, sched_max = 0;
     bool out_cloud_ready = false;
     // f1: device copy of a PointCloud2 payload, one buffer per stream group (the copy and the unpack kernel of a slot
@@ -423,16 +434,19 @@ int layer_index(gg_handle h, int slot, const char* name, int* idx) {
 }
 
 // One entry of the parameter staging ring: the SlotParams of up to n_slots scans and, in arrays parallel to them, their
-// output destinations (OutDest) and PointCloud2 payloads (UnpackDesc), each pinned on the host with a device copy.
+// output destinations (OutDest), PointCloud2 payloads (UnpackDesc) and query sets (QueryDesc), each pinned on the host
+// with a device copy.
 struct Staging {
     int pos = 0;                 // position in the ring
     int m = 0;                   // records filled
     int max_points = 0;          // largest n_points of the records
     bool dests = false;          // commit also copies the OutDest records
     bool unpack = false;         // ... and the UnpackDesc records
+    bool query = false;          // ... and the QueryDesc records
     gg::SlotParams *hp = nullptr, *dp = nullptr;
     gg::OutDest *hdest = nullptr, *ddest = nullptr;
     gg::UnpackDesc *hunpack = nullptr, *dunpack = nullptr;
+    gg::QueryDesc *hquery = nullptr, *dquery = nullptr;
 
     // Reserve the next entry (waits only if the ring wrapped onto an in-flight entry).
     int acquire(gg_handle h) {
@@ -446,12 +460,15 @@ struct Staging {
         ddest = h->d_dest + at;
         hunpack = h->h_unpack + at;
         dunpack = h->d_unpack + at;
+        hquery = h->h_query + at;
+        dquery = h->d_query + at;
         return GG_OK;
     }
     int commit(cudaStream_t st) const {
         GG_CUDA(cudaMemcpyAsync(dp, hp, (size_t)m * sizeof(gg::SlotParams), cudaMemcpyHostToDevice, st));
         if (dests) GG_CUDA(cudaMemcpyAsync(ddest, hdest, (size_t)m * sizeof(gg::OutDest), cudaMemcpyHostToDevice, st));
         if (unpack) GG_CUDA(cudaMemcpyAsync(dunpack, hunpack, (size_t)m * sizeof(gg::UnpackDesc), cudaMemcpyHostToDevice, st));
+        if (query) GG_CUDA(cudaMemcpyAsync(dquery, hquery, (size_t)m * sizeof(gg::QueryDesc), cudaMemcpyHostToDevice, st));
         return GG_OK;
     }
     // The entry may be reused once the kernels that read it have finished (they may run on any of the handle's streams,
@@ -1017,6 +1034,8 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     GG_TRY(dev_alloc(h, &h->d_dest, (size_t)kRing * S));
     GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_unpack), sizeof(gg::UnpackDesc) * kRing * S, cudaHostAllocDefault));
     GG_TRY(dev_alloc(h, &h->d_unpack, (size_t)kRing * S));
+    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_query), sizeof(gg::QueryDesc) * kRing * S, cudaHostAllocDefault));
+    GG_TRY(dev_alloc(h, &h->d_query, (size_t)kRing * S));
     for (int i = 0; i < kRing; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->ring_ev[i], cudaEventDisableTiming));
     GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_in, cudaEventDisableTiming));
     for (int i = 0; i < kStreams; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_out[i], cudaEventDisableTiming));
@@ -1052,6 +1071,7 @@ int gg_destroy(gg_handle h) {
     if (h->h_ring) cudaFreeHost(h->h_ring);
     if (h->h_dest) cudaFreeHost(h->h_dest);
     if (h->h_unpack) cudaFreeHost(h->h_unpack);
+    if (h->h_query) cudaFreeHost(h->h_query);
     for (int i = 0; i < kRing; ++i)
         if (h->ring_ev[i]) cudaEventDestroy(h->ring_ev[i]);
     if (h->own_streams)
@@ -1699,7 +1719,8 @@ const char* gg_profile_kernel_name(int id) {
     static const char* names[gg::K_NUM] = {"k_rasterize",   "k_cell_tiles",    "k_cell_place",    "k_scatter",
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
-                                           "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image"};
+                                           "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
+                                           "k_sample_layers"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2243,6 +2264,81 @@ int gg_get_layers_to_device(gg_handle h, int count, const int* slots, int n_name
 int gg_set_layers_from_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, const float* src,
                               void* stream) {
     return layer_transfer(h, count, slots, n_names, names, const_cast<float*>(src), true, stream);
+}
+
+// Terrain lookups: one k_sample_layers per stream group with non-empty sets in the batch.
+int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const gg_positions* queries, int n_names, const char* const* names,
+                               int mode, void* stream) {
+    gg::LayerList list{};
+    int points_at = -1, rc;
+    if ((rc = check_slot_batch(h, count, slots, n_names, names, {}, &list, &points_at)) || count == 0 || n_names == 0) return rc;
+    if (!queries) return fail(GG_E_ARG, "null queries");
+    if (mode != GG_SAMPLE_NEAREST && mode != GG_SAMPLE_LINEAR) return fail(GG_E_ARG, "unknown sample mode %d", mode);
+    const gg::View& v = h->view;
+    const void* arena = v.layers;
+    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    std::vector<ByteRange>& ranges = h->range_scratch;
+    ranges.clear();
+    size_t total = 0;
+    for (int k = 0; k < count; ++k) {
+        const gg_positions& q = queries[k];
+        if (q.n == 0) continue;
+        if (q.n > (size_t)INT32_MAX) return fail(GG_E_ARG, "set %d: %zu positions, at most %d", k, q.n, INT32_MAX);
+        if (!q.data || !q.dst) return fail(GG_E_ARG, "set %d: null data or dst", k);
+        if (q.point_step < 8 || q.point_step % 4) return fail(GG_E_ARG, "set %d: point_step %d is not a multiple of 4 of at least 8", k, q.point_step);
+        if (q.off_x < 0 || q.off_y < 0 || q.off_x % 4 || q.off_y % 4 || q.off_x > q.point_step - 4 || q.off_y > q.point_step - 4)
+            return fail(GG_E_ARG, "set %d: offsets (%d, %d) are not multiples of 4 inside point_step %d", k, q.off_x, q.off_y, q.point_step);
+        if (reinterpret_cast<uintptr_t>(q.data) % 4 || reinterpret_cast<uintptr_t>(q.dst) % 4 || reinterpret_cast<uintptr_t>(q.cell) % 4)
+            return fail(GG_E_ARG, "set %d: data, dst or cell is not 4-byte aligned", k);
+        const size_t dst_bytes = (size_t)n_names * q.n * sizeof(float), cell_bytes = q.n * sizeof(int32_t);
+        if (ranges_overlap(q.dst, dst_bytes, arena, arena_bytes) || ranges_overlap(q.cell, cell_bytes, arena, arena_bytes))
+            return fail(GG_E_ARG, "set %d: an output overlaps the handle's layers", k);
+        const uintptr_t data = reinterpret_cast<uintptr_t>(q.data), dst = reinterpret_cast<uintptr_t>(q.dst);
+        ranges.push_back({data, data + q.n * (size_t)q.point_step, k, false});
+        ranges.push_back({dst, dst + dst_bytes, k, true});
+        if (q.cell) ranges.push_back({reinterpret_cast<uintptr_t>(q.cell), reinterpret_cast<uintptr_t>(q.cell) + cell_bytes, k, true});
+        total += q.n;
+    }
+    // Outputs must not overlap any range; inputs may share memory.  Sorted by start, a range overlaps an earlier one iff
+    // it starts below the largest end among them, so one sweep keeps the farthest-reaching range and the farthest output.
+    std::sort(ranges.begin(), ranges.end(), [](const ByteRange& a, const ByteRange& b) { return a.begin < b.begin; });
+    const ByteRange *far_any = nullptr, *far_out = nullptr;
+    for (const ByteRange& r : ranges) {
+        const ByteRange* o = r.output ? far_any : far_out;
+        if (o && o->end > r.begin)
+            return fail(GG_E_ARG, "set %d: %s overlaps %s of set %d", r.set, r.output ? "an output" : "the positions",
+                        o->output ? "an output" : "the positions", o->set);
+        if (!far_any || r.end > far_any->end) far_any = &r;
+        if (r.output && (!far_out || r.end > far_out->end)) far_out = &r;
+    }
+    if (total == 0) return GG_OK;
+    GG_CUDA(cudaSetDevice(h->device));
+    auto fill = [&](int i, Staging& e) {
+        const gg_positions& q = queries[i];
+        const SlotState& s = h->slots[slots[i]];
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        p.points_layer = points_layer(h, slots[i]);
+        p.px = s.px;
+        p.py = s.py;
+        p.n_points = (int)q.n;
+        gg::QueryDesc& d = e.hquery[e.m];
+        std::memset(&d, 0, sizeof(d));
+        d.data = static_cast<const unsigned char*>(q.data);
+        d.dst = q.dst;
+        d.cell = q.cell;
+        d.point_step = q.point_step;
+        d.off_x = q.off_x;
+        d.off_y = q.off_y;
+        e.query = true;
+        return q.n > 0;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) {
+        return gg::launch_sample(h->view, e.dp, e.dquery, e.m, e.max_points, list, mode, st, h->prof);
+    };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
 }  // extern "C"

@@ -178,7 +178,7 @@ constexpr int OUT_TILE = 1024;
 // kernels of the pipeline, as reported by the profiling hooks (gg_profile_read)
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
-    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_NUM
+    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_NUM
 };
 
 // Optional per-kernel CUDA-event timing (bench.py's roofline needs the dominant kernel's own
@@ -251,5 +251,19 @@ int launch_terrain_images(const View& v, const SlotParams* batch, int count, flo
 // max_points: the largest n_points of the batch.
 int launch_eval(const View& v, const SlotParams* batch, int count, int max_points, unsigned long long* counts, cudaStream_t st, Profiler* prof);
 constexpr int EVAL_LABELS = GG_EVAL_IDS;  // ring values (SemanticKITTI label ids <= 259) x {ground, non-ground}
+// Terrain lookups (gg_sample_layers_to_device): one set of query positions of a slot and where its results go.  It sits
+// in the staging entry next to the scans' SlotParams, in a parallel array with the same index (like OutDest).
+struct QueryDesc {
+    const unsigned char* data;  // batch[k].n_points records of point_step bytes, float32 x / y at off_x / off_y (map frame)
+    float* dst;                 // [names.n][n]: value of name l at query q at dst[l * n + q]
+    int32_t* cell;              // [n] i + j * N of the query's cell, -1 outside; null: none
+    int point_step, off_x, off_y;
+    int reserved;               // zero
+};
+// The values of `names` at the positions of descs[k] in the map of batch[k].slot at (batch[k].px, batch[k].py);
+// mode GG_SAMPLE_NEAREST / GG_SAMPLE_LINEAR.  Per scan the staging entry carries slot, px, py, n_points (the set's size)
+// and points_layer.  max_points: the largest n_points of the batch.
+int launch_sample(const View& v, const SlotParams* batch, const QueryDesc* descs, int count, int max_points, const LayerList& names, int mode,
+                  cudaStream_t st, Profiler* prof);
 
 }  // namespace gg

@@ -65,6 +65,12 @@ __device__ __forceinline__ bool grid_inside(const Const& k, double px, double py
     return tx >= 0.0 && ty >= 0.0 && tx < k.len && ty < k.len;
 }
 
+// grid_map getPositionFromIndex along one axis (start index (0,0)): pos + (len/2 - res/2) + res * (-(double)index)
+__device__ __forceinline__ double cell_centre(const Const& k, double pos, int index) {
+    const double off = __dsub_rn(k.half, __dmul_rn(0.5, k.res));
+    return __dadd_rn(__dadd_rn(pos, off), __dmul_rn(k.res, (double)(-index)));
+}
+
 // Eigen 3.3.7 redux_novec_unroller: binary split over the block's coefficients (column-major).
 template <int Start, int Len>
 struct TreeSum {
@@ -180,10 +186,8 @@ __global__ void __launch_bounds__(256) k_roll_gather(View v, const SlotParams* _
         if (seed[u]) {
             const int cell = cell0 + u;
             const int r = cell % N, cc = cell / N;
-            // grid_map getPositionFromIndex: pos + (len/2 - res/2) + res * (-(double)index)
-            const double off = __dsub_rn(k.half, __dmul_rn(0.5, k.res));
-            const double x = __dadd_rn(__dadd_rn(sp.px, off), __dmul_rn(k.res, (double)(-r)));
-            const double y = __dadd_rn(__dadd_rn(sp.py, off), __dmul_rn(k.res, (double)(-cc)));
+            const double x = cell_centre(k, sp.px, r);
+            const double y = cell_centre(k, sp.py, cc);
             // tf2::Transform * Vector3(x, y, 0): row2.dot(v) + origin.z
             const double tz = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sp.t20, x), __dmul_rn(sp.t21, y)), __dmul_rn(sp.t22, 0.0)), sp.t23);
             g[u] = (float)(-tz);
@@ -2099,6 +2103,108 @@ __global__ void __launch_bounds__(EVAL_THREADS) k_eval_counts(View v, const Slot
         if (s_cnt[t]) atomicAdd(&dst[t], (unsigned long long)s_cnt[t]);
 }
 
+// Terrain lookups (gg_sample_layers_to_device).  Blocks (x, set): every thread takes SAMPLE_ILP queries of set
+// batch[set] SAMPLE_THREADS apart, issues their position loads up front (as k_label does), finds each query's cell with
+// the rasterizer's grid_index / grid_inside and, in linear mode, its bilinear weights once; then per name it gathers 1
+// or 4 cells per query and stores the values coalesced at dst[l * n + q].  Arithmetic: fp64, correctly rounded, no
+// contraction (the header's definition).  A linear value that is NaN, and every value outside the map, is stored as
+// the quiet NaN 0x7fc00000 (device fp64 arithmetic does not keep NaN payloads); nearest values keep their bits.
+constexpr int SAMPLE_THREADS = 256, SAMPLE_ILP = 2;   // 4 queries per thread need 107 registers; 2 keep 64 and four blocks per SM
+constexpr uint32_t SAMPLE_NAN = 0x7fc00000u;
+
+__global__ void __launch_bounds__(SAMPLE_THREADS) k_sample_layers(View v, const SlotParams* __restrict__ batch, const QueryDesc* __restrict__ descs,
+                                                                  LayerList names, int mode) {
+    const SlotParams& sp = batch[blockIdx.y];
+    const unsigned n = (unsigned)sp.n_points;
+    const unsigned q0 = blockIdx.x * (SAMPLE_THREADS * SAMPLE_ILP) + threadIdx.x;
+    if (q0 >= n) return;
+    const QueryDesc& d = descs[blockIdx.y];
+    const Const& k = v.k;
+    const int N = k.N;
+    const double px = sp.px, py = sp.py;
+    const unsigned char* __restrict__ data = d.data;
+    const size_t step = (size_t)d.point_step;
+    float x[SAMPLE_ILP], y[SAMPLE_ILP];
+#pragma unroll
+    for (int u = 0; u < SAMPLE_ILP; ++u) {
+        const unsigned q = q0 + u * SAMPLE_THREADS;
+        x[u] = y[u] = __uint_as_float(SAMPLE_NAN);
+        if (q < n) {
+            const unsigned char* p = data + (size_t)q * step;
+            x[u] = __ldg(reinterpret_cast<const float*>(p + d.off_x));
+            y[u] = __ldg(reinterpret_cast<const float*>(p + d.off_y));
+        }
+    }
+    // per query: its cell a (-1 outside) and, when it interpolates, the neighbours b = (i + si, j), c = (i, j + sj),
+    // d = (i + si, j + sj) with their weights (cb = -1: the nearest value)
+    int ca[SAMPLE_ILP], cb[SAMPLE_ILP], cc[SAMPLE_ILP], cd[SAMPLE_ILP];
+    double wa[SAMPLE_ILP], wb[SAMPLE_ILP], wc[SAMPLE_ILP], wd[SAMPLE_ILP];
+#pragma unroll
+    for (int u = 0; u < SAMPLE_ILP; ++u) {
+        const double dx = (double)x[u], dy = (double)y[u];
+        int i, j;
+        grid_index(k, px, py, dx, dy, i, j);
+        const bool in = grid_inside(k, px, py, dx, dy) && i >= 0 && j >= 0 && i < N && j < N;
+        ca[u] = in ? i + j * N : -1;
+        cb[u] = cc[u] = cd[u] = -1;
+        wa[u] = wb[u] = wc[u] = wd[u] = 0.0;
+        if (in && mode == GG_SAMPLE_LINEAR) {
+            const double cx = cell_centre(k, px, i), cy = cell_centre(k, py, j);
+            const int si = dx >= cx ? -1 : 1, sj = dy >= cy ? -1 : 1;   // i grows toward -x
+            if (i + si >= 0 && i + si < N && j + sj >= 0 && j + sj < N) {
+                const double tx = __ddiv_rn(fabs(__dsub_rn(dx, cx)), k.res), ty = __ddiv_rn(fabs(__dsub_rn(dy, cy)), k.res);
+                const double ux = __dsub_rn(1.0, tx), uy = __dsub_rn(1.0, ty);
+                wa[u] = __dmul_rn(ux, uy);
+                wb[u] = __dmul_rn(tx, uy);
+                wc[u] = __dmul_rn(ux, ty);
+                wd[u] = __dmul_rn(tx, ty);
+                cb[u] = ca[u] + si;
+                cc[u] = ca[u] + sj * N;
+                cd[u] = ca[u] + si + sj * N;
+            }
+        }
+    }
+    if (d.cell) {
+#pragma unroll
+        for (int u = 0; u < SAMPLE_ILP; ++u) {
+            const unsigned q = q0 + u * SAMPLE_THREADS;
+            if (q < n) d.cell[q] = ca[u];
+        }
+    }
+#pragma unroll
+    for (int l = 0; l < L_NUM; ++l) {   // static indexing keeps `names` in the parameter bank
+        if (l >= names.n) break;
+        const int idx = names.idx[l];
+        const float* __restrict__ P = v.layer(sp.slot, idx == LAYER_POINTS ? sp.points_layer : idx);
+        float fa[SAMPLE_ILP], fb[SAMPLE_ILP], fc[SAMPLE_ILP], fd[SAMPLE_ILP];
+#pragma unroll
+        for (int u = 0; u < SAMPLE_ILP; ++u) {
+            fa[u] = ca[u] >= 0 ? P[ca[u]] : __uint_as_float(SAMPLE_NAN);
+            fb[u] = fc[u] = fd[u] = 0.0f;
+            if (cb[u] >= 0) {
+                fb[u] = P[cb[u]];
+                fc[u] = P[cc[u]];
+                fd[u] = P[cd[u]];
+            }
+        }
+        float* __restrict__ out = d.dst + (size_t)l * n;
+#pragma unroll
+        for (int u = 0; u < SAMPLE_ILP; ++u) {
+            const unsigned q = q0 + u * SAMPLE_THREADS;
+            if (q >= n) break;
+            float r = fa[u];
+            if (cb[u] >= 0) {
+                const double s = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(wa[u], (double)fa[u]), __dmul_rn(wb[u], (double)fb[u])),
+                                                     __dmul_rn(wc[u], (double)fc[u])),
+                                           __dmul_rn(wd[u], (double)fd[u]));
+                r = (float)s;
+                if (r != r) r = __uint_as_float(SAMPLE_NAN);
+            }
+            out[q] = r;
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
@@ -2366,6 +2472,15 @@ int launch_terrain_images(const View& v, const SlotParams* batch, int count, flo
 
 int launch_eval(const View& v, const SlotParams* batch, int count, int max_points, unsigned long long* counts, cudaStream_t st, Profiler* prof) {
     GG_LAUNCH(K_EVAL, k_eval_counts<<<dim3(max(1, cdiv(max_points, EVAL_TILE)), count), EVAL_THREADS, 0, st>>>(v, batch, counts));
+    return 1;
+}
+
+int launch_sample(const View& v, const SlotParams* batch, const QueryDesc* descs, int count, int max_points, const LayerList& names, int mode,
+                  cudaStream_t st, Profiler* prof) {
+    constexpr long long per_block = SAMPLE_THREADS * SAMPLE_ILP;   // max_points may be INT32_MAX: no int rounding-up
+    const long long blocks = ((long long)max_points + per_block - 1) / per_block;
+    const unsigned nb = blocks > 0 ? (unsigned)blocks : 1u;
+    GG_LAUNCH(K_SAMPLE, k_sample_layers<<<dim3(nb, count), SAMPLE_THREADS, 0, st>>>(v, batch, descs, names, mode));
     return 1;
 }
 

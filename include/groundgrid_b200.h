@@ -459,6 +459,69 @@ int gg_get_layers_to_device(gg_handle h, int count, const int* slots, int n_name
 int gg_set_layers_from_device(gg_handle h, int count, const int* slots, int n_names, const char* const* names, const float* src,
                               void* stream);
 
+/* Terrain lookups: the values of layers of `count` distinct slots at arbitrary map-frame positions (a planner's samples,
+ * another sensor's detections, the points of the next cloud), written into caller-owned device memory and ordered on
+ * the caller's stream -- what grid_map's getIndex followed by a layer read gives a consumer of the published map
+ * (GroundGridNodelet.cpp:211-214), without exporting whole planes.
+ *   slots      : `count` distinct slots, each with an initialised map (no scan needed: the prior after gg_init_map or
+ *                after a roll is a valid terrain).  The map position used is the slot's position after its last
+ *                enqueued roll (what gg_get_map_position returns at the time of the call).
+ *   queries    : queries[k] is the set of positions of slots[k] and where its results go; all DEVICE memory on the
+ *                handle's device:
+ *                  data       n records of point_step bytes, 4-byte aligned (NULL allowed when n == 0)
+ *                  n          <= INT32_MAX, independent of the handle's max_points
+ *                  point_step multiple of 4, >= 8: 32 for gg_point records, 8 for float32 [n, 2], 16 for [n, 4] ...
+ *                  off_x/y    byte offsets of float32 x, y in the MAP frame; multiples of 4, off + 4 <= point_step
+ *                  dst        float32 [n_names][n], 4-byte aligned: the value of name l at query q lands at dst[l*n + q]
+ *                  cell       NULL or int32 [n], 4-byte aligned: i + j*N of the query's cell, -1 outside the map
+ *   names      : `n_names` (<= 12) distinct layer names, resolved as in gg_get_layers_to_device ("points" per slot)
+ *   mode       : GG_SAMPLE_NEAREST or GG_SAMPLE_LINEAR
+ *   stream     : cudaStream_t; NULL is the legacy default stream.  The contract of gg_get_layers_to_device: the work
+ *                starts after everything already enqueued on `stream` and on the stream group of every slot in the
+ *                batch, work enqueued on `stream` afterwards sees the results, and nothing waits on the host except the
+ *                flow control of the parameter staging ring.  A stream-ordered allocator may therefore free the
+ *                position sets, or reuse their memory, on `stream` right after the call; the slot's next scan, enqueued
+ *                after the call, does not change what the call reads.
+ * Cell: the rasterizer's own arithmetic (a query lands in exactly the cell a scan point at the same position would):
+ * (x, y) widened to double, (i, j) = grid_map getIndexFromPosition (fp64 division, truncation toward zero); the query
+ * is inside when checkIfPositionWithinMap holds and 0 <= i, j < N.  Border cells (i or j >= N-3) are ordinary cells
+ * here: their value is what the layer holds.  A query outside the map, NaN and +-inf coordinates included, gets
+ * cell = -1 and NaN (0x7fc00000) for every name: grid_map throws there, one bad query must not fail a batch.
+ * GG_SAMPLE_NEAREST: value = plane[i + j*N], bits unchanged (NaN payloads and -0 included).
+ * GG_SAMPLE_LINEAR: this project's own definition (not a restatement of grid_map's atPosition(INTER_LINEAR)).  All
+ * arithmetic is fp64, correctly rounded, without contraction:
+ *   - the centre of cell (i, j) is grid_map's getPositionFromIndex: off = half - 0.5*res (half = N*res / 2),
+ *     cx = (px + off) + res*(double)(-i), cy likewise with j and py;
+ *   - neighbour direction si = (x >= cx) ? -1 : +1 (i grows toward -x), sj = (y >= cy) ? -1 : +1;
+ *   - fractions tx = |x - cx| / res, ty = |y - cy| / res;
+ *   - if i + si or j + sj is outside [0, N), the result is the nearest value;
+ *   - otherwise, with a = (i, j), b = (i+si, j), c = (i, j+sj), d = (i+si, j+sj):
+ *     v = (((1-tx)(1-ty)*fa + tx(1-ty)*fb) + (1-tx)ty*fc) + tx*ty*fd, each weight rounded once, the sum taken left to
+ *     right, and (float)v stored.
+ *   Non-finite cells propagate as IEEE arithmetic gives (a zero weight times inf is NaN); a NaN result is stored as
+ *   0x7fc00000.
+ * count == 0, n_names == 0, or sets that are all empty (n == 0) enqueue nothing and return GG_OK.  Rejected with
+ * nothing enqueued (the error text names the set):
+ *   GG_E_ARG   what gg_get_layers_to_device rejects for slots and names; null queries; an unknown mode; per set a null
+ *              data or dst with n > 0, n > INT32_MAX, a point_step that is not a multiple of 4 or below 8, offsets that
+ *              are negative, not multiples of 4 or do not fit point_step, a misaligned data / dst / cell; an output
+ *              range (dst, cell) overlapping the handle's layers, any set's positions or another output range (the
+ *              sets of different slots run concurrently)
+ *   GG_E_LAYER an unknown name, a GG_FLAG_FULL_LAYERS layer without the flag, "expectedPoints"
+ *   GG_E_STATE a slot whose map is not initialised */
+#define GG_SAMPLE_NEAREST 0
+#define GG_SAMPLE_LINEAR 1
+typedef struct gg_positions {
+    const void* data;
+    size_t n;
+    int point_step;
+    int off_x, off_y;
+    float* dst;
+    int32_t* cell;
+} gg_positions;
+int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const gg_positions* queries, int n_names, const char* const* names,
+                               int mode, void* stream);
+
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
  * touches a slot is enqueued on its stream.  gg_stream() is the primary stream;
