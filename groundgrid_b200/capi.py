@@ -157,6 +157,11 @@ POSITIONS_DTYPE = np.dtype({"names": ["data", "n", "point_step", "off_x", "off_y
                             "itemsize": C.sizeof(Positions)})
 SAMPLE_MODES = {"nearest": 0, "linear": 1}   # GG_SAMPLE_NEAREST, GG_SAMPLE_LINEAR
 
+# numpy image of an array of gg_point_info: device addresses of one slot's codes and heights (0 = none)
+POINT_INFO_DTYPE = np.dtype({"names": ["codes", "height"], "formats": [np.uint64, np.uint64], "offsets": [0, 8], "itemsize": 16})
+# per-point classes of gg_get_point_classes / gg_point_info_to_device (code >> 24)
+PC_ABSENT, PC_KEPT, PC_KEPT_BORDER, PC_IGNORED, PC_IGNORED_BORDER, PC_OUTLIER = range(6)
+
 # numpy image of an array of gg_scan_desc (ScanDesc)
 SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "n_points", "origin", "base_z"], "formats": [np.int32, np.uint64, (np.float32, 3), np.float64],
                             "offsets": [0, 8, 16, 32], "itemsize": C.sizeof(ScanDesc)})
@@ -246,6 +251,8 @@ def load(build_if_missing=True):
         "gg_eval_accumulate": (i, [vp, i]),
         "gg_eval_read": (i, [vp, vp, i]),
         "gg_eval_counts_to_device": (i, [vp, i, vp, vp, vp]),
+        "gg_point_info_to_device": (i, [vp, i, vp, vp, vp]),
+        "gg_last_scan_points": (i, [vp, i, C.POINTER(sz)]),
         "gg_profile_enable": (i, [vp, i]),
         "gg_profile_read": (i, [vp, vp, vp, i]),
         "gg_profile_kernel_count": (i, []),
@@ -909,6 +916,50 @@ class GroundGridB200:
         codes = np.zeros(n, np.uint32)
         _check(self._l.gg_get_point_classes(self._h, slot, _ptr(codes), n))
         return codes
+
+    def last_scan_points(self, slot=0):
+        """Points of the slot's last scan (gg_last_scan_points): the length of its point_info_to_device outputs."""
+        n = C.c_size_t(0)
+        _check(self._l.gg_last_scan_points(self._h, slot, C.byref(n)))
+        return n.value
+
+    def point_info_to_device_ptrs(self, slots, codes_ptrs, height_ptrs, stream_ptr):
+        """gg_point_info_to_device with raw device addresses: codes_ptrs / height_ptrs one address per slot (int; 0 or None
+        = none) or None for none at all; stream_ptr an int or None (None = the legacy default stream)."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        o = np.zeros(max(1, len(sl)), POINT_INFO_DTYPE)
+        for field, ptrs in (("codes", codes_ptrs), ("height", height_ptrs)):
+            if ptrs is not None:
+                o[field][:len(sl)] = [0 if p is None else int(p) for p in ptrs]
+        _check(self._l.gg_point_info_to_device(self._h, len(sl), _ptr(sl), _ptr(o), stream_ptr))
+
+    def point_info_to_device(self, slots, codes=True, height=True, out=None, stream=None):
+        """Per input point of each slot's last completed scan, its class code and height above the terrain
+        (gg_point_info_to_device).  Returns (codes, height): each a list of one CUDA tensor per slot of the scan's
+        n_points, or None when not asked for.
+          codes  : int32 tensors, class << 24 | cell (the bits of gg_get_point_classes; the class is codes >> 24, PC_*)
+          height : float32 tensors, z - ground[cell]; NaN for absent points
+          out    : None, or a pair (codes list or None, height list or None) of contiguous tensors to fill
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream); outputs are allocated on it.
+        The call returns without waiting for the device; work enqueued on `stream` afterwards sees the outputs."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        ns = [self.last_scan_points(int(s)) for s in slots]
+        result = []
+        for k, (want, dtype) in enumerate(((codes, torch.int32), (height, torch.float32))):
+            given = None if out is None else out[k]
+            if given is not None:
+                if len(given) != len(slots):
+                    raise ValueError("out needs one tensor per slot")
+                result.append([self._stream_out(torch, dev, current, stream, t, (n,), dtype, f"out[{k}][{j}]")
+                               for j, (t, n) in enumerate(zip(given, ns))])
+            elif want:
+                with torch.cuda.stream(stream):
+                    result.append(list(torch.split(torch.empty(sum(ns), dtype=dtype, device=dev), ns)))
+            else:
+                result.append(None)
+        ptrs = [None if r is None else [t.data_ptr() if n else 0 for t, n in zip(r, ns)] for r in result]
+        self.point_info_to_device_ptrs(slots, ptrs[0], ptrs[1], stream.cuda_stream or None)
+        return result[0], result[1]
 
     def detect_ground_patches(self, slot=0):
         _check(self._l.gg_detect_ground_patches(self._h, slot))

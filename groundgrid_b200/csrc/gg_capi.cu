@@ -281,6 +281,8 @@ struct SlotState {
     bool output_valid = false;
     const gg_point* src = nullptr;  // caller-owned device cloud of the last scan (null: the slot's own buffer)
     const float* packed_input = nullptr;  // last scan came through the packed host path (no 32-byte records on the device)
+    size_t scan_points = 0;    // points of the last scan (n_points may already count the next upload)
+    bool moved_since_scan = false;  // a roll shifted the cells after the last scan: its cell indices are stale
 };
 
 // A caller's device byte range [begin, end) of one query set: its positions (input) or one of its outputs.
@@ -317,6 +319,8 @@ struct gg_handle_s {
     gg::UnpackDesc* d_unpack = nullptr;
     gg::QueryDesc* h_query = nullptr;    // terrain lookups: query sets of the entry's slots, same shape as h_ring / d_ring
     gg::QueryDesc* d_query = nullptr;
+    gg::PointInfoDest* h_pinfo = nullptr;  // point classes and heights: destinations of the entry's slots, same shape
+    gg::PointInfoDest* d_pinfo = nullptr;  // (both allocated on first use)
     cudaEvent_t ring_ev[kRing] = {};
     cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
     cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
@@ -434,8 +438,8 @@ int layer_index(gg_handle h, int slot, const char* name, int* idx) {
 }
 
 // One entry of the parameter staging ring: the SlotParams of up to n_slots scans and, in arrays parallel to them, their
-// output destinations (OutDest), PointCloud2 payloads (UnpackDesc) and query sets (QueryDesc), each pinned on the host
-// with a device copy.
+// output destinations (OutDest), PointCloud2 payloads (UnpackDesc), query sets (QueryDesc) and point-info destinations
+// (PointInfoDest), each pinned on the host with a device copy.
 struct Staging {
     int pos = 0;                 // position in the ring
     int m = 0;                   // records filled
@@ -443,10 +447,12 @@ struct Staging {
     bool dests = false;          // commit also copies the OutDest records
     bool unpack = false;         // ... and the UnpackDesc records
     bool query = false;          // ... and the QueryDesc records
+    bool pinfo = false;          // ... and the PointInfoDest records
     gg::SlotParams *hp = nullptr, *dp = nullptr;
     gg::OutDest *hdest = nullptr, *ddest = nullptr;
     gg::UnpackDesc *hunpack = nullptr, *dunpack = nullptr;
     gg::QueryDesc *hquery = nullptr, *dquery = nullptr;
+    gg::PointInfoDest *hpinfo = nullptr, *dpinfo = nullptr;
 
     // Reserve the next entry (waits only if the ring wrapped onto an in-flight entry).
     int acquire(gg_handle h) {
@@ -462,6 +468,8 @@ struct Staging {
         dunpack = h->d_unpack + at;
         hquery = h->h_query + at;
         dquery = h->d_query + at;
+        hpinfo = h->h_pinfo ? h->h_pinfo + at : nullptr;   // allocated on the first gg_point_info_to_device
+        dpinfo = h->d_pinfo ? h->d_pinfo + at : nullptr;
         return GG_OK;
     }
     int commit(cudaStream_t st) const {
@@ -469,6 +477,7 @@ struct Staging {
         if (dests) GG_CUDA(cudaMemcpyAsync(ddest, hdest, (size_t)m * sizeof(gg::OutDest), cudaMemcpyHostToDevice, st));
         if (unpack) GG_CUDA(cudaMemcpyAsync(dunpack, hunpack, (size_t)m * sizeof(gg::UnpackDesc), cudaMemcpyHostToDevice, st));
         if (query) GG_CUDA(cudaMemcpyAsync(dquery, hquery, (size_t)m * sizeof(gg::QueryDesc), cudaMemcpyHostToDevice, st));
+        if (pinfo) GG_CUDA(cudaMemcpyAsync(dpinfo, hpinfo, (size_t)m * sizeof(gg::PointInfoDest), cudaMemcpyHostToDevice, st));
         return GG_OK;
     }
     // The entry may be reused once the kernels that read it have finished (they may run on any of the handle's streams,
@@ -717,6 +726,8 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         s.output_valid = false;
         s.src = dev_points ? dev_points[i] : nullptr;
         s.packed_input = packed;
+        s.scan_points = d.n_points;
+        s.moved_since_scan = false;
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) {
@@ -1072,6 +1083,7 @@ int gg_destroy(gg_handle h) {
     if (h->h_dest) cudaFreeHost(h->h_dest);
     if (h->h_unpack) cudaFreeHost(h->h_unpack);
     if (h->h_query) cudaFreeHost(h->h_query);
+    if (h->h_pinfo) cudaFreeHost(h->h_pinfo);
     for (int i = 0; i < kRing; ++i)
         if (h->ring_ev[i]) cudaEventDestroy(h->ring_ev[i]);
     if (h->own_streams)
@@ -1191,6 +1203,7 @@ int gg_update_pose_batch(gg_handle h, int count, const int* slots, const double*
         p.slot = slots[i];
         const bool mv = p.shift_i != 0 || p.shift_j != 0;   // else: "We havent moved so we have nothing to do", GroundGrid.cpp:136-137
         if (moved) moved[i] = mv ? 1 : 0;
+        if (mv) s.moved_since_scan = true;
         return mv;
     };
     return run_groups(h, count, slots, false, nullptr, fill,
@@ -1720,7 +1733,7 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
-                                           "k_sample_layers"};
+                                           "k_sample_layers", "k_point_info"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2339,6 +2352,74 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
         return gg::launch_sample(h->view, e.dp, e.dquery, e.m, e.max_points, list, mode, st, h->prof);
     };
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
+// Point classes and heights: one k_point_info per stream group with something to write.
+int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_point_info* outs, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0) return GG_OK;
+    if (!slots || !outs) return fail(GG_E_ARG, "null argument");
+    int rc;
+    if ((rc = check_slots(h, count, slots))) return rc;
+    const gg::View& v = h->view;
+    const void* arena = v.layers;
+    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    std::vector<ByteRange>& ranges = h->range_scratch;
+    ranges.clear();
+    for (int k = 0; k < count; ++k) {
+        const int slot = slots[k];
+        const SlotState& s = h->slots[slot];
+        if ((rc = check_completed_scan(h, slot))) return rc;
+        if (s.moved_since_scan) return fail(GG_E_STATE, "slot %d: the map moved since its last scan (the cell indices are stale)", slot);
+        const gg_point_info& o = outs[k];
+        if (reinterpret_cast<uintptr_t>(o.codes) % 4 || reinterpret_cast<uintptr_t>(o.height) % 4)
+            return fail(GG_E_ARG, "slot %d: codes or height is not 4-byte aligned", slot);
+        const size_t bytes = s.scan_points * sizeof(uint32_t);
+        for (const void* p : {static_cast<const void*>(o.codes), static_cast<const void*>(o.height)}) {
+            if (!p || !bytes) continue;
+            if (ranges_overlap(p, bytes, arena, arena_bytes)) return fail(GG_E_ARG, "slot %d: an output overlaps the handle's layers", slot);
+            ranges.push_back({reinterpret_cast<uintptr_t>(p), reinterpret_cast<uintptr_t>(p) + bytes, k, true});
+        }
+    }
+    // every range is an output: sorted by start, a range overlaps an earlier one iff it starts below their largest end
+    std::sort(ranges.begin(), ranges.end(), [](const ByteRange& a, const ByteRange& b) { return a.begin < b.begin; });
+    const ByteRange* far = nullptr;
+    for (const ByteRange& r : ranges) {
+        if (far && far->end > r.begin) return fail(GG_E_ARG, "an output of slot %d overlaps an output of slot %d", slots[r.set], slots[far->set]);
+        if (!far || r.end > far->end) far = &r;
+    }
+    if (ranges.empty()) return GG_OK;
+    GG_CUDA(cudaSetDevice(h->device));
+    // the staging of the destinations, parallel to the ring, on first use (a handle that never asks has none)
+    if (!h->d_pinfo && (rc = dev_alloc(h, &h->d_pinfo, (size_t)kRing * h->n_slots))) return rc;
+    if (!h->h_pinfo)
+        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * kRing * h->n_slots, cudaHostAllocDefault));
+    auto fill = [&](int i, Staging& e) {
+        const SlotState& s = h->slots[slots[i]];
+        const gg_point_info& o = outs[i];
+        const bool write = s.scan_points > 0 && (o.codes || o.height);
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        p.n_points = write ? (int)s.scan_points : 0;
+        gg::PointInfoDest& d = e.hpinfo[e.m];
+        d.codes = o.codes;
+        d.height = o.height;
+        e.pinfo = true;
+        return write;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_point_info(h->view, e.dp, e.dpinfo, e.m, e.max_points, st, h->prof); };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
+int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
+    int rc = check_slot(h, slot);
+    if (rc) return rc;
+    if (!n_points) return fail(GG_E_ARG, "null argument");
+    *n_points = h->slots[slot].scan_points;
+    return GG_OK;
 }
 
 }  // extern "C"

@@ -178,7 +178,7 @@ constexpr int OUT_TILE = 1024;
 // kernels of the pipeline, as reported by the profiling hooks (gg_profile_read)
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
-    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_NUM
+    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_NUM
 };
 
 // Optional per-kernel CUDA-event timing (bench.py's roofline needs the dominant kernel's own
@@ -265,5 +265,15 @@ struct QueryDesc {
 // and points_layer.  max_points: the largest n_points of the batch.
 int launch_sample(const View& v, const SlotParams* batch, const QueryDesc* descs, int count, int max_points, const LayerList& names, int mode,
                   cudaStream_t st, Profiler* prof);
+// Point classes and heights (gg_point_info_to_device): where one slot's results go.  It sits in the staging entry next
+// to the slots' SlotParams, in a parallel array with the same index (like OutDest).
+struct PointInfoDest {
+    uint32_t* codes;   // [n] class << 24 | cell; null: none
+    float* height;     // [n] z - ground[cell], NaN for absent points; null: none
+};
+// The codes and heights of the last scan of batch[k].slot into dests[k]; batch[k].n_points is that scan's point count
+// (0: nothing to write).  max_points: the largest n_points of the batch.
+int launch_point_info(const View& v, const SlotParams* batch, const PointInfoDest* dests, int count, int max_points, cudaStream_t st,
+                      Profiler* prof);
 
 }  // namespace gg

@@ -2205,6 +2205,50 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample_layers(View v, const 
     }
 }
 
+// Point classes and heights (gg_point_info_to_device).  Blocks (x, slot): every thread takes PINFO_ILP points of the
+// slot's last scan PINFO_THREADS apart (as k_label does), issues their code and z loads up front, then gathers "ground"
+// at each point's cell (N^2 floats per slot, L2-resident), then stores codes and heights coalesced.  Heights are
+// z - ground[cell] in fp32; an absent point has no cell and gets the quiet NaN 0x7fc00000.
+constexpr int PINFO_THREADS = 256, PINFO_ILP = 4;
+constexpr uint32_t PINFO_NAN = 0x7fc00000u;
+
+__global__ void __launch_bounds__(PINFO_THREADS) k_point_info(View v, const SlotParams* __restrict__ batch, const PointInfoDest* __restrict__ dests) {
+    const SlotParams& sp = batch[blockIdx.y];
+    const int n = sp.n_points;
+    const int i0 = blockIdx.x * (PINFO_THREADS * PINFO_ILP) + threadIdx.x;
+    if (i0 >= n) return;   // the grid covers the largest scan of the batch
+    const PointInfoDest d = dests[blockIdx.y];
+    const size_t base = (size_t)sp.slot * v.pcap;
+    const float* __restrict__ G = v.layer(sp.slot, L_GROUND);
+    uint32_t code[PINFO_ILP];
+    float z[PINFO_ILP];
+#pragma unroll
+    for (int u = 0; u < PINFO_ILP; ++u) {
+        const int i = i0 + u * PINFO_THREADS;
+        code[u] = i < n ? v.code[base + i] : (PC_ABSENT << 24);
+        z[u] = (i < n && d.height) ? __uint_as_float(v.zw[base + i].x) : 0.0f;
+    }
+    if (d.height) {
+        float g[PINFO_ILP];
+#pragma unroll
+        for (int u = 0; u < PINFO_ILP; ++u) g[u] = (code[u] >> 24) != PC_ABSENT ? G[code[u] & 0xffffffu] : 0.0f;
+#pragma unroll
+        for (int u = 0; u < PINFO_ILP; ++u) {
+            const int i = i0 + u * PINFO_THREADS;
+            if (i >= n) break;
+            d.height[i] = (code[u] >> 24) != PC_ABSENT ? __fsub_rn(z[u], g[u]) : __uint_as_float(PINFO_NAN);
+        }
+    }
+    if (d.codes) {
+#pragma unroll
+        for (int u = 0; u < PINFO_ILP; ++u) {
+            const int i = i0 + u * PINFO_THREADS;
+            if (i >= n) break;
+            d.codes[i] = code[u];
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
@@ -2481,6 +2525,12 @@ int launch_sample(const View& v, const SlotParams* batch, const QueryDesc* descs
     const long long blocks = ((long long)max_points + per_block - 1) / per_block;
     const unsigned nb = blocks > 0 ? (unsigned)blocks : 1u;
     GG_LAUNCH(K_SAMPLE, k_sample_layers<<<dim3(nb, count), SAMPLE_THREADS, 0, st>>>(v, batch, descs, names, mode));
+    return 1;
+}
+
+int launch_point_info(const View& v, const SlotParams* batch, const PointInfoDest* dests, int count, int max_points, cudaStream_t st,
+                      Profiler* prof) {
+    GG_LAUNCH(K_POINT_INFO, k_point_info<<<dim3(max(1, cdiv(max_points, PINFO_THREADS * PINFO_ILP)), count), PINFO_THREADS, 0, st>>>(v, batch, dests));
     return 1;
 }
 

@@ -407,6 +407,51 @@ int gg_eval_read(gg_handle h, uint64_t* counts, int reset);
  * _wait) first. */
 int gg_eval_counts_to_device(gg_handle h, int count, const int* slots, uint64_t* dev_counts, void* stream);
 
+/* Caller-owned DEVICE destinations of one slot of gg_point_info_to_device (on the handle's device; each may be NULL).
+ * n = the point count of the slot's last scan (gg_last_scan_points). */
+typedef struct gg_point_info {
+    uint32_t* codes;   /* [n], 4-byte aligned: class << 24 | cell, bit-identical to gg_get_point_classes */
+    float* height;     /* [n], 4-byte aligned: z - ground[cell] */
+} gg_point_info;
+
+/* Per-point class and height above the terrain of the last completed scan of `count` distinct slots, written into
+ * caller-owned device memory and ordered on the caller's stream: the batched, device-side form of gg_get_point_classes,
+ * plus the quantity the label rule compares against its tolerance (src/GroundSegmentation.cpp:171-173).
+ *   codes  : for every input point, in input order (for a merged scan: part order), the word gg_get_point_classes returns
+ *            for it at the same point of the slot's stream: class << 24 | cell with class 0 absent, 1 kept, 2 kept
+ *            (border cell), 3 ignored (ring > max_ring or near range), 4 ignored (border cell), 5 below-ground outlier
+ *            (labelled ground) -- the point_index / ignored / outliers lists of insert_cloud (:112-117)
+ *   height : for a point with a cell (classes 1-5), __fsub_rn(z, ground[cell]) in fp32, bit-identical to
+ *            np.float32(z) - np.float32(G[cell]).  z is the map-frame z the scan rasterized (after any unpack and
+ *            transform); G is the "ground" plane at the point of the slot's stream where the call runs: after the scan's
+ *            spiral, or what a later gg_set_layer[s_from_device] wrote.  Border and outlier points get heights too (an
+ *            outlier's is typically negative).  Absent points get the quiet NaN 0x7fc00000 (as gg_sample_layers_to_device
+ *            outside the map).
+ *   stream : cudaStream_t; NULL is the legacy default stream.  The contract of gg_get_layers_to_device: the work starts
+ *            after everything already enqueued on `stream` and on the stream group of every slot in the batch, work
+ *            enqueued on `stream` afterwards sees the outputs, and nothing waits on the host except the flow control of
+ *            the parameter staging ring.  The slot's next roll or scan, enqueued after the call, does not change them.
+ *            The first call on a handle also allocates the staging of the destinations (cudaMalloc, cudaHostAlloc).
+ * Nothing is read from the caller's cloud or payload: both values come from the handle's per-point state and layers.  So,
+ * unlike gg_eval_counts_to_device, the call works after gg_run_cloud_msgs_to_device, gg_run_merged_cloud_msgs_to_device
+ * or gg_run_scans_to_device with the input already freed, and after gg_filter_cloud_batch with host-packed clouds.
+ * count == 0, or a batch with nothing to write (every n == 0 or both pointers NULL), enqueues nothing and returns GG_OK.
+ * Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle, slots or outs; count > n_slots; a slot out of range or repeated; a misaligned output; an
+ *              output range overlapping the handle's layers or another output range of the call (the slots run
+ *              concurrently)
+ *   GG_E_STATE a slot whose map is not initialised, with no completed scan (none since gg_init_map, or the last one
+ *              stopped early), or whose map moved since that scan: a roll with a nonzero cell shift moves every cell
+ *              index, so the codes would no longer address the terrain the scan saw.  A roll that does not move is fine.
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_point_info* outs, void* stream);
+
+/* *n_points = the point count of the slot's last scan, completed or stopped early (0 before any scan since gg_init_map).
+ * An upload of the next cloud does not change it.  Host state: no device wait.  GG_E_ARG: null handle or n_points, slot
+ * out of range. */
+int gg_last_scan_points(gg_handle h, int slot, size_t* n_points);
+
 /* Per-kernel CUDA-event timing on the launching stream (bench.py roofline).  While enabled every
  * kernel launch is bracketed by an event pair; gg_profile_read synchronises and returns the
  * accumulated milliseconds and launch counts per kernel id (arrays of gg_profile_kernel_count()). */
