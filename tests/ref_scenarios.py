@@ -15,6 +15,7 @@ import os
 
 import numpy as np
 
+import cloud_orders as co
 from groundgrid_b200 import synth
 from groundgrid_b200.synth import base_from_map_qt, tf2_matrix
 
@@ -156,12 +157,12 @@ def push_below_ground(pts, count, seed):
     pts["z"][idx] -= rng.uniform(0.25, 2.0, count).astype(np.float32)
 
 
-def created(make, rec, dim, res, **cfg):
+def created(make, rec, dim, res, position=(0.0, 0.0), **cfg):
     m = make(dim, res)
     rec("cells", m.n)
     if cfg:
         m.set_config(**cfg)
-    m.init_map(0.0, 0.0, 0.0)
+    m.init_map(float(position[0]), float(position[1]), 0.0)
     for name in ("points", "ground", "groundpatch", "minGroundHeight", "maxGroundHeight"):
         rec(f"creation/{name}", m.layer(name))
     return m
@@ -372,6 +373,108 @@ def full_size_stream(make, rec, cfg):
         scan(m, rec, pts, org, 0.0, f"scan {k}", cloud=False)
 
 
+# ---- point orders, cell densities, non-finite heights, maps far from the origin (tests/cloud_orders.py) -----------------
+def input_orders(make, rec):
+    """Three scans on one 300 x 300 map, each in another point order (firing, shuffled, one point of a cell per warp), so
+    the prior is non-trivial and the order changes from scan to scan; the third with points pushed below the ground."""
+    m = created(make, rec, 99.0, 0.33)
+    scene = synth.make_scene(seed=2024)
+    for k, order in enumerate(("firing", "shuffled", "cell_round_robin")):
+        pts, org = synth.scan_64(scene, seed=2100 + k)
+        if k == 2:
+            push_below_ground(pts, 3000, 7)
+        pts, _ = co.reorder(order, pts, org, m.n, 0.33, seed=k)
+        scan(m, rec, pts, org, 0.0, f"scan {k} {order}")
+
+
+DENSE_GEOMETRY = {100: (33.0, 0.33), 101: (33.0, float(np.float32(33.0 / 101.0)))}
+
+
+def dense_cells(make, rec, n):
+    """Cells with a chosen number of runs (1 .. 120) and of points (1 .. 8 192) on an even and an odd map."""
+    dim, res = DENSE_GEOMETRY[n]
+    m = created(make, rec, dim, res)
+    assert m.n == n
+    for k, (pts, org, _) in enumerate((co.runs_ladder(n, res, seed=1), co.count_ladder(n, res, seed=2),
+                                       co.count_ladder(n, res, seed=3, scattered=True), co.runs_ladder(n, res, seed=4))):
+        scan(m, rec, pts, org, 0.0, f"scan {k}")
+
+
+def nonfinite_heights(make, rec):
+    """NaN, +inf and -inf heights at finite x, y: two scans (the second on the NaN-laden prior the first left), a roll,
+    and a finite scan on what remains."""
+    m = created(make, rec, 99.0, 0.33)
+    scene = synth.make_scene(seed=606)
+    for k in range(3):
+        ex, ey = (0.0, 0.0) if k < 2 else (1.7, -0.8)
+        pts, org = synth.scan_64(scene, (ex, ey), seed=610 + k)
+        if k < 2:
+            pts = co.nonfinite_heights(pts, seed=620 + k)
+        else:
+            q, t = base_from_map_qt(ex, ey, 0.0, 0.0, pitch=0.01)
+            assert update(m, rec, ex, ey, q, t, "roll") == 1
+        scan(m, rec, pts, org, 0.0, f"scan {k}")
+        if k == 0:
+            assert np.isnan(m.layer("ground")).sum() > 1000
+
+
+FAR_POSITIONS = {"1.2e5": (1.2e5 + 0.37, -3.4e5 - 0.11), "5.6e6": (4.1e5 - 0.21, 5.6e6 + 0.43)}
+
+
+def far_stream(where):
+    """The poses and clouds of far_from_origin: (k, ex, ey, yaw, base_z, (q, t), points, origin) per scan; scan 4 follows
+    a jump of more than the map's length."""
+    px, py = FAR_POSITIONS[where]
+    scene = co.far_scene((px, py), seed=31, undulation=0.2)
+    for k in range(5):
+        ex, ey, yaw = px + 0.9 * k, py - 0.7 * k, 0.02 * k
+        if k == 4:
+            ex, ey = px + 150.0, py - 120.0
+            scene = co.far_scene((ex, ey), seed=32)
+        pts, org = synth.scan_64(scene, (ex, ey), yaw, seed=3100 + k, az_steps=1024)
+        if k:
+            push_below_ground(pts, 800, 3200 + k)
+        yield k, ex, ey, yaw, 0.01 * k, base_from_map_qt(ex, ey, yaw, 0.01 * k, pitch=0.02), pts, org
+
+
+def far_from_origin(make, rec, where):
+    """A map created 1e5 .. 6e6 m from the origin, where float32 coordinates are 0.008 .. 0.5 m apart: five scans rolling
+    along a diagonal with yaw and a pitched base frame, the last after a jump that clears the map."""
+    m = created(make, rec, 99.0, 0.33, position=FAR_POSITIONS[where])
+    for k, ex, ey, yaw, base_z, (q, t), pts, org in far_stream(where):
+        if k:
+            assert update(m, rec, ex, ey, q, t, f"roll {k}") == 1
+        lab = scan(m, rec, pts, org, base_z, f"scan {k}")
+        assert (lab == 49).sum() > 20000 and (lab == 99).sum() > 2000
+
+
+def far_geometry(make, rec, where):
+    """grid_map's index and inside arithmetic at the cell edges of a far map and their float32 / float64 neighbours,
+    before and after a move."""
+    pos = FAR_POSITIONS[where]
+    m = created(make, rec, 33.0, 0.33, position=pos)
+    rng = np.random.default_rng(8)
+
+    def check(ctx):
+        c = m.position()
+        edge = np.array([m.cell_position(int(i), int(i)) for i in range(m.n)]) + 0.5 * float(np.float32(0.33))
+        idx = []
+        for ex, ey in edge[rng.permutation(m.n)[:40]]:
+            fx, fy = np.float32(ex), np.float32(ey)
+            for x, y in ((ex, ey), (np.nextafter(ex, np.inf), ey), (np.nextafter(ex, -np.inf), np.nextafter(ey, -np.inf)),
+                         (fx, fy), (np.nextafter(fx, np.float32(np.inf)), fy), (fx, np.nextafter(fy, np.float32(-np.inf))),
+                         (np.nextafter(fx, np.float32(-np.inf)), np.nextafter(fy, np.float32(np.inf)))):
+                i, j, inside = m.grid_index(float(x), float(y))
+                idx.append((int(inside), i if inside else 0, j if inside else 0))
+        rec(f"{ctx}/grid_index", np.array(idx, np.int64))
+        rec(f"{ctx}/centre", c)
+
+    check("created")
+    q, t = base_from_map_qt(pos[0] + 3.21, pos[1] - 1.77, 0.1, 0.0)
+    assert update(m, rec, pos[0] + 3.21, pos[1] - 1.77, q, t, "move", layers=()) == 1
+    check("moved")
+
+
 SCENARIOS = {
     "expected_points_table": (expected_points_table, [()]),
     "cfg1_cfg2_64_beam_300": (cfg1_cfg2_64_beam_300, [()]),
@@ -383,6 +486,11 @@ SCENARIOS = {
     "geometry_primitives_agree": (geometry_primitives_agree, [()]),
     "single_phase_calls_agree": (single_phase_calls_agree, [()]),
     "full_size_stream": (full_size_stream, [(c,) for c in FULL_SIZES]),
+    "input_orders": (input_orders, [()]),
+    "dense_cells": (dense_cells, [(n,) for n in DENSE_GEOMETRY]),
+    "nonfinite_heights": (nonfinite_heights, [()]),
+    "far_from_origin": (far_from_origin, [(w,) for w in FAR_POSITIONS]),
+    "far_geometry": (far_geometry, [(w,) for w in FAR_POSITIONS]),
 }
 
 

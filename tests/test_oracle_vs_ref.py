@@ -3,7 +3,8 @@ src/GroundSegmentation.cpp + GroundGrid.cpp of the reference compiled on CPU sta
 
 This is what pins the oracle: every layer, label, output position and map roll must agree bit for bit at
 thread_count = 1 on the BASELINE.json configurations (cfg1/2: 64 beams, 300x300; cfg3: 128 beams, 600x600;
-cfg4: four LiDARs ~480k points, 364x364), on rolling streams with outliers, and on random geometries / configs.
+cfg4: four LiDARs ~480k points, 364x364), on rolling streams with outliers, on random geometries / configs, and on
+re-ordered clouds, dense cells, non-finite heights and maps far from the origin (tests/cloud_orders.py).
 The reference's answers are stored as digests (tests/golden/ref_digests.json, tests/ref_scenarios.py), so these
 tests need no build of the reference.
 """
@@ -50,6 +51,29 @@ def test_geometry_primitives_agree():
 
 def test_single_phase_calls_agree():
     rs.run("single_phase_calls_agree", rs.Oracle)
+
+
+def test_input_orders():
+    rs.run("input_orders", rs.Oracle)
+
+
+@pytest.mark.parametrize("n", list(rs.DENSE_GEOMETRY))
+def test_dense_cells(n):
+    rs.run("dense_cells", rs.Oracle, n)
+
+
+def test_nonfinite_heights():
+    rs.run("nonfinite_heights", rs.Oracle)
+
+
+@pytest.mark.parametrize("where", list(rs.FAR_POSITIONS))
+def test_far_from_origin(where):
+    rs.run("far_from_origin", rs.Oracle, where)
+
+
+@pytest.mark.parametrize("where", list(rs.FAR_POSITIONS))
+def test_far_geometry(where):
+    rs.run("far_geometry", rs.Oracle, where)
 
 
 def test_reference_threading_as_shipped_runs():
