@@ -46,7 +46,7 @@ class Config(C.Structure):
 class ScanDesc(C.Structure):
     _fields_ = [
         ("slot", C.c_int),
-        ("_reserved", C.c_int),
+        ("flags", C.c_int),
         ("n_points", C.c_size_t),
         ("origin", C.c_float * 3),
         ("_pad", C.c_float),
@@ -163,8 +163,22 @@ POINT_INFO_DTYPE = np.dtype({"names": ["codes", "height"], "formats": [np.uint64
 PC_ABSENT, PC_KEPT, PC_KEPT_BORDER, PC_IGNORED, PC_IGNORED_BORDER, PC_OUTLIER = range(6)
 
 # numpy image of an array of gg_scan_desc (ScanDesc)
-SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "n_points", "origin", "base_z"], "formats": [np.int32, np.uint64, (np.float32, 3), np.float64],
-                            "offsets": [0, 8, 16, 32], "itemsize": C.sizeof(ScanDesc)})
+SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "flags", "n_points", "origin", "base_z"],
+                            "formats": [np.int32, np.int32, np.uint64, (np.float32, 3), np.float64],
+                            "offsets": [ScanDesc.slot.offset, ScanDesc.flags.offset, ScanDesc.n_points.offset, ScanDesc.origin.offset,
+                                        ScanDesc.base_z.offset], "itemsize": C.sizeof(ScanDesc)})
+SCAN_DEVICE_POSE = 1   # GG_SCAN_DEVICE_POSE: the scan's origin / base_z come from the slot's device scan pose
+
+
+class DevicePoses(C.Structure):
+    """gg_device_poses: device addresses of the per-slot pose arrays of gg_update_poses_from_device (None = not given)."""
+
+    _fields_ = [
+        ("xy", C.c_void_p),
+        ("T_base_from_map", C.c_void_p),
+        ("origin", C.c_void_p),
+        ("base_z", C.c_void_p),
+    ]
 
 
 class DeviceOutputs:
@@ -252,6 +266,7 @@ def load(build_if_missing=True):
         "gg_eval_read": (i, [vp, vp, i]),
         "gg_eval_counts_to_device": (i, [vp, i, vp, vp, vp]),
         "gg_point_info_to_device": (i, [vp, i, vp, vp, vp]),
+        "gg_update_poses_from_device": (i, [vp, i, vp, C.POINTER(DevicePoses), vp, vp]),
         "gg_last_scan_points": (i, [vp, i, C.POINTER(sz)]),
         "gg_profile_enable": (i, [vp, i]),
         "gg_profile_read": (i, [vp, vp, vp, i]),
@@ -279,6 +294,7 @@ def load(build_if_missing=True):
         "gg_host_expected_points": (i, [d, C.c_float, vp]),
         "gg_host_spiral_schedule": (i, [i, vp, i, vp, i, C.POINTER(i), C.POINTER(i)]),
         "gg_host_move_map": (i, [d, vp, d, d, vp]),
+        "gg_host_resolve_move": (i, [d, vp, d, d, vp]),
         "gg_host_geometry_constants": (i, [d, C.c_float, C.c_uint, vp]),
         "gg_host_config_constants": (i, [C.POINTER(Config), vp]),
         "gg_host_config_registry": (i, [i, i, vp, vp, vp]),
@@ -328,6 +344,15 @@ def host_move_map(res, pos_xy, new_xy):
     shift = np.zeros(2, np.int32)
     moved = load().gg_host_move_map(float(res), _ptr(pos), float(new_xy[0]), float(new_xy[1]), _ptr(shift))
     return bool(moved), pos, (int(shift[0]), int(shift[1]))
+
+
+def host_resolve_move(res, pos_xy, new_xy):
+    """The cell-shift resolve of gg_update_poses_from_device run on the host: (1 moved / 0 not / -1 invalid, new position,
+    shift).  An invalid pose (non-finite, or a shift outside int32) leaves the position and the zero shift untouched."""
+    pos = np.array(pos_xy, np.float64)
+    shift = np.zeros(2, np.int32)
+    status = load().gg_host_resolve_move(float(res), _ptr(pos), float(new_xy[0]), float(new_xy[1]), _ptr(shift))
+    return int(status), pos, (int(shift[0]), int(shift[1]))
 
 
 GEOMETRY_CONSTANTS = ("N", "N2", "full_layers", "res_f", "res", "rres", "len", "half", "res_sq")
@@ -436,6 +461,47 @@ class GroundGridB200:
         moved = np.zeros(len(slots), np.int32)
         _check(self._l.gg_update_pose_batch(self._h, len(slots), _ptr(slots), _ptr(xy), _ptr(T), _ptr(moved)))
         return moved.astype(bool)
+
+    def update_poses_from_device_ptrs(self, slots, xy_ptr, T_ptr, origin_ptr, base_z_ptr, moved_ptr, stream_ptr):
+        """gg_update_poses_from_device with raw device addresses (ints, or None for NULL); stream_ptr None = the legacy
+        default stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        p = DevicePoses(xy_ptr, T_ptr, origin_ptr, base_z_ptr)
+        _check(self._l.gg_update_poses_from_device(self._h, len(sl), _ptr(sl), C.byref(p), moved_ptr, stream_ptr))
+
+    def update_poses_from_device(self, slots, xy=None, T=None, origins=None, base_z=None, moved=False, stream=None):
+        """Rolls and / or scan poses of `slots` from CUDA tensors, resolved on the device (gg_update_poses_from_device).
+          xy      : float64 [count, 2] odometry positions, with T float64 [count, 3, 4] (or [count, 12]) of
+                    lookupTransform("base_link", "map"): rolls bit-identical to update_pose_batch
+          origins : float32 [count, 3] cloudOrigin, with base_z float64 [count]: the scan pose that scans run with
+                    origins="device" use
+          moved   : also return an int32 [count] tensor: 1 the cells shifted, 0 not, -1 invalid pose (map untouched)
+          stream  : torch.cuda.Stream the work is ordered on (default: the current stream); `moved` is allocated on it.
+        Every tensor must be contiguous on this handle's device.  The call returns without waiting for the device; the
+        pose tensors may be freed or refilled right after it when they belong to `stream` (others are marked in use on
+        `stream`).  Afterwards the slots' map positions live on the device: position() and the other host calls that
+        need them wait for the slots' work first."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count = len(slots)
+        want = {"xy": (xy, torch.float64, (count, 2)), "T": (T, torch.float64, (count, 12)), "origins": (origins, torch.float32, (count, 3)),
+                "base_z": (base_z, torch.float64, (count,))}
+        ptrs = {}
+        for name, (t, dtype, shape) in want.items():
+            if t is None:
+                ptrs[name] = None
+                continue
+            if t.dtype != dtype or t.device != dev or not t.is_contiguous() or t.numel() != int(np.prod(shape)) or t.shape[0] != count:
+                raise ValueError(f"{name} must be a contiguous {dtype} tensor {shape} on {dev}")
+            if stream != current:
+                t.record_stream(stream)
+            ptrs[name] = t.data_ptr() if count else None
+        out = None
+        if moved:
+            with torch.cuda.stream(stream):
+                out = torch.empty(count, dtype=torch.int32, device=dev)
+        self.update_poses_from_device_ptrs(slots, ptrs["xy"], ptrs["T"], ptrs["origins"], ptrs["base_z"],
+                                           out.data_ptr() if out is not None and count else None, stream.cuda_stream or None)
+        return out
 
     def position(self, slot=0):
         xy = np.zeros(2, np.float64)
@@ -686,10 +752,15 @@ class GroundGridB200:
 
     @staticmethod
     def make_descs(slots, n_points, origins, base_z):
+        """ScanDesc array; origins="device" flags every scan GG_SCAN_DEVICE_POSE (base_z is then ignored)."""
         arr = (ScanDesc * len(slots))()
+        device = isinstance(origins, str) and origins == "device"
         for k, s in enumerate(slots):
             arr[k].slot = int(s)
             arr[k].n_points = int(n_points[k])
+            if device:
+                arr[k].flags = SCAN_DEVICE_POSE
+                continue
             arr[k].origin[0], arr[k].origin[1], arr[k].origin[2] = [float(v) for v in origins[k]]
             arr[k].base_z = float(base_z[k])
         return arr
@@ -715,7 +786,8 @@ class GroundGridB200:
     def run_scans_to_device(self, clouds, slots, origins, base_z, labels=True, select="nonground", index=False, stream=None):
         """One scan per slot on caller-owned CUDA tensors, results left in new CUDA tensors (gg_run_scans_to_device).
           clouds : contiguous CUDA tensors of 32-byte point records (e.g. float32 [n, 8] or uint8 [n * 32]), 16-byte aligned
-          origins: [count][3] sensor positions in the map frame; base_z: one value or one per scan
+          origins: [count][3] sensor positions in the map frame; base_z: one value or one per scan.  origins="device"
+                   (base_z unused): every scan takes the slot's latest device scan pose (update_poses_from_device)
           select : labels of the output cloud to return: "nonground" (the obstacle points), "ground", "all" (what get_output
                    returns) or None (no cloud)
           index  : also return the input index of each returned point
@@ -849,6 +921,9 @@ class GroundGridB200:
         descs = np.zeros(count, SCAN_DESC_DTYPE)
         descs["slot"] = np.asarray(slots, np.int32)
         descs["n_points"] = n
+        if isinstance(origins, str) and origins == "device":   # the slots' device scan poses (update_poses_from_device)
+            descs["flags"] = SCAN_DEVICE_POSE
+            return descs
         descs["origin"] = np.asarray(origins, np.float32).reshape(count, 3)
         descs["base_z"] = np.broadcast_to(np.asarray(base_z, np.float64), (count,))
         return descs

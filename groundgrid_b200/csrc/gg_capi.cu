@@ -283,6 +283,10 @@ struct SlotState {
     const float* packed_input = nullptr;  // last scan came through the packed host path (no 32-byte records on the device)
     size_t scan_points = 0;    // points of the last scan (n_points may already count the next upload)
     bool moved_since_scan = false;  // a roll shifted the cells after the last scan: its cell indices are stale
+    // gg_update_poses_from_device
+    bool device_position = false;   // px / py are stale: the position lives in the device table (PoseTables::position)
+    bool device_scan_pose = false;  // the device holds a scan pose of the slot (flagged scans may run)
+    bool device_rolled = false;     // a device roll since the last scan (it may have moved the cells)
 };
 
 // A caller's device byte range [begin, end) of one query set: its positions (input) or one of its outputs.
@@ -321,6 +325,9 @@ struct gg_handle_s {
     gg::QueryDesc* d_query = nullptr;
     gg::PointInfoDest* h_pinfo = nullptr;  // point classes and heights: destinations of the entry's slots, same shape
     gg::PointInfoDest* d_pinfo = nullptr;  // (both allocated on first use)
+    int* h_pose_bits = nullptr;            // gg::PoseBits of the entry's records, same shape (allocated with `poses`)
+    int* d_pose_bits = nullptr;
+    gg::PoseTables poses{};                // per-slot device positions and scan poses (first gg_update_poses_from_device)
     cudaEvent_t ring_ev[kRing] = {};
     cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
     cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
@@ -448,11 +455,15 @@ struct Staging {
     bool unpack = false;         // ... and the UnpackDesc records
     bool query = false;          // ... and the QueryDesc records
     bool pinfo = false;          // ... and the PointInfoDest records
+    bool pose_bits = false;      // ... and the PoseBits of the records
+    bool position = false;       // fill staged slot positions (run_groups then patches device-owned ones on the device)
+    bool stage = false;          // some record takes its position or scan pose from the device tables (k_stage_poses)
     gg::SlotParams *hp = nullptr, *dp = nullptr;
     gg::OutDest *hdest = nullptr, *ddest = nullptr;
     gg::UnpackDesc *hunpack = nullptr, *dunpack = nullptr;
     gg::QueryDesc *hquery = nullptr, *dquery = nullptr;
     gg::PointInfoDest *hpinfo = nullptr, *dpinfo = nullptr;
+    int *hbits = nullptr, *dbits = nullptr;
 
     // Reserve the next entry (waits only if the ring wrapped onto an in-flight entry).
     int acquire(gg_handle h) {
@@ -470,6 +481,8 @@ struct Staging {
         dquery = h->d_query + at;
         hpinfo = h->h_pinfo ? h->h_pinfo + at : nullptr;   // allocated on the first gg_point_info_to_device
         dpinfo = h->d_pinfo ? h->d_pinfo + at : nullptr;
+        hbits = h->h_pose_bits ? h->h_pose_bits + at : nullptr;   // allocated on the first gg_update_poses_from_device
+        dbits = h->d_pose_bits ? h->d_pose_bits + at : nullptr;
         return GG_OK;
     }
     int commit(cudaStream_t st) const {
@@ -478,6 +491,7 @@ struct Staging {
         if (unpack) GG_CUDA(cudaMemcpyAsync(dunpack, hunpack, (size_t)m * sizeof(gg::UnpackDesc), cudaMemcpyHostToDevice, st));
         if (query) GG_CUDA(cudaMemcpyAsync(dquery, hquery, (size_t)m * sizeof(gg::QueryDesc), cudaMemcpyHostToDevice, st));
         if (pinfo) GG_CUDA(cudaMemcpyAsync(dpinfo, hpinfo, (size_t)m * sizeof(gg::PointInfoDest), cudaMemcpyHostToDevice, st));
+        if (pose_bits) GG_CUDA(cudaMemcpyAsync(dbits, hbits, (size_t)m * sizeof(int), cudaMemcpyHostToDevice, st));
         return GG_OK;
     }
     // The entry may be reused once the kernels that read it have finished (they may run on any of the handle's streams,
@@ -539,6 +553,8 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
         if (seen[slot]++) return fail(GG_E_ARG, "slot %d appears twice in one batch (scans of a batch run concurrently)", slot);
         if (!h->slots[slot].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slot);
         if (!slots.scans) continue;
+        if ((slots.scans[i].flags & GG_SCAN_DEVICE_POSE) && !h->slots[slot].device_scan_pose)
+            return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_POSE without a device scan pose since gg_init_map", slot);
         const size_t n = slots.scans[i].n_points;
         if (n > h->pcap) return fail(GG_E_ARG, "slot %d: %zu points exceed capacity %zu", slot, n, h->pcap);
         if (clouds && n && !clouds[i]) return fail(GG_E_ARG, "scan %d: null cloud", i);
@@ -553,6 +569,9 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
 // release of the entry.  A group whose records need nothing (a roll that moves no slot) only takes and releases its
 // entry.  With `fenced`, the groups start after everything enqueued on `caller` so far, and `caller` waits for them: no
 // host wait but the flow control of the staging ring.
+// Poses: when fill staged slot positions (e.position), a record of a slot whose position is device-owned, or of a scan
+// flagged GG_SCAN_DEVICE_POSE, is patched from the device tables by k_stage_poses right after the copy.  Without such
+// records (every all-host flow) nothing more is copied or launched.
 template <typename Fill, typename Launch>
 int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t caller, Fill&& fill, Launch&& launch) {
     int rc;
@@ -564,6 +583,12 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
             if (stream_index(h, slots[i]) != g) continue;
             if (e.m == 0 && (rc = e.acquire(h))) return rc;
             work |= fill(i, e);
+            if (e.position && e.hbits) {
+                int bits = h->slots[slots[i]].device_position ? gg::POSE_POSITION : 0;
+                if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_POSE)) bits |= gg::POSE_ORIGIN;
+                e.hbits[e.m] = bits;
+                if (bits) e.stage = e.pose_bits = true;
+            }
             e.max_points = std::max(e.max_points, e.hp[e.m].n_points);
             ++e.m;
         }
@@ -571,6 +596,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
         cudaStream_t st = h->streams[g];
         if (work) {
             if ((rc = e.commit(st))) return rc;
+            if (e.stage) h->launches += gg::launch_stage_poses(h->poses, e.dp, e.dbits, e.m, st, h->prof);
             if (fenced) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
             const int n = launch(e, st);
             if (n < 0) return n;
@@ -699,6 +725,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         const gg_scan_desc& d = scans[i];
         const float* packed = packed_ptrs ? packed_ptrs[i] : nullptr;
         fill_params(h, d, e.hp[e.m], dev_points ? dev_points[i] : nullptr, packed);
+        e.position = true;
         if (caller) {
             if (e.m == 0) write = false;
             gg::OutDest& od = e.hdest[e.m];
@@ -728,6 +755,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         s.packed_input = packed;
         s.scan_points = d.n_points;
         s.moved_since_scan = false;
+        s.device_rolled = false;
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) {
@@ -843,9 +871,26 @@ int run_phase(gg_handle h, int slot, double base_z, Launch&& launch) {
         d.n_points = h->slots[slot].n_points;
         d.base_z = base_z;
         fill_params(h, d, e.hp[0], h->slots[slot].src);
+        e.position = true;
         return true;
     };
     return run_groups(h, 1, &slot, false, nullptr, fill, launch);
+}
+
+// A call that needs the map position on the host: a device-owned position is read back once the slot's stream group
+// has finished what is enqueued (a host wait), and the slot is host-owned again.
+int take_position_back(gg_handle h, int slot) {
+    SlotState& s = h->slots[slot];
+    if (!s.device_position) return GG_OK;
+    GG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream_of(h, slot);
+    double2 p;
+    GG_CUDA(cudaMemcpyAsync(&p, h->poses.position + slot, sizeof(p), cudaMemcpyDeviceToHost, st));
+    GG_CUDA(cudaStreamSynchronize(st));
+    s.px = p.x;
+    s.py = p.y;
+    s.device_position = false;
+    return GG_OK;
 }
 
 }  // namespace
@@ -1084,6 +1129,7 @@ int gg_destroy(gg_handle h) {
     if (h->h_unpack) cudaFreeHost(h->h_unpack);
     if (h->h_query) cudaFreeHost(h->h_query);
     if (h->h_pinfo) cudaFreeHost(h->h_pinfo);
+    if (h->h_pose_bits) cudaFreeHost(h->h_pose_bits);
     for (int i = 0; i < kRing; ++i)
         if (h->ring_ev[i]) cudaEventDestroy(h->ring_ev[i]);
     if (h->own_streams)
@@ -1171,6 +1217,7 @@ int gg_get_slot_config(gg_handle h, int slot, gg_config* cfg) {
 int gg_init_map(gg_handle h, int slot, double x, double y, double z) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
+    if ((rc = take_position_back(h, slot))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     SlotState& s = h->slots[slot];
     s = SlotState();
@@ -1187,6 +1234,8 @@ int gg_update_pose_batch(gg_handle h, int count, const int* slots, const double*
     if (count <= 0) return GG_OK;
     int rc;
     if ((rc = check_slots(h, count, slots))) return rc;
+    for (int i = 0; i < count; ++i)
+        if ((rc = take_position_back(h, slots[i]))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     auto fill = [&](int i, Staging& e) {
         SlotState& s = h->slots[slots[i]];
@@ -1219,6 +1268,7 @@ int gg_get_map_position(gg_handle h, int slot, double xy[2]) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (!xy) return fail(GG_E_ARG, "null argument");
+    if ((rc = take_position_back(h, slot))) return rc;
     xy[0] = h->slots[slot].px;
     xy[1] = h->slots[slot].py;
     return GG_OK;
@@ -1227,6 +1277,7 @@ int gg_get_map_position(gg_handle h, int slot, double xy[2]) {
 int gg_set_map_position(gg_handle h, int slot, double x, double y) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
+    if ((rc = take_position_back(h, slot))) return rc;
     h->slots[slot].px = x;
     h->slots[slot].py = y;
     return GG_OK;
@@ -1733,7 +1784,7 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
-                                           "k_sample_layers", "k_point_info"};
+                                           "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2336,6 +2387,7 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
         p.points_layer = points_layer(h, slots[i]);
         p.px = s.px;
         p.py = s.py;
+        e.position = true;
         p.n_points = (int)q.n;
         gg::QueryDesc& d = e.hquery[e.m];
         std::memset(&d, 0, sizeof(d));
@@ -2372,6 +2424,8 @@ int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_p
         const SlotState& s = h->slots[slot];
         if ((rc = check_completed_scan(h, slot))) return rc;
         if (s.moved_since_scan) return fail(GG_E_STATE, "slot %d: the map moved since its last scan (the cell indices are stale)", slot);
+        if (s.device_rolled)
+            return fail(GG_E_STATE, "slot %d: a device roll since its last scan may have moved the map (the cell indices may be stale)", slot);
         const gg_point_info& o = outs[k];
         if (reinterpret_cast<uintptr_t>(o.codes) % 4 || reinterpret_cast<uintptr_t>(o.height) % 4)
             return fail(GG_E_ARG, "slot %d: codes or height is not 4-byte aligned", slot);
@@ -2411,6 +2465,60 @@ int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_p
         return write;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_point_info(h->view, e.dp, e.dpinfo, e.m, e.max_points, st, h->prof); };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
+// Poses from device memory: per stream group one k_pose_resolve over the group's slots, then (with xy) the roll kernels
+// on the same staging entry.
+int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const gg_device_poses* poses, int32_t* dev_moved, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0) return GG_OK;
+    if (!slots || !poses) return fail(GG_E_ARG, "null argument");
+    int rc;
+    if ((rc = check_slots(h, count, slots))) return rc;
+    const gg_device_poses& in = *poses;
+    if (!in.xy != !in.T_base_from_map) return fail(GG_E_ARG, "xy and T_base_from_map must both be given or both be NULL");
+    if (!in.origin != !in.base_z) return fail(GG_E_ARG, "origin and base_z must both be given or both be NULL");
+    auto misaligned = [](const void* p, size_t a) { return reinterpret_cast<uintptr_t>(p) % a != 0; };
+    if (misaligned(in.xy, 8) || misaligned(in.T_base_from_map, 8) || misaligned(in.base_z, 8))
+        return fail(GG_E_ARG, "xy, T_base_from_map or base_z is not 8-byte aligned");
+    if (misaligned(in.origin, 4) || misaligned(dev_moved, 4)) return fail(GG_E_ARG, "origin or dev_moved is not 4-byte aligned");
+    const size_t n = (size_t)count, moved_bytes = n * sizeof(int32_t);
+    const gg::View& v = h->view;
+    if (ranges_overlap(dev_moved, moved_bytes, v.layers, (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float)))
+        return fail(GG_E_ARG, "dev_moved overlaps the handle's layers");
+    if (ranges_overlap(dev_moved, moved_bytes, in.xy, n * 2 * sizeof(double)) || ranges_overlap(dev_moved, moved_bytes, in.T_base_from_map, n * 12 * sizeof(double)) ||
+        ranges_overlap(dev_moved, moved_bytes, in.origin, n * 3 * sizeof(float)) || ranges_overlap(dev_moved, moved_bytes, in.base_z, n * sizeof(double)))
+        return fail(GG_E_ARG, "dev_moved overlaps the poses");
+    if (!in.xy && !in.origin) return GG_OK;
+    GG_CUDA(cudaSetDevice(h->device));
+    // the device tables and the staging of the pose bits, on first use (a handle that never asks has none)
+    const size_t S = (size_t)h->n_slots;
+    if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
+    if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
+    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
+    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    const gg::DevicePoses dp{in.xy, in.T_base_from_map, in.origin, in.base_z, dev_moved};
+    auto fill = [&](int i, Staging& e) {
+        SlotState& s = h->slots[slots[i]];
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        p.px = s.px;   // the position k_pose_resolve starts from, unless the device table holds it
+        p.py = s.py;
+        e.hbits[e.m] = s.device_position ? gg::POSE_POSITION : 0;
+        e.pose_bits = true;
+        if (in.xy) s.device_position = s.device_rolled = true;
+        if (in.origin) s.device_scan_pose = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) {
+        int launched = gg::launch_pose_resolve(h->view, h->poses, e.dp, e.dbits, e.m, dp, st, h->prof);
+        if (in.xy) launched += gg::launch_roll(h->view, e.dp, e.m, st, h->prof);
+        return launched;
+    };
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 

@@ -798,6 +798,11 @@ int gg_host_move_map(double res, double* pos_xy, double nx, double ny, int* shif
     return (shift_ij[0] != 0 || shift_ij[1] != 0) ? 1 : 0;
 }
 
+// the resolve of k_pose_resolve (gg_internal.h:resolve_move) on the host: 1 moved, 0 not, -1 invalid (nothing written)
+int gg_host_resolve_move(double res, double* pos_xy, double nx, double ny, int* shift_ij) {
+    return gg::resolve_move(res, pos_xy[0], pos_xy[1], nx, ny, shift_ij[0], shift_ij[1]);
+}
+
 // out[9]: N, N2, full_layers, res_f, res, rres, len, half, res_sq
 int gg_host_geometry_constants(double dimension_m, float resolution, unsigned flags, double* out) {
     gg::Const k;

@@ -95,6 +95,7 @@ int gg_host_expected_points(double dimension_m, float resolution, float* dst);
 int gg_host_spiral_schedule(int n, int* level_start, int level_cap, uint32_t* visits, int visit_cap, int* n_levels, int* n_visits);
 int gg_host_spiral_records(int n, float resolution, int dist, uint32_t* recs, int rec_cap_words, int* max_recent);
 int gg_host_move_map(double res, double* pos_xy, double nx, double ny, int* shift_ij);
+int gg_host_resolve_move(double res, double* pos_xy, double nx, double ny, int* shift_ij);
 int gg_host_geometry_constants(double dimension_m, float resolution, unsigned flags, double* out);
 int gg_host_config_constants(const gg_config* cfg, double* out);
 int gg_host_config_registry(int n_slots, int n_ops, const int* op_slot, const gg_config* op_cfg, int* out);

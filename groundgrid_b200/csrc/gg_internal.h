@@ -178,7 +178,8 @@ constexpr int OUT_TILE = 1024;
 // kernels of the pipeline, as reported by the profiling hooks (gg_profile_read)
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
-    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_NUM
+    K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_STAGE_POSES, K_POSE_RESOLVE,
+    K_NUM
 };
 
 // Optional per-kernel CUDA-event timing (bench.py's roofline needs the dominant kernel's own
@@ -275,5 +276,82 @@ struct PointInfoDest {
 // (0: nothing to write).  max_points: the largest n_points of the batch.
 int launch_point_info(const View& v, const SlotParams* batch, const PointInfoDest* dests, int count, int max_points, cudaStream_t st,
                       Profiler* prof);
+
+// ---- poses from device memory (gg_update_poses_from_device) ----
+// fp64 arithmetic, correctly rounded and never contracted, on the host and on the device
+__host__ __device__ __forceinline__ double pose_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ double pose_sub(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ double pose_mul(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ double pose_div(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __ddiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+
+// gg_host.cpp:move_map for one position, for a roll resolved on the device: the whole-cell shift toward (nx, ny),
+// rounded half away from zero, and the map position advanced by it.  Returns 1 (the cells shift), 0 (no shift) or -1:
+// a non-finite quotient or a shift outside int32 (move_map's int conversion is undefined there), which leaves px, py
+// and the shift untouched.
+__host__ __device__ __forceinline__ int resolve_move(double res, double& px, double& py, double nx, double ny, int& shift_i, int& shift_j) {
+    const double tx = pose_div(pose_sub(nx, px), res), ty = pose_div(pose_sub(ny, py), res);
+    const double rx = pose_add(tx, tx > 0 ? 0.5 : -0.5), ry = pose_add(ty, ty > 0 ? 0.5 : -0.5);
+    // truncation toward zero lands in (-2^31, 2^31) and -cx fits as well; NaN fails every comparison
+    if (!(rx > -2147483648.0 && rx < 2147483648.0 && ry > -2147483648.0 && ry < 2147483648.0)) return -1;
+    const int cx = (int)rx, cy = (int)ry;
+    shift_i = -cx;
+    shift_j = -cy;
+    px = pose_add(px, pose_mul((double)cx, res));
+    py = pose_add(py, pose_mul((double)cy, res));
+    return (cx != 0 || cy != 0) ? 1 : 0;
+}
+
+// Per-record bits of a staging entry (PoseBits[m] next to its SlotParams): where k_stage_poses takes the record's
+// pose from.
+enum PoseBits : int {
+    POSE_POSITION = 1,   // px / py from the slot's entry of the device position table (the position is device-owned)
+    POSE_ORIGIN = 2,     // ox / oy / oz / base_z_f from the slot's device scan pose (GG_SCAN_DEVICE_POSE)
+};
+// The handle's per-slot device tables (allocated on the first gg_update_poses_from_device).
+struct PoseTables {
+    double2* position;   // [n_slots] map position of a device-owned slot
+    float4* scan_pose;   // [n_slots] origin x, y, z and (float)base_z
+};
+// Patches the `count` records of batch whose bits ask for it from the tables; runs after the entry's copy and before
+// the kernels that read it.
+int launch_stage_poses(const PoseTables& t, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof);
+// The poses of one gg_update_poses_from_device call (entry batch[j].pos of each array); null xy: no roll, null origin:
+// no scan pose.
+struct DevicePoses {
+    const double* xy;
+    const double* T;
+    const float* origin;
+    const double* base_z;
+    int32_t* moved;
+};
+// One thread per record: resolves the roll of batch[j] from its staged position (bits POSE_POSITION: the device table's),
+// writes shift_i / shift_j, px / py and t20..t23 into the record for launch_roll, the new position into the table and
+// moved[pos]; stores the scan pose.
+int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, const int* bits, int count, const DevicePoses& in, cudaStream_t st,
+                        Profiler* prof);
 
 }  // namespace gg

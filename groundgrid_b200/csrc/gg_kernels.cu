@@ -2249,6 +2249,68 @@ __global__ void __launch_bounds__(PINFO_THREADS) k_point_info(View v, const Slot
     }
 }
 
+// Poses from device memory (gg_update_poses_from_device).  One thread per staged record; both kernels are tiny and
+// exist to keep the host out of the loop, not for throughput.
+constexpr int POSE_THREADS = 128;
+
+// A staging entry's records take the slot's device-owned position and / or its device scan pose, after the entry's
+// copy and before the kernels that read them (the same stream).
+__global__ void __launch_bounds__(POSE_THREADS) k_stage_poses(PoseTables t, SlotParams* __restrict__ batch, const int* __restrict__ bits, int count) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count) return;
+    const int b = bits[j];
+    if (!b) return;
+    SlotParams& p = batch[j];
+    if (b & POSE_POSITION) {
+        const double2 q = t.position[p.slot];
+        p.px = q.x;
+        p.py = q.y;
+    }
+    if (b & POSE_ORIGIN) {
+        const float4 o = t.scan_pose[p.slot];
+        p.ox = o.x;
+        p.oy = o.y;
+        p.oz = o.z;
+        p.base_z_f = o.w;
+    }
+}
+
+// GroundGrid::update's pose step for record j of a roll entry: the cell shift from the caller's odometry position
+// (resolve_move, the arithmetic of gg_host.cpp:move_map), the seed row of T_base_from_map, the new position; then
+// k_roll_gather / k_roll_commit run on the same records.  A record whose pose is invalid keeps shift 0: the roll
+// kernels skip it.  The scan pose is stored as fill_params stages a host one: (float)base_z.
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_resolve(double res, PoseTables t, SlotParams* __restrict__ batch, const int* __restrict__ bits,
+                                                               int count, DevicePoses in) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count) return;
+    SlotParams& p = batch[j];
+    const int s = p.slot;
+    const size_t k = (size_t)p.pos;
+    int moved = 0;
+    if (in.xy) {
+        double px = p.px, py = p.py;
+        if (bits[j] & POSE_POSITION) {
+            const double2 q = t.position[s];
+            px = q.x;
+            py = q.y;
+        }
+        int si = 0, sj = 0;
+        moved = resolve_move(res, px, py, in.xy[2 * k], in.xy[2 * k + 1], si, sj);
+        p.shift_i = si;
+        p.shift_j = sj;
+        p.px = px;
+        p.py = py;
+        const double* T = in.T + 12 * k;
+        p.t20 = T[8];
+        p.t21 = T[9];
+        p.t22 = T[10];
+        p.t23 = T[11];
+        t.position[s] = make_double2(px, py);
+    }
+    if (in.origin) t.scan_pose[s] = make_float4(in.origin[3 * k], in.origin[3 * k + 1], in.origin[3 * k + 2], (float)in.base_z[k]);
+    if (in.moved) in.moved[k] = moved;
+}
+
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
@@ -2531,6 +2593,17 @@ int launch_sample(const View& v, const SlotParams* batch, const QueryDesc* descs
 int launch_point_info(const View& v, const SlotParams* batch, const PointInfoDest* dests, int count, int max_points, cudaStream_t st,
                       Profiler* prof) {
     GG_LAUNCH(K_POINT_INFO, k_point_info<<<dim3(max(1, cdiv(max_points, PINFO_THREADS * PINFO_ILP)), count), PINFO_THREADS, 0, st>>>(v, batch, dests));
+    return 1;
+}
+
+int launch_stage_poses(const PoseTables& t, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_STAGE_POSES, k_stage_poses<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(t, batch, bits, count));
+    return 1;
+}
+
+int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, const int* bits, int count, const DevicePoses& in, cudaStream_t st,
+                        Profiler* prof) {
+    GG_LAUNCH(K_POSE_RESOLVE, k_pose_resolve<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(v.k.res, t, batch, bits, count, in));
     return 1;
 }
 
