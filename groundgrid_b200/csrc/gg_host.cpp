@@ -793,6 +793,20 @@ int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* 
     return 1;
 }
 
+// the confidence decay of every spiral path (gg_internal.h:decay_confidence) for the configuration cfg, on the host
+int gg_host_decay_confidence(const gg_config* cfg, const float* occ, size_t n, float* out) {
+    gg::CfgConst k;
+    gg::derive_config(*cfg, k);
+    for (size_t i = 0; i < n; ++i) out[i] = gg::decay_confidence(k, occ[i]);
+    return 0;
+}
+
+// the confidence a visit of k_spiral_skew leaves: its SD entry d, or the visited cell's own occ where d is SKEW_NEAR
+int gg_host_skew_visit_confidence(const float* d, const float* occ, size_t n, float* out) {
+    for (size_t i = 0; i < n; ++i) out[i] = gg::skew_decays(d[i]) ? d[i] : occ[i];
+    return 0;
+}
+
 int gg_host_move_map(double res, double* pos_xy, double nx, double ny, int* shift_ij) {
     gg::move_map(res, pos_xy[0], pos_xy[1], nx, ny, shift_ij[0], shift_ij[1]);
     return (shift_ij[0] != 0 || shift_ij[1] != 0) ? 1 : 0;

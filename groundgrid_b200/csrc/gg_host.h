@@ -104,4 +104,6 @@ int gg_host_pack_cloud_cached(const gg_point* src, size_t n, unsigned char* dst)
 int gg_host_packer_selftest(int threads, int n_jobs, size_t n_points, int ring_slots, int rounds, int lag);
 int gg_host_spiral_plan(int n, float resolution, int* out);
 int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* lane_end, int* cell_home, int* irr_level_start, uint32_t* irr_recs, int irr_cap_words);
+int gg_host_decay_confidence(const gg_config* cfg, const float* occ, size_t n, float* out);
+int gg_host_skew_visit_confidence(const float* d, const float* occ, size_t n, float* out);
 }

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cfloat>
+
 #include "groundgrid_b200.h"
 
 namespace gg {
@@ -307,6 +309,23 @@ __host__ __device__ __forceinline__ double pose_div(double a, double b) {
     return a / b;
 #endif
 }
+
+// ---- confidence decay of the spiral sweep (interpolate_cell :463-464), shared by every spiral path ----
+// std::max(c - c / decrease_factor, 0.001) in fp64.  The result is >= 0.001 or NaN: +-inf decays to NaN (inf - inf),
+// and so does NaN (std::max keeps its first argument when the comparison fails).
+__host__ __device__ __forceinline__ float decay_confidence(const CfgConst& kc, float occ) {
+    // Confidences sit at the 0.001 floor in most of the map; from there down to -FLT_MAX the result is the floor again
+    // (host-checked for the configured factor, CfgConst::decay_floor_ok), which skips the fp64 division.  -inf is not
+    // in that range: it decays to NaN like every other non-finite confidence.
+    if (kc.decay_floor_ok && occ <= 0.001f && occ >= -FLT_MAX) return 0.001f;
+    const double o = (double)occ;
+    const double dec = pose_sub(o, pose_div(o, kc.dec_factor));
+    return (float)((dec < 0.001) ? 0.001 : dec);
+}
+// The skewed spiral stores, per visit, the confidence the visit leaves (SD, written by k_detect): the decay of a cell
+// beyond minDistSquared, SKEW_NEAR (never a decay) for a cell the visit does not decay.
+constexpr float SKEW_NEAR = -1.0f;
+__host__ __device__ __forceinline__ bool skew_decays(float d) { return d != SKEW_NEAR; }
 
 // gg_host.cpp:move_map for one position, for a roll resolved on the device: the whole-cell shift toward (nx, ny),
 // rounded half away from zero, and the map position advanced by it.  Returns 1 (the cells shift), 0 (no shift) or -1:

@@ -739,15 +739,7 @@ constexpr int DT_X = 32, DT_Y = 8, DT_H = 2;
 constexpr int DT_W = DT_X + 2 * DT_H;   // 36
 constexpr int DT_R = DT_Y + 2 * DT_H;   // 12
 
-// confidence decay of interpolate_cell (:464): std::max(c - c / decrease_factor, 0.001) in fp64
-__device__ __forceinline__ float decay_confidence(const CfgConst& kc, float occ) {
-    // Confidences sit at the 0.001 floor in most of the map; from there (and below) the result is the floor
-    // again (host-checked for the configured factor, CfgConst::decay_floor_ok), which skips the fp64 division.
-    if (kc.decay_floor_ok && occ <= 0.001f) return 0.001f;
-    const double o = (double)occ;
-    const double dec = __dsub_rn(o, __ddiv_rn(o, kc.dec_factor));
-    return (float)((dec < 0.001) ? 0.001 : dec);
-}
+// the confidence decay of interpolate_cell (:464) is gg_internal.h:decay_confidence
 
 // Fused into k_detect: every cell is copied to its home slot(s) as soon as its final G, C are known.
 __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams& sp, int cell, int x, int y, float g, float c, bool far) {
@@ -761,7 +753,7 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
         c = 1.0f;
     }
     // :463: beyond minDistSquared (`far`, from the per-cell table) the visit stores the decayed confidence (:464)
-    const float d1 = far ? decay_confidence(kc, c) : -1.0f;
+    const float d1 = far ? decay_confidence(kc, c) : SKEW_NEAR;
     float2* SK = v.skew.sk + (size_t)sp.slot * v.skew.slots;
     float* SD = v.skew.sd + (size_t)sp.slot * v.skew.slots;
     const float2 gc = make_float2(g, c);
@@ -769,7 +761,7 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
     SD[home.x] = d1;
     if (home.y >= 0) {
         SK[home.y] = gc;
-        SD[home.y] = far ? decay_confidence(kc, d1) : -1.0f;  // second visit of a ring corner
+        SD[home.y] = far ? decay_confidence(kc, d1) : SKEW_NEAR;  // second visit of a ring corner
     }
     if (home.z >= 0) SK[home.z] = gc;
     if (home.w >= 0) SK[home.w] = gc;
@@ -1427,7 +1419,7 @@ __device__ __forceinline__ float2 spiral_visit(const float2* nb, float d) {
     const float ssum = __fadd_rn(tree9(cc), FLT_MIN);  // :457
     const float avg = __fdiv_rn(tree9(pr), ssum);      // :458
     const float newg = __fadd_rn(__fmul_rn(__fsub_rn(1.0f, occ), avg), __fmul_rn(occ, h));  // :460
-    return make_float2(newg, d >= 0.0f ? d : occ);     // :463-464 via the table of k_skew
+    return make_float2(newg, skew_decays(d) ? d : occ);  // :463-464 via the table of k_skew
 }
 
 // The level time of this kernel is set by the longest per-warp INSTRUCTION sequence between two
@@ -1525,7 +1517,7 @@ __device__ __forceinline__ void skew_lane_thread(const View& v, const SlotParams
             s_xch[(l__ & XM) * lanes + xid] = r__;                                                  \
             SK[base0 + l__ * KP] = r__;                                                             \
             Gn[cell0 + l__ * cstep] = r__.x;                                                        \
-            if (CURD >= 0.0f) Cn[cell0 + l__ * cstep] = r__.y;                                      \
+            if (skew_decays(CURD)) Cn[cell0 + l__ * cstep] = r__.y;                                 \
         }                                                                                           \
         __syncthreads();                                                                            \
     }
@@ -1643,7 +1635,7 @@ __device__ __forceinline__ void skew_irregular_thread(const View& v, const SlotP
                 SK[own] = r;
                 if (mirror >= 0) SK[mirror] = r;
                 Gn[hd[3]] = r.x;
-                if (s_dd[ti] >= 0.0f) Cn[hd[3]] = r.y;
+                if (skew_decays(s_dd[ti])) Cn[hd[3]] = r.y;
             }
         }
         __syncthreads();

@@ -146,6 +146,9 @@ class Cuda:
     def filter_cloud(self, pts, org, base_z, cloud=True):
         return self.m.filter_cloud(pts, org, base_z, want_index=True, want_cloud=cloud)
 
+    def spiral(self, base_z):
+        self.m.spiral_ground_interpolation(base_z)
+
     def __getattr__(self, name):
         return getattr(self.m, name)
 
@@ -475,6 +478,32 @@ def far_geometry(make, rec, where):
     check("moved")
 
 
+def nonfinite_confidence(make, rec):
+    """Imported priors (set_layer, as a migrated slot brings them) with +-inf, NaN and other edge confidences
+    (tests/spiral_priors.py) on far, near, ring-corner, centre and border cells: each non-finite value in its own map,
+    the finite ones densely in one, for the default decrease factor and 1000; a scan and the per-phase spiral on each."""
+    import spiral_priors as sp
+
+    cases = sp.edge_cases(100, 0.33)
+    pts, org = synth.lidar_scan(synth.make_scene(seed=5, n_boxes=6, rmin=1.0, rmax=13.0), beams=16, az_steps=256, seed=5)
+    for factor in (5.0, 1000.0):
+        for seed, (name, planted) in enumerate(cases.items()):
+            G, C = sp.planted_prior(100, 0.33, planted, seed=seed)
+            ctx = f"{factor:g}/{name}"
+            for how in ("scan", "spiral"):
+                m = make(33.0, 0.33)
+                m.set_config(occupied_cells_decrease_factor=factor)
+                m.init_map(0.0, 0.0, 0.0)
+                m.set_layer("ground", G)
+                m.set_layer("groundpatch", C)
+                if how == "scan":
+                    rec(f"{ctx}/scan/labels", m.filter_cloud(pts, org, 0.1, cloud=False)[0])
+                else:
+                    m.spiral(0.1)
+                for layer in ("ground", "groundpatch"):
+                    rec(f"{ctx}/{how}/{layer}", m.layer(layer))
+
+
 SCENARIOS = {
     "expected_points_table": (expected_points_table, [()]),
     "cfg1_cfg2_64_beam_300": (cfg1_cfg2_64_beam_300, [()]),
@@ -491,6 +520,7 @@ SCENARIOS = {
     "nonfinite_heights": (nonfinite_heights, [()]),
     "far_from_origin": (far_from_origin, [(w,) for w in FAR_POSITIONS]),
     "far_geometry": (far_geometry, [(w,) for w in FAR_POSITIONS]),
+    "nonfinite_confidence": (nonfinite_confidence, [()]),
 }
 
 

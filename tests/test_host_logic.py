@@ -7,6 +7,7 @@ import re
 import numpy as np
 import pytest
 
+import spiral_priors as sp
 from groundgrid_b200 import capi
 from oracle import Oracle
 
@@ -86,6 +87,35 @@ def test_move_map_matches_oracle():
         pos = new_pos
 
 
+def decay_confidence(c, factor=5.0):
+    """gg_internal.h:decay_confidence (the decay k_skew / k_detect store for the skewed and the pipelined spiral) for
+    occupied_cells_decrease_factor = factor, elementwise on the host."""
+    import ctypes as C
+
+    L = capi.load()
+    L.gg_host_decay_confidence.restype = C.c_int
+    L.gg_host_decay_confidence.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    cfg = capi.default_config()
+    cfg.occupied_cells_decrease_factor = factor
+    c = np.ascontiguousarray(c, np.float32)
+    out = np.empty_like(c)
+    assert L.gg_host_decay_confidence(C.byref(cfg), c.ctypes.data, c.size, out.ctypes.data) == 0
+    return out
+
+
+def skew_visit_confidence(d, occ):
+    """The confidence a visit of k_spiral_skew leaves, from its SD entry d (the decay, or the near-cell sentinel)."""
+    import ctypes as C
+
+    L = capi.load()
+    L.gg_host_skew_visit_confidence.restype = C.c_int
+    L.gg_host_skew_visit_confidence.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    d, occ = np.ascontiguousarray(d, np.float32), np.ascontiguousarray(occ, np.float32)
+    out = np.empty_like(d)
+    assert L.gg_host_skew_visit_confidence(d.ctypes.data, occ.ctypes.data, d.size, out.ctypes.data) == 0
+    return out
+
+
 def _tree9(v):
     return ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + (v[7] + v[8])))
 
@@ -112,7 +142,9 @@ def run_level_schedule(G, C, base_z, level_start, visits, res_f, dec_factor=5.0)
         fy = (y.astype(np.float32) - f32(c)).astype(np.float64)
         far = (fx * fx + fy * fy) * res2 > 12.0
         o64 = occ.astype(np.float64)
-        dec = np.maximum(o64 - o64 / np.float64(dec_factor), 0.001).astype(np.float32)
+        dec = o64 - o64 / np.float64(dec_factor)
+        with np.errstate(invalid="ignore"):
+            dec = np.where(dec < 0.001, 0.001, dec).astype(np.float32)   # std::max(dec, 0.001): NaN stays NaN
         C[x[far], y[far]] = dec[far]
     return G, C
 
@@ -170,9 +202,6 @@ def test_pipelined_spiral_records_emulation(dim, res, dist):
     from the table.  Must reproduce the oracle's sequential sweep bit for bit."""
     o = Oracle(dim, res)
     n = o.n
-    ok, max_recent, ls, recs = host_spiral_records(n, res, dist)
-    assert ok == 1 and max_recent <= 4
-    L = len(ls) - 1
     rng = np.random.default_rng(4)
     o.init_map(0.0, 0.0, 0.0)
     G = rng.uniform(-1, 1, (n, n)).astype(np.float32)
@@ -180,15 +209,23 @@ def test_pipelined_spiral_records_emulation(dim, res, dist):
     o.set_layer("ground", G)
     o.set_layer("groundpatch", C)
     o.spiral(0.3)
+    G, C = emulate_pipe(n, res, dist, G, C, 0.3)
+    assert np.array_equal(o.layer("ground"), G)
+    assert np.array_equal(o.layer("groundpatch"), C)
 
+
+def emulate_pipe(n, res, dist, G, C, base_z, factor=5.0):
+    """k_detect's decay table (D1, and D2 for the second visit of a ring corner) -> k_spiral_pipe with `dist` levels of
+    prefetch, on the CPU; returns the sweep's (ground, groundpatch)."""
+    ok, max_recent, ls, recs = host_spiral_records(n, res, dist)
+    assert ok == 1 and max_recent <= 4
+    L = len(ls) - 1
     c = n // 2 - 1
     G, C = G.copy(), C.copy()
-    o64 = C.astype(np.float64)
-    D1 = np.maximum(o64 - o64 / 5.0, 0.001).astype(np.float32)
-    d64 = D1.astype(np.float64)
-    D2 = np.maximum(d64 - d64 / 5.0, 0.001).astype(np.float32)
+    D1 = decay_confidence(C, factor)
+    D2 = decay_confidence(D1, factor)
     C[c, c] = 1.0
-    G[c, c] = f32(0.3)
+    G[c, c] = f32(base_z)
     ring = {}       # level -> (newg, newc) arrays by slot
     snaps = {}      # level -> (cc[9], gg[9]) snapshot taken dist levels ahead
 
@@ -231,8 +268,7 @@ def test_pipelined_spiral_records_emulation(dim, res, dist):
         ring.pop(lvl - dist - 1, None)
         G[x, y] = newg
         C[x[far], y[far]] = newc[far]
-    assert np.array_equal(o.layer("ground"), G)
-    assert np.array_equal(o.layer("groundpatch"), C)
+    return G, C
 
 
 @pytest.mark.parametrize("n", [0, 1, 7, 8, 9, 16383, 16384, 16385, 40001])
@@ -295,10 +331,6 @@ def test_skewed_spiral_tables_emulation(dim, res):
     Must equal the oracle's sequential sweep bit for bit."""
     o = Oracle(dim, res)
     n = o.n
-    t = host_spiral_skew(n)
-    assert t is not None
-    KP, rows, row0, lanes, L = t["KP"], t["rows"], t["row0"], t["lanes"], t["levels"]
-    prev_q = [1, 3, 7, 5]
     rng = np.random.default_rng(17)
     o.init_map(0.0, 0.0, 0.0)
     G = rng.uniform(-1, 1, (n, n)).astype(np.float32)
@@ -306,16 +338,27 @@ def test_skewed_spiral_tables_emulation(dim, res):
     o.set_layer("ground", G)
     o.set_layer("groundpatch", C)
     o.spiral(0.3)
+    G, C = emulate_skew(n, res, G, C, 0.3)
+    assert np.array_equal(o.layer("ground"), G)
+    assert np.array_equal(o.layer("groundpatch"), C)
+
+
+def emulate_skew(n, res, G, C, base_z, factor=5.0, t=None, lanes_at=None):
+    """k_skew (the skewed copy and its SD table, fused into k_detect) -> k_spiral_skew -> k_unskew on the CPU; returns
+    the sweep's (ground, groundpatch).  lanes_at(level): the lanes whose regular visit of that level runs (default: the
+    lanes whose [lane_begin, lane_end) holds it), e.g. from a replay of the lane threads."""
+    t = host_spiral_skew(n) if t is None else t
+    assert t is not None
+    KP, rows, row0, lanes, L = t["KP"], t["rows"], t["row0"], t["lanes"], t["levels"]
+    prev_q = [1, 3, 7, 5]
 
     # ---- k_skew (column-major cell index = i + j * n)
     c = n // 2 - 1
     Gf, Cf = G.reshape(-1, order="F").copy(), C.reshape(-1, order="F").copy()
-    Gf[c + c * n] = f32(0.3)
+    Gf[c + c * n] = f32(base_z)
     Cf[c + c * n] = 1.0
-    o64 = Cf.astype(np.float64)
-    D1 = np.maximum(o64 - o64 / 5.0, 0.001).astype(np.float32)
-    d64 = D1.astype(np.float64)
-    D2 = np.maximum(d64 - d64 / 5.0, 0.001).astype(np.float32)
+    D1 = decay_confidence(Cf, factor)
+    D2 = decay_confidence(D1, factor)
     ii, jj = np.meshgrid(np.arange(n), np.arange(n), indexing="ij")
     fx = (ii.astype(np.float32) - f32(c)).astype(np.float64)
     fy = (jj.astype(np.float32) - f32(c)).astype(np.float64)
@@ -336,6 +379,8 @@ def test_skewed_spiral_tables_emulation(dim, res):
     irr, ils = t["irr"], t["irr_level_start"]
 
     def reg_lanes(lvl):
+        if lanes_at is not None:
+            return np.asarray(lanes_at(lvl), np.int64)
         return lane[(t["lane_begin"] <= lvl) & (lvl < t["lane_end"])]
 
     def fetch(lvl):  # what the prefetch of level `lvl` sees
@@ -354,8 +399,7 @@ def test_skewed_spiral_tables_emulation(dim, res):
         avg = tree(cc * gg) / s
         occ = cc[:, 4]
         newg = (f32(1.0) - occ) * avg + occ * gg[:, 4]
-        newc = np.where(dd >= 0, dd, occ).astype(np.float32)
-        return newg.astype(np.float32), newc
+        return newg.astype(np.float32), skew_visit_confidence(dd, occ)
 
     nxt = fetch(0)
     for lvl in range(L):
@@ -393,8 +437,90 @@ def test_skewed_spiral_tables_emulation(dim, res):
     # ---- k_unskew
     m = home[:, 0] >= 0
     Gf[m], Cf[m] = SKg[home[m, 0]], SKc[home[m, 0]]
-    assert np.array_equal(o.layer("ground"), Gf.reshape(n, n, order="F"))
-    assert np.array_equal(o.layer("groundpatch"), Cf.reshape(n, n, order="F"))
+    return Gf.reshape(n, n, order="F"), Cf.reshape(n, n, order="F")
+
+
+def reference_decay(c, factor):
+    """interpolate_cell :464 as the reference writes it: std::max(c - c / F, 0.001) in double, std::max(a, b) = a < b ? b : a
+    (so a NaN difference stays NaN), stored as float."""
+    o = np.float64(c)
+    with np.errstate(invalid="ignore"):
+        d = o - o / np.float64(factor)
+        return f32(0.001) if d < 0.001 else f32(d)
+
+
+def test_decay_confidence_at_the_edges_of_its_domain():
+    """The decay every spiral path stores for a far cell, against the reference's expression, on both sides of the
+    floor shortcut (decay_floor_ok = 1 for factors 1 .. 100, 0 for 1000)."""
+    vals = np.array(list(sp.FINITE_EDGES) + list(sp.NONFINITE.values()) + [f32(-1.0), f32(1e-30), f32(2e-3), f32(1e30)], np.float32)
+    for factor in sp.FACTORS:
+        consts = capi.host_config_constants(_config(occupied_cells_decrease_factor=factor))
+        assert consts["decay_floor_ok"] == (0 if factor == 1000.0 else 1), factor
+        got = decay_confidence(vals, factor)
+        want = np.array([reference_decay(v, factor) for v in vals], np.float32)
+        assert np.array_equal(got, want, equal_nan=True), (factor, got, want)
+    assert np.isnan(decay_confidence(np.array([np.inf, -np.inf, np.nan], np.float32), 5.0)).all()
+    # the skewed layout's table: a decay (>= 0.001 or NaN) is stored; only the near-cell sentinel keeps the cell's value
+    d = np.array([np.nan, 0.001, 7.0, -1.0], np.float32)
+    occ = np.array([np.inf, -np.inf, 0.5, np.inf], np.float32)
+    assert np.array_equal(skew_visit_confidence(d, occ), np.array([np.nan, 0.001, 7.0, np.inf], np.float32), equal_nan=True)
+
+
+def _config(**kw):
+    cfg = capi.default_config()
+    for k, v in kw.items():
+        setattr(cfg, k, v)
+    return cfg
+
+
+def _nan_equal_report(name, a, b):
+    bad = ~((a == b) | (np.isnan(a) & np.isnan(b)))
+    if not bad.any():
+        return None
+    idx = np.argwhere(bad)
+    return f"{name}: {bad.sum()} cells differ, e.g. " + ", ".join(f"{tuple(i)}: emulated={a[tuple(i)]!r} oracle={b[tuple(i)]!r}" for i in idx[:4])
+
+
+EDGE_PATHS = ("plain", "pipe", "skew")
+
+
+@pytest.mark.parametrize("factor", sp.FACTORS)
+@pytest.mark.parametrize("path", EDGE_PATHS)
+@pytest.mark.parametrize("dim,res", [(33.0, 0.33), (33.33, 0.33)])   # N = 100, 101
+def test_spiral_emulations_on_edge_confidences(dim, res, path, factor):
+    """Imported priors with +-inf, NaN, -0, negative, denormal, FLT_MAX and 0.001 (and its neighbours) confidences on far,
+    near, ring-corner, centre and border cells (tests/spiral_priors.py), through the plain level schedule, the pipelined
+    records (two levels ahead) and the skewed tables with their decay tables: NaN-aware equal to the oracle's sweep, and
+    at every planted cell the value the reference's decay gives."""
+    n = Oracle(dim, res).n
+    ls, vs = capi.host_spiral_schedule(n)
+    t = host_spiral_skew(n) if path == "skew" else None
+    fails = []
+    for seed, (name, planted) in enumerate(sp.edge_cases(n, res).items()):
+        G, C = sp.planted_prior(n, res, planted, seed=seed)
+        o = Oracle(dim, res)
+        o.set_config(occupied_cells_decrease_factor=factor)
+        o.init_map(0.0, 0.0, 0.0)
+        o.set_layer("ground", G)
+        o.set_layer("groundpatch", C)
+        o.spiral(0.3)
+        with np.errstate(invalid="ignore", over="ignore"):   # inf - inf, FLT_MAX sums: the arithmetic under test
+            if path == "plain":
+                Ge, Ce = run_level_schedule(G, C, 0.3, ls, vs, res, dec_factor=factor)
+            elif path == "pipe":
+                Ge, Ce = emulate_pipe(n, res, 2, G, C, 0.3, factor)
+            else:
+                Ge, Ce = emulate_skew(n, res, G, C, 0.3, factor, t=t)
+        Go, Co = o.layer("ground"), o.layer("groundpatch")
+        errs = [r for r in (_nan_equal_report("ground", Ge, Go), _nan_equal_report("groundpatch", Ce, Co)) if r]
+        for (x, y), kind, v in planted:
+            want = sp.expected_confidence(kind, v, lambda c: reference_decay(c, factor))
+            for who, got in (("oracle", Co[x, y]), ("emulation", Ce[x, y])):
+                if not np.array_equal(got, want, equal_nan=True):
+                    errs.append(f"{who} groundpatch at {kind} cell {(x, y)} planted {v!r}: {got!r}, the reference's decay gives {want!r}")
+        if errs:
+            fails.append(f"[{name}] " + " | ".join(errs[:4]))
+    assert not fails, f"{path}, N {n}, factor {factor}: " + "\n".join(fails)
 
 
 # Parent-build values: the choice gg_create made before it moved into plan_spiral (skew tables, records, and the

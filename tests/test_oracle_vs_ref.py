@@ -76,6 +76,12 @@ def test_far_geometry(where):
     rs.run("far_geometry", rs.Oracle, where)
 
 
+def test_nonfinite_confidence():
+    """The reference's NaN for a far cell whose imported confidence is +-inf (std::max(inf - inf, 0.001)), and its
+    floor for -0, negative and denormal confidences, on the oracle port."""
+    rs.run("nonfinite_confidence", rs.Oracle)
+
+
 def test_reference_threading_as_shipped_runs():
     """thread_count = 8 (the shipped default: 8 insert + 4 patch-detection threads) is racy and therefore not a parity
     target; it must still run and label nearly everything like the reference's sequential execution (stored in
