@@ -1662,9 +1662,14 @@ int gg_terrain_images_to_device(gg_handle h, int count, const int* slots, float*
 }
 
 // ---- single phases (GroundSegmentation.h:56-62 of the reference) ------------------------------
+// Both read the plane "points" names (layer_index); the whole-map call first recomputes the variance from "m2" (:323)
+// where the handle keeps it (GG_FLAG_FULL_LAYERS), else it reads the stored variance.
 int gg_detect_ground_patches(gg_handle h, int slot) {
+    int rc = check_slot(h, slot), points = gg::L_COUNT;
+    if (rc || (rc = layer_index(h, slot, "points", &points))) return rc;
+    const bool recompute = (h->flags & GG_FLAG_FULL_LAYERS) != 0;
     return run_phase(h, slot, 0.0, [&](const Staging& e, cudaStream_t st) {
-        return gg::launch_detect_only(h->view, e.dp, 1, st, h->prof, h->have_layer_map ? &h->layer_map : nullptr);
+        return gg::launch_detect_only(h->view, e.dp, 1, st, h->prof, h->have_layer_map ? &h->layer_map : nullptr, points, recompute);
     });
 }
 
@@ -1689,8 +1694,11 @@ int gg_detect_ground_patch(gg_handle h, int slot, int patch_size, int i, int j) 
     if (patch_size != 3 && patch_size != 5) return fail(GG_E_ARG, "patch size must be 3 or 5");
     const int N = h->view.k.N, H = patch_size / 2;
     if (i < H || j < H || i >= N - H || j >= N - H) return fail(GG_E_ARG, "cell (%d, %d) has no %dx%d neighbourhood", i, j, patch_size, patch_size);
+    int points = gg::L_COUNT;
+    if ((rc = layer_index(h, slot, "points", &points))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
-    h->launches += gg::launch_detect_cell(h->view, h->variants.constants(h->variants.variant_of(slot)), slot, patch_size, i, j, stream_of(h, slot));
+    h->launches += gg::launch_detect_cell(h->view, h->variants.constants(h->variants.variant_of(slot)), slot, patch_size, i, j, points,
+                                          stream_of(h, slot));
     GG_CUDA(cudaGetLastError());
     return GG_OK;
 }

@@ -202,10 +202,13 @@ int launch_roll(const View& v, const SlotParams* batch, int count, cudaStream_t 
 int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int max_points, int stop_after, cudaStream_t st,
                          Profiler* prof, const CUtensorMap* layer_map);
 // single phases / single cells (the reference's public per-phase methods)
-int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map);
+// count_layer: the plane detection reads as "points"; recompute: the variance is L_M2 / (points + FLT_MIN) (:323),
+// computed inside the detection kernel and stored to L_VARIANCE (full layers only)
+int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map,
+                       int count_layer, bool recompute);
 int launch_spiral_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof);
 int launch_interpolate_cell(const View& v, const CfgConst& c, int slot, int x, int y, cudaStream_t st);
-int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, cudaStream_t st);
+int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, int count_layer, cudaStream_t st);
 // The output cloud of `count` completed scans, compacted into dests[k] (dests[k] goes with batch[k]).
 // compact: count + scan passes (needed for index / cloud / count); write: the write pass (needed for index / cloud /
 // labels).  A batch that wants only labels needs only the write pass.

@@ -769,7 +769,8 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
 
 // Per-cell quantities of detect_ground_patches that depend only on the grid and the configuration, computed
 // once per configuration variant (gg_capi.cu:build_variant) with the very operations of the per-scan code they replace:
-//   x: max(3, floor(threshold * S * expectedPoints))  (:364; integer valued, exact in float, capped at 2^24)
+//   x: max(3, floor(threshold * S * expectedPoints))  (:364), rounded up to float: for a float psum, psum < x is then the
+//      reference's double comparison psum < max(...) at any magnitude (no float lies between the bound and x)
 //   y: variance threshold (:369)      z: expectedPoints      w: flags
 constexpr int DTF_S5 = 1, DTF_FAR = 2, DTF_INNER = 4;
 
@@ -793,11 +794,10 @@ __global__ void k_build_detect_table(View v, const CfgConst kc, float4* __restri
     const double S = (flags & DTF_S5) ? 5.0 : 3.0;
     double need = floor(__dmul_rn(__dmul_rn(kc.gp_thresh, S), (double)e));
     need = (need < 3.0) ? 3.0 : need;                 // NaN -> NaN: the comparison below stays false, as in the reference
-    if (need > 16777216.0) need = 16777216.0;         // patch sums are counts far below 2^24
     const double a = __dmul_rn((double)sqdist, kc.df_sq);
     const double m = (a < kc.mdf_sq) ? kc.mdf_sq : a;
     const float vt = (float)((kc.mdf10_sq < m) ? kc.mdf10_sq : m);
-    tab[cell] = make_float4((float)need, vt, e, __int_as_float(flags));
+    tab[cell] = make_float4(__double2float_ru(need), vt, e, __int_as_float(flags));
 }
 
 // returns true when (g, c) changed
@@ -812,7 +812,7 @@ __device__ __forceinline__ bool detect_patch(const CfgConst& kc, const float (*s
     const float psum = TreeSum<0, S * S>::run([&](int q) { return sP[c0 + q / S][r0 + q % S]; });
     const float oc = c, og = g;
 
-    // early skipping of (almost) empty areas, :364 (both sides integer valued: the float compare is the double one)
+    // early skipping of (almost) empty areas, :364 (need is rounded up to float: the float compare is the double one)
     if (psum < need) return false;
 
     float localmin = sM[c0][r0];
@@ -851,7 +851,10 @@ __device__ __forceinline__ bool detect_patch(const CfgConst& kc, const float (*s
     return false;
 }
 
-__global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const SlotParams* __restrict__ batch) {
+// count_layer: the plane read as "points" -- L_COUNT in the pipeline, whatever "points" names for a call on its own.
+// recompute (a call on its own, full layers): the variance is m2 / (points + FLT_MIN) (:323), computed from L_M2 for
+// every tile entry and stored for every cell, instead of read from L_VARIANCE (the pipeline's k_cell_stats just wrote it).
+__global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const SlotParams* __restrict__ batch, int count_layer, bool recompute) {
     __shared__ float sP[DT_R][DT_W], sPV[DT_R][DT_W], sPM[DT_R][DT_W], sM[DT_R][DT_W];
     const SlotParams& sp = batch[blockIdx.z];
     const Const& k = v.k;
@@ -861,8 +864,8 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const Slot
     // one 64-bit base per scan, 32-bit offsets below it (all layers of a slot span far less than 2^31 floats)
     float* const L0 = v.layer(sp.slot, 0);
     const int N2 = k.N2;
-    const float* P = L0 + L_COUNT * N2;
-    const float* V = L0 + L_VARIANCE * N2;
+    const float* P = L0 + count_layer * N2;
+    const float* V = L0 + (recompute ? L_M2 : L_VARIANCE) * N2;
     const float* M = L0 + L_MINH * N2;
     // tile + halo (36 x 12): a thread fetches column tx of rows ty and ty + 8 (ty < 4) and, for tx < 4, the halo
     // columns 32 + tx of the same rows; four fixed positions o, o + 32, o + 8 N, o + 8 N + 32, every global load issued
@@ -880,6 +883,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const Slot
         tp[u] = in[u] ? P[off[u]] : 0.0f;
         tv[u] = in[u] ? V[off[u]] : 0.0f;
         tm[u] = in[u] ? M[off[u]] : FLT_MAX;
+        if (recompute) tv[u] = __fdiv_rn(tv[u], __fadd_rn(tp[u], FLT_MIN));   // outside the map 0 / FLT_MIN = 0, as before
     }
     const int i = i0 + tx, j = j0 + ty;
     const bool live = i < N && j < N;
@@ -891,6 +895,10 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const Slot
         c = L0[L_GROUNDPATCH * N2 + cell];
         variance = V[cell];
         tb = __ldg(sp.detect_tab + cell);
+        if (recompute) {
+            variance = __fdiv_rn(variance, __fadd_rn(P[cell], FLT_MIN));
+            L0[L_VARIANCE * N2 + cell] = variance;   // no block reads L_VARIANCE in this mode
+        }
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -942,9 +950,13 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const Slot
 // coefficients e[k] = block(k % S, k / S) (SURVEY App. A.0).  Most inner nodes of that tree are runs of 2 or 3
 // consecutive rows of ONE column: pair(r, c) = q(r, c) + q(r+1, c) and triple(r, c) = q(r, c) + pair(r+1, c) -- the
 // very additions of the tree, so they can be computed once per tile position and shared by every window that contains
-// them (a 5x5 tree then needs 14 shared loads and 13 additions instead of 25 and 24).  The point-count sum is a sum of
-// small integers (exact in fp32 in any order) and the block minimum is order-free: both are separable (column
-// partials of 3 / 5 rows).  Tiles without a single candidate cell (psum >= need nowhere) skip the product stage.
+// them (a 5x5 tree then needs 14 shared loads and 13 additions instead of 25 and 24).  The point-count sum is taken
+// from column partials of 3 / 5 rows: exact in any order while every count of the tile is an integer in
+// [0, DT_EXACT_COUNT] (25 of them stay below 2^24); a tile holding any other count (an imported plane: fractions,
+// negatives, NaN, huge counts) sums every window in Eigen's tree order instead.  The block minimum is taken from
+// column minima that skip NaN, then across the columns, and is the NaN of element 0 when there is one: the minCoeff
+// fold keeps its first element unless a later one is strictly smaller, so a NaN elsewhere never counts.  Tiles
+// without a single candidate cell (psum >= need nowhere) skip the product stage.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
@@ -1051,8 +1063,13 @@ __device__ __forceinline__ bool detect_decide(const CfgConst& kc, float psum, fl
 // A CTA walks DT_TILES consecutive tiles along j; the TMA loads of tile k + 1 are issued before tile k is computed
 // (two stages of raw tiles, one mbarrier each, phase parity flips every second use).
 constexpr int DT_TILES = 4;
+constexpr float DT_EXACT_COUNT = 524288.0f;   // 2^19: 25 such counts sum to less than 2^24
 
-__global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const SlotParams* __restrict__ batch, const __grid_constant__ CUtensorMap tmap) {
+// the minimum of a, b that keeps a unless b is strictly smaller, or a is NaN (column minima that skip NaN)
+__device__ __forceinline__ float min_skip_nan(float a, float b) { return (b < a || a != a) ? b : a; }
+
+__global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const SlotParams* __restrict__ batch, const __grid_constant__ CUtensorMap tmap,
+                                                             int count_layer, bool recompute) {
     __shared__ DetectTile s;
     __shared__ __align__(8) uint64_t s_bar[2];
     const SlotParams& sp = batch[blockIdx.z];
@@ -1070,8 +1087,8 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
         uint64_t* bar = &s_bar[kk & 1];
         const int j0 = (tile0 + kk) * DT_Y;
         mbar_expect_tx(bar, kBytes);
-        tma_load_3d(&r.P[0][0], &tmap, bar, i0 - DT_HX, j0 - DT_H, plane0 + L_COUNT);
-        tma_load_3d(&r.V[0][0], &tmap, bar, i0 - DT_HX, j0 - DT_H, plane0 + L_VARIANCE);
+        tma_load_3d(&r.P[0][0], &tmap, bar, i0 - DT_HX, j0 - DT_H, plane0 + count_layer);
+        tma_load_3d(&r.V[0][0], &tmap, bar, i0 - DT_HX, j0 - DT_H, plane0 + (recompute ? L_M2 : L_VARIANCE));
         tma_load_3d(&r.M[0][0], &tmap, bar, i0 - DT_HX, j0 - DT_H, plane0 + L_MINH);
     };
     if (tid == 0) {
@@ -1100,23 +1117,43 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
         }
         const int flags = __float_as_int(tb.w);
         mbar_wait(&s_bar[kk & 1], (uint32_t)((kk >> 1) & 1));
+        if (recompute) {   // :323 on the tile: V holds m2 (see k_detect_ldg); outside the map 0 / FLT_MIN = 0, as before
+            DetectRaw& rw = s.raw[kk & 1];
+            for (int p = tid; p < DT_R * DT_WT; p += DT_X * DT_Y) {
+                const int row = p / DT_WT, col = p % DT_WT;
+                rw.V[row][col] = __fdiv_rn(rw.V[row][col], __fadd_rn(rw.P[row][col], FLT_MIN));
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the stage is refilled by the TMA unit later
+            __syncthreads();
+            if (live) L0[L_VARIANCE * N2 + cell] = rw.V[lj][li];   // no block reads L_VARIANCE in this mode
+        }
 
-        // stage A: column partials of the point counts (exact) -- positions p = tid, tid + 256 of the 12 x 40 tile
-        // (only columns 0 .. 35 are ever the first row of a window: col + 4 <= 39 stays inside the tile, no bounds tests)
+        // stage A: column partials of the point counts -- positions p = tid, tid + 256 of the 12 x 40 tile
+        // (only columns 0 .. 35 are ever the first row of a window: col + 4 <= 39 stays inside the tile, no bounds tests;
+        // together they read every entry of the tile, so they also tell whether all its counts are small integers)
+        bool exact = true;
         for (int p = tid; p < DT_R * DT_WC; p += DT_X * DT_Y) {
             const int row = p / DT_WC, col = p % DT_WC;   // row = j index of the tile, col = i index
             float a[5];
 #pragma unroll
-            for (int q = 0; q < 5; ++q) a[q] = raw.P[row][col + q];
+            for (int q = 0; q < 5; ++q) {
+                a[q] = raw.P[row][col + q];
+                exact = exact && a[q] >= 0.0f && a[q] <= DT_EXACT_COUNT && a[q] == truncf(a[q]);
+            }
             const float c3 = __fadd_rn(__fadd_rn(a[0], a[1]), a[2]);
             s.C3[row][col] = c3;
             s.C5[row][col] = __fadd_rn(__fadd_rn(c3, a[3]), a[4]);
         }
-        __syncthreads();
+        exact = __syncthreads_and(exact);
         const bool inner = live && (flags & DTF_INNER);
         const bool s5 = (flags & DTF_S5) != 0;
         float psum = 0.0f;
-        if (inner) {
+        if (inner && !exact) {   // the window sum in Eigen's order (:359)
+            if (s5)
+                psum = TreeSum<0, 25>::run([&](int q) { return raw.P[lj - 2 + q / 5][li - 2 + q % 5]; });
+            else
+                psum = TreeSum<0, 9>::run([&](int q) { return raw.P[lj - 1 + q / 3][li - 1 + q % 3]; });
+        } else if (inner) {
             if (s5) {
                 const int r0 = li - 2, c0 = lj - 2;
                 psum = __fadd_rn(__fadd_rn(__fadd_rn(s.C5[c0][r0], s.C5[c0 + 1][r0]), __fadd_rn(s.C5[c0 + 2][r0], s.C5[c0 + 3][r0])), s.C5[c0 + 4][r0]);
@@ -1125,7 +1162,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
                 psum = __fadd_rn(__fadd_rn(s.C3[c0][r0], s.C3[c0 + 1][r0]), s.C3[c0 + 2][r0]);
             }
         }
-        // early skipping of (almost) empty areas, :364 (both sides integer valued: the float compare is the double one)
+        // early skipping of (almost) empty areas, :364 (need is rounded up to float: the float compare is the double one)
         const bool cand = inner && !(psum < tb.x);
         const bool any = __syncthreads_or(cand);
         bool changed = false;
@@ -1152,13 +1189,9 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
                 s.PM2[row][col] = __fadd_rn(qm[0], qm[1]);
                 s.TV[row][col] = __fadd_rn(qv[0], pv12);
                 s.TM[row][col] = __fadd_rn(qm[0], pm12);
-                float n3 = m[0];
-                n3 = (m[1] < n3) ? m[1] : n3;
-                n3 = (m[2] < n3) ? m[2] : n3;
+                const float n3 = min_skip_nan(min_skip_nan(m[0], m[1]), m[2]);
                 s.N3[row][col] = n3;
-                float n5 = (m[3] < n3) ? m[3] : n3;
-                n5 = (m[4] < n5) ? m[4] : n5;
-                s.N5[row][col] = n5;
+                s.N5[row][col] = min_skip_nan(min_skip_nan(n3, m[3]), m[4]);
             }
             __syncthreads();
             if (cand) {
@@ -1171,6 +1204,8 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
                         const float t = s.N5[c0 + q][r0];
                         localmin = (t < localmin) ? t : localmin;
                     }
+                    const float m0 = raw.M[c0][r0];
+                    localmin = (m0 != m0) ? m0 : localmin;
                     changed = detect_decide<5>(kc, psum, localmin, tree25(s.QV, s.PV2, s.TV, r0, c0), tree25(s.QM, s.PM2, s.TM, r0, c0), centerP, variance,
                                                tb.y, tb.z, g, c);
                 } else {
@@ -1181,6 +1216,8 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
                         const float t = s.N3[c0 + q][r0];
                         localmin = (t < localmin) ? t : localmin;
                     }
+                    const float m0 = raw.M[c0][r0];
+                    localmin = (m0 != m0) ? m0 : localmin;
                     changed = detect_decide<3>(kc, psum, localmin, tree9s(s.QV, s.PV2, r0, c0), tree9s(s.QM, s.PM2, r0, c0), centerP, variance, tb.y, tb.z, g, c);
                 }
             }
@@ -2359,11 +2396,13 @@ int launch_roll(const View& v, const SlotParams* batch, int count, cudaStream_t 
 }
 
 // patch detection: the TMA-staged tile when the arena has a descriptor (it needs a 16-byte row pitch: N % 4 == 0), else plain loads
-static void enqueue_detect(const View& v, const SlotParams* batch, int count, cudaStream_t st, const CUtensorMap* layer_map) {
+static void enqueue_detect(const View& v, const SlotParams* batch, int count, cudaStream_t st, const CUtensorMap* layer_map, int count_layer,
+                           bool recompute) {
     if (layer_map)
-        k_detect_tma<<<dim3(cdiv(v.k.N, DT_X), cdiv(cdiv(v.k.N, DT_Y), DT_TILES), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch, *layer_map);
+        k_detect_tma<<<dim3(cdiv(v.k.N, DT_X), cdiv(cdiv(v.k.N, DT_Y), DT_TILES), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch, *layer_map, count_layer,
+                                                                                                                     recompute);
     else
-        k_detect_ldg<<<dim3(cdiv(v.k.N, DT_X), cdiv(v.k.N, DT_Y), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch);
+        k_detect_ldg<<<dim3(cdiv(v.k.N, DT_X), cdiv(v.k.N, DT_Y), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch, count_layer, recompute);
 }
 
 int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int max_points, int stop_after, cudaStream_t st,
@@ -2384,7 +2423,7 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
     ++launches;
     if (stop_after == 1) return launches;
 
-    GG_LAUNCH(K_DETECT, enqueue_detect(v, batch, count, st, layer_map));
+    GG_LAUNCH(K_DETECT, enqueue_detect(v, batch, count, st, layer_map, L_COUNT, false));
     ++launches;
     if (stop_after == 2) return launches;
 
@@ -2463,12 +2502,12 @@ __global__ void k_interpolate_cell(View v, const CfgConst kc, int slot, int x, i
     }
 }
 
-// GroundSegmentation::detect_ground_patch<S> (:343-395) for one cell, reading the layers directly
+// GroundSegmentation::detect_ground_patch<S> (:343-395) for one cell, reading the layers directly ("points" = count_layer)
 template <int S>
-__global__ void k_detect_cell(View v, const CfgConst kc, int slot, int i, int j) {
+__global__ void k_detect_cell(View v, const CfgConst kc, int slot, int i, int j, int count_layer) {
     const Const& k = v.k;
     const int N = k.N, H = S / 2;
-    const float* P = v.layer(slot, L_COUNT);
+    const float* P = v.layer(slot, count_layer);
     const float* V = v.layer(slot, L_VARIANCE);
     const float* M = v.layer(slot, L_MINH);
     float* G = v.layer(slot, L_GROUND);
@@ -2499,8 +2538,9 @@ __global__ void k_detect_cell(View v, const CfgConst kc, int slot, int i, int j)
     }
 }
 
-int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map) {
-    GG_LAUNCH(K_DETECT, enqueue_detect(v, batch, count, st, layer_map));
+int launch_detect_only(const View& v, const SlotParams* batch, int count, cudaStream_t st, Profiler* prof, const CUtensorMap* layer_map,
+                       int count_layer, bool recompute) {
+    GG_LAUNCH(K_DETECT, enqueue_detect(v, batch, count, st, layer_map, count_layer, recompute));
     return 1;
 }
 
@@ -2515,11 +2555,11 @@ int launch_interpolate_cell(const View& v, const CfgConst& c, int slot, int x, i
     return 1;
 }
 
-int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, cudaStream_t st) {
+int launch_detect_cell(const View& v, const CfgConst& c, int slot, int S, int i, int j, int count_layer, cudaStream_t st) {
     if (S == 3)
-        k_detect_cell<3><<<1, 1, 0, st>>>(v, c, slot, i, j);
+        k_detect_cell<3><<<1, 1, 0, st>>>(v, c, slot, i, j, count_layer);
     else
-        k_detect_cell<5><<<1, 1, 0, st>>>(v, c, slot, i, j);
+        k_detect_cell<5><<<1, 1, 0, st>>>(v, c, slot, i, j, count_layer);
     return 1;
 }
 

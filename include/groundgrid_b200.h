@@ -253,8 +253,18 @@ int gg_synchronize(gg_handle h);
  *                                       3 ignored, 4 ignored (border cell), 5 outlier -- the contents of the
  *                                       point_index / ignored / outliers lists of :112-117
  *   gg_detect_ground_patches          = detect_ground_patches for all four sections (:314-340; sections are disjoint
- *                                       and every cell only writes itself, so their union is order-free)
- *   gg_detect_ground_patch            = detect_ground_patch<patch_size>(map, i, j) for one cell (:343-395)
+ *                                       and every cell only writes itself, so their union is order-free).  Reads the
+ *                                       planes "points" (whatever gg_get_layer's "points" names at the call: the kept-
+ *                                       point count after a scan stopped before labelling, else the non-ground count),
+ *                                       "minGroundHeight", "ground", "groundpatch", and writes "ground", "groundpatch".
+ *                                       With GG_FLAG_FULL_LAYERS it first sets "variance" = m2 / (points + FLT_MIN)
+ *                                       (:323) as the reference does; a handle without the flag keeps no "m2" and reads
+ *                                       the stored "variance" in its place -- the one difference from the reference.
+ *                                       Any float in these planes (NaN, +-inf, fractional or negative counts) gives the
+ *                                       reference's result.
+ *   gg_detect_ground_patch            = detect_ground_patch<patch_size>(map, i, j) for one cell (:343-395): reads
+ *                                       "points" (as above), the stored "variance", "minGroundHeight", "ground",
+ *                                       "groundpatch"; no variance recompute, as in the reference
  *   gg_spiral_ground_interpolation    = spiral_ground_interpolation (:398-441), base_z = z of toBase * (0,0,0)
  *   gg_interpolate_cell               = interpolate_cell(map, x, y) (:445-465)                                   */
 int gg_get_point_classes(gg_handle h, int slot, uint32_t* codes, size_t n);

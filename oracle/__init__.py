@@ -85,6 +85,9 @@ def lib():
                                        C.c_void_p, C.c_void_p, C.c_void_p]
         L.ggo_interpolate_cell.argtypes = [C.c_void_p, C.c_int, C.c_int]
         L.ggo_spiral.argtypes = [C.c_void_p, C.c_double]
+        L.ggo_detect_ground_patches.argtypes = [C.c_void_p]
+        L.ggo_detect_ground_patch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
+        L.ggo_add_layer.argtypes = [C.c_void_p, C.c_char_p, C.c_double]
         L.ggo_grid_index.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_void_p]
         L.ggo_cell_position.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.ggo_block_sum3.restype = C.c_float
@@ -177,6 +180,21 @@ class Oracle:
 
     def spiral(self, base_z):
         self._l.ggo_spiral(self._h, float(base_z))
+
+    def detect_ground_patches(self):
+        """detect_ground_patches over all four sections, with the variance recompute each starts with (:323)."""
+        if self._l.ggo_detect_ground_patches(self._h) != 0:
+            raise RuntimeError("oracle: detection needs a map with 'm2' and 'variance' layers")
+
+    def detect_ground_patch(self, size, i, j):
+        """detect_ground_patch<size>(map, i, j): one cell, the stored variance."""
+        if self._l.ggo_detect_ground_patch(self._h, int(size), int(i), int(j)) != 0:
+            raise RuntimeError("oracle: detection needs a map with a 'variance' layer")
+
+    def add_layer(self, name, value=0.0):
+        """grid_map::GridMap::add(name, value)."""
+        if self._l.ggo_add_layer(self._h, name.encode(), float(value)) != 0:
+            raise KeyError(name)
 
     def grid_index(self, x, y):
         idx = np.zeros(2, np.int32)

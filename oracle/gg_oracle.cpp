@@ -554,6 +554,34 @@ void ggo_interpolate_cell(void* h, int x, int y) {
     static_cast<ggo::Oracle*>(h)->interpolate_cell(x, y);
 }
 void ggo_spiral(void* h, double base_z) { static_cast<ggo::Oracle*>(h)->spiral_ground_interpolation(base_z); }
+// detect_ground_patches for all four sections, each starting with the variance recompute of :323, as filter_cloud
+// calls them; -1 if the map has no "m2" / "variance" layer yet (the reference's map["m2"] would throw)
+int ggo_detect_ground_patches(void* h) {
+    auto* o = static_cast<ggo::Oracle*>(h);
+    if (!o->have_map || !o->present[o->find_layer("m2")] || !o->present[o->find_layer("variance")]) return -1;
+    o->bind_hot();
+    for (unsigned short s = 0; s < 4; ++s) o->detect_ground_patches(s);
+    return 0;
+}
+// detect_ground_patch<S>(map, i, j) alone: reads "variance" as stored (no recompute)
+int ggo_detect_ground_patch(void* h, int S, int i, int j) {
+    auto* o = static_cast<ggo::Oracle*>(h);
+    if (!o->have_map || !o->present[o->find_layer("variance")] || (S != 3 && S != 5)) return -1;
+    o->bind_hot();
+    if (S == 3)
+        o->detect_ground_patch<3>(i, j);
+    else
+        o->detect_ground_patch<5>(i, j);
+    return 0;
+}
+// grid_map::GridMap::add(name, value): a new layer, or an existing one overwritten, with the constant value
+int ggo_add_layer(void* h, const char* name, double value) {
+    auto* o = static_cast<ggo::Oracle*>(h);
+    const int k = o->find_layer(name);
+    if (k < 0 || !o->have_map) return -1;
+    o->L(name).assign(static_cast<size_t>(o->geo.n) * o->geo.n, static_cast<float>(value));
+    return 0;
+}
 void ggo_grid_index(void* h, double x, double y, int* idx2, int* inside) {
     auto* o = static_cast<ggo::Oracle*>(h);
     ggo::get_index(o->geo, x, y, idx2[0], idx2[1]);

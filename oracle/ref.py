@@ -79,6 +79,10 @@ class Reference:
         L.ggr_filter_cloud.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.ggr_detect_ground_patches.argtypes = [C.c_void_p, C.c_int]
+        # a library built elsewhere from an older harness may lack the one-cell entry point; only that call needs it
+        self._has_detect_patch = hasattr(L, "ggr_detect_ground_patch")
+        if self._has_detect_patch:
+            L.ggr_detect_ground_patch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
         L.ggr_interpolate_cell.argtypes = [C.c_void_p, C.c_int, C.c_int]
         L.ggr_spiral.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.ggr_add_layer.argtypes = [C.c_void_p, C.c_char_p, C.c_double]
@@ -163,8 +167,17 @@ class Reference:
         self.last_filter_seconds = sec.value
         return labels, out_index[:nout], (out_cloud[:nout] if want_cloud else None)
 
-    def detect_ground_patches(self, section):
-        self._l.ggr_detect_ground_patches(self._h, int(section))
+    def detect_ground_patches(self, section=None):
+        """One section (0 .. 3) of GroundSegmentation::detect_ground_patches, or all four in order (section=None)."""
+        for s in range(4) if section is None else (section,):
+            self._l.ggr_detect_ground_patches(self._h, int(s))
+
+    def detect_ground_patch(self, size, i, j):
+        """GroundSegmentation::detect_ground_patch<size>(map, i, j)."""
+        assert size in (3, 5)
+        if not self._has_detect_patch:
+            raise RuntimeError("reference: this oracle/_ref library predates ggr_detect_ground_patch; rebuild it with oracle/build_ref.py")
+        self._l.ggr_detect_ground_patch(self._h, int(size), int(i), int(j))
 
     def interpolate_cell(self, x, y):
         self._l.ggr_interpolate_cell(self._h, x, y)

@@ -257,6 +257,13 @@ void ggr_detect_ground_patches(void* h, int section) {
     auto* r = static_cast<Ref*>(h);
     r->seg.detect_ground_patches(*r->map, static_cast<unsigned short>(section));
 }
+void ggr_detect_ground_patch(void* h, int S, int i, int j) {
+    auto* r = static_cast<Ref*>(h);
+    if (S == 3)
+        r->seg.detect_ground_patch<3>(*r->map, static_cast<size_t>(i), static_cast<size_t>(j));
+    else
+        r->seg.detect_ground_patch<5>(*r->map, static_cast<size_t>(i), static_cast<size_t>(j));
+}
 void ggr_interpolate_cell(void* h, int x, int y) {
     auto* r = static_cast<Ref*>(h);
     r->seg.interpolate_cell(*r->map, static_cast<size_t>(x), static_cast<size_t>(y));

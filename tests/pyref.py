@@ -146,47 +146,9 @@ def filter_cloud(points, origin, base_z, G, C, E, geo, cfg=None, stop_after=0):
     with np.errstate(all="ignore"):
         var[...] = m2 / (cnt + FLT_MIN)
     res_f = f32(geo.res)
-    gp = f64(cfg["ground_patch_detection_minimum_point_count_threshold"])
     for i in range(2, N - 2):
         for j in range(2, N - 2):
-            di = f64(i) - f64(N) / f64(2.0)
-            dj = f64(j) - f64(N) / f64(2.0)
-            sqd = f32((di * di + dj * dj) * (f64(res_f) * f64(res_f)))
-            S = 3 if f64(sqd) <= f64(cfg["patch_size_change_distance"]) ** 2 else 5
-            h = S // 2
-            Pb = block(cnt, i - h, j - h, S)
-            psum = tree_sum(Pb)
-            e = E[i, j]
-            oc, og = C[i, j], G[i, j]
-            if f64(psum) < max(math.floor(float(gp * f64(S) * f64(e))), 3.0):
-                continue
-            dfac = f64(cfg["distance_factor"])
-            mdf = f64(cfg["minimum_distance_factor"])
-            vt = f32(min(max(f64(sqd) * (dfac * dfac), mdf * mdf), (mdf * f64(10)) * (mdf * f64(10))))
-            Vb = block(var, i - h, j - h, S)
-            Mb = block(minh, i - h, j - h, S)
-            variance = var[i, j]
-            localmin = min(Mb)
-            with np.errstate(all="ignore"):
-                if cnt[i, j] >= f32(cfg["point_count_cell_variance_threshold"]):
-                    maxVar = variance
-                else:
-                    maxVar = f32(tree_sum([f32(p * v) for p, v in zip(Pb, Vb)]) / psum)
-                groundlevel = f32(tree_sum([f32(p * m) for p, m in zip(Pb, Mb)]) / psum)
-            groundDiff = max(f32(f32(groundlevel - og) * f32(f32(2.0) * oc)), f32(1.0))
-            if f64(oc) > 0.5 and f64(groundlevel) >= f64(og) + f64(cfg["outlier_tolerance"]):
-                continue
-            factor = f64(cfg["occupied_cells_point_count_factor"])
-            if (f64(vt) > f64(maxVar) * f64(maxVar) and maxVar > 0
-                    and f64(psum) > f64(f32(f32(groundDiff * e) * f32(S))) * gp):
-                nc = f32(min(f64(psum) / factor, f64(1.0)))
-                num = f32(f32(groundlevel * nc) + f32(f32(oc * og) * f32(2)))
-                den = f32(nc + f32(oc * f32(2)))
-                G[i, j] = f32(num / den)
-                C[i, j] = f32(min((f64(psum) / (factor * f64(2.0)) + f64(oc)) / f64(2.0), f64(1.0)))
-            elif localmin < og:
-                G[i, j] = localmin
-                C[i, j] = min(f32(oc + f32(0.1)), f32(0.5))
+            detect_cell(cnt, var, minh, G, C, E, i, j, patch_size(N, res_f, cfg, i, j), cfg, res_f)
     if stop_after == 2:
         return out
 
@@ -248,3 +210,79 @@ def filter_cloud(points, origin, base_z, G, C, E, geo, cfg=None, stop_after=0):
         order.append(i)
     out.update(labels=labels, order=np.array(order, np.uint32), points=obst)
     return out
+
+
+def patch_size(N, res_f, cfg, i, j):
+    """3 or 5: the window detect_ground_patches picks for cell (i, j) (:332-337)."""
+    di = f64(i) - f64(N) / f64(2.0)
+    dj = f64(j) - f64(N) / f64(2.0)
+    sqd = f32((di * di + dj * dj) * (f64(res_f) * f64(res_f)))
+    return 3 if f64(sqd) <= f64(cfg["patch_size_change_distance"]) ** 2 else 5
+
+
+def variance_threshold(N, res_f, cfg, i, j):
+    """varThresholdsq of cell (i, j) (:369)."""
+    di = f64(i) - f64(N) / f64(2.0)
+    dj = f64(j) - f64(N) / f64(2.0)
+    sqd = f32((di * di + dj * dj) * (f64(res_f) * f64(res_f)))
+    dfac = f64(cfg["distance_factor"])
+    mdf = f64(cfg["minimum_distance_factor"])
+    return f32(min(max(f64(sqd) * (dfac * dfac), mdf * mdf), (mdf * f64(10)) * (mdf * f64(10))))
+
+
+def min_point_count(cfg, S, e):
+    """The early-skip bound of :364, a double (NaN stays NaN: std::max(NaN, 3.0) is NaN)."""
+    x = f64(cfg["ground_patch_detection_minimum_point_count_threshold"]) * f64(S) * f64(e)
+    x = f64(math.floor(x)) if math.isfinite(x) else x
+    return f64(3.0) if x < 3.0 else x
+
+
+def detect_cell(cnt, var, minh, G, C, E, i, j, S, cfg, res_f):
+    """GroundSegmentation::detect_ground_patch<S>(map, i, j) (A.4, :343-395) on the planes as stored: updates G, C in place
+    and returns which way the cell went: "need" (skipped, too few points, :364), "upward" (skipped, known high confidence
+    estimate not raised, :379), "confident" (:382-388), "localmin" (:389-394) or "unchanged"."""
+    N = cnt.shape[0]
+    cfg = dict(DEFAULT_CFG, **(cfg or {}))
+    h = S // 2
+    Pb = block(cnt, i - h, j - h, S)
+    psum = tree_sum(Pb)
+    e = E[i, j]
+    oc, og = C[i, j], G[i, j]
+    if f64(psum) < min_point_count(cfg, S, e):
+        return "need"
+    vt = variance_threshold(N, res_f, cfg, i, j)
+    Vb = block(var, i - h, j - h, S)
+    Mb = block(minh, i - h, j - h, S)
+    variance = var[i, j]
+    localmin = Mb[0]
+    for t in Mb[1:]:                     # minCoeff: column by column, the first strict minimum (a NaN only from element 0)
+        if t < localmin:
+            localmin = t
+    with np.errstate(all="ignore"):
+        if cnt[i, j] >= f32(cfg["point_count_cell_variance_threshold"]):
+            maxVar = variance
+        else:
+            maxVar = f32(tree_sum([f32(p * v) for p, v in zip(Pb, Vb)]) / psum)
+        groundlevel = f32(tree_sum([f32(p * m) for p, m in zip(Pb, Mb)]) / psum)
+        gd = f32(f32(groundlevel - og) * f32(f32(2.0) * oc))
+        groundDiff = f32(1.0) if gd < f32(1.0) else gd
+        if f64(oc) > 0.5 and f64(groundlevel) >= f64(og) + f64(cfg["outlier_tolerance"]):
+            return "upward"
+        factor = f64(cfg["occupied_cells_point_count_factor"])
+        gp = f64(cfg["ground_patch_detection_minimum_point_count_threshold"])
+        if (f64(vt) > f64(maxVar) * f64(maxVar) and maxVar > 0
+                and f64(psum) > f64(f32(f32(groundDiff * e) * f32(S))) * gp):
+            q = f64(psum) / factor
+            nc = f32(f64(1.0) if f64(1.0) < q else q)
+            num = f32(f32(groundlevel * nc) + f32(f32(oc * og) * f32(2)))
+            den = f32(nc + f32(oc * f32(2)))
+            G[i, j] = f32(num / den)
+            c = (f64(psum) / (factor * f64(2.0)) + f64(oc)) / f64(2.0)
+            C[i, j] = f32(f64(1.0) if f64(1.0) < c else c)
+            return "confident"
+        if localmin < og:
+            G[i, j] = localmin
+            t = f32(oc + f32(0.1))
+            C[i, j] = f32(0.5) if f32(0.5) < t else t
+            return "localmin"
+    return "unchanged"

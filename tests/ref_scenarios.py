@@ -149,6 +149,16 @@ class Cuda:
     def spiral(self, base_z):
         self.m.spiral_ground_interpolation(base_z)
 
+    def add_layer(self, name, value=0.0):
+        """Every layer exists on the device: grid_map's add(name, value) only sets it."""
+        self.m.set_layer(name, np.full((self.n, self.n), value, np.float32))
+
+    def detect_ground_patches(self):
+        self.m.detect_ground_patches()
+
+    def detect_ground_patch(self, size, i, j):
+        self.m.detect_ground_patch(size, i, j)
+
     def __getattr__(self, name):
         return getattr(self.m, name)
 
@@ -504,6 +514,59 @@ def nonfinite_confidence(make, rec):
                     rec(f"{ctx}/{how}/{layer}", m.layer(layer))
 
 
+# ---- patch detection on imported planes (tests/detect_planes.py) ----------------------------------------------------------
+DETECT_SIZES = (12, 100, 101, 102, 300, 364)
+
+
+def detection_map(make, c):
+    """A fresh map of case c with its planes imported; the layers detection needs that a fresh map of the reference
+    does not have yet ("groundCandidates", "m2", "variance", :61-75) are added first, as filter_cloud adds them."""
+    m = make(c.dim, c.res)
+    m.set_config(**c.config)
+    m.init_map(0.0, 0.0, 0.0)
+    for name in ("groundCandidates", "m2", "variance"):
+        m.add_layer(name, 0.0)
+    for name in c.planes:
+        m.set_layer(name, c.planes[name])
+    return m
+
+
+def detection_scan(n, dim=None):
+    """A small scan of an N x N map (of tests/detect_planes.geometry(n) unless the length is given): (points, origin)."""
+    import detect_planes as dp
+
+    dim = dp.geometry(n)[0] if dim is None else dim
+    scene = synth.make_scene(seed=n, n_boxes=6, rmin=1.0, rmax=max(1.5, 0.4 * dim))
+    return synth.lidar_scan(scene, beams=16, az_steps=256, seed=n)
+
+
+def detect_planes(make, rec, n):
+    """Every case of tests/detect_planes.py: detect_ground_patches over the four sections (with the variance recompute
+    each starts with), then, on a fresh import, detect_ground_patch<S> at every planted cell and at the limits of the
+    window; and detect_ground_patches right after a complete scan, on the layers filter_cloud left."""
+    import detect_planes as dp
+
+    for c in dp.cases(n):
+        ctx = f"{c.kind}/{c.cfg_name}"
+        m = detection_map(make, c)
+        m.detect_ground_patches()
+        for name in ("ground", "groundpatch", "variance"):
+            rec(f"{ctx}/patches/{name}", m.layer(name))
+        m = detection_map(make, c)
+        for S, i, j in [(S, i, j) for i, j, S, _ in c.planted] + dp.window_limit_cells(n):
+            m.detect_ground_patch(S, i, j)
+        for name in ("ground", "groundpatch"):
+            rec(f"{ctx}/patch/{name}", m.layer(name))
+    dim, res = dp.geometry(n)
+    m = make(dim, res)
+    m.init_map(0.0, 0.0, 0.0)
+    pts, org = detection_scan(n)
+    rec("scan/labels", m.filter_cloud(pts, org, 0.0, cloud=False)[0])
+    m.detect_ground_patches()
+    for name in ("ground", "groundpatch", "variance"):
+        rec(f"scan/patches/{name}", m.layer(name))
+
+
 SCENARIOS = {
     "expected_points_table": (expected_points_table, [()]),
     "cfg1_cfg2_64_beam_300": (cfg1_cfg2_64_beam_300, [()]),
@@ -521,6 +584,7 @@ SCENARIOS = {
     "far_from_origin": (far_from_origin, [(w,) for w in FAR_POSITIONS]),
     "far_geometry": (far_geometry, [(w,) for w in FAR_POSITIONS]),
     "nonfinite_confidence": (nonfinite_confidence, [()]),
+    "detect_planes": (detect_planes, [(n,) for n in DETECT_SIZES]),
 }
 
 

@@ -82,6 +82,13 @@ def test_nonfinite_confidence():
     rs.run("nonfinite_confidence", rs.Oracle)
 
 
+@pytest.mark.parametrize("n", rs.DETECT_SIZES)
+def test_detect_planes(n):
+    """detect_ground_patches and detect_ground_patch<S> on the imported planes of tests/detect_planes.py (NaN, +-inf,
+    -0, denormal, fractional and huge counts, cells on every boundary of the decision and on the patch size switch)."""
+    rs.run("detect_planes", rs.Oracle, n)
+
+
 def test_reference_threading_as_shipped_runs():
     """thread_count = 8 (the shipped default: 8 insert + 4 patch-detection threads) is racy and therefore not a parity
     target; it must still run and label nearly everything like the reference's sequential execution (stored in
