@@ -807,6 +807,25 @@ int gg_host_skew_visit_confidence(const float* d, const float* occ, size_t n, fl
     return 0;
 }
 
+// The outlier ray-march of k_rasterize from step `from` on (gg_internal.h:outlier_walk), for the ray from `origin` to
+// `point` (x, y, z) over the prior G / C of an N x N map at pos_xy: 1 an occluding cell is found, 0 none, -1 the ray does
+// not march (vz is not below -0.01f).  The direction is k_rasterize's (:250-257).
+int gg_host_outlier_walk(double dimension_m, float resolution, const double* pos_xy, const float* G, const float* C, double thr, double tol,
+                         const float* origin, const float* point, long long from) {
+    gg::Const k;
+    gg::derive_geometry(dimension_m, resolution, 0, k);
+    float vx = point[0] - origin[0], vy = point[1] - origin[1], vz = point[2] - origin[2];
+    const float sq = (vx * vx + vy * vy) + vz * vz;
+    const float len = std::sqrt(sq);
+    vx = vx / len;
+    vy = vy / len;
+    vz = vz / len;
+    if (!(vz < -0.01f)) return -1;
+    if (from < 0) return -1;
+    const gg::OutlierRay ray{pos_xy[0], pos_xy[1], k.half, k.res, (double)len * (double)len, thr, tol, origin[0], origin[1], origin[2], vx, vy, vz, k.N};
+    return gg::outlier_walk(ray, G, C, from > 2147483648LL ? 2147483648u : (unsigned)from) ? 1 : 0;
+}
+
 int gg_host_move_map(double res, double* pos_xy, double nx, double ny, int* shift_ij) {
     gg::move_map(res, pos_xy[0], pos_xy[1], nx, ny, shift_ij[0], shift_ij[1]);
     return (shift_ij[0] != 0 || shift_ij[1] != 0) ? 1 : 0;

@@ -106,4 +106,6 @@ int gg_host_spiral_plan(int n, float resolution, int* out);
 int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* lane_end, int* cell_home, int* irr_level_start, uint32_t* irr_recs, int irr_cap_words);
 int gg_host_decay_confidence(const gg_config* cfg, const float* occ, size_t n, float* out);
 int gg_host_skew_visit_confidence(const float* d, const float* occ, size_t n, float* out);
+int gg_host_outlier_walk(double dimension_m, float resolution, const double* pos_xy, const float* G, const float* C, double thr, double tol,
+                         const float* origin, const float* point, long long from);
 }

@@ -347,6 +347,122 @@ __host__ __device__ __forceinline__ int resolve_move(double res, double& px, dou
     return (cx != 0 || cy != 0) ? 1 : 0;
 }
 
+// ---- the outlier ray-march of k_rasterize past its first steps (insert_cloud :255-272) ----
+// fp32 arithmetic, correctly rounded and never contracted, on the host and on the device
+__host__ __device__ __forceinline__ float ray_mul(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ float ray_add(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+
+// One point's ray after the pre-test (:244-257): the unit direction v (vz < -0.01f), len^2 and the map it walks.
+struct OutlierRay {
+    double px, py, half, res;  // map position, len / 2, resolution
+    double len2;               // std::pow(len, 2.0)
+    double thr, tol;           // min_outlier_detection_ground_confidence, outlier_tolerance
+    float ox, oy, oz;          // cloud origin
+    float vx, vy, vz;
+    int N;
+};
+
+// What one step of the march computes from `step` (:258-262).  Each quantity is a monotone function of step:
+// (float)step, fl(fs * v), fl(s + o), the index -trunc((p - len/2 - pos) / res), lhs and the height bound all are.
+__host__ __device__ __forceinline__ int ray_trunc(double v) {
+    // grid_map's cast<int>() of the quotient, clamped as k_rasterize's trunc_index clamps it (beyond +-1e9 the index is
+    // outside the map either way; the clamp keeps it monotone)
+    if (!(v == v)) return 1000000000;
+    if (v > 1.0e9) return 1000000000;
+    if (v < -1.0e9) return -1000000000;
+    return (int)v;
+}
+// the cell index along axis a (0: x, 1: y) of step `step`
+__host__ __device__ __forceinline__ int ray_index(const volatile OutlierRay& r, unsigned step, int a) {
+    const float s = ray_mul((float)step, a ? r.vy : r.vx);
+    const double p = (double)ray_add(s, a ? r.oy : r.ox);
+    return -ray_trunc(pose_div(pose_sub(pose_sub(p, r.half), a ? r.py : r.px), r.res));
+}
+// lhs < len2: the loop still runs at `step`
+__host__ __device__ __forceinline__ bool ray_runs(const volatile OutlierRay& r, unsigned step) {
+    const float fs = (float)step;
+    const float sx = ray_mul(fs, r.vx), sy = ray_mul(fs, r.vy), sz = ray_mul(fs, r.vz);
+    return pose_add(pose_add(pose_mul((double)sx, (double)sx), pose_mul((double)sy, (double)sy)), pose_mul((double)sz, (double)sz)) < r.len2;
+}
+
+// The first step t in [lo, hi) with d0 * ix(t) > b0 or d1 * iy(t) > b1, hi if there is none (d = 0: that axis is not
+// tested).  d0 * ix and d1 * iy do not decrease along the ray, so the predicate is false up to some step and true from
+// there on.
+__host__ __device__ __forceinline__ unsigned ray_first(const volatile OutlierRay& r, unsigned lo, unsigned hi, int d0, int b0, int d1, int b1) {
+    while (lo < hi) {
+        const unsigned mid = lo + (hi - lo) / 2;
+        if ((d0 && d0 * ray_index(r, mid, 0) > b0) || (d1 && d1 * ray_index(r, mid, 1) > b1))
+            hi = mid;
+        else
+            lo = mid + 1;
+    }
+    return lo;
+}
+
+// The march from step `from` on, without walking it step by step: true when some step in [from, S) finds an occluding
+// cell, S being the first step whose lhs reaches len2.  The cells the ray visits are a monotone staircase and the steps
+// of one cell form an interval; the cell tests (interior, the clamped 3x3 sum, C > 0.01f) do not depend on the step and
+// the height bound fl(fl(fs * vz) + oz) + tol does not increase along the ray, so a cell occludes at some step of its
+// interval exactly when it does at the interval's last step.  The walk finds S, the interior part of the ray and each
+// cell's last step by bisection over step: O(cells * 31) instead of O(steps).
+// The reference counts in `int step`; a ray whose loop would run past INT_MAX overflows it (undefined behaviour).  Here
+// the march ends after step INT_MAX, as if the loop condition failed there.
+// G / C: the prior's "ground" / "groundpatch" (column-major, N x N, N > 4).  k_rasterize keeps r in local memory (it is
+// volatile here) and runs the walk inline, so that the walk's few registers fit beside the kernel's.
+__host__ __device__ __forceinline__ bool outlier_walk(const volatile OutlierRay& r, const float* G, const float* C, unsigned from) {
+    const unsigned end = 2147483648u;  // one past INT_MAX
+    if (from >= end) return false;
+    unsigned lo = from, hi = end;
+    while (lo < hi) {  // S: lhs does not decrease along the ray
+        const unsigned mid = lo + (hi - lo) / 2;
+        if (ray_runs(r, mid))
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    const unsigned S = lo;
+    if (S <= from) return false;
+    const int N = r.N;
+    const int d0 = ray_index(r, S - 1, 0) >= ray_index(r, from, 0) ? 1 : -1;
+    const int d1 = ray_index(r, S - 1, 1) >= ray_index(r, from, 1) ? 1 : -1;
+    // interior steps (0 < ix < N-1 and 0 < iy < N-1): an interval per axis, so an interval
+    unsigned s = ray_first(r, from, S, d0, d0 > 0 ? 0 : 1 - N, 0, 0);
+    const unsigned s1 = ray_first(r, from, S, 0, 0, d1, d1 > 0 ? 0 : 1 - N);
+    s = s > s1 ? s : s1;
+    unsigned e = ray_first(r, from, S, d0, d0 > 0 ? N - 2 : -1, 0, 0);
+    const unsigned e1 = ray_first(r, from, S, 0, 0, d1, d1 > 0 ? N - 2 : -1);
+    e = e < e1 ? e : e1;
+    while (s < e) {
+        const int ix = ray_index(r, s, 0), iy = ray_index(r, s, 1);
+        s = ray_first(r, s + 1, e, d0, d0 * ix, d1, d1 * iy);  // one past the cell's last step
+        const int r0 = ix - 1 > 2 ? ix - 1 : 2, c0 = iy - 1 > 2 ? iy - 1 : 2;  // :268 (clamped, not centred)
+        const float* B = C + r0 + (size_t)c0 * N;
+        const size_t n = N;
+        // Eigen 3.3.7's binary split over the column-major block (k_rasterize's tree9)
+        const float bs = ray_add(ray_add(ray_add(B[0], B[1]), ray_add(B[2], B[n])),
+                                 ray_add(ray_add(B[n + 1], B[n + 2]), ray_add(B[2 * n], ray_add(B[2 * n + 1], B[2 * n + 2]))));
+        const size_t cell = (size_t)ix + (size_t)iy * n;
+        // the height bound at the cell's last step, the lowest of the cell
+        if ((double)bs > r.thr && C[cell] > 0.01f && (double)G[cell] >= pose_add((double)ray_add(ray_mul((float)(s - 1), r.vz), r.oz), r.tol))
+            return true;
+    }
+    return false;
+}
+// The plain loop hands a ray to outlier_walk at this step (physical rays end long before it).
+constexpr int RAY_WALK_FROM = 4096;
+
 // Per-record bits of a staging entry (PoseBits[m] next to its SlotParams): where k_stage_poses takes the record's
 // pose from.
 enum PoseBits : int {

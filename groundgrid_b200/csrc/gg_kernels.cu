@@ -289,8 +289,14 @@ __device__ __forceinline__ uint32_t rasterize_point(const View& v, const SlotPar
                 vz = __fdiv_rn(vz, len);
                 const double len2 = __dmul_rn((double)len, (double)len);
                 if (vz < -0.01f) {
-                    // step cap: the reference loop is unbounded for non-finite lengths
-                    for (int step = 3; step < (1 << 20); ++step) {
+                    // len is finite here (a non-finite one makes vz NaN or -0), so the loop ends; a ray still running
+                    // at RAY_WALK_FROM is finished by the exact walk, whatever its length
+                    bool walk = false;
+                    for (int step = 3;; ++step) {
+                        if (step == RAY_WALK_FROM) {
+                            walk = true;
+                            break;
+                        }
                         const float fs = (float)step;
                         const float sx = __fmul_rn(fs, vx), sy = __fmul_rn(fs, vy), sz = __fmul_rn(fs, vz);
                         const double lhs = __dadd_rn(__dadd_rn(__dmul_rn((double)sx, (double)sx), __dmul_rn((double)sy, (double)sy)),
@@ -309,6 +315,14 @@ __device__ __forceinline__ uint32_t rasterize_point(const View& v, const SlotPar
                             outlier = true;
                             break;
                         }
+                    }
+                    if (walk) {
+                        // the ray's constants stay in local memory while the walk runs (see outlier_walk)
+                        volatile OutlierRay ray;
+                        ray.px = px, ray.py = py, ray.half = k.half, ray.res = k.res, ray.len2 = len2;
+                        ray.thr = kc.min_outlier_conf, ray.tol = kc.outlier_tol;
+                        ray.ox = ox, ray.oy = oy, ray.oz = oz, ray.vx = vx, ray.vy = vy, ray.vz = vz, ray.N = N;
+                        outlier = outlier_walk(ray, G, C, RAY_WALK_FROM);
                     }
                 }
             }

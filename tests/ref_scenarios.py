@@ -567,6 +567,26 @@ def detect_planes(make, rec, n):
         rec(f"scan/patches/{name}", m.layer(name))
 
 
+# ---- the outlier test on imported priors (tests/outlier_rays.py) ---------------------------------------------------------
+OUTLIER_SIZES = ("100", "101", "far")
+
+
+def outlier_priors(make, rec, which):
+    """Every case of tests/outlier_rays.py (the rays on each decision of the outlier test, long rays past step 2^20, an
+    origin 2e6 m outside the map): the prior imported with set_layer, then a one-point scan."""
+    import outlier_rays as orr
+
+    n, pos = {"100": (100, (0.0, 0.0)), "101": (101, (0.0, 0.0)), "far": (100, orr.FAR)}[which]
+    for c in orr.cases(n, pos, heavy=False):
+        m = make(c.dim, c.res)
+        if c.cfg:
+            m.set_config(**c.cfg)
+        m.init_map(float(pos[0]), float(pos[1]), 0.0)
+        m.set_layer("ground", c.G)
+        m.set_layer("groundpatch", c.C)
+        scan(m, rec, c.cloud(), c.origin, 0.0, c.name, layers=("points", "ground", "groundpatch", "minGroundHeight", "variance"))
+
+
 SCENARIOS = {
     "expected_points_table": (expected_points_table, [()]),
     "cfg1_cfg2_64_beam_300": (cfg1_cfg2_64_beam_300, [()]),
@@ -585,6 +605,7 @@ SCENARIOS = {
     "far_geometry": (far_geometry, [(w,) for w in FAR_POSITIONS]),
     "nonfinite_confidence": (nonfinite_confidence, [()]),
     "detect_planes": (detect_planes, [(n,) for n in DETECT_SIZES]),
+    "outlier_priors": (outlier_priors, [(w,) for w in OUTLIER_SIZES]),
 }
 
 

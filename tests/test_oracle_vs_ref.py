@@ -89,6 +89,13 @@ def test_detect_planes(n):
     rs.run("detect_planes", rs.Oracle, n)
 
 
+@pytest.mark.parametrize("which", rs.OUTLIER_SIZES)
+def test_outlier_priors(which):
+    """The outlier test on the priors and rays of tests/outlier_rays.py (every decision of the march on both sides, rays
+    past step 2^20, an origin 2e6 m outside the map), on the oracle port."""
+    rs.run("outlier_priors", rs.Oracle, which)
+
+
 def test_reference_threading_as_shipped_runs():
     """thread_count = 8 (the shipped default: 8 insert + 4 patch-detection threads) is racy and therefore not a parity
     target; it must still run and label nearly everything like the reference's sequential execution (stored in
