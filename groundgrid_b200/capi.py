@@ -168,6 +168,7 @@ SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "flags", "n_points", "origin", "ba
                             "offsets": [ScanDesc.slot.offset, ScanDesc.flags.offset, ScanDesc.n_points.offset, ScanDesc.origin.offset,
                                         ScanDesc.base_z.offset], "itemsize": C.sizeof(ScanDesc)})
 SCAN_DEVICE_POSE = 1   # GG_SCAN_DEVICE_POSE: the scan's origin / base_z come from the slot's device scan pose
+SCAN_DEVICE_COUNT = 2  # GG_SCAN_DEVICE_COUNT: n_points is the capacity; the scan runs on the slot's stored device count
 
 
 class DevicePoses(C.Structure):
@@ -187,7 +188,9 @@ class DeviceOutputs:
       cloud[k]  : float32 [n_k, 8], the selected output points as 32-byte records, intensity 49 / 99 (None without select)
       index[k]  : int32 [n_k], input index of each selected point (None unless asked for)
       counts    : int32 [count] on the device, selected points of each scan (None without select)
-    Only the first counts[k] entries of cloud[k] / index[k] are written.  They are complete in the order of `stream`."""
+    Only the first counts[k] entries of cloud[k] / index[k] are written.  They are complete in the order of `stream`.
+    With device_counts=True every n_k is the scan's capacity: labels[k] then has capacity length and only its first u
+    entries are written, u being the count the scan used (last_scan_points)."""
 
     def __init__(self, labels, cloud, index, counts, stream):
         self.labels, self.cloud, self.index, self.counts, self.stream = labels, cloud, index, counts, stream
@@ -268,6 +271,7 @@ def load(build_if_missing=True):
         "gg_point_info_to_device": (i, [vp, i, vp, vp, vp]),
         "gg_update_poses_from_device": (i, [vp, i, vp, C.POINTER(DevicePoses), vp, vp]),
         "gg_last_scan_points": (i, [vp, i, C.POINTER(sz)]),
+        "gg_set_point_counts_from_device": (i, [vp, i, vp, vp, vp]),
         "gg_profile_enable": (i, [vp, i]),
         "gg_profile_read": (i, [vp, vp, vp, i]),
         "gg_profile_kernel_count": (i, []),
@@ -502,6 +506,31 @@ class GroundGridB200:
         self.update_poses_from_device_ptrs(slots, ptrs["xy"], ptrs["T"], ptrs["origins"], ptrs["base_z"],
                                            out.data_ptr() if out is not None and count else None, stream.cuda_stream or None)
         return out
+
+    def set_point_counts_from_device_ptrs(self, slots, counts_ptr, stream_ptr):
+        """gg_set_point_counts_from_device with a raw device address (int32 [count]); stream_ptr None = the legacy default
+        stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        _check(self._l.gg_set_point_counts_from_device(self._h, len(sl), _ptr(sl), counts_ptr, stream_ptr))
+
+    def set_point_counts_from_device(self, slots, counts, stream=None):
+        """The point counts of the slots' next scans from a CUDA tensor (gg_set_point_counts_from_device): scans run with
+        device_counts=True use them.
+          counts : int32 [count] (int64 is converted on `stream`, without a host wait), contiguous on this handle's device
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        The call returns without waiting for the device; `counts` may be freed or overwritten right after it when it
+        belongs to `stream` (another stream's tensor is marked in use on `stream`).  A count outside [0, capacity] runs the
+        scan empty."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count = len(slots)
+        if counts.device != dev or counts.numel() != count or counts.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"counts must be an int32 or int64 tensor of {count} entries on {dev}")
+        if stream != current:
+            counts.record_stream(stream)
+        if counts.dtype != torch.int32 or not counts.is_contiguous():
+            with torch.cuda.stream(stream):
+                counts = counts.reshape(-1).to(torch.int32).contiguous()
+        self.set_point_counts_from_device_ptrs(slots, counts.data_ptr() if count else None, stream.cuda_stream or None)
 
     def position(self, slot=0):
         xy = np.zeros(2, np.float64)
@@ -768,10 +797,16 @@ class GroundGridB200:
     def run_scans(self, descs, stop_after=0):
         _check(self._l.gg_run_scans(self._h, len(descs), descs, stop_after))
 
-    def run_scans_device(self, descs, dev_ptrs, stop_after=0):
-        """dev_ptrs: device addresses (ints) of the per-scan clouds (32-byte records)."""
+    def run_scans_device(self, descs, dev_ptrs, stop_after=0, device_counts=False):
+        """dev_ptrs: device addresses (ints) of the per-scan clouds (32-byte records).  device_counts: flag every scan
+        GG_SCAN_DEVICE_COUNT (its n_points is then the capacity; set_point_counts_from_device stores the counts)."""
+        if device_counts and isinstance(descs, np.ndarray):
+            descs["flags"] |= SCAN_DEVICE_COUNT
+        elif device_counts:
+            for d in descs:
+                d.flags |= SCAN_DEVICE_COUNT
         pp = (C.c_void_p * len(descs))(*dev_ptrs)
-        _check(self._l.gg_run_scans_device(self._h, len(descs), descs, pp, stop_after))
+        _check(self._l.gg_run_scans_device(self._h, len(descs), _ptr(descs) if isinstance(descs, np.ndarray) else descs, pp, stop_after))
 
     def run_scans_to_device_ptrs(self, descs, dev_ptrs, out_ptrs, select, counts_ptr, stream_ptr):
         """gg_run_scans_to_device with raw device addresses.  descs: ScanDesc array or SCAN_DESC_DTYPE array;
@@ -783,7 +818,8 @@ class GroundGridB200:
         op = None if out_ptrs is None else np.ascontiguousarray(out_ptrs, dtype=np.uint64).reshape(count, 3)
         _check(self._l.gg_run_scans_to_device(self._h, count, d, _ptr(pp), _ptr(op), int(select), counts_ptr, stream_ptr))
 
-    def run_scans_to_device(self, clouds, slots, origins, base_z, labels=True, select="nonground", index=False, stream=None):
+    def run_scans_to_device(self, clouds, slots, origins, base_z, labels=True, select="nonground", index=False, stream=None,
+                            device_counts=False):
         """One scan per slot on caller-owned CUDA tensors, results left in new CUDA tensors (gg_run_scans_to_device).
           clouds : contiguous CUDA tensors of 32-byte point records (e.g. float32 [n, 8] or uint8 [n * 32]), 16-byte aligned
           origins: [count][3] sensor positions in the map frame; base_z: one value or one per scan.  origins="device"
@@ -792,6 +828,8 @@ class GroundGridB200:
                    returns) or None (no cloud)
           index  : also return the input index of each returned point
           stream : torch.cuda.Stream the work is ordered on (default: the current stream); the outputs are allocated on it.
+          device_counts : each cloud's length is the scan's capacity, and the scan runs on the slot's stored device count
+                   (set_point_counts_from_device, GG_SCAN_DEVICE_COUNT); the outputs are allocated at capacity.
         The call returns without waiting for the device.  Work enqueued on `stream` afterwards sees complete outputs, and
         the inputs may be freed right after the call when they were allocated on `stream` (other streams' inputs are
         marked in use on `stream`).  Returns DeviceOutputs."""
@@ -802,7 +840,7 @@ class GroundGridB200:
             if c.device != dev or not c.is_contiguous() or nbytes % 32:
                 raise ValueError(f"clouds must be contiguous tensors of 32-byte records on {dev}")
             n.append(nbytes // 32)
-        descs = self._device_descs(slots, n, origins, base_z)
+        descs = self._device_descs(slots, n, origins, base_z, device_counts)
         out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, clouds)
         self.run_scans_to_device_ptrs(descs, [c.data_ptr() for c in clouds], ptrs, sel,
                                       out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
@@ -833,7 +871,7 @@ class GroundGridB200:
         _check(self._l.gg_run_cloud_msgs_to_device(self._h, count, d, _ptr(msgs), _ptr(op), int(select), counts_ptr, stream_ptr))
 
     def run_cloud_msgs_to_device(self, payloads, point_step, field_offsets, T, slots, origins, base_z, labels=True, select="nonground",
-                                 index=False, stream=None):
+                                 index=False, stream=None, device_counts=False):
         """One sensor_msgs/PointCloud2 payload per slot, in caller-owned CUDA memory, unpacked and transformed to the map frame
         on the device and then run like run_scans_to_device (gg_run_cloud_msgs_to_device).
           payloads      : contiguous CUDA tensors of any dtype whose byte size is a multiple of the scan's point_step
@@ -842,9 +880,9 @@ class GroundGridB200:
           field_offsets : byte offsets of x, y, z, intensity, ring (-1 absent), one 5-tuple or one per scan
           T             : None (every payload in the map frame), an array [count, 3, 4] of lookupTransform("map", frame_id), or
                           a list with None entries
-        origins, base_z, labels, select, index and stream as in run_scans_to_device.  Each payload may be freed right
-        after the call when it was allocated on `stream` (other streams' payloads are marked in use on `stream`).
-        Returns DeviceOutputs."""
+        origins, base_z, labels, select, index, stream and device_counts (each payload's length is then the capacity) as
+        in run_scans_to_device.  Each payload may be freed right after the call when it was allocated on `stream` (other
+        streams' payloads are marked in use on `stream`).  Returns DeviceOutputs."""
         torch, dev, stream, sel = self._device_call(select, index, stream)
         count = len(payloads)
         steps = np.broadcast_to(np.asarray(point_step, np.int64), (count,))
@@ -854,7 +892,7 @@ class GroundGridB200:
             if c.device != dev or not c.is_contiguous() or step <= 0 or nbytes % step:
                 raise ValueError(f"payloads must be contiguous tensors on {dev} whose byte size is a multiple of point_step")
             n.append(int(nbytes // step))
-        descs = self._device_descs(slots, n, origins, base_z)
+        descs = self._device_descs(slots, n, origins, base_z, device_counts)
         out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, payloads)
         self.run_cloud_msgs_to_device_ptrs(descs, [c.data_ptr() for c in payloads], steps, field_offsets, T, ptrs, sel,
                                            out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
@@ -916,13 +954,15 @@ class GroundGridB200:
         return torch, dev, (torch.cuda.current_stream(dev) if stream is None else stream), sel
 
     @staticmethod
-    def _device_descs(slots, n, origins, base_z):
+    def _device_descs(slots, n, origins, base_z, device_counts=False):
         count = len(n)
         descs = np.zeros(count, SCAN_DESC_DTYPE)
         descs["slot"] = np.asarray(slots, np.int32)
         descs["n_points"] = n
+        if device_counts:   # n is the capacity; the slots' stored device counts (set_point_counts_from_device)
+            descs["flags"] = SCAN_DEVICE_COUNT
         if isinstance(origins, str) and origins == "device":   # the slots' device scan poses (update_poses_from_device)
-            descs["flags"] = SCAN_DEVICE_POSE
+            descs["flags"] |= SCAN_DEVICE_POSE
             return descs
         descs["origin"] = np.asarray(origins, np.float32).reshape(count, 3)
         descs["base_z"] = np.broadcast_to(np.asarray(base_z, np.float64), (count,))
@@ -993,7 +1033,8 @@ class GroundGridB200:
         return codes
 
     def last_scan_points(self, slot=0):
-        """Points of the slot's last scan (gg_last_scan_points): the length of its point_info_to_device outputs."""
+        """Points of the slot's last scan (gg_last_scan_points): the length of its point_info_to_device outputs.  After a
+        device_counts scan this waits for the slot's work (the count is on the device until then)."""
         n = C.c_size_t(0)
         _check(self._l.gg_last_scan_points(self._h, slot, C.byref(n)))
         return n.value
@@ -1016,7 +1057,9 @@ class GroundGridB200:
           height : float32 tensors, z - ground[cell]; NaN for absent points
           out    : None, or a pair (codes list or None, height list or None) of contiguous tensors to fill
           stream : torch.cuda.Stream the work is ordered on (default: the current stream); outputs are allocated on it.
-        The call returns without waiting for the device; work enqueued on `stream` afterwards sees the outputs."""
+        The call returns without waiting for the device; work enqueued on `stream` afterwards sees the outputs.  The
+        lengths come from last_scan_points, which waits after a device_counts scan; point_info_to_device_ptrs with
+        buffers sized for the scan's capacity does not."""
         torch, dev, current, stream = self._layer_stream(stream)
         ns = [self.last_scan_points(int(s)) for s in slots]
         result = []

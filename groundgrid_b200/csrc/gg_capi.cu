@@ -287,6 +287,9 @@ struct SlotState {
     bool device_position = false;   // px / py are stale: the position lives in the device table (PoseTables::position)
     bool device_scan_pose = false;  // the device holds a scan pose of the slot (flagged scans may run)
     bool device_rolled = false;     // a device roll since the last scan (it may have moved the cells)
+    // gg_set_point_counts_from_device
+    bool stored_count = false;      // the device holds a stored count of the slot (GG_SCAN_DEVICE_COUNT scans may run)
+    bool device_count = false;      // n_points / scan_points are the last scan's capacity: its count lives in CountTables::last
 };
 
 // A caller's device byte range [begin, end) of one query set: its positions (input) or one of its outputs.
@@ -328,6 +331,7 @@ struct gg_handle_s {
     int* h_pose_bits = nullptr;            // gg::PoseBits of the entry's records, same shape (allocated with `poses`)
     int* d_pose_bits = nullptr;
     gg::PoseTables poses{};                // per-slot device positions and scan poses (first gg_update_poses_from_device)
+    gg::CountTables counts{};              // per-slot device point counts (first gg_set_point_counts_from_device)
     cudaEvent_t ring_ev[kRing] = {};
     cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
     cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
@@ -457,7 +461,8 @@ struct Staging {
     bool pinfo = false;          // ... and the PointInfoDest records
     bool pose_bits = false;      // ... and the PoseBits of the records
     bool position = false;       // fill staged slot positions (run_groups then patches device-owned ones on the device)
-    bool stage = false;          // some record takes its position or scan pose from the device tables (k_stage_poses)
+    bool count = false;          // fill staged last-scan counts (run_groups then takes device-owned ones on the device)
+    bool stage = false;          // some record takes its position, scan pose or count from the device tables (k_stage_poses)
     gg::SlotParams *hp = nullptr, *dp = nullptr;
     gg::OutDest *hdest = nullptr, *ddest = nullptr;
     gg::UnpackDesc *hunpack = nullptr, *dunpack = nullptr;
@@ -555,10 +560,20 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
         if (!slots.scans) continue;
         if ((slots.scans[i].flags & GG_SCAN_DEVICE_POSE) && !h->slots[slot].device_scan_pose)
             return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_POSE without a device scan pose since gg_init_map", slot);
+        if ((slots.scans[i].flags & GG_SCAN_DEVICE_COUNT) && !h->slots[slot].stored_count)
+            return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_COUNT without a stored count since gg_init_map", slot);
         const size_t n = slots.scans[i].n_points;
         if (n > h->pcap) return fail(GG_E_ARG, "slot %d: %zu points exceed capacity %zu", slot, n, h->pcap);
         if (clouds && n && !clouds[i]) return fail(GG_E_ARG, "scan %d: null cloud", i);
     }
+    return GG_OK;
+}
+
+// The calls whose scans take their point counts from the host (gg_run_scans, gg_filter_cloud_batch[_begin],
+// gg_run_merged_cloud_msgs_to_device) reject GG_SCAN_DEVICE_COUNT.
+int check_host_counts(int count, const gg_scan_desc* scans) {
+    for (int i = 0; i < count; ++i)
+        if (scans[i].flags & GG_SCAN_DEVICE_COUNT) return fail(GG_E_ARG, "scan %d: GG_SCAN_DEVICE_COUNT on a call whose counts are on the host", i);
     return GG_OK;
 }
 
@@ -570,8 +585,10 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
 // entry.  With `fenced`, the groups start after everything enqueued on `caller` so far, and `caller` waits for them: no
 // host wait but the flow control of the staging ring.
 // Poses: when fill staged slot positions (e.position), a record of a slot whose position is device-owned, or of a scan
-// flagged GG_SCAN_DEVICE_POSE, is patched from the device tables by k_stage_poses right after the copy.  Without such
-// records (every all-host flow) nothing more is copied or launched.
+// flagged GG_SCAN_DEVICE_POSE, is patched from the device tables by k_stage_poses right after the copy.  Counts: a scan
+// flagged GG_SCAN_DEVICE_COUNT takes its count from the slot's stored one; when fill staged last-scan counts (e.count),
+// a non-empty record of a slot whose last count is device-owned takes that count.  Without such records (every all-host
+// flow) nothing more is copied or launched.
 template <typename Fill, typename Launch>
 int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t caller, Fill&& fill, Launch&& launch) {
     int rc;
@@ -583,9 +600,14 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
             if (stream_index(h, slots[i]) != g) continue;
             if (e.m == 0 && (rc = e.acquire(h))) return rc;
             work |= fill(i, e);
-            if (e.position && e.hbits) {
-                int bits = h->slots[slots[i]].device_position ? gg::POSE_POSITION : 0;
-                if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_POSE)) bits |= gg::POSE_ORIGIN;
+            if ((e.position || e.count) && e.hbits) {
+                int bits = 0;
+                if (e.position) {
+                    if (h->slots[slots[i]].device_position) bits |= gg::POSE_POSITION;
+                    if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_POSE)) bits |= gg::POSE_ORIGIN;
+                    if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_COUNT)) bits |= gg::POSE_COUNT;
+                }
+                if (e.count && h->slots[slots[i]].device_count && e.hp[e.m].n_points > 0) bits |= gg::POSE_LAST_COUNT;
                 e.hbits[e.m] = bits;
                 if (bits) e.stage = e.pose_bits = true;
             }
@@ -596,7 +618,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
         cudaStream_t st = h->streams[g];
         if (work) {
             if ((rc = e.commit(st))) return rc;
-            if (e.stage) h->launches += gg::launch_stage_poses(h->poses, e.dp, e.dbits, e.m, st, h->prof);
+            if (e.stage) h->launches += gg::launch_stage_poses(h->poses, h->counts, e.dp, e.dbits, e.m, st, h->prof);
             if (fenced) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
             const int n = launch(e, st);
             if (n < 0) return n;
@@ -756,6 +778,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         s.scan_points = d.n_points;
         s.moved_since_scan = false;
         s.device_rolled = false;
+        s.device_count = (d.flags & GG_SCAN_DEVICE_COUNT) != 0;   // a host-count scan makes the count host-owned again
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) {
@@ -826,6 +849,7 @@ int run_output_on(gg_handle h, int slot, bool want_cloud) {
         od.cloud = want_cloud ? h->view.out_cloud + (size_t)slot * h->pcap : nullptr;
         od.select = GG_SELECT_GROUND | GG_SELECT_NONGROUND;
         e.dests = true;
+        e.count = true;
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_output(h->view, e.dp, e.ddest, 1, e.max_points, true, true, st, h->prof); };
@@ -890,6 +914,21 @@ int take_position_back(gg_handle h, int slot) {
     s.px = p.x;
     s.py = p.y;
     s.device_position = false;
+    return GG_OK;
+}
+
+// A call that needs the last scan's point count on the host: a device-owned count (a GG_SCAN_DEVICE_COUNT scan) is read
+// back once the slot's stream group has finished what is enqueued (a host wait), and the slot is host-owned again.
+int take_count_back(gg_handle h, int slot) {
+    SlotState& s = h->slots[slot];
+    if (!s.device_count) return GG_OK;
+    GG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream_of(h, slot);
+    int32_t u = 0;
+    GG_CUDA(cudaMemcpyAsync(&u, h->counts.last + slot, sizeof(u), cudaMemcpyDeviceToHost, st));
+    GG_CUDA(cudaStreamSynchronize(st));
+    s.n_points = s.scan_points = (size_t)u;
+    s.device_count = false;
     return GG_OK;
 }
 
@@ -1288,6 +1327,7 @@ int gg_upload_points(gg_handle h, int slot, const gg_point* points, size_t n) {
     if (rc) return rc;
     if (n > h->pcap) return fail(GG_E_ARG, "%zu points exceed capacity %zu", n, h->pcap);
     if (n && !points) return fail(GG_E_ARG, "null points");
+    if ((rc = take_count_back(h, slot))) return rc;   // the upload replaces n_points, not the last scan's count
     h->inputs_busy = true;
     GG_CUDA(cudaSetDevice(h->device));
     if (n) GG_CUDA(cudaMemcpyAsync(h->view.points + (size_t)slot * h->pcap, points, n * sizeof(gg_point), cudaMemcpyHostToDevice, stream_of(h, slot)));
@@ -1298,6 +1338,8 @@ int gg_upload_points(gg_handle h, int slot, const gg_point* points, size_t n) {
 int gg_run_scans(gg_handle h, int count, const gg_scan_desc* scans, int stop_after) {
     if (!h || !scans) return fail(GG_E_ARG, "null argument");
     if (stop_after < 0 || stop_after > 3) return fail(GG_E_ARG, "stop_after must be 0..3");
+    int rc;
+    if ((rc = check_host_counts(count, scans))) return rc;
     h->inputs_busy = true;
     GG_CUDA(cudaSetDevice(h->device));
     return run_scans_grouped(h, count, scans, stop_after);
@@ -1369,6 +1411,8 @@ namespace {
 // buffer d_raw (grown to their total bytes), then each part is a one-scan batch of the unpack kernel of
 // gg_run_cloud_msgs_to_device, landing after the parts before it.
 int upload_parts(gg_handle h, int slot, int n_parts, const gg_cloud_part* parts) {
+    int rc;
+    if ((rc = take_count_back(h, slot))) return rc;   // the upload replaces n_points, not the last scan's count
     GG_CUDA(cudaSetDevice(h->device));
     h->inputs_busy = true;
     cudaStream_t st = stream_of(h, slot);
@@ -1383,7 +1427,6 @@ int upload_parts(gg_handle h, int slot, int n_parts, const gg_cloud_part* parts)
         GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&h->d_raw[sg]), bytes + 256));
         h->d_raw_cap[sg] = bytes;
     }
-    int rc;
     size_t at = 0;
     for (int p = 0; p < n_parts; ++p) {
         const gg_cloud_part& part = parts[p];
@@ -1457,6 +1500,7 @@ int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_des
                                        const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream) {
     if (!h || !scans || (count > 0 && (!n_parts || !parts))) return fail(GG_E_ARG, "null argument");
     int rc;
+    if ((rc = check_host_counts(count, scans))) return rc;   // per-part device counts would need device part offsets
     if ((rc = check_outputs(outs, -1, select, dev_counts))) return rc;
     std::vector<int>& base = h->part_base;
     base.assign((size_t)std::max(count, 0), 0);
@@ -1586,6 +1630,7 @@ int eval_counts(gg_handle h, int count, const int* slots, unsigned long long* ds
         p.n_points = (int)s.n_points;
         p.src = s.src ? s.src : h->view.points + (size_t)slots[i] * h->pcap;
         p.packed = s.packed_input;
+        e.count = true;
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_eval(h->view, e.dp, e.m, max_points, dst, st, h->prof); };
@@ -1707,6 +1752,7 @@ int gg_detect_ground_patch(gg_handle h, int slot, int patch_size, int i, int j) 
 int gg_get_point_classes(gg_handle h, int slot, uint32_t* codes, size_t n) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
+    if ((rc = take_count_back(h, slot))) return rc;
     if (n > h->slots[slot].n_points || (n && !codes)) return fail(GG_E_ARG, "bad class buffer");
     if (!h->slots[slot].ran) return fail(GG_E_STATE, "slot %d: no rasterised scan", slot);
     GG_CUDA(cudaSetDevice(h->device));
@@ -1792,7 +1838,7 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
-                                           "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve"};
+                                           "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve", "k_store_counts"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -1896,6 +1942,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
     if (!h || !scans || !points) return fail(GG_E_ARG, "null argument");
     if (count < 0) return fail(GG_E_ARG, "negative count");
     int rc;
+    if ((rc = check_host_counts(count, scans))) return rc;
     if ((rc = check_slots(h, count, scans, points))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     if (h->host_pack && !h->packer) {
@@ -2470,6 +2517,7 @@ int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_p
         d.codes = o.codes;
         d.height = o.height;
         e.pinfo = true;
+        e.count = true;
         return write;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_point_info(h->view, e.dp, e.dpinfo, e.m, e.max_points, st, h->prof); };
@@ -2530,10 +2578,42 @@ int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const 
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
+// Point counts from device memory: per stream group one k_store_counts over the group's slots.
+int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_n_points, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0) return GG_OK;
+    if (!slots || !dev_n_points) return fail(GG_E_ARG, "null argument");
+    if (reinterpret_cast<uintptr_t>(dev_n_points) % alignof(int32_t)) return fail(GG_E_ARG, "dev_n_points is not 4-byte aligned");
+    const gg::View& v = h->view;
+    if (ranges_overlap(dev_n_points, (size_t)count * sizeof(int32_t), v.layers, (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float)))
+        return fail(GG_E_ARG, "dev_n_points overlaps the handle's layers");
+    int rc;
+    if ((rc = check_slots(h, count, slots))) return rc;
+    GG_CUDA(cudaSetDevice(h->device));
+    // the device tables and the staging of the per-record bits, on first use (a handle that never asks has none)
+    const size_t S = (size_t)h->n_slots;
+    if (!h->counts.stored && (rc = dev_alloc(h, &h->counts.stored, S))) return rc;
+    if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
+    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
+    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    auto fill = [&](int i, Staging& e) {
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        h->slots[slots[i]].stored_count = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_store_counts(h->counts, e.dp, e.m, dev_n_points, st, h->prof); };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
 int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (!n_points) return fail(GG_E_ARG, "null argument");
+    if ((rc = take_count_back(h, slot))) return rc;
     *n_points = h->slots[slot].scan_points;
     return GG_OK;
 }

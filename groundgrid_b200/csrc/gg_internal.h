@@ -181,6 +181,7 @@ constexpr int OUT_TILE = 1024;
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
     K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_STAGE_POSES, K_POSE_RESOLVE,
+    K_STORE_COUNTS,
     K_NUM
 };
 
@@ -468,15 +469,25 @@ constexpr int RAY_WALK_FROM = 4096;
 enum PoseBits : int {
     POSE_POSITION = 1,   // px / py from the slot's entry of the device position table (the position is device-owned)
     POSE_ORIGIN = 2,     // ox / oy / oz / base_z_f from the slot's device scan pose (GG_SCAN_DEVICE_POSE)
+    POSE_COUNT = 4,      // a scan of GG_SCAN_DEVICE_COUNT: n_points (staged: the capacity) from the slot's stored count,
+                         // 0 when that is outside [0, capacity); the result also goes to the slot's last count
+    POSE_LAST_COUNT = 8, // n_points from the slot's last count (the count of its last scan is device-owned)
 };
 // The handle's per-slot device tables (allocated on the first gg_update_poses_from_device).
 struct PoseTables {
     double2* position;   // [n_slots] map position of a device-owned slot
     float4* scan_pose;   // [n_slots] origin x, y, z and (float)base_z
 };
+// The handle's per-slot point counts from device memory (allocated on the first gg_set_point_counts_from_device).
+struct CountTables {
+    int32_t* stored;     // [n_slots] the latest count gg_set_point_counts_from_device stored, as the caller gave it
+    int32_t* last;       // [n_slots] the count the slot's last GG_SCAN_DEVICE_COUNT scan ran on
+};
 // Patches the `count` records of batch whose bits ask for it from the tables; runs after the entry's copy and before
 // the kernels that read it.
-int launch_stage_poses(const PoseTables& t, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof);
+int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof);
+// One thread per record: the count of batch[j] (at dev_n[batch[j].pos]) into the slot's entry of c.stored.
+int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof);
 // The poses of one gg_update_poses_from_device call (entry batch[j].pos of each array); null xy: no roll, null origin:
 // no scan pose.
 struct DevicePoses {

@@ -2296,14 +2296,23 @@ __global__ void __launch_bounds__(PINFO_THREADS) k_point_info(View v, const Slot
 // exist to keep the host out of the loop, not for throughput.
 constexpr int POSE_THREADS = 128;
 
-// A staging entry's records take the slot's device-owned position and / or its device scan pose, after the entry's
-// copy and before the kernels that read them (the same stream).
-__global__ void __launch_bounds__(POSE_THREADS) k_stage_poses(PoseTables t, SlotParams* __restrict__ batch, const int* __restrict__ bits, int count) {
+// A staging entry's records take the slot's device-owned position and / or its device scan pose, and their point count
+// from the count tables, after the entry's copy and before the kernels that read them (the same stream).
+__global__ void __launch_bounds__(POSE_THREADS) k_stage_poses(PoseTables t, CountTables c, SlotParams* __restrict__ batch, const int* __restrict__ bits,
+                                                              int count) {
     const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
     if (j >= count) return;
     const int b = bits[j];
     if (!b) return;
     SlotParams& p = batch[j];
+    if (b & POSE_COUNT) {
+        // the staged n_points is the scan's capacity: a count outside [0, capacity] runs the scan empty, never clamped
+        const int v = c.stored[p.slot];
+        const int u = (v >= 0 && v <= p.n_points) ? v : 0;
+        p.n_points = u;
+        c.last[p.slot] = u;
+    }
+    if (b & POSE_LAST_COUNT) p.n_points = c.last[p.slot];
     if (b & POSE_POSITION) {
         const double2 q = t.position[p.slot];
         p.px = q.x;
@@ -2352,6 +2361,16 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_resolve(double res, PoseT
     }
     if (in.origin) t.scan_pose[s] = make_float4(in.origin[3 * k], in.origin[3 * k + 1], in.origin[3 * k + 2], (float)in.base_z[k]);
     if (in.moved) in.moved[k] = moved;
+}
+
+// Point counts from device memory (gg_set_point_counts_from_device): record j stores the caller's count of its slot.
+// Values are stored as given; k_stage_poses applies the capacity rule when a scan uses them.
+__global__ void __launch_bounds__(POSE_THREADS) k_store_counts(CountTables c, const SlotParams* __restrict__ batch, int count,
+                                                               const int32_t* __restrict__ dev_n) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count) return;
+    const SlotParams& p = batch[j];
+    c.stored[p.slot] = dev_n[p.pos];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2642,8 +2661,13 @@ int launch_point_info(const View& v, const SlotParams* batch, const PointInfoDes
     return 1;
 }
 
-int launch_stage_poses(const PoseTables& t, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof) {
-    GG_LAUNCH(K_STAGE_POSES, k_stage_poses<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(t, batch, bits, count));
+int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_STAGE_POSES, k_stage_poses<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(t, c, batch, bits, count));
+    return 1;
+}
+
+int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_STORE_COUNTS, k_store_counts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(c, batch, count, dev_n));
     return 1;
 }
 

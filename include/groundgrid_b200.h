@@ -83,8 +83,12 @@ typedef struct gg_handle_s* gg_handle;
  *   origin  = cloudOrigin (x, y, z of the sensor in the map frame, GroundGridNodelet.cpp:139-146,190-194)
  *   base_z  = z of mapToBase * (0,0,0) (GroundSegmentation.cpp:405-411)
  *   flags   = GG_SCAN_DEVICE_POSE: origin / base_z come from the slot's device scan pose (gg_update_poses_from_device)
- *             instead of this descriptor; the other bits are reserved and ignored (pass 0)                */
+ *             instead of this descriptor;
+ *             GG_SCAN_DEVICE_COUNT: n_points is the scan's capacity and the scan runs on the slot's stored device count
+ *             (gg_set_point_counts_from_device);
+ *             the other bits are reserved and ignored (pass 0)                */
 #define GG_SCAN_DEVICE_POSE 1
+#define GG_SCAN_DEVICE_COUNT 2
 typedef struct gg_scan_desc {
     int slot;
     int flags;
@@ -195,6 +199,42 @@ typedef struct gg_device_poses {
  * _wait) first. */
 int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const gg_device_poses* poses, int32_t* dev_moved,
                                 void* stream);
+
+/* ---- point counts from caller GPU memory ----
+ * The point count of the slots' next scans, read from DEVICE memory, for callers whose scan sizes are only known on the
+ * GPU (a crop box or range gate run on the GPU, organized clouds compacted to their valid returns, a simulator's ray
+ * caster that drops misses, the dev_counts of another call), which would otherwise copy them to the host every step.
+ *   dev_n_points : int32 [count], 4-byte aligned, on the handle's device; dev_n_points[k] becomes the stored count of
+ *                  slots[k].  Values are not validated here (see the capacity rule below).
+ *   stream       : cudaStream_t; NULL is the legacy default stream.  The contract of gg_update_poses_from_device: the
+ *                  work starts after everything already enqueued on `stream` and on the stream groups of the slots, and
+ *                  nothing waits on the host except the flow control of the parameter staging ring.  The counts are
+ *                  consumed by the first kernel of each stream group, so a stream-ordered allocator may free or
+ *                  overwrite them on `stream` right after the call.
+ * A scan whose gg_scan_desc sets GG_SCAN_DEVICE_COUNT runs on the latest stored count v of its slot in the slot's stream
+ * order; every later flagged scan reuses it until the next call stores another.  Its n_points is the scan's CAPACITY
+ * (<= max_points): the cloud or payload must be readable for the records the scan uses, and each output needs room for
+ * n_points entries, as for a host count.  The scan uses u = v if 0 <= v <= n_points, else u = 0 (it runs as on an empty
+ * cloud): there is no clamping, and nothing past the capacity is ever read.  Outputs (labels, index, cloud,
+ * dev_counts), layers, gg_get_output, the evaluation tallies and the point info are bit-identical to the same scan run
+ * with a host n_points = u on the same first u records; only the first u labels are written.  The grids of a flagged
+ * scan are sized from its capacity.  The flag is honoured by gg_run_scans_device, gg_run_scans_to_device and
+ * gg_run_cloud_msgs_to_device, with or without GG_SCAN_DEVICE_POSE and with any stop_after.  The calls whose counts are
+ * on the host -- gg_run_scans, gg_filter_cloud_batch[_begin] and gg_run_merged_cloud_msgs_to_device -- reject it with
+ * GG_E_ARG, and a flagged scan of a slot with no stored count since its gg_init_map is GG_E_STATE, with nothing enqueued.
+ * After a flagged scan the slot's last-scan count u is device-owned: gg_point_info_to_device, gg_eval_counts_to_device,
+ * gg_eval_accumulate and gg_get_output take it from the device in stream order, without a host wait (point-info
+ * destinations are sized for the capacity; only the first u entries are written).  gg_last_scan_points,
+ * gg_get_point_classes, gg_upload_points and gg_upload_cloud_msg[s] first WAIT on the host for the work enqueued on the
+ * slot's stream group, take the count back (the slot is host-owned again) and then proceed as on a host-owned slot.  A
+ * scan with a host count, on any path, makes the count host-owned again; gg_init_map forgets the stored count.
+ * count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle, slots or dev_n_points; count > n_slots; a slot out of range or repeated; dev_n_points not
+ *              4-byte aligned or overlapping the handle's layers
+ *   GG_E_STATE a slot whose map is not initialised
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_n_points, void* stream);
 
 /* Replaces GroundSegmentation::filter_cloud (src/GroundSegmentation.cpp:50-197) for one slot with
  * HOST buffers: copies the cloud to the device, runs rasterise -> patch detection -> spiral
@@ -469,7 +509,8 @@ int gg_eval_read(gg_handle h, uint64_t* counts, int reset);
 int gg_eval_counts_to_device(gg_handle h, int count, const int* slots, uint64_t* dev_counts, void* stream);
 
 /* Caller-owned DEVICE destinations of one slot of gg_point_info_to_device (on the handle's device; each may be NULL).
- * n = the point count of the slot's last scan (gg_last_scan_points). */
+ * n = the point count the slot's last scan used (gg_last_scan_points); after a GG_SCAN_DEVICE_COUNT scan, destinations
+ * are sized for that scan's capacity and only the first n entries are written. */
 typedef struct gg_point_info {
     uint32_t* codes;   /* [n], 4-byte aligned: class << 24 | cell, bit-identical to gg_get_point_classes */
     float* height;     /* [n], 4-byte aligned: z - ground[cell] */
@@ -508,9 +549,10 @@ typedef struct gg_point_info {
  * _wait) first. */
 int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_point_info* outs, void* stream);
 
-/* *n_points = the point count of the slot's last scan, completed or stopped early (0 before any scan since gg_init_map).
- * An upload of the next cloud does not change it.  Host state: no device wait.  GG_E_ARG: null handle or n_points, slot
- * out of range. */
+/* *n_points = the point count the slot's last scan used, completed or stopped early (0 before any scan since
+ * gg_init_map).  An upload of the next cloud does not change it.  Host state: no device wait, except after a
+ * GG_SCAN_DEVICE_COUNT scan, whose count it first waits for (gg_set_point_counts_from_device).  GG_E_ARG: null handle or
+ * n_points, slot out of range. */
 int gg_last_scan_points(gg_handle h, int slot, size_t* n_points);
 
 /* Per-kernel CUDA-event timing on the launching stream (bench.py roofline).  While enabled every
