@@ -4,6 +4,7 @@ path and no CPU fallback: every compute call raises GroundGridError without an H
 """
 import ctypes as C
 import os
+import weakref
 
 import numpy as np
 
@@ -182,6 +183,24 @@ class DevicePoses(C.Structure):
     ]
 
 
+class StepDesc(C.Structure):
+    """gg_step_desc: the fixed batch and caller device buffers of a step plan (gg_step_plan_create)."""
+
+    _fields_ = [
+        ("count", C.c_int),
+        ("scans", C.c_void_p),
+        ("dev_points", C.c_void_p),
+        ("msgs", C.c_void_p),
+        ("dev_T_map_from_frame", C.c_void_p),
+        ("dev_n_points", C.c_void_p),
+        ("poses", DevicePoses),
+        ("dev_moved", C.c_void_p),
+        ("outs", C.c_void_p),
+        ("select", C.c_uint),
+        ("dev_counts", C.c_void_p),
+    ]
+
+
 class DeviceOutputs:
     """What GroundGridB200.run_scans_to_device returns: per-scan views into flat CUDA tensors.
       labels[k] : uint8 [n_k], the labels of every input point (None unless asked for)
@@ -206,6 +225,46 @@ class DeviceOutputs:
             return None if views is None else [v[:k] for v, k in zip(views, n)]
 
         return cut(self.cloud), cut(self.index)
+
+
+class StepPlan:
+    """What GroundGridB200.step_plan returns: one step of a fixed batch recorded as a CUDA graph (gg_step_plan_create).
+      launch(stream=None) : replays the step on `stream` (default: the current stream), without a host wait; inside a
+                            torch.cuda.graph capture it adds the step to the captured graph
+      outputs             : DeviceOutputs of the step (allocated at capacity), rewritten by every replay
+      moved               : int32 [count] dev_moved of the roll, or None
+      kernels             : kernel launches per replay
+      close()             : gg_step_plan_destroy (waits for the device); the slots accept every call again
+    The plan keeps its input and output tensors alive; write the next step's inputs into them (e.g. with copy_) on the
+    stream before launching."""
+
+    def __init__(self, owner, p, outputs, moved, keep):
+        self._owner, self._p, self.outputs, self.moved, self._keep = owner, p, outputs, moved, keep
+        owner._plans.add(self)
+
+    def launch(self, stream=None):
+        import torch
+
+        if not self._p:
+            raise GroundGridError(-3, "the step plan is closed")
+        st = torch.cuda.current_stream(torch.device("cuda", self._owner.device)) if stream is None else stream
+        _check(self._owner._l.gg_step_plan_launch(self._p, st.cuda_stream or None))
+
+    @property
+    def kernels(self):
+        return self._owner._l.gg_step_plan_kernels(self._p)
+
+    def close(self):
+        if getattr(self, "_p", None):
+            p, self._p = self._p, None
+            self._owner._plans.discard(self)
+            _check(self._owner._l.gg_step_plan_destroy(p))
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 _lib = None
@@ -272,6 +331,10 @@ def load(build_if_missing=True):
         "gg_update_poses_from_device": (i, [vp, i, vp, C.POINTER(DevicePoses), vp, vp]),
         "gg_last_scan_points": (i, [vp, i, C.POINTER(sz)]),
         "gg_set_point_counts_from_device": (i, [vp, i, vp, vp, vp]),
+        "gg_step_plan_create": (i, [vp, C.POINTER(StepDesc), C.POINTER(vp)]),
+        "gg_step_plan_launch": (i, [vp, vp]),
+        "gg_step_plan_kernels": (i, [vp]),
+        "gg_step_plan_destroy": (i, [vp]),
         "gg_profile_enable": (i, [vp, i]),
         "gg_profile_read": (i, [vp, vp, vp, i]),
         "gg_profile_kernel_count": (i, []),
@@ -414,9 +477,12 @@ class GroundGridB200:
         self.n = self._l.gg_cells_per_side(h)
         self.n_slots = n_slots
         self.max_points = max_points
+        self._plans = weakref.WeakSet()   # live step plans (gg_destroy destroys them)
 
     def close(self):
         if getattr(self, "_h", None):
+            for plan in list(getattr(self, "_plans", ())):   # gg_destroy destroys them
+                plan._p = None
             self._l.gg_destroy(self._h)
             self._h = None
 
@@ -939,6 +1005,101 @@ class GroundGridB200:
                                                   stream.cuda_stream or None)
         del Tarr                   # the transforms `parts` points to: read during the call only
         return out
+
+    def step_plan(self, slots, clouds=None, payloads=None, point_step=32, field_offsets=(0, 4, 8, 16, 20), T=None, origins="device",
+                  base_z=None, counts=None, xy=None, T_base_from_map=None, pose_origins=None, pose_base_z=None, moved=False, labels=True,
+                  select="nonground", index=False):
+        """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
+        Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
+        pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
+        its inputs are given, and every replay is bit-identical to it run on the tensors' contents at replay time.
+          clouds / payloads : exactly one: contiguous CUDA tensors as in run_scans_to_device / run_cloud_msgs_to_device;
+                              their lengths are the scans' capacities
+          point_step, field_offsets : the payloads' layout (one value or one per scan)
+          T        : payloads only.  None (map frame); a CUDA float64 tensor [count, 12] (or [count, 3, 4]) or a list of
+                     CUDA float64 [12] tensors / None: lookupTransform("map", frame_id) read at every replay; a numpy
+                     [count, 3, 4] or a list of numpy 3x4 / None: fixed host transforms
+          origins  : "device" (the slots' device scan poses, GG_SCAN_DEVICE_POSE) or host [count][3] with base_z
+          counts   : CUDA int32 [count] or None: the scans' point counts, read at every replay (GG_SCAN_DEVICE_COUNT)
+          xy, T_base_from_map, pose_origins, pose_base_z : CUDA tensors as in update_poses_from_device, or None
+          moved    : also allocate dev_moved (plan.moved)
+          labels, select, index : the outputs, as in run_scans_to_device
+        Returns a StepPlan.  Until it is closed the slots are bound to it (see the C header)."""
+        import torch
+
+        torch_, dev, stream, sel = self._device_call(select, index, None)
+        count = len(slots)
+        if (clouds is None) == (payloads is None):
+            raise ValueError("give exactly one of clouds and payloads")
+        keep = []
+
+        def dptr(t, dtype, shape, name):
+            if t is None:
+                return None
+            if t.dtype != dtype or t.device != dev or not t.is_contiguous() or t.numel() != int(np.prod(shape)):
+                raise ValueError(f"{name} must be a contiguous {dtype} tensor {shape} on {dev}")
+            keep.append(t)
+            return t.data_ptr()
+
+        d = StepDesc()
+        d.count = count
+        if clouds is not None:
+            n = []
+            for c in clouds:
+                nbytes = c.numel() * c.element_size()
+                if c.device != dev or not c.is_contiguous() or nbytes % 32:
+                    raise ValueError(f"clouds must be contiguous tensors of 32-byte records on {dev}")
+                n.append(nbytes // 32)
+            pp = np.array([c.data_ptr() for c in clouds], np.uint64)
+            keep += [clouds, pp]
+            d.dev_points = pp.ctypes.data
+        else:
+            steps = np.broadcast_to(np.asarray(point_step, np.int64), (count,))
+            n = []
+            for c, step in zip(payloads, steps):
+                nbytes = c.numel() * c.element_size()
+                if c.device != dev or not c.is_contiguous() or step <= 0 or nbytes % step:
+                    raise ValueError(f"payloads must be contiguous tensors on {dev} whose byte size is a multiple of point_step")
+                n.append(int(nbytes // step))
+            msgs = np.zeros(count, CLOUD_MSG_DTYPE)
+            msgs["data"] = [c.data_ptr() for c in payloads]
+            msgs["point_step"] = steps
+            msgs["field_offsets"] = np.asarray(field_offsets, np.int32).reshape(-1, 5)
+            keep += [payloads, msgs]
+            d.msgs = msgs.ctypes.data
+            if isinstance(T, torch.Tensor):
+                T = list(T.reshape(count, 12))
+            if T is not None:
+                if len(T) != count:
+                    raise ValueError("T needs one entry per scan")
+                tp = np.zeros(count, np.uint64)
+                Tarr = np.zeros((count, 12), np.float64)   # host transforms: read by gg_step_plan_create
+                for k, t in enumerate(T):
+                    if isinstance(t, torch.Tensor):
+                        tp[k] = dptr(t, torch.float64, (12,), "T")
+                    elif t is not None:
+                        Tarr[k] = np.asarray(t, np.float64).reshape(12)
+                        msgs["T_map_from_frame"][k] = Tarr.ctypes.data + 96 * k
+                keep += [tp, Tarr]
+                if tp.any():
+                    d.dev_T_map_from_frame = tp.ctypes.data
+        descs = self._device_descs(slots, n, origins, base_z, counts is not None)
+        sl = np.ascontiguousarray(slots, np.int32)
+        keep += [descs, sl]
+        d.scans = descs.ctypes.data
+        d.dev_n_points = dptr(counts, torch.int32, (count,), "counts")
+        d.poses = DevicePoses(dptr(xy, torch.float64, (count, 2), "xy"), dptr(T_base_from_map, torch.float64, (count, 12), "T_base_from_map"),
+                              dptr(pose_origins, torch.float32, (count, 3), "pose_origins"), dptr(pose_base_z, torch.float64, (count,), "pose_base_z"))
+        mv = torch.empty(count, dtype=torch.int32, device=dev) if moved else None
+        d.dev_moved = mv.data_ptr() if mv is not None else None
+        out, ptrs = self._device_outputs(torch_, dev, stream, n, labels, sel, index, [])
+        keep.append(ptrs)
+        d.outs = ptrs.ctypes.data
+        d.select = sel
+        d.dev_counts = out.counts.data_ptr() if out.counts is not None else None
+        p = C.c_void_p()
+        _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
+        return StepPlan(self, p, out, mv, keep)
 
     # shared by run_scans_to_device / run_cloud_msgs_to_device / run_merged_cloud_msgs_to_device
     def _device_call(self, select, index, stream):

@@ -292,6 +292,26 @@ struct SlotState {
     bool device_count = false;      // n_points / scan_points are the last scan's capacity: its count lives in CountTables::last
 };
 
+// While gg_step_plan_create records a step, run_groups takes its staging entries from here instead of the ring: per stream
+// group with slots in the plan one block of 3 * per_call[g] records (one entry per call of the step), each record array
+// (SlotParams, OutDest, UnpackDesc, PoseBits) contiguous in the block.  The records are filled in the host image; the
+// plan keeps a pristine device copy of it, and each replay first restores the working block of every group from it
+// (the pose and staging kernels patch the working records in place).  Nothing is committed from the host and no ring
+// event is recorded: the launches go to the recorder's capture streams.
+struct PlanRecorder {
+    struct Block {
+        size_t at = 0, bytes = 0;                    // byte range of the group's block in the image
+        size_t params = 0, dest = 0, unpack = 0, bits = 0;   // byte offsets of its arrays in the image
+        int per_call = 0, next = 0;                  // records per entry; records handed out
+        int first = 0;                               // index of the group's first record over all blocks
+    };
+    Block blk[kStreams];
+    cudaStream_t streams[kStreams] = {};             // capture branch of each group with slots in the plan
+    std::vector<unsigned char> host;                 // host image of the blocks
+    unsigned char* work = nullptr;                   // device working copy (what the recorded kernels address)
+    int records = 0;                                 // records over all blocks
+};
+
 // A caller's device byte range [begin, end) of one query set: its positions (input) or one of its outputs.
 struct ByteRange {
     uintptr_t begin, end;
@@ -387,6 +407,25 @@ struct gg_handle_s {
     EventProfiler* prof = nullptr;   // non-null while profiling is enabled
     double prof_ms[gg::K_NUM] = {};
     uint32_t prof_count[gg::K_NUM] = {};
+    // step plans
+    PlanRecorder* rec = nullptr;            // non-null while gg_step_plan_create records a step
+    std::vector<gg_step_plan> slot_plan;    // per slot: the plan it is bound to, or null
+    std::vector<gg_step_plan> plans;        // live plans (gg_destroy destroys them)
+};
+
+// A recorded step (gg_step_plan_create): its graph, the records it restores and the slots' host state after a step.
+struct gg_step_plan_s {
+    gg_handle h = nullptr;
+    std::vector<int> slots;
+    std::vector<SlotState> after;     // the slots' host state after a step (the same after every replay)
+    std::vector<int> groups;          // stream groups with slots in the plan
+    gg::View view{};                  // the handle's view the kernels were recorded with
+    unsigned char* pristine = nullptr;   // device image of the records as recorded
+    unsigned char* work = nullptr;       // the records the kernels address, restored at the start of every replay
+    const double** dev_T = nullptr;      // [records] caller transform of each UnpackDesc record, or null
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    int kernels = 0;                  // kernel launches per replay
 };
 
 namespace {
@@ -489,6 +528,23 @@ struct Staging {
         hbits = h->h_pose_bits ? h->h_pose_bits + at : nullptr;   // allocated on the first gg_update_poses_from_device
         dbits = h->d_pose_bits ? h->d_pose_bits + at : nullptr;
         return GG_OK;
+    }
+    // While a step is recorded: the next entry of group g's block (PlanRecorder).
+    int acquire_recorded(gg_handle h, int g) {
+        PlanRecorder::Block& b = h->rec->blk[g];
+        if (b.next + b.per_call > 3 * b.per_call) return fail(GG_E_STATE, "stream group %d: more entries than a recorded step holds", g);
+        const int at = b.next;
+        b.next += b.per_call;
+        unsigned char *host = h->rec->host.data(), *dev = h->rec->work;
+        hp = reinterpret_cast<gg::SlotParams*>(host + b.params) + at;
+        dp = reinterpret_cast<gg::SlotParams*>(dev + b.params) + at;
+        hdest = reinterpret_cast<gg::OutDest*>(host + b.dest) + at;
+        ddest = reinterpret_cast<gg::OutDest*>(dev + b.dest) + at;
+        hunpack = reinterpret_cast<gg::UnpackDesc*>(host + b.unpack) + at;
+        dunpack = reinterpret_cast<gg::UnpackDesc*>(dev + b.unpack) + at;
+        hbits = reinterpret_cast<int*>(host + b.bits) + at;
+        dbits = reinterpret_cast<int*>(dev + b.bits) + at;
+        return GG_OK;   // no query sets or point-info destinations: no call of a step uses them
     }
     int commit(cudaStream_t st) const {
         GG_CUDA(cudaMemcpyAsync(dp, hp, (size_t)m * sizeof(gg::SlotParams), cudaMemcpyHostToDevice, st));
@@ -598,7 +654,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
         bool work = false;
         for (int i = 0; i < count; ++i) {
             if (stream_index(h, slots[i]) != g) continue;
-            if (e.m == 0 && (rc = e.acquire(h))) return rc;
+            if (e.m == 0 && (rc = h->rec ? e.acquire_recorded(h, g) : e.acquire(h))) return rc;
             work |= fill(i, e);
             if ((e.position || e.count) && e.hbits) {
                 int bits = 0;
@@ -615,9 +671,10 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
             ++e.m;
         }
         if (e.m == 0) continue;
-        cudaStream_t st = h->streams[g];
+        // a recorded step launches on its capture branches, and its records come from the plan's image
+        cudaStream_t st = h->rec ? h->rec->streams[g] : h->streams[g];
         if (work) {
-            if ((rc = e.commit(st))) return rc;
+            if (!h->rec && (rc = e.commit(st))) return rc;
             if (e.stage) h->launches += gg::launch_stage_poses(h->poses, h->counts, e.dp, e.dbits, e.m, st, h->prof);
             if (fenced) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
             const int n = launch(e, st);
@@ -625,7 +682,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
             h->launches += n;
             GG_CUDA(cudaGetLastError());
         }
-        if ((rc = e.release(h, st))) return rc;
+        if (!h->rec && (rc = e.release(h, st))) return rc;
         if (fenced) {
             GG_CUDA(cudaEventRecord(h->caller_out[g], st));
             GG_CUDA(cudaStreamWaitEvent(caller, h->caller_out[g], 0));
@@ -901,18 +958,35 @@ int run_phase(gg_handle h, int slot, double base_z, Launch&& launch) {
     return run_groups(h, 1, &slot, false, nullptr, fill, launch);
 }
 
-// A call that needs the map position on the host: a device-owned position is read back once the slot's stream group
-// has finished what is enqueued (a host wait), and the slot is host-owned again.
-int take_position_back(gg_handle h, int slot) {
-    SlotState& s = h->slots[slot];
-    if (!s.device_position) return GG_OK;
+// The calls that would give a slot a host position or change the configuration a step plan's records carry by value
+// are refused on a slot bound to a plan.
+int check_unbound(gg_handle h, int slot, const char* call) {
+    if (h->slot_plan[slot]) return fail(GG_E_STATE, "slot %d is bound to a step plan: %s is refused until gg_step_plan_destroy", slot, call);
+    return GG_OK;
+}
+
+// The device-owned position of a slot, once the slot's stream group has finished what is enqueued (a host wait).
+int read_device_position(gg_handle h, int slot, double xy[2]) {
     GG_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = stream_of(h, slot);
     double2 p;
     GG_CUDA(cudaMemcpyAsync(&p, h->poses.position + slot, sizeof(p), cudaMemcpyDeviceToHost, st));
     GG_CUDA(cudaStreamSynchronize(st));
-    s.px = p.x;
-    s.py = p.y;
+    xy[0] = p.x;
+    xy[1] = p.y;
+    return GG_OK;
+}
+
+// A call that needs the map position on the host: a device-owned position is read back once the slot's stream group
+// has finished what is enqueued (a host wait), and the slot is host-owned again.
+int take_position_back(gg_handle h, int slot) {
+    SlotState& s = h->slots[slot];
+    if (!s.device_position) return GG_OK;
+    double xy[2] = {0.0, 0.0};
+    int rc = read_device_position(h, slot, xy);
+    if (rc) return rc;
+    s.px = xy[0];
+    s.py = xy[1];
     s.device_position = false;
     return GG_OK;
 }
@@ -985,6 +1059,7 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     h->resolution = resolution;
     gg_default_config(&h->cfg);
     h->slots.resize(n_slots);
+    h->slot_plan.assign((size_t)n_slots, nullptr);
     h->slot_cfg.assign((size_t)n_slots, h->cfg);
     {
         gg::CfgConst kc;
@@ -1144,6 +1219,7 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
 int gg_destroy(gg_handle h) {
     if (!h) return GG_OK;
     cudaSetDevice(h->device);
+    while (!h->plans.empty()) gg_step_plan_destroy(h->plans.back());
     cudaDeviceSynchronize();
     delete h->prof;
     delete h->packer;
@@ -1193,6 +1269,7 @@ int gg_spiral_schedule_info(gg_handle h, int* levels, int* visits, int* max_per_
 
 int gg_set_config(gg_handle h, const gg_config* cfg) {
     if (!h || !cfg) return fail(GG_E_ARG, "null argument");
+    if (!h->plans.empty()) return fail(GG_E_STATE, "slots are bound to step plans: gg_set_config is refused until gg_step_plan_destroy");
     GG_CUDA(cudaSetDevice(h->device));
     int rc = gg_synchronize(h);  // kernels in flight keep the tables of the old configuration
     if (rc) return rc;
@@ -1214,6 +1291,7 @@ int gg_set_slot_config(gg_handle h, int slot, const gg_config* cfg) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (!cfg) return fail(GG_E_ARG, "null argument");
+    if ((rc = check_unbound(h, slot, "gg_set_slot_config"))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     // Every kernel that reads the slot's variant runs on the slot's stream: once that stream is idle, the old variant
     // is read by nobody if the slot was its last user (and may be rebuilt for the new constants below).  Other stream
@@ -1255,7 +1333,7 @@ int gg_get_slot_config(gg_handle h, int slot, gg_config* cfg) {
 
 int gg_init_map(gg_handle h, int slot, double x, double y, double z) {
     int rc = check_slot(h, slot);
-    if (rc) return rc;
+    if (rc || (rc = check_unbound(h, slot, "gg_init_map"))) return rc;
     if ((rc = take_position_back(h, slot))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     SlotState& s = h->slots[slot];
@@ -1273,6 +1351,8 @@ int gg_update_pose_batch(gg_handle h, int count, const int* slots, const double*
     if (count <= 0) return GG_OK;
     int rc;
     if ((rc = check_slots(h, count, slots))) return rc;
+    for (int i = 0; i < count; ++i)
+        if ((rc = check_unbound(h, slots[i], "gg_update_pose[_batch]"))) return rc;
     for (int i = 0; i < count; ++i)
         if ((rc = take_position_back(h, slots[i]))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
@@ -1307,6 +1387,7 @@ int gg_get_map_position(gg_handle h, int slot, double xy[2]) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (!xy) return fail(GG_E_ARG, "null argument");
+    if (h->slot_plan[slot]) return read_device_position(h, slot, xy);   // a bound slot stays device-owned
     if ((rc = take_position_back(h, slot))) return rc;
     xy[0] = h->slots[slot].px;
     xy[1] = h->slots[slot].py;
@@ -1315,7 +1396,7 @@ int gg_get_map_position(gg_handle h, int slot, double xy[2]) {
 
 int gg_set_map_position(gg_handle h, int slot, double x, double y) {
     int rc = check_slot(h, slot);
-    if (rc) return rc;
+    if (rc || (rc = check_unbound(h, slot, "gg_set_map_position"))) return rc;
     if ((rc = take_position_back(h, slot))) return rc;
     h->slots[slot].px = x;
     h->slots[slot].py = y;
@@ -1884,6 +1965,7 @@ int gg_filter_cloud(gg_handle h, int slot, const gg_point* points, size_t n, con
     if (rc) return rc;
     if (!origin) return fail(GG_E_ARG, "null origin");
     if (!h->slots[slot].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slot);
+    if ((rc = check_unbound(h, slot, "gg_filter_cloud"))) return rc;
     if ((rc = gg_upload_points(h, slot, points, n))) return rc;
     gg_scan_desc d;
     std::memset(&d, 0, sizeof(d));
@@ -1944,6 +2026,8 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
     int rc;
     if ((rc = check_host_counts(count, scans))) return rc;
     if ((rc = check_slots(h, count, scans, points))) return rc;
+    for (int i = 0; i < count; ++i)
+        if ((rc = check_unbound(h, scans[i].slot, "gg_filter_cloud_batch[_begin]"))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     if (h->host_pack && !h->packer) {
         // GG_HOST_THREADS forces a thread count; by default all usable CPUs (affinity, cgroup quota,
@@ -2616,6 +2700,265 @@ int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
     if ((rc = take_count_back(h, slot))) return rc;
     *n_points = h->slots[slot].scan_points;
     return GG_OK;
+}
+
+// ---- step plans -------------------------------------------------------------------------------
+namespace {
+size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+void free_plan(gg_step_plan p) {
+    if (p->exec) cudaGraphExecDestroy(p->exec);
+    if (p->graph) cudaGraphDestroy(p->graph);
+    if (p->pristine) cudaFree(p->pristine);
+    if (p->work) cudaFree(p->work);
+    if (p->dev_T) cudaFree(p->dev_T);
+    delete p;
+}
+
+// What gg_step_plan_create checks beyond the step's calls (those check their own arguments while the step is recorded).
+int check_step_desc(gg_handle h, const gg_step_desc& d) {
+    if (d.count <= 0) return fail(GG_E_ARG, "a step plan needs count > 0 scans, got %d", d.count);
+    if (!d.scans) return fail(GG_E_ARG, "null scans");
+    if (d.count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", d.count, h->n_slots);
+    if (!d.dev_points == !d.msgs) return fail(GG_E_ARG, "a step plan takes exactly one of dev_points and msgs");
+    if (d.dev_T_map_from_frame && !d.msgs) return fail(GG_E_ARG, "dev_T_map_from_frame needs msgs");
+    int rc;
+    for (int i = 0; i < d.count; ++i) {
+        const int slot = d.scans[i].slot;
+        if ((rc = check_slot(h, slot))) return rc;
+        if (h->slot_plan[slot]) return fail(GG_E_STATE, "slot %d is already bound to a step plan", slot);
+    }
+    if (!d.dev_T_map_from_frame) return GG_OK;
+    std::vector<uintptr_t> ts;
+    for (int k = 0; k < d.count; ++k) {
+        const uintptr_t t = reinterpret_cast<uintptr_t>(d.dev_T_map_from_frame[k]);
+        if (!t) continue;
+        if (t % alignof(double)) return fail(GG_E_ARG, "scan %d: dev_T_map_from_frame is not 8-byte aligned", k);
+        if (d.msgs[k].T_map_from_frame) return fail(GG_E_ARG, "scan %d: both a device and a host T_map_from_frame", k);
+        ts.push_back(t);
+    }
+    std::sort(ts.begin(), ts.end());
+    for (size_t j = 1; j < ts.size(); ++j)
+        if (ts[j] < ts[j - 1] + 12 * sizeof(double)) return fail(GG_E_ARG, "two dev_T_map_from_frame entries overlap");
+    return GG_OK;
+}
+
+// The step of plan p, recorded on the capture root `root` (gg_step_plan_create): per branch the restore of its records
+// and, where a payload takes a device transform, the transform staging; then the step's three calls.
+int record_step(gg_handle h, const gg_step_desc& d, const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root,
+                cudaEvent_t fork, gg_step_plan p) {
+    const PlanRecorder& r = *h->rec;
+    GG_CUDA(cudaEventRecord(fork, root));
+    for (int g : p->groups) {
+        const PlanRecorder::Block& b = r.blk[g];
+        cudaStream_t st = r.streams[g];
+        GG_CUDA(cudaStreamWaitEvent(st, fork, 0));
+        GG_CUDA(cudaMemcpyAsync(p->work + b.at, p->pristine + b.at, b.bytes, cudaMemcpyDeviceToDevice, st));
+        if (T_group[g])
+            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.unpack), p->dev_T + b.first, 3 * b.per_call, st);
+    }
+    int rc;
+    const gg_device_poses& q = d.poses;
+    if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, d.count, slots.data(), d.dev_n_points, root))) return rc;
+    if ((q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, d.count, slots.data(), &q, d.dev_moved, root)))
+        return rc;
+    if (d.dev_points) return gg_run_scans_to_device(h, d.count, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root);
+    return gg_run_cloud_msgs_to_device(h, d.count, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
+}
+
+// Everything the recorded kernels address that the step's calls would allocate on first use, and the spiral's shared
+// memory opt-in: a recording may not allocate, and the View it records must not change afterwards.
+int prepare_recording(gg_handle h) {
+    const size_t S = (size_t)h->n_slots;
+    int rc;
+    if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
+    if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
+    if (!h->counts.stored && (rc = dev_alloc(h, &h->counts.stored, S))) return rc;
+    if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
+    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
+    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    if ((rc = ensure_out_cloud(h))) return rc;
+    if (gg::prepare_scan_pipeline(h->view)) return fail(GG_E_CUDA, "spiral shared-memory opt-in: %s", cudaGetErrorString(cudaGetLastError()));
+    return GG_OK;
+}
+
+// gg_step_plan_create after check_step_desc and prepare_recording: lays out the record blocks, seeds the positions,
+// records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
+// step leaves in p->after.
+int record_plan(gg_handle h, const gg_step_desc& d, gg_step_plan p) {
+    const int count = d.count;
+    std::vector<int>& slots = p->slots;
+    slots.resize(count);
+    for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
+    PlanRecorder rec;
+    std::vector<char> T_group(kStreams, 0);
+    size_t at = 0;
+    for (int g = 0; g < h->n_streams; ++g) {
+        int c = 0;
+        for (int i = 0; i < count; ++i)
+            if (stream_index(h, slots[i]) == g) {
+                ++c;
+                if (d.dev_T_map_from_frame && d.dev_T_map_from_frame[i]) T_group[g] = 1;
+            }
+        if (c == 0) continue;
+        PlanRecorder::Block& b = rec.blk[g];
+        b.per_call = c;
+        b.first = rec.records;
+        rec.records += 3 * c;
+        b.at = b.params = at;
+        b.dest = at = align16(at + 3 * c * sizeof(gg::SlotParams));
+        b.unpack = at = align16(at + 3 * c * sizeof(gg::OutDest));
+        b.bits = at = align16(at + 3 * c * sizeof(gg::UnpackDesc));
+        at = align16(at + 3 * c * sizeof(int));
+        b.bytes = at - b.at;
+        p->groups.push_back(g);
+    }
+    rec.host.assign(at, 0);
+    GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->pristine), at));
+    GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->work), at));
+    rec.work = p->work;
+    if (d.dev_T_map_from_frame) GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->dev_T), (size_t)rec.records * sizeof(double*)));
+
+    // the slots' stream groups are idle from here on: nothing in flight reads or writes what is seeded below
+    for (int g : p->groups) GG_CUDA(cudaStreamSynchronize(h->streams[g]));
+    std::vector<SlotState> before(count);
+    for (int j = 0; j < count; ++j) before[j] = h->slots[slots[j]];
+    auto restore = [&] {
+        for (int j = 0; j < count; ++j) h->slots[slots[j]] = before[j];
+    };
+    for (int j = 0; j < count; ++j) {
+        SlotState& s = h->slots[slots[j]];
+        if (s.device_position || !s.have_map) continue;
+        const double2 q = make_double2(s.px, s.py);
+        const cudaError_t e = cudaMemcpy(h->poses.position + slots[j], &q, sizeof(q), cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            restore();
+            return fail(GG_E_CUDA, "seeding the device position of slot %d: %s", slots[j], cudaGetErrorString(e));
+        }
+        s.device_position = true;
+    }
+
+    cudaStream_t root = nullptr;
+    cudaEvent_t fork = nullptr;
+    int rc = GG_OK;
+    cudaError_t e = cudaStreamCreateWithFlags(&root, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fork, cudaEventDisableTiming);
+    for (int g : p->groups)
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&rec.streams[g], cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamBeginCapture(root, cudaStreamCaptureModeThreadLocal);
+    if (e != cudaSuccess) {
+        rc = fail(GG_E_CUDA, "step plan recording: %s", cudaGetErrorString(e));
+    } else {
+        EventProfiler* prof = h->prof;   // replays are not profiled: no event pairs in the graph
+        const uint64_t launches = h->launches;
+        h->prof = nullptr;
+        h->rec = &rec;
+        rc = record_step(h, d, slots, T_group, root, fork, p);
+        h->rec = nullptr;
+        h->prof = prof;
+        p->kernels = (int)(h->launches - launches);
+        h->launches = launches;
+        cudaGraph_t graph = nullptr;
+        e = cudaStreamEndCapture(root, &graph);
+        if (!rc && e != cudaSuccess) rc = fail(GG_E_CUDA, "step plan recording: %s", cudaGetErrorString(e));
+        if (rc && graph) cudaGraphDestroy(graph);
+        if (!rc) p->graph = graph;
+        cudaGetLastError();   // a failed recording leaves nothing behind
+    }
+    for (int g : p->groups)
+        if (rec.streams[g]) cudaStreamDestroy(rec.streams[g]);
+    if (fork) cudaEventDestroy(fork);
+    if (root) cudaStreamDestroy(root);
+    if (!rc) {
+        p->after.resize(count);
+        for (int j = 0; j < count; ++j) p->after[j] = h->slots[slots[j]];
+    }
+    // the recording ran nothing: the slots keep their state, with the seeded positions device-owned on success
+    restore();
+    if (rc) return rc;
+    for (int j = 0; j < count; ++j) h->slots[slots[j]].device_position = true;
+
+    // the records as recorded, the caller transforms of the payload records, and the executable graph
+    std::vector<const double*> T_rec(rec.records, nullptr);
+    for (int g : p->groups) {
+        const PlanRecorder::Block& b = rec.blk[g];
+        int j = b.first + b.next - b.per_call;   // the scan call's entry is the group's last
+        for (int i = 0; i < count; ++i)
+            if (stream_index(h, slots[i]) == g) T_rec[j++] = d.dev_T_map_from_frame ? d.dev_T_map_from_frame[i] : nullptr;
+    }
+    GG_CUDA(cudaMemcpy(p->pristine, rec.host.data(), at, cudaMemcpyHostToDevice));
+    if (p->dev_T) GG_CUDA(cudaMemcpy(p->dev_T, T_rec.data(), T_rec.size() * sizeof(double*), cudaMemcpyHostToDevice));
+    GG_CUDA(cudaGraphInstantiate(&p->exec, p->graph, 0));
+    std::memcpy(&p->view, &h->view, sizeof(p->view));   // bytewise: gg_step_plan_launch compares it bytewise
+    return GG_OK;
+}
+}  // namespace
+
+int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out) {
+    if (!out) return fail(GG_E_ARG, "null out pointer");
+    *out = nullptr;
+    if (!h || !desc) return fail(GG_E_ARG, "null argument");
+    int rc;
+    if ((rc = check_step_desc(h, *desc))) return rc;
+    GG_CUDA(cudaSetDevice(h->device));
+    if ((rc = prepare_recording(h))) return rc;
+    gg_step_plan p = new gg_step_plan_s();
+    p->h = h;
+    if ((rc = record_plan(h, *desc, p))) {
+        free_plan(p);
+        return rc;
+    }
+    for (int s : p->slots) h->slot_plan[s] = p;
+    h->plans.push_back(p);
+    *out = p;
+    return GG_OK;
+}
+
+int gg_step_plan_launch(gg_step_plan p, void* stream) {
+    if (!p) return fail(GG_E_ARG, "null plan");
+    gg_handle h = p->h;
+    if (std::memcmp(&h->view, &p->view, sizeof(p->view)) != 0)
+        return fail(GG_E_STATE, "the handle's buffers changed since the plan was recorded (gg_filter_cloud_batch_begin swaps the label buffers)");
+    GG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    cudaStreamCaptureStatus status = cudaStreamCaptureStatusNone;
+    cudaGraph_t graph = nullptr;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t n_deps = 0;
+    GG_CUDA(cudaStreamGetCaptureInfo(st, &status, nullptr, &graph, &deps, &n_deps));
+    if (status == cudaStreamCaptureStatusInvalidated) return fail(GG_E_CUDA, "the stream's capture has been invalidated");
+    if (status == cudaStreamCaptureStatusActive) {
+        // a node of the caller's capture after its current dependencies; no fences with the handle's streams
+        cudaGraphNode_t node;
+        GG_CUDA(cudaGraphAddChildGraphNode(&node, graph, deps, n_deps, p->graph));
+        GG_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+    } else {
+        // after the work enqueued on the plan's stream groups, and before the work enqueued on them afterwards
+        for (int g : p->groups) {
+            GG_CUDA(cudaEventRecord(h->caller_out[g], h->streams[g]));
+            GG_CUDA(cudaStreamWaitEvent(st, h->caller_out[g], 0));
+        }
+        GG_CUDA(cudaGraphLaunch(p->exec, st));
+        GG_CUDA(cudaEventRecord(h->caller_in, st));
+        for (int g : p->groups) GG_CUDA(cudaStreamWaitEvent(h->streams[g], h->caller_in, 0));
+    }
+    for (size_t j = 0; j < p->slots.size(); ++j) h->slots[p->slots[j]] = p->after[j];
+    h->launches += (uint64_t)p->kernels;
+    h->inputs_busy = true;
+    return GG_OK;
+}
+
+int gg_step_plan_kernels(gg_step_plan p) { return p ? p->kernels : fail(GG_E_ARG, "null plan"); }
+
+int gg_step_plan_destroy(gg_step_plan p) {
+    if (!p) return GG_OK;
+    gg_handle h = p->h;
+    cudaSetDevice(h->device);
+    const cudaError_t e = cudaDeviceSynchronize();   // replays in flight read the plan's records
+    for (int s : p->slots) h->slot_plan[s] = nullptr;
+    h->plans.erase(std::remove(h->plans.begin(), h->plans.end(), p), h->plans.end());
+    free_plan(p);
+    return e == cudaSuccess ? GG_OK : fail(GG_E_CUDA, "gg_step_plan_destroy: %s", cudaGetErrorString(e));
 }
 
 }  // extern "C"

@@ -503,4 +503,12 @@ struct DevicePoses {
 int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, const int* bits, int count, const DevicePoses& in, cudaStream_t st,
                         Profiler* prof);
 
+// ---- step plans (gg_step_plan_create) ----
+// One thread per record: descs[j] takes the 12 doubles at T[j] as its transform (transform = 1) when T[j] is given, and
+// is left alone otherwise.  Runs on a replay's working records, before k_unpack_transform reads them.
+int launch_stage_transforms(UnpackDesc* descs, const double* const* T, int count, cudaStream_t st);
+// The dynamic shared-memory opt-in of the spiral kernel launch_scan_pipeline picks for v (it sets it at launch time
+// too; a recorded step sets it before the recording).
+int prepare_scan_pipeline(const View& v);
+
 }  // namespace gg

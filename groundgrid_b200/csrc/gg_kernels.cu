@@ -2373,6 +2373,20 @@ __global__ void __launch_bounds__(POSE_THREADS) k_store_counts(CountTables c, co
     c.stored[p.slot] = dev_n[p.pos];
 }
 
+// Step plans (gg_step_plan_create): record j of a replay's working UnpackDescs takes its sensor-to-map transform from
+// the caller's device memory, read at replay time; the copy is bitwise, so k_unpack_transform computes what it computes
+// for the same doubles staged from the host.
+__global__ void __launch_bounds__(POSE_THREADS) k_stage_transforms(UnpackDesc* __restrict__ descs, const double* const* __restrict__ T, int count) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count) return;
+    const double* t = T[j];
+    if (!t) return;
+    UnpackDesc& d = descs[j];
+#pragma unroll
+    for (int q = 0; q < 12; ++q) d.T[q] = t[q];
+    d.transform = 1;
+}
+
 // ------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------
@@ -2438,6 +2452,15 @@ static void enqueue_detect(const View& v, const SlotParams* batch, int count, cu
         k_detect_ldg<<<dim3(cdiv(v.k.N, DT_X), cdiv(v.k.N, DT_Y), count), dim3(DT_X, DT_Y), 0, st>>>(v, batch, count_layer, recompute);
 }
 
+// dynamic shared memory of the skewed / pipelined spiral launch for v
+static size_t skew_shm(const View& v) {
+    return (size_t)SKEW_RING * v.skew.irr_chunks * sizeof(uint4) + (size_t)SKEW_XCH_DEPTH * v.skew.lanes * sizeof(float2) +
+           (size_t)v.skew.irr_max * 9 * sizeof(float2) + (size_t)v.skew.irr_max * sizeof(float) + 16;
+}
+static size_t pipe_shm(const View& v) {
+    return (size_t)((v.levels + 4) & ~3) * sizeof(int) + (size_t)(SPIRAL_PIPE_DIST + 1) * v.spiral_threads * sizeof(float2);
+}
+
 int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int max_points, int stop_after, cudaStream_t st,
                          Profiler* prof, const CUtensorMap* layer_map) {
     int launches = 0;
@@ -2462,8 +2485,7 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
 
     const int threads = v.spiral_threads;
     if (v.skew.sk) {
-        const size_t shm = (size_t)SKEW_RING * v.skew.irr_chunks * sizeof(uint4) + (size_t)SKEW_XCH_DEPTH * v.skew.lanes * sizeof(float2) +
-                           (size_t)v.skew.irr_max * 9 * sizeof(float2) + (size_t)v.skew.irr_max * sizeof(float) + 16;
+        const size_t shm = skew_shm(v);
 #define GG_SKEW_LAUNCH(T, C)                                                                                                     \
     {                                                                                                                            \
         if (shm > 48 * 1024)   /* large maps: opt in to more dynamic shared memory */                                           \
@@ -2480,7 +2502,7 @@ int launch_scan_pipeline(const View& v, const SlotParams* batch, int count, int 
             GG_SKEW_LAUNCH(1024, 1)
 #undef GG_SKEW_LAUNCH
     } else if (v.spiral_recs) {
-        const size_t shm = (size_t)((v.levels + 4) & ~3) * sizeof(int) + (size_t)(SPIRAL_PIPE_DIST + 1) * threads * sizeof(float2);
+        const size_t shm = pipe_shm(v);
 #define GG_PIPE_LAUNCH(T)                                                                                                        \
     {                                                                                                                            \
         if (shm > 48 * 1024) cudaFuncSetAttribute(k_spiral_pipe<T, SPIRAL_PIPE_DIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm); \
@@ -2669,6 +2691,35 @@ int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* ba
 int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof) {
     GG_LAUNCH(K_STORE_COUNTS, k_store_counts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(c, batch, count, dev_n));
     return 1;
+}
+
+int launch_stage_transforms(UnpackDesc* descs, const double* const* T, int count, cudaStream_t st) {
+    k_stage_transforms<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(descs, T, count);
+    return 1;
+}
+
+int prepare_scan_pipeline(const View& v) {
+    const int threads = v.spiral_threads;
+    cudaError_t e = cudaSuccess;
+    if (v.skew.sk) {
+        const size_t shm = skew_shm(v);
+        if (shm > 48 * 1024) {
+            if (threads <= 320)
+                e = cudaFuncSetAttribute(k_spiral_skew<320, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+            else if (threads <= 448)
+                e = cudaFuncSetAttribute(k_spiral_skew<448, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+            else if (threads <= 768)
+                e = cudaFuncSetAttribute(k_spiral_skew<768, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+            else
+                e = cudaFuncSetAttribute(k_spiral_skew<1024, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+        }
+    } else if (v.spiral_recs) {
+        const size_t shm = pipe_shm(v);
+        if (shm > 48 * 1024)
+            e = threads == 512 ? cudaFuncSetAttribute(k_spiral_pipe<512, SPIRAL_PIPE_DIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm)
+                               : cudaFuncSetAttribute(k_spiral_pipe<1024, SPIRAL_PIPE_DIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm);
+    }
+    return e == cudaSuccess ? 0 : -1;
 }
 
 int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, const int* bits, int count, const DevicePoses& in, cudaStream_t st,

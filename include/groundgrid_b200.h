@@ -236,6 +236,9 @@ int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const 
  * _wait) first. */
 int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_n_points, void* stream);
 
+/* A whole step -- counts, poses and scans -- recorded once and replayed from caller GPU memory: see the step plans
+ * (gg_step_plan_create) after gg_run_cloud_msgs_to_device. */
+
 /* Replaces GroundSegmentation::filter_cloud (src/GroundSegmentation.cpp:50-197) for one slot with
  * HOST buffers: copies the cloud to the device, runs rasterise -> patch detection -> spiral
  * interpolation -> labelling, copies results back and returns when they are in host memory.
@@ -401,6 +404,68 @@ typedef struct gg_cloud_msg {
  * gg_upload_cloud_msg: null data with n_points > 0, point_step < 12, x, y or z absent, a field outside point_step. */
 int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const gg_cloud_msg* msgs,
                                 const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream);
+
+/* ---- step plans: one step of a batch recorded once as a CUDA graph and replayed ----
+ * For callers that keep every per-step input on the GPU and run their step as a CUDA graph (simulators stepping many
+ * robots, replay services, GPU perception stacks).  A plan is a fixed batch of `count` distinct slots and a fixed set of
+ * caller DEVICE buffers; the host issues the launches, copies and fences of a step once, at gg_step_plan_create, and a
+ * replay issues none of them.  Its step is, by definition, this call sequence on those slots and buffers:
+ *   1. if dev_n_points: gg_set_point_counts_from_device(dev_n_points);
+ *   2. if any pointer of `poses` is given: gg_update_poses_from_device(poses, dev_moved);
+ *   3. gg_run_scans_to_device over dev_points, or gg_run_cloud_msgs_to_device over msgs, with scans, outs, select and
+ *      dev_counts (stop_after 0).
+ * Every replay is bit-identical to that sequence run with the buffers' contents at replay time: labels, index, cloud,
+ * dev_counts, dev_moved, every layer, the map position, gg_get_output, point info, tallies and gg_last_scan_points.  The
+ * flags GG_SCAN_DEVICE_POSE and GG_SCAN_DEVICE_COUNT mean what they mean for those calls; the buffers' ADDRESSES are
+ * fixed for the plan's life, their contents are read at replay time.
+ *   dev_T_map_from_frame : NULL, or with msgs a host array [count] of DEVICE pointers (8-byte aligned, 12 doubles each,
+ *                          pairwise disjoint) or NULL entries.  Entry k given: payload k is transformed with the 12
+ *                          doubles found there AT REPLAY TIME, bit-identical to the same doubles given as
+ *                          msgs[k].T_map_from_frame (which must then be NULL).  Entry NULL: msgs[k]'s own rule (its host
+ *                          T_map_from_frame is read at gg_step_plan_create).
+ * Bound slots: a slot belongs to at most one plan, and its map position is device-owned from gg_step_plan_create (a
+ * host-owned position is seeded into the device table) until gg_step_plan_destroy.  On a bound slot, gg_update_pose[_batch],
+ * gg_set_map_position, gg_init_map, gg_set_slot_config and gg_filter_cloud[_batch[_begin]] return GG_E_STATE with
+ * nothing enqueued, and so does gg_set_config while any slot of the handle is bound: they would give the slot a host
+ * position or change the configuration the plan's records carry by value.  gg_get_map_position waits for the slot's
+ * stream group and returns the device position; the slot stays device-owned.  Every other call behaves as on any slot
+ * whose position is device-owned.
+ * gg_step_plan_create validates what the three calls validate, with the same codes, and also rejects (GG_E_ARG) a null
+ * handle, desc or out, count <= 0, both or neither of dev_points / msgs, dev_T_map_from_frame without msgs, an entry of
+ * it that is misaligned, overlaps another or goes with a non-NULL msgs[k].T_map_from_frame; GG_E_STATE: a slot bound to
+ * another plan.  It waits for the slots' stream groups, allocates what the recorded kernels address, and does not run
+ * the step.  Replays are not profiled (gg_profile_enable).
+ * gg_step_plan_launch(stream): stream is a cudaStream_t (NULL: the legacy default stream).
+ *   - stream not capturing: the contract of gg_run_scans_to_device -- the replay starts after everything already
+ *     enqueued on `stream` and on the plan's stream groups, work enqueued afterwards on `stream` or on those groups sees
+ *     it complete, and the host never waits.
+ *   - stream capturing (e.g. inside torch.cuda.graph): the plan's graph is added to the caller's capture as a child-graph
+ *     node after the capture's current dependencies.  There are no fences with the handle's streams (a capture cannot
+ *     depend on uncaptured work): the caller orders the handle's other calls on the same slots by passing them the same
+ *     stream, and the plan must outlive every graph it was captured into.
+ *   In both cases the slots' host state is what the call sequence leaves (the same after every replay), and
+ *   gg_kernel_launches grows by the plan's kernel count.  GG_E_STATE: the handle's buffers changed since the plan was
+ *   recorded (a gg_filter_cloud_batch_begin swaps the label buffers of the handle).
+ * gg_step_plan_destroy waits for the device, unbinds the slots (they keep their device-owned positions) and frees the
+ * plan; gg_destroy destroys the handle's remaining plans. */
+typedef struct gg_step_plan_s* gg_step_plan;
+typedef struct gg_step_desc {
+    int count;
+    const gg_scan_desc* scans;                  /* host [count]: slot, flags, n_points (the capacity with GG_SCAN_DEVICE_COUNT), origin, base_z */
+    const gg_point* const* dev_points;          /* host [count] of device clouds, or NULL ... */
+    const gg_cloud_msg* msgs;                   /* ... or host [count] of payloads (exactly one of the two) */
+    const double* const* dev_T_map_from_frame;  /* NULL or host [count] of device pointers / NULL entries (msgs only) */
+    const int32_t* dev_n_points;                /* device [count] or NULL: step 1 */
+    gg_device_poses poses;                      /* step 2; all four NULL: no step 2 */
+    int32_t* dev_moved;                         /* as in gg_update_poses_from_device */
+    const gg_scan_outputs* outs;                /* as in gg_run_scans_to_device */
+    unsigned select;
+    int32_t* dev_counts;
+} gg_step_desc;
+int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out);
+int gg_step_plan_launch(gg_step_plan plan, void* stream);
+int gg_step_plan_kernels(gg_step_plan plan);   /* kernels per replay */
+int gg_step_plan_destroy(gg_step_plan plan);
 
 /* ---- a multi-LiDAR rig: several sensor payloads per scan ----
  * One scan of a rig with several sensors arrives as one PointCloud2 payload per sensor, each in its own frame.  The
