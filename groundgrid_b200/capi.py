@@ -183,6 +183,15 @@ class DevicePoses(C.Structure):
     ]
 
 
+class DeviceResets(C.Structure):
+    """gg_device_resets: device addresses of the odometry poses and the mask of gg_init_maps_from_device (None = NULL)."""
+
+    _fields_ = [
+        ("xyz", C.c_void_p),
+        ("mask", C.c_void_p),
+    ]
+
+
 class StepDesc(C.Structure):
     """gg_step_desc: the fixed batch and caller device buffers of a step plan (gg_step_plan_create)."""
 
@@ -332,6 +341,8 @@ def load(build_if_missing=True):
         "gg_last_scan_points": (i, [vp, i, C.POINTER(sz)]),
         "gg_set_point_counts_from_device": (i, [vp, i, vp, vp, vp]),
         "gg_step_plan_create": (i, [vp, C.POINTER(StepDesc), C.POINTER(vp)]),
+        "gg_init_maps_from_device": (i, [vp, i, vp, C.POINTER(DeviceResets), vp]),
+        "gg_step_plan_create_with_resets": (i, [vp, C.POINTER(StepDesc), C.POINTER(DeviceResets), C.POINTER(vp)]),
         "gg_step_plan_launch": (i, [vp, vp]),
         "gg_step_plan_kernels": (i, [vp]),
         "gg_step_plan_destroy": (i, [vp]),
@@ -597,6 +608,38 @@ class GroundGridB200:
             with torch.cuda.stream(stream):
                 counts = counts.reshape(-1).to(torch.int32).contiguous()
         self.set_point_counts_from_device_ptrs(slots, counts.data_ptr() if count else None, stream.cuda_stream or None)
+
+    def init_maps_from_device_ptrs(self, slots, xyz_ptr, mask_ptr, stream_ptr):
+        """gg_init_maps_from_device with raw device addresses (ints, or None for NULL); stream_ptr None = the legacy
+        default stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        r = DeviceResets(xyz_ptr, mask_ptr)
+        _check(self._l.gg_init_maps_from_device(self._h, len(sl), _ptr(sl), C.byref(r), stream_ptr))
+
+    def init_maps_from_device(self, slots, xyz, mask=None, stream=None):
+        """init_map of the slots a device mask picks, at device poses (gg_init_maps_from_device).
+          xyz    : float64 [count, 3] odometry x, y, z, as init_map takes them
+          mask   : int32 [count], nonzero = start slots[k] over; None = every slot (which then needs no map beforehand)
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        Every tensor must be contiguous on this handle's device.  The call returns without waiting for the device; the
+        tensors may be freed or refilled right after it when they belong to `stream` (others are marked in use on
+        `stream`).  Afterwards every slot of the call has a device-owned position, keeps its stored device scan pose and
+        count, and refuses point_info_to_device until its next scan, reset or not (see the C header)."""
+        if xyz is None:
+            raise ValueError("xyz is required")
+        torch, dev, current, stream = self._layer_stream(stream)
+        count = len(slots)
+        ptrs = []
+        for name, t, dtype, shape in (("xyz", xyz, torch.float64, (count, 3)), ("mask", mask, torch.int32, (count,))):
+            if t is None:
+                ptrs.append(None)
+                continue
+            if t.dtype != dtype or t.device != dev or not t.is_contiguous() or t.numel() != int(np.prod(shape)) or (count and t.shape[0] != count):
+                raise ValueError(f"{name} must be a contiguous {dtype} tensor {shape} on {dev}")
+            if stream != current:
+                t.record_stream(stream)
+            ptrs.append(t.data_ptr() if count else None)
+        self.init_maps_from_device_ptrs(slots, ptrs[0], ptrs[1], stream.cuda_stream or None)
 
     def position(self, slot=0):
         xy = np.zeros(2, np.float64)
@@ -1008,11 +1051,12 @@ class GroundGridB200:
 
     def step_plan(self, slots, clouds=None, payloads=None, point_step=32, field_offsets=(0, 4, 8, 16, 20), T=None, origins="device",
                   base_z=None, counts=None, xy=None, T_base_from_map=None, pose_origins=None, pose_base_z=None, moved=False, labels=True,
-                  select="nonground", index=False):
+                  select="nonground", index=False, reset_xyz=None, reset_mask=None):
         """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
         Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
         pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
-        its inputs are given, and every replay is bit-identical to it run on the tensors' contents at replay time.
+        its inputs are given, and every replay is bit-identical to it run on the tensors' contents at replay time.  With
+        reset_xyz the step starts with init_maps_from_device(reset_xyz, reset_mask) (gg_step_plan_create_with_resets).
           clouds / payloads : exactly one: contiguous CUDA tensors as in run_scans_to_device / run_cloud_msgs_to_device;
                               their lengths are the scans' capacities
           point_step, field_offsets : the payloads' layout (one value or one per scan)
@@ -1024,6 +1068,8 @@ class GroundGridB200:
           xy, T_base_from_map, pose_origins, pose_base_z : CUDA tensors as in update_poses_from_device, or None
           moved    : also allocate dev_moved (plan.moved)
           labels, select, index : the outputs, as in run_scans_to_device
+          reset_xyz, reset_mask : CUDA float64 [count, 3] and int32 [count] (or None: every slot) as in
+                     init_maps_from_device, read at every replay; reset_mask without reset_xyz is an error
         Returns a StepPlan.  Until it is closed the slots are bound to it (see the C header)."""
         import torch
 
@@ -1098,7 +1144,13 @@ class GroundGridB200:
         d.select = sel
         d.dev_counts = out.counts.data_ptr() if out.counts is not None else None
         p = C.c_void_p()
-        _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
+        if reset_xyz is None:
+            if reset_mask is not None:
+                raise ValueError("reset_mask needs reset_xyz")
+            _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
+        else:
+            r = DeviceResets(dptr(reset_xyz, torch.float64, (count, 3), "reset_xyz"), dptr(reset_mask, torch.int32, (count,), "reset_mask"))
+            _check(self._l.gg_step_plan_create_with_resets(self._h, C.byref(d), C.byref(r), C.byref(p)))
         return StepPlan(self, p, out, mv, keep)
 
     # shared by run_scans_to_device / run_cloud_msgs_to_device / run_merged_cloud_msgs_to_device

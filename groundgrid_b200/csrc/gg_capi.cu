@@ -293,11 +293,12 @@ struct SlotState {
 };
 
 // While gg_step_plan_create records a step, run_groups takes its staging entries from here instead of the ring: per stream
-// group with slots in the plan one block of 3 * per_call[g] records (one entry per call of the step), each record array
+// group with slots in the plan one block of kStepCalls * per_call[g] records (one entry per call of the step), each record array
 // (SlotParams, OutDest, UnpackDesc, PoseBits) contiguous in the block.  The records are filled in the host image; the
 // plan keeps a pristine device copy of it, and each replay first restores the working block of every group from it
 // (the pose and staging kernels patch the working records in place).  Nothing is committed from the host and no ring
 // event is recorded: the launches go to the recorder's capture streams.
+constexpr int kStepCalls = 4;   // calls of a recorded step: resets, counts, poses, scans
 struct PlanRecorder {
     struct Block {
         size_t at = 0, bytes = 0;                    // byte range of the group's block in the image
@@ -532,7 +533,7 @@ struct Staging {
     // While a step is recorded: the next entry of group g's block (PlanRecorder).
     int acquire_recorded(gg_handle h, int g) {
         PlanRecorder::Block& b = h->rec->blk[g];
-        if (b.next + b.per_call > 3 * b.per_call) return fail(GG_E_STATE, "stream group %d: more entries than a recorded step holds", g);
+        if (b.next + b.per_call > kStepCalls * b.per_call) return fail(GG_E_STATE, "stream group %d: more entries than a recorded step holds", g);
         const int at = b.next;
         b.next += b.per_call;
         unsigned char *host = h->rec->host.data(), *dev = h->rec->work;
@@ -600,10 +601,10 @@ struct SlotList {
 };
 
 // The checks of every call on a list of slots, in this order: at most n_slots entries, then per entry a slot in range,
-// no slot twice (the scans of a batch run concurrently), an initialised map and, for a list of scans, at most pcap points
-// and (with `clouds`) a cloud for every non-empty scan.  h->seen_scratch is free again when it returns, so a checked call
-// may run checked sub-batches.
-int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* clouds = nullptr) {
+// no slot twice (the scans of a batch run concurrently), an initialised map (unless need_map is false) and, for a list of
+// scans, at most pcap points and (with `clouds`) a cloud for every non-empty scan.  h->seen_scratch is free again when it
+// returns, so a checked call may run checked sub-batches.
+int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* clouds = nullptr, bool need_map = true) {
     if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
     std::vector<unsigned char>& seen = h->seen_scratch;
     seen.assign((size_t)h->n_slots, 0);
@@ -612,7 +613,7 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
         const int slot = slots[i];
         if ((rc = check_slot(h, slot))) return rc;
         if (seen[slot]++) return fail(GG_E_ARG, "slot %d appears twice in one batch (scans of a batch run concurrently)", slot);
-        if (!h->slots[slot].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slot);
+        if (need_map && !h->slots[slot].have_map) return fail(GG_E_STATE, "slot %d: map not initialised", slot);
         if (!slots.scans) continue;
         if ((slots.scans[i].flags & GG_SCAN_DEVICE_POSE) && !h->slots[slot].device_scan_pose)
             return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_POSE without a device scan pose since gg_init_map", slot);
@@ -1919,7 +1920,8 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_cell_stats",  "k_detect",        "k_spiral",           "k_label",         "k_roll_gather",
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
-                                           "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve", "k_store_counts"};
+                                           "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve", "k_store_counts",
+                                           "k_reset_maps"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2693,6 +2695,53 @@ int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, co
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
+// Map resets from device memory: per stream group one k_reset_maps over the group's slots.  The host cannot see the mask,
+// so every slot of the call leaves it in the same state: a device-owned position (k_reset_maps seeds the host-owned
+// positions of masked-off slots), the stored scan pose and count kept, the last scan's outputs still readable, and its
+// point info refused until the next scan, as after a device roll.
+int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_device_resets* resets, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0) return GG_OK;
+    if (!slots || !resets || !resets->xyz) return fail(GG_E_ARG, "null argument");
+    const gg_device_resets& in = *resets;
+    if (reinterpret_cast<uintptr_t>(in.xyz) % alignof(double)) return fail(GG_E_ARG, "xyz is not 8-byte aligned");
+    if (reinterpret_cast<uintptr_t>(in.mask) % alignof(int32_t)) return fail(GG_E_ARG, "mask is not 4-byte aligned");
+    const gg::View& v = h->view;
+    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    if (ranges_overlap(in.xyz, (size_t)count * 3 * sizeof(double), v.layers, arena_bytes) ||
+        ranges_overlap(in.mask, (size_t)count * sizeof(int32_t), v.layers, arena_bytes))
+        return fail(GG_E_ARG, "xyz or mask overlaps the handle's layers");
+    int rc;
+    // without a mask every slot gets a map, so a slot needs none beforehand
+    if ((rc = check_slots(h, count, slots, nullptr, in.mask != nullptr))) return rc;
+    GG_CUDA(cudaSetDevice(h->device));
+    // the device tables and the staging of the pose bits, on first use (a handle that never asks has none)
+    const size_t S = (size_t)h->n_slots;
+    if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
+    if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
+    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
+    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    auto fill = [&](int i, Staging& e) {
+        SlotState& s = h->slots[slots[i]];
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        p.px = s.px;   // what a masked-off record seeds into the table, unless the table already holds the position
+        p.py = s.py;
+        e.hbits[e.m] = s.device_position ? gg::POSE_POSITION : 0;
+        e.pose_bits = true;
+        s.have_map = true;
+        s.device_position = s.device_rolled = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) {
+        return gg::launch_reset_maps(h->view, h->poses, e.dp, e.dbits, e.m, in.xyz, in.mask, st, h->prof);
+    };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
 int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
@@ -2716,7 +2765,8 @@ void free_plan(gg_step_plan p) {
 }
 
 // What gg_step_plan_create checks beyond the step's calls (those check their own arguments while the step is recorded).
-int check_step_desc(gg_handle h, const gg_step_desc& d) {
+int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets) {
+    if (resets && !resets->xyz) return fail(GG_E_ARG, "resets without xyz");
     if (d.count <= 0) return fail(GG_E_ARG, "a step plan needs count > 0 scans, got %d", d.count);
     if (!d.scans) return fail(GG_E_ARG, "null scans");
     if (d.count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", d.count, h->n_slots);
@@ -2743,10 +2793,11 @@ int check_step_desc(gg_handle h, const gg_step_desc& d) {
     return GG_OK;
 }
 
-// The step of plan p, recorded on the capture root `root` (gg_step_plan_create): per branch the restore of its records
-// and, where a payload takes a device transform, the transform staging; then the step's three calls.
-int record_step(gg_handle h, const gg_step_desc& d, const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root,
-                cudaEvent_t fork, gg_step_plan p) {
+// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_resets): per branch the restore of
+// its records and, where a payload takes a device transform, the transform staging; then the step's calls, the resets
+// (when given) first.
+int record_step(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, const std::vector<int>& slots, const std::vector<char>& T_group,
+                cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
     const PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
@@ -2755,10 +2806,11 @@ int record_step(gg_handle h, const gg_step_desc& d, const std::vector<int>& slot
         GG_CUDA(cudaStreamWaitEvent(st, fork, 0));
         GG_CUDA(cudaMemcpyAsync(p->work + b.at, p->pristine + b.at, b.bytes, cudaMemcpyDeviceToDevice, st));
         if (T_group[g])
-            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.unpack), p->dev_T + b.first, 3 * b.per_call, st);
+            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.unpack), p->dev_T + b.first, kStepCalls * b.per_call, st);
     }
     int rc;
     const gg_device_poses& q = d.poses;
+    if (resets && (rc = gg_init_maps_from_device(h, d.count, slots.data(), resets, root))) return rc;
     if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, d.count, slots.data(), d.dev_n_points, root))) return rc;
     if ((q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, d.count, slots.data(), &q, d.dev_moved, root)))
         return rc;
@@ -2785,7 +2837,7 @@ int prepare_recording(gg_handle h) {
 // gg_step_plan_create after check_step_desc and prepare_recording: lays out the record blocks, seeds the positions,
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
-int record_plan(gg_handle h, const gg_step_desc& d, gg_step_plan p) {
+int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, gg_step_plan p) {
     const int count = d.count;
     std::vector<int>& slots = p->slots;
     slots.resize(count);
@@ -2804,12 +2856,12 @@ int record_plan(gg_handle h, const gg_step_desc& d, gg_step_plan p) {
         PlanRecorder::Block& b = rec.blk[g];
         b.per_call = c;
         b.first = rec.records;
-        rec.records += 3 * c;
+        rec.records += kStepCalls * c;
         b.at = b.params = at;
-        b.dest = at = align16(at + 3 * c * sizeof(gg::SlotParams));
-        b.unpack = at = align16(at + 3 * c * sizeof(gg::OutDest));
-        b.bits = at = align16(at + 3 * c * sizeof(gg::UnpackDesc));
-        at = align16(at + 3 * c * sizeof(int));
+        b.dest = at = align16(at + kStepCalls * c * sizeof(gg::SlotParams));
+        b.unpack = at = align16(at + kStepCalls * c * sizeof(gg::OutDest));
+        b.bits = at = align16(at + kStepCalls * c * sizeof(gg::UnpackDesc));
+        at = align16(at + kStepCalls * c * sizeof(int));
         b.bytes = at - b.at;
         p->groups.push_back(g);
     }
@@ -2853,7 +2905,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, gg_step_plan p) {
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, slots, T_group, root, fork, p);
+        rc = record_step(h, d, resets, slots, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -2894,17 +2946,19 @@ int record_plan(gg_handle h, const gg_step_desc& d, gg_step_plan p) {
 }
 }  // namespace
 
-int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out) {
+int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out) { return gg_step_plan_create_with_resets(h, desc, nullptr, out); }
+
+int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
     if (!h || !desc) return fail(GG_E_ARG, "null argument");
     int rc;
-    if ((rc = check_step_desc(h, *desc))) return rc;
+    if ((rc = check_step_desc(h, *desc, resets))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     if ((rc = prepare_recording(h))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, p))) {
+    if ((rc = record_plan(h, *desc, resets, p))) {
         free_plan(p);
         return rc;
     }

@@ -181,7 +181,7 @@ constexpr int OUT_TILE = 1024;
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
     K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_STAGE_POSES, K_POSE_RESOLVE,
-    K_STORE_COUNTS,
+    K_STORE_COUNTS, K_RESET_MAPS,
     K_NUM
 };
 
@@ -502,6 +502,11 @@ struct DevicePoses {
 // moved[pos]; stores the scan pose.
 int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, const int* bits, int count, const DevicePoses& in, cudaStream_t st,
                         Profiler* prof);
+// Map resets (gg_init_maps_from_device): record j re-initialises the layers of batch[j].slot as k_init_map does at the
+// odometry xyz[batch[j].pos] and writes its x, y into the position table, unless mask (may be null) is zero at pos; a
+// masked-off record whose bits lack POSE_POSITION seeds its staged px / py into the table instead.
+int launch_reset_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const double* xyz, const int32_t* mask,
+                      cudaStream_t st, Profiler* prof);
 
 // ---- step plans (gg_step_plan_create) ----
 // One thread per record: descs[j] takes the 12 doubles at T[j] as its transform (transform = 1) when T[j] is given, and

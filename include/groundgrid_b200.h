@@ -236,7 +236,44 @@ int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const 
  * _wait) first. */
 int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_n_points, void* stream);
 
-/* A whole step -- counts, poses and scans -- recorded once and replayed from caller GPU memory: see the step plans
+/* ---- map resets from caller GPU memory ----
+ * GroundGrid::initGroundGrid (src/GroundGrid.cpp:50-80) for the slots a DEVICE mask picks, at DEVICE odometry poses,
+ * ordered on the caller's stream.  For callers that start maps over on the GPU's say-so (a simulator's episode resets
+ * and teleports, a relocalization), which would otherwise read the flags back to the host every step and, inside a step
+ * plan, destroy and re-record the plan.  Entry k of both arrays belongs to slots[k]. */
+typedef struct gg_device_resets {
+    const double* xyz;    /* DEVICE [count][3], 8-byte aligned: odometry x, y, z of initGroundGrid */
+    const int32_t* mask;  /* DEVICE [count] or NULL, 4-byte aligned: nonzero = re-initialise slots[k]; NULL = every slot */
+} gg_device_resets;
+
+/* Effect: for each k with mask[k] != 0 (every k when mask is NULL), slot slots[k] ends up bit-identical to
+ *   gg_init_map(slots[k], xyz[k][0], xyz[k][1], xyz[k][2]) run at the same point of the slot's stream: every layer
+ *   (GG_FLAG_FULL_LAYERS layers included) and the map position as exact doubles.  A slot whose mask entry is zero is
+ *   untouched.  Values are not validated, as in gg_init_map.
+ * stream: cudaStream_t; NULL is the legacy default stream.  The contract of gg_update_poses_from_device: the work starts
+ *   after everything already enqueued on `stream` and on the stream groups of the slots, work enqueued on `stream`
+ *   afterwards sees the reset, and nothing waits on the host except the flow control of the parameter staging ring.  xyz
+ *   and mask are consumed by the first kernel of each stream group, so a stream-ordered allocator may free or refill them
+ *   on `stream` right after the call.
+ * Host state afterwards -- the host cannot see the mask, so it is the same for every slot of the call, reset or not:
+ *   - the map position is device-owned, as after a device roll of gg_update_poses_from_device (a host-owned position of
+ *     a slot that is not reset is kept as it was); the host calls listed at gg_get_map_position wait for it;
+ *   - the stored device scan pose and stored point count are KEPT (gg_init_map forgets them): a GG_SCAN_DEVICE_POSE or
+ *     GG_SCAN_DEVICE_COUNT scan after the reset uses them;
+ *   - the last scan's outputs stay readable: gg_get_output, gg_eval_accumulate and gg_eval_counts_to_device read its
+ *     outputs and labels, which a reset does not touch;
+ *   - gg_point_info_to_device is GG_E_STATE until the slot's next scan, as after a device roll.
+ * With mask NULL a slot needs no map beforehand (it gets one); with a mask every slot must have one.  Slots bound to a
+ * step plan are accepted.
+ * count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle, slots, resets or xyz; count > n_slots; a slot out of range or repeated; xyz not 8-byte or mask
+ *              not 4-byte aligned; xyz or mask overlapping the handle's layers
+ *   GG_E_STATE a slot whose map is not initialised, when a mask is given
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_device_resets* resets, void* stream);
+
+/* A whole step -- resets, counts, poses and scans -- recorded once and replayed from caller GPU memory: see the step plans
  * (gg_step_plan_create) after gg_run_cloud_msgs_to_device. */
 
 /* Replaces GroundSegmentation::filter_cloud (src/GroundSegmentation.cpp:50-197) for one slot with
@@ -463,6 +500,12 @@ typedef struct gg_step_desc {
     int32_t* dev_counts;
 } gg_step_desc;
 int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out);
+/* A step plan whose step starts with a step 0: gg_init_maps_from_device(resets) over the plan's slots in desc->scans
+ * order, then steps 1-3 as above.  Every replay is bit-identical to that four-call sequence run with the buffers'
+ * contents at replay time (resets->xyz and resets->mask are read at replay time, so the mask may change every step).
+ * resets NULL is exactly gg_step_plan_create.  Validation: what gg_step_plan_create validates, what
+ * gg_init_maps_from_device validates, and GG_E_ARG for resets without xyz.  The plan adds one kernel per stream group. */
+int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out);
 int gg_step_plan_launch(gg_step_plan plan, void* stream);
 int gg_step_plan_kernels(gg_step_plan plan);   /* kernels per replay */
 int gg_step_plan_destroy(gg_step_plan plan);
