@@ -44,6 +44,11 @@ int fail(int code, const char* fmt, ...) {
 
 constexpr int kStreams = 8;   // upper bound; GG_STREAMS (default 8) picks how many are used
 constexpr int kRing = 256;
+// gg_filter_cloud_batch with host packing
+constexpr int kPackSlots = 32;           // staging-ring slots of the packers
+constexpr int kPackedCopyStreams = 4;    // H2D streams of packed clouds (raw clouds take 2 more)
+constexpr size_t kBusTarget = 8u << 20;  // raw clouds are added while fewer bytes than this are in flight on the bus
+constexpr int kRawDepth = 4;             // ... and fewer raw copies than this are pending
 
 // CUDA-event pairs around every kernel launch while profiling is enabled.
 struct EventProfiler : gg::Profiler {
@@ -130,8 +135,8 @@ class HostPacker {
     int threads() const { return (int)workers_.size(); }
 
     // Staging ring: packed job number `seq` (counted over the lifetime of the handle) is written to slot
-    // seq % slots.  The ring is small enough to stay in the last-level cache, so the packers' (plain) stores
-    // and the DMA reads that follow mostly stay out of DRAM; a slot is reused once `copied` -- the number of
+    // seq % slots.  The packers write it with streaming stores, which do not leave modified lines in the
+    // cores' caches for the DMA reads that follow to snoop; a slot is reused once `copied` -- the number of
     // packed jobs whose H2D copy has completed, advanced by the feeding thread -- has passed its last user.
     void set_ring(unsigned char* base, size_t stride, int slots) {
         ring_ = base;
@@ -198,10 +203,6 @@ class HostPacker {
     bool packed(const PackJob& job) const { return job.remaining.load(std::memory_order_acquire) <= 0; }
     bool help() { return work_one(false); }  // the calling thread packs one chunk if one can be started right away
 
-    static void pack_range(const gg_point* src, size_t n, unsigned char* dst, size_t i0, size_t i1, bool cached = false) {
-        gg::pack_cloud_range(src, n, dst, i0, i1, cached);
-    }
-
   private:
     bool work_one(bool may_wait) {
         std::vector<PackJob>* jobs;
@@ -230,7 +231,7 @@ class HostPacker {
         if (go) {
             PackJob& job = (*jobs)[chunk.first];
             const size_t i0 = (size_t)chunk.second * kChunk;
-            pack_range(job.src, job.n, slot_of(seq), i0, std::min(job.n, i0 + kChunk), true);
+            gg::pack_cloud_range(job.src, job.n, slot_of(seq), i0, std::min(job.n, i0 + kChunk));
             job.remaining.fetch_sub(1, std::memory_order_release);
         }
         const auto t2 = std::chrono::steady_clock::now();
@@ -377,9 +378,8 @@ struct gg_handle_s {
     HostPacker* packer = nullptr;    // created on the first packed batch call
     // gg_filter_cloud_batch[_begin] alternates between two sets of input / label buffers ("parity"), so the
     // clouds of batch t+1 can be packed and copied while the kernels of batch t still read theirs
-    unsigned char* h_stage = nullptr;  // pinned staging ring of the packers, [pack_slots][14 * pcap] (HostPacker::set_ring)
-    int pack_slots = 32;               // GG_PACK_RING
-    std::vector<cudaEvent_t> slot_ev;  // [pack_slots] H2D of the slot's current cloud
+    unsigned char* h_stage = nullptr;  // pinned staging ring of the packers, [kPackSlots][14 * pcap] (HostPacker::set_ring)
+    cudaEvent_t slot_ev[kPackSlots] = {};  // H2D of the slot's current cloud
     uint64_t pack_issued = 0;          // packed jobs whose copy has been enqueued (HostPacker::copied counts the completed ones)
     unsigned char* in_packed[2] = {};  // device, same shape
     gg_point* in_raw[2] = {};          // device 32-byte records; [0] is the slots' own buffer (view.points)
@@ -390,17 +390,13 @@ struct gg_handle_s {
     int host_pack = 1;               // GG_HOST_PACK=0 sends the 32-byte records as they are
     int launch_unit = 32;            // GG_LAUNCH_UNIT: scans per kernel launch set in gg_filter_cloud_batch
     int host_pack_mix = 1;           // GG_HOST_PACK=1 pins "pack everything"; default: pack and send raw side by side
-    cudaStream_t copy_in[10] = {}, copy_out = nullptr;  // [0, n_copy_in): packed clouds, then 2 for raw clouds;  // H2D / D2H of gg_filter_cloud_batch, never behind kernels
-    int n_copy_in = 4;                                   // GG_COPY_STREAMS
-    int main_help = 1;                                   // GG_MAIN_HELP
+    // H2D / D2H of gg_filter_cloud_batch, never behind kernels; copy_in: kPackedCopyStreams for packed clouds, then 2 for raw ones
+    cudaStream_t copy_in[kPackedCopyStreams + 2] = {}, copy_out = nullptr;
     CUtensorMap layer_map{};        // TMA descriptor of the layer arena (k_detect_tma); valid iff have_layer_map
     bool have_layer_map = false;
     bool inputs_busy = false;  // asynchronous work that reads or writes the slots' input buffers may be in flight
     std::vector<cudaEvent_t> batch_ev;                    // unit hand-over events of gg_filter_cloud_batch
-    cudaEvent_t raw_ev[8] = {};      // throttle of the raw copies issued by the mixing loop
-    int raw_gate = 2;                // GG_RAW_GATE (legacy, only with GG_BUS_TARGET_MB=0): no raw copies while this many packed clouds wait for the bus
-    size_t bus_target = 8u << 20;    // GG_BUS_TARGET_MB: raw clouds are added while fewer bytes than this are in flight on the bus
-    int raw_depth = 4;               // GG_RAW_DEPTH: raw copies in flight before the loop stops claiming more
+    cudaEvent_t raw_ev[kRawDepth] = {};  // throttle of the raw copies issued by the mixing loop
     size_t last_raw = 0, last_packed = 0;  // scans sent raw / packed by the last batch call
     size_t last_raw_bytes = 0, last_packed_bytes = 0;
     size_t last_feed_us = 0, last_total_us = 0;
@@ -1179,11 +1175,6 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
     }
 
     if (const char* e = getenv("GG_LAUNCH_UNIT")) h->launch_unit = std::max(1, atoi(e));
-    if (const char* e = getenv("GG_COPY_STREAMS")) h->n_copy_in = std::min(8, std::max(1, atoi(e)));
-    if (const char* e = getenv("GG_MAIN_HELP")) h->main_help = atoi(e);
-    if (const char* e = getenv("GG_RAW_GATE")) h->raw_gate = std::max(1, atoi(e));
-    if (const char* e = getenv("GG_BUS_TARGET_MB")) h->bus_target = (size_t)std::max(0, atoi(e)) << 20;
-    if (const char* e = getenv("GG_RAW_DEPTH")) h->raw_depth = std::min(8, std::max(1, atoi(e)));
     if (const char* e = getenv("GG_HOST_PACK")) {
         h->host_pack = atoi(e) ? 1 : 0;
         h->host_pack_mix = 0;
@@ -1227,17 +1218,18 @@ int gg_destroy(gg_handle h) {
     for (int g = 0; g < kStreams; ++g)
         if (h->d_raw[g]) cudaFree(h->d_raw[g]);
     if (h->h_stage) cudaFreeHost(h->h_stage);
-    for (cudaEvent_t e : h->slot_ev) cudaEventDestroy(e);
+    for (cudaEvent_t e : h->slot_ev)
+        if (e) cudaEventDestroy(e);
     for (int i = 0; i < kStreams; ++i)
         if (h->caller_out[i]) cudaEventDestroy(h->caller_out[i]);
     if (h->caller_in) cudaEventDestroy(h->caller_in);
     for (int e = 0; e < 2; ++e)
         if (h->batch_done[e]) cudaEventDestroy(h->batch_done[e]);
-    for (int e = 0; e < 8; ++e)
-        if (h->raw_ev[e]) cudaEventDestroy(h->raw_ev[e]);
+    for (cudaEvent_t e : h->raw_ev)
+        if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : h->batch_ev) cudaEventDestroy(e);
-    for (int e = 0; e < 10; ++e)
-        if (h->copy_in[e]) cudaStreamDestroy(h->copy_in[e]);
+    for (cudaStream_t s : h->copy_in)
+        if (s) cudaStreamDestroy(s);
     if (h->copy_out) cudaStreamDestroy(h->copy_out);
     for (void* p : h->dev_allocs) cudaFree(p);
     if (h->h_ring) cudaFreeHost(h->h_ring);
@@ -1998,9 +1990,9 @@ int batch_wait(gg_handle h, int parity) {
 int batch_prepare(gg_handle h) {
     int rc;
     if (!h->copy_out) {
-        for (int e = 0; e < 8; ++e) GG_CUDA(cudaEventCreateWithFlags(&h->raw_ev[e], cudaEventDisableTiming));
+        for (cudaEvent_t& e : h->raw_ev) GG_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (int e = 0; e < 2; ++e) GG_CUDA(cudaEventCreateWithFlags(&h->batch_done[e], cudaEventDisableTiming));
-        for (int e = 0; e < h->n_copy_in + 2; ++e) GG_CUDA(cudaStreamCreateWithFlags(&h->copy_in[e], cudaStreamNonBlocking));
+        for (cudaStream_t& s : h->copy_in) GG_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
         GG_CUDA(cudaStreamCreateWithFlags(&h->copy_out, cudaStreamNonBlocking));
         h->in_raw[0] = h->view.points;
         h->labels_buf[0] = h->view.labels;
@@ -2010,11 +2002,9 @@ int batch_prepare(gg_handle h) {
         if ((rc = dev_alloc(h, &h->labels_buf[1], (size_t)h->n_slots * h->pcap))) return rc;
         for (int e = 0; e < 2; ++e)
             if ((rc = dev_alloc(h, &h->in_packed[e], (size_t)h->n_slots * 14 * h->pcap))) return rc;
-        if (const char* e = getenv("GG_PACK_RING")) h->pack_slots = std::min(256, std::max(2, atoi(e)));
-        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_stage), (size_t)h->pack_slots * 14 * h->pcap, cudaHostAllocDefault));
-        h->slot_ev.resize(h->pack_slots);
+        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_stage), (size_t)kPackSlots * 14 * h->pcap, cudaHostAllocDefault));
         for (cudaEvent_t& e : h->slot_ev) GG_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        h->packer->set_ring(h->h_stage, 14 * h->pcap, h->pack_slots);
+        h->packer->set_ring(h->h_stage, 14 * h->pcap, kPackSlots);
     }
     return GG_OK;
 }
@@ -2062,7 +2052,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
         // Two ways to get a cloud across PCIe: repacked by host worker threads into x | y | z | ring
         // (14 useful bytes of every 32-byte record, costs CPU time) or as it is (costs bus time).  Both
         // resources are used at once: the packers walk the scans from the front; whenever fewer than
-        // raw_depth raw copies of this loop are pending, the calling thread takes the LAST scan nobody has
+        // kRawDepth raw copies of this loop are pending, the calling thread takes the LAST scan nobody has
         // started packing and sends it raw.  Whatever the CPU quota of the host, neither the packers
         // nor the bus sit idle.
         //
@@ -2075,7 +2065,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
         gg_point* const draw = h->in_raw[par];
         uint8_t* const dlab = h->labels_buf[par];
         h->view.labels = dlab;  // what gg_download_labels / gg_get_output read after this batch
-        const int KP = h->n_copy_in, KC = KP + 2;  // packed clouds rotate over the first KP copy streams, raw ones over the last 2
+        const int KP = kPackedCopyStreams, KC = KP + 2;  // packed clouds rotate over the first KP copy streams, raw ones over the last 2
         std::vector<int> order;
         for (int g = 0; g < h->n_streams; ++g)
             for (int i = 0; i < count; ++i)
@@ -2148,7 +2138,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
         const uint64_t seq_base = h->pack_issued;
         auto poll_copies = [&] {  // staging slots whose cloud has reached the device go back to the packers, in order
             uint64_t done = h->packer->copied.load(std::memory_order_relaxed);
-            while (done < h->pack_issued && cudaEventQuery(h->slot_ev[done % (uint64_t)h->pack_slots]) == cudaSuccess) ++done;
+            while (done < h->pack_issued && cudaEventQuery(h->slot_ev[done % kPackSlots]) == cudaSuccess) ++done;
             h->packer->copied.store(done, std::memory_order_release);
         };
         h->packer->pack_ns = 0;
@@ -2172,7 +2162,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
                 cudaStream_t cs = h->copy_in[n_copies++ % KP];
                 if (d.n_points)
                     GG_CUDA(cudaMemcpyAsync(dpk + (size_t)d.slot * 14 * h->pcap, h->packer->slot_of(h->pack_issued), 14 * n_pad, cudaMemcpyHostToDevice, cs));
-                GG_CUDA(cudaEventRecord(h->slot_ev[h->pack_issued % (uint64_t)h->pack_slots], cs));
+                GG_CUDA(cudaEventRecord(h->slot_ev[h->pack_issued % kPackSlots], cs));
                 ++h->pack_issued;
                 sent_packed[front] = 1;
                 ++h->last_packed;
@@ -2188,18 +2178,17 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
             // before the next packed cloud arrives, so a raw one is added; above it the bus is the limit and a raw cloud
             // would only delay cheaper packed ones.  The split therefore follows the measured rates of the packers and of
             // the bus on this host (CPU quota, ranks sharing the socket) instead of a fixed gate.
-            while (raw_done < raw_issued && cudaEventQuery(h->raw_ev[raw_done % h->raw_depth]) == cudaSuccess) ++raw_done;
+            while (raw_done < raw_issued && cudaEventQuery(h->raw_ev[raw_done % kRawDepth]) == cudaSuccess) ++raw_done;
             const uint64_t packed_in_flight = h->pack_issued - h->packer->copied.load(std::memory_order_relaxed);
             const size_t in_flight_bytes = (size_t)packed_in_flight * last_packed_bytes + (size_t)(raw_issued - raw_done) * last_raw_bytes;
-            const bool below_target = h->bus_target ? in_flight_bytes < h->bus_target : packed_in_flight < (uint64_t)h->raw_gate;
-            const bool bus_free = h->host_pack_mix && below_target && (raw_issued - raw_done) < h->raw_depth;
+            const bool bus_free = h->host_pack_mix && in_flight_bytes < kBusTarget && (raw_issued - raw_done) < kRawDepth;
             int j = bus_free ? h->packer->claim_raw_from_back() : -1;
             if (j >= 0) {
                 const gg_scan_desc& d = scans[order[j]];
                 if (d.n_points)
                     GG_CUDA(cudaMemcpyAsync(draw + (size_t)d.slot * h->pcap, jobs[j].src, d.n_points * sizeof(gg_point), cudaMemcpyHostToDevice,
                                             h->copy_in[KP + (raw_issued & 1)]));
-                GG_CUDA(cudaEventRecord(h->raw_ev[raw_issued % h->raw_depth], h->copy_in[KP + (raw_issued & 1)]));
+                GG_CUDA(cudaEventRecord(h->raw_ev[raw_issued % kRawDepth], h->copy_in[KP + (raw_issued & 1)]));
                 ++raw_issued;
                 ++h->last_raw;
                 h->last_raw_bytes += d.n_points * sizeof(gg_point);
@@ -2210,7 +2199,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
             }
             // nothing to enqueue: with the raw queue full (or no mixing) this thread packs a chunk as well
             const auto i0 = std::chrono::steady_clock::now();
-            if ((h->host_pack_mix && (bus_free || !h->main_help)) || !h->packer->help()) std::this_thread::yield();
+            if (bus_free || !h->packer->help()) std::this_thread::yield();
             idle_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - i0).count();
         }
         h->last_pack_us = h->packer->pack_ns.load() / 1000;
@@ -2298,19 +2287,16 @@ int gg_num_streams(gg_handle h) { return h ? h->n_streams : GG_E_ARG; }
 
 // host-only: the repacking of gg_filter_cloud_batch for one cloud (dst: 14 * ((n + 7) & ~7) bytes,
 // 32-byte aligned), chunked like the worker threads do it -- exported for the CPU tests
-static int pack_whole_cloud(const gg_point* src, size_t n, unsigned char* dst, bool cached) {
+int gg_host_pack_cloud(const gg_point* src, size_t n, unsigned char* dst) {
     if ((!src && n) || !dst) return GG_E_ARG;
     size_t i0 = 0;
     do {
         const size_t i1 = std::min(n, i0 + HostPacker::kChunk);
-        HostPacker::pack_range(src, n, dst, i0, i1, cached);
+        gg::pack_cloud_range(src, n, dst, i0, i1);
         i0 = i1;
     } while (i0 < n);
     return GG_OK;
 }
-int gg_host_pack_cloud(const gg_point* src, size_t n, unsigned char* dst) { return pack_whole_cloud(src, n, dst, false); }
-// same with plain (cache-allocating) stores
-int gg_host_pack_cloud_cached(const gg_point* src, size_t n, unsigned char* dst) { return pack_whole_cloud(src, n, dst, true); }
 
 // host-only self-test of the packer pool (no CUDA): `rounds` batches of n_jobs clouds go through a ring of
 // `ring_slots` staging slots; this thread plays the feeder of gg_filter_cloud_batch_begin -- it checks every packed
@@ -2333,7 +2319,7 @@ int gg_host_packer_selftest(int threads, int n_jobs, size_t n_points, int ring_s
         }
         want[j].assign(stride + 32, 0);
         unsigned char* w = want[j].data() + ((32 - (reinterpret_cast<uintptr_t>(want[j].data()) & 31)) & 31);
-        pack_whole_cloud(src[j].data(), n, w, false);
+        gg_host_pack_cloud(src[j].data(), n, w);
     }
     auto want_ptr = [&](int j) { return want[j].data() + ((32 - (reinterpret_cast<uintptr_t>(want[j].data()) & 31)) & 31); };
     std::vector<unsigned char> ring_mem((size_t)ring_slots * stride + 64);

@@ -8,7 +8,6 @@
 #include <cstdio>
 #include <thread>
 #include <cstdint>
-#include <cpuid.h>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -593,7 +592,6 @@ static void pack_sse2(const gg_point* src, size_t n, unsigned char* dst, size_t 
 // 32 records (1 KB) per iteration: every destination cache line (2 of x, y and z each, 1 of rings) is
 // written completely by back-to-back streaming stores, so each write-combining buffer drains as one full
 // line.  The rings come out of the upper record halves by the same in-lane transpose as the coordinates.
-template <bool NT>
 __attribute__((target("avx2"))) static inline void pack8_avx2(const gg_point* p, float* x, float* y, float* z, __m256i& ring_dwords) {
     // lane 0: records 0..3, lane 1: records 4..7; transpose 4x4 inside each 128-bit lane
     const __m256 a = _mm256_loadu2_m128(&p[4].x, &p[0].x), b = _mm256_loadu2_m128(&p[5].x, &p[1].x);
@@ -601,15 +599,9 @@ __attribute__((target("avx2"))) static inline void pack8_avx2(const gg_point* p,
     const __m256 t0 = _mm256_unpacklo_ps(a, b), t1 = _mm256_unpackhi_ps(a, b);
     const __m256 t2 = _mm256_unpacklo_ps(c, d), t3 = _mm256_unpackhi_ps(c, d);
     const __m256 vx = _mm256_shuffle_ps(t0, t2, 0x44), vy = _mm256_shuffle_ps(t0, t2, 0xEE), vz = _mm256_shuffle_ps(t1, t3, 0x44);  // x0..x3 | x4..x7
-    if (NT) {
-        _mm256_stream_ps(x, vx);
-        _mm256_stream_ps(y, vy);
-        _mm256_stream_ps(z, vz);
-    } else {
-        _mm256_store_ps(x, vx);
-        _mm256_store_ps(y, vy);
-        _mm256_store_ps(z, vz);
-    }
+    _mm256_stream_ps(x, vx);
+    _mm256_stream_ps(y, vy);
+    _mm256_stream_ps(z, vz);
     // upper halves: intensity | ring (u16) + 2 padding bytes | padding | padding
     const __m256 e = _mm256_loadu2_m128(&p[4].intensity, &p[0].intensity), f = _mm256_loadu2_m128(&p[5].intensity, &p[1].intensity);
     const __m256 g = _mm256_loadu2_m128(&p[6].intensity, &p[2].intensity), h = _mm256_loadu2_m128(&p[7].intensity, &p[3].intensity);
@@ -617,7 +609,9 @@ __attribute__((target("avx2"))) static inline void pack8_avx2(const gg_point* p,
     ring_dwords = _mm256_and_si256(_mm256_castps_si256(_mm256_shuffle_ps(u0, u2, 0xEE)), _mm256_set1_epi32(0xffff));
 }
 
-template <bool NT>
+// records to prefetch ahead of the 32 being packed: 256 records are 8 KB, which lands in L1 before they are read
+constexpr int kPackPrefetchRecords = 256;
+
 __attribute__((target("avx2"))) static void pack_avx2(const gg_point* src, size_t n, unsigned char* dst, size_t i0, size_t i1) {
     const size_t n_pad = (n + 7) & ~(size_t)7;
     float* x = reinterpret_cast<float*>(dst);
@@ -627,38 +621,25 @@ __attribute__((target("avx2"))) static void pack_avx2(const gg_point* src, size_
     size_t i = i0;
     const size_t stop = std::min(i1, n);
     const size_t end32 = i0 + ((stop - i0) & ~(size_t)31), end8 = i0 + ((stop - i0) & ~(size_t)7);
-    static const int pf_dist = getenv("GG_PACK_PF_DIST") ? atoi(getenv("GG_PACK_PF_DIST")) : 256;
-    static const int pf_hint = getenv("GG_PACK_PF_HINT") ? atoi(getenv("GG_PACK_PF_HINT")) : 1;
     for (; i < end32; i += 32) {
         const gg_point* p = src + i;
-        // 1 KB of records per iteration, prefetched `pf_dist` records ahead into L1 (prefetcht0 8 KB
-        // ahead by default; GG_PACK_PF_DIST / _HINT choose others)
-        const char* pf = reinterpret_cast<const char*>(p + pf_dist);
-        if (pf_hint == 0)
-            for (int l = 0; l < 16; ++l) _mm_prefetch(pf + 64 * l, _MM_HINT_NTA);
-        else if (pf_hint == 1)
-            for (int l = 0; l < 16; ++l) _mm_prefetch(pf + 64 * l, _MM_HINT_T0);
-        else if (pf_hint == 2)
-            for (int l = 0; l < 16; ++l) _mm_prefetch(pf + 64 * l, _MM_HINT_T2);
+        // 1 KB of records per iteration, prefetched into L1 (prefetcht0) 8 KB ahead
+        const char* pf = reinterpret_cast<const char*>(p + kPackPrefetchRecords);
+        for (int l = 0; l < 16; ++l) _mm_prefetch(pf + 64 * l, _MM_HINT_T0);
         __m256i r0, r1, r2, r3;
         // coordinates line by line: 16 records fill one 64-byte line of x, y and z each
-        pack8_avx2<NT>(p, x + i, y + i, z + i, r0);
-        pack8_avx2<NT>(p + 8, x + i + 8, y + i + 8, z + i + 8, r1);
-        pack8_avx2<NT>(p + 16, x + i + 16, y + i + 16, z + i + 16, r2);
-        pack8_avx2<NT>(p + 24, x + i + 24, y + i + 24, z + i + 24, r3);
+        pack8_avx2(p, x + i, y + i, z + i, r0);
+        pack8_avx2(p + 8, x + i + 8, y + i + 8, z + i + 8, r1);
+        pack8_avx2(p + 16, x + i + 16, y + i + 16, z + i + 16, r2);
+        pack8_avx2(p + 24, x + i + 24, y + i + 24, z + i + 24, r3);
         // packus interleaves the 128-bit lanes of its operands: restore record order with a 64-bit permute
         const __m256i w0 = _mm256_permute4x64_epi64(_mm256_packus_epi32(r0, r1), 0xD8), w1 = _mm256_permute4x64_epi64(_mm256_packus_epi32(r2, r3), 0xD8);
-        if (NT) {
-            _mm256_stream_si256(reinterpret_cast<__m256i*>(r + i), w0);
-            _mm256_stream_si256(reinterpret_cast<__m256i*>(r + i + 16), w1);
-        } else {
-            _mm256_store_si256(reinterpret_cast<__m256i*>(r + i), w0);
-            _mm256_store_si256(reinterpret_cast<__m256i*>(r + i + 16), w1);
-        }
+        _mm256_stream_si256(reinterpret_cast<__m256i*>(r + i), w0);
+        _mm256_stream_si256(reinterpret_cast<__m256i*>(r + i + 16), w1);
     }
     for (; i < end8; i += 8) {
         __m256i r0;
-        pack8_avx2<NT>(src + i, x + i, y + i, z + i, r0);
+        pack8_avx2(src + i, x + i, y + i, z + i, r0);
         const __m256i w = _mm256_permute4x64_epi64(_mm256_packus_epi32(r0, r0), 0xD8);
         _mm_store_si128(reinterpret_cast<__m128i*>(r + i), _mm256_castsi256_si128(w));
     }
@@ -666,38 +647,10 @@ __attribute__((target("avx2"))) static void pack_avx2(const gg_point* src, size_
     _mm_sfence();
 }
 
-// write the cache lines of [p, p + bytes) back to memory (they stay cached): the DMA engine then reads clean lines
-// instead of snooping modified ones out of the packing core's cache
-static bool have_clwb() {
-    unsigned a = 0, b = 0, c = 0, d = 0;
-    return __get_cpuid_count(7, 0, &a, &b, &c, &d) && (b & (1u << 24));
-}
-static inline void write_back(const void* p, size_t bytes) {
-    const char* q = reinterpret_cast<const char*>(reinterpret_cast<uintptr_t>(p) & ~(uintptr_t)63);
-    const char* e = reinterpret_cast<const char*>(p) + bytes;
-    for (; q < e; q += 64) __asm__ volatile("clwb %0" : "+m"(*const_cast<char*>(q)));
-}
-
-void pack_cloud_range(const gg_point* src, size_t n, unsigned char* dst, size_t i0, size_t i1, bool cached) {
+void pack_cloud_range(const gg_point* src, size_t n, unsigned char* dst, size_t i0, size_t i1) {
     static const bool have_avx2 = __builtin_cpu_supports("avx2");
-    // GG_PACK_STORE: 0 streaming stores (default), 1 plain stores, 2 plain stores + clwb of the chunk.  Plain stores
-    // pack fastest but the DMA engine then reads modified lines out of the cores' caches; clwb avoids that at the price
-    // of the packers' time; streaming stores into the small ring avoid both.
-    static const int store_mode = getenv("GG_PACK_STORE") ? atoi(getenv("GG_PACK_STORE")) : 0;
-    if (cached && store_mode == 0) cached = false;
-    if (have_avx2 && (reinterpret_cast<uintptr_t>(dst) & 31) == 0) {
-        if (cached)
-            pack_avx2<false>(src, n, dst, i0, i1);
-        else
-            pack_avx2<true>(src, n, dst, i0, i1);
-        if (cached && store_mode == 2 && have_clwb()) {
-            const size_t n_pad = (n + 7) & ~(size_t)7, e1 = (i1 >= n) ? n_pad : i1;
-            float* x = reinterpret_cast<float*>(dst);
-            for (int a = 0; a < 3; ++a) write_back(x + a * n_pad + i0, (e1 - i0) * 4);
-            write_back(reinterpret_cast<uint16_t*>(x + 3 * n_pad) + i0, (e1 - i0) * 2);
-            _mm_sfence();
-        }
-    }
+    if (have_avx2 && (reinterpret_cast<uintptr_t>(dst) & 31) == 0)
+        pack_avx2(src, n, dst, i0, i1);
     else
         pack_sse2(src, n, dst, i0, i1);
 }

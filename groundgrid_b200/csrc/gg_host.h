@@ -42,9 +42,7 @@ class ConfigRegistry {
 };
 void move_map(double res, double& px, double& py, double nx, double ny, int& shift_i, int& shift_j);
 void build_spiral_schedule(int n, std::vector<int>& level_start, std::vector<uint32_t>& visits);
-// cached: plain stores (destination meant to stay in the last-level cache until the DMA engine reads it)
-// instead of streaming stores
-void pack_cloud_range(const gg_point* src, size_t n, unsigned char* dst, size_t i0, size_t i1, bool cached = false);
+void pack_cloud_range(const gg_point* src, size_t n, unsigned char* dst, size_t i0, size_t i1);
 int usable_cpus();
 
 // Tables of the skewed-layout spiral kernel (k_spiral_skew), see gg_host.cpp:build_spiral_skew.
@@ -100,7 +98,6 @@ int gg_host_geometry_constants(double dimension_m, float resolution, unsigned fl
 int gg_host_config_constants(const gg_config* cfg, double* out);
 int gg_host_config_registry(int n_slots, int n_ops, const int* op_slot, const gg_config* op_cfg, int* out);
 int gg_host_pack_cloud(const gg_point* src, size_t n, unsigned char* dst);
-int gg_host_pack_cloud_cached(const gg_point* src, size_t n, unsigned char* dst);
 int gg_host_packer_selftest(int threads, int n_jobs, size_t n_points, int ring_slots, int rounds, int lag);
 int gg_host_spiral_plan(int n, float resolution, int* out);
 int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* lane_end, int* cell_home, int* irr_level_start, uint32_t* irr_recs, int irr_cap_words);

@@ -294,8 +294,8 @@ int gg_filter_cloud(gg_handle h, int slot, const gg_point* points, size_t n, con
  * PCIe is the bottleneck of this path.  Host worker threads (GG_HOST_THREADS; default: the usable
  * CPUs of the process minus one) repack clouds into pinned staging memory as x | y | z | ring
  * (14 of the 32 bytes of a PointXYZIR record are used by the algorithm) so that only those bytes
- * cross the bus; whenever the packers fall behind the bus (fewer than two packed clouds queued for
- * copying), the calling thread sends scans from the back of the batch, which no packer has reached
+ * cross the bus.  While fewer than 8 MiB are in flight on the bus and fewer than four raw copies are
+ * pending, the calling thread adds scans from the back of the batch, which no packer has reached
  * yet, as plain 32-byte records.  GG_HOST_PACK=1 packs every scan, GG_HOST_PACK=0 none.  Results
  * are identical in all modes.  Every scan runs with its slot's configuration (gg_set_slot_config). */
 int gg_filter_cloud_batch(gg_handle h, int count, const gg_scan_desc* scans, const gg_point* const* points,
