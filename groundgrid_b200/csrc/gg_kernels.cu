@@ -571,6 +571,10 @@ __global__ void __launch_bounds__(256) k_scatter(View v, const SlotParams* __res
 // ------------------------------------------------------------------------------------------
 constexpr int CS_THREADS = 256;
 
+// "pointsRaw" of a cell with r inside points.  The reference counts up by 1.0f (:234), which stops at 2^24 (2^24 + 1
+// rounds back to 2^24); raw_i counts in int, so the float it stores is clamped to where the float count stops.
+__device__ __forceinline__ float raw_count(int r) { return (float)min(r, 1 << 24); }
+
 template <bool FULL>
 __global__ void __launch_bounds__(CS_THREADS, FULL ? 2 : 4) k_cell_stats(View v, const SlotParams* __restrict__ batch) {
     const SlotParams& sp = batch[blockIdx.y];
@@ -589,7 +593,7 @@ __global__ void __launch_bounds__(CS_THREADS, FULL ? 2 : 4) k_cell_stats(View v,
             *reinterpret_cast<float4*>(v.layer(sp.slot, L_OBSTACLES) + t) = make_float4(0.f, 0.f, 0.f, 0.f);  // map["points"].setConstant(0.0), :147
             if (FULL) {
                 const int4 r = *reinterpret_cast<const int4*>(v.raw_i + coff + t);
-                *reinterpret_cast<float4*>(v.layer(sp.slot, L_RAW) + t) = make_float4((float)r.x, (float)r.y, (float)r.z, (float)r.w);
+                *reinterpret_cast<float4*>(v.layer(sp.slot, L_RAW) + t) = make_float4(raw_count(r.x), raw_count(r.y), raw_count(r.z), raw_count(r.w));
                 *reinterpret_cast<int4*>(v.raw_i + coff + t) = make_int4(0, 0, 0, 0);
             }
         }
@@ -600,7 +604,7 @@ __global__ void __launch_bounds__(CS_THREADS, FULL ? 2 : 4) k_cell_stats(View v,
             if ((k.N2 & 3) != 0) {
                 v.layer(sp.slot, L_OBSTACLES)[cell] = 0.0f;
                 if (FULL) {
-                    v.layer(sp.slot, L_RAW)[cell] = (float)v.raw_i[coff + cell];
+                    v.layer(sp.slot, L_RAW)[cell] = raw_count(v.raw_i[coff + cell]);
                     v.raw_i[coff + cell] = 0;
                 }
             }

@@ -82,7 +82,7 @@ def lib():
         L.ggo_set_layer.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
         L.ggo_filter_cloud.restype = C.c_long
         L.ggo_filter_cloud.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_double, C.c_int, C.c_int,
-                                       C.c_void_p, C.c_void_p, C.c_void_p]
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.ggo_interpolate_cell.argtypes = [C.c_void_p, C.c_int, C.c_int]
         L.ggo_spiral.argtypes = [C.c_void_p, C.c_double]
         L.ggo_detect_ground_patches.argtypes = [C.c_void_p]
@@ -160,20 +160,24 @@ class Oracle:
         if self._l.ggo_set_layer(self._h, name.encode(), _ptr(a)) != 0:
             raise KeyError(name)
 
-    def filter_cloud(self, points, origin, base_z, threads=1, stop_after=0, want_cloud=False):
+    def filter_cloud(self, points, origin, base_z, threads=1, stop_after=0, want_cloud=False, want_classes=False):
         """Returns (labels[u8 per input point: 0 absent / 49 ground / 99 non-ground],
-        out_index[u32: input index of each output point in reference order], out_cloud or None)."""
+        out_index[u32: input index of each output point in reference order], out_cloud or None); with want_classes
+        also classes[u8 per input point]: 0 outside the map, 1 kept, 2 kept in a border cell, 3 ignored, 4 ignored in a
+        border cell, 5 outlier (the classes of gg_get_point_classes)."""
         pts = np.ascontiguousarray(points, dtype=POINT_DTYPE)
         n = pts.shape[0]
         labels = np.zeros(n, np.uint8)
         out_index = np.zeros(n, np.uint32)
         out_cloud = np.zeros(n, POINT_DTYPE) if want_cloud else None
+        classes = np.zeros(n, np.uint8) if want_classes else None
         org = np.ascontiguousarray(origin, dtype=np.float32)
         nout = self._l.ggo_filter_cloud(self._h, _ptr(pts), n, _ptr(org), float(base_z), int(threads), int(stop_after),
-                                        _ptr(labels), _ptr(out_cloud), _ptr(out_index))
+                                        _ptr(labels), _ptr(out_cloud), _ptr(out_index), _ptr(classes))
         if nout < 0:
             raise RuntimeError("oracle: map not initialised")
-        return labels, out_index[:nout], (out_cloud[:nout] if want_cloud else None)
+        out = (labels, out_index[:nout], (out_cloud[:nout] if want_cloud else None))
+        return out + (classes,) if want_classes else out
 
     def interpolate_cell(self, x, y):
         self._l.ggo_interpolate_cell(self._h, x, y)

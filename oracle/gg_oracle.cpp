@@ -408,7 +408,7 @@ class Oracle {
     // 3 = after spiral interpolation (for per-phase parity tests; layers can then be read).
     // threads <= 0 -> cfg.thread_count.  labels[i] = 0 (absent from output), 49 or 99.
     size_t filter_cloud(const Point* cloud, size_t npts, const Point& origin, double base_z, int threads,
-                        int stop_after, uint8_t* labels, Point* out_cloud, uint32_t* out_index) {
+                        int stop_after, uint8_t* labels, Point* out_cloud, uint32_t* out_index, uint8_t* classes = nullptr) {
         reset_scan_layers();
         bind_hot();
         const int N = geo.n;
@@ -437,6 +437,17 @@ class Oracle {
         for (auto& part : outliers_list) outliers.insert(outliers.end(), part.begin(), part.end());
         for (auto& part : ignored_list) ignored.insert(ignored.end(), part.begin(), part.end());
         if (labels) std::memset(labels, 0, npts);
+        if (classes) {  // the point classes of the CUDA path (gg_get_point_classes >> 24): 0 outside, 1 / 2 kept, 3 / 4 ignored
+                        // (inner / border cell, :167-168), 5 outlier
+            std::memset(classes, 0, npts);
+            auto mark = [&](const std::vector<IndexedCell>& part, uint8_t inner) {
+                for (const IndexedCell& e : part)
+                    classes[e.first] = (N <= e.second.first + 3 || N <= e.second.second + 3) ? inner + 1 : inner;
+            };
+            mark(point_index, 1);
+            mark(ignored, 3);
+            for (size_t i : outliers) classes[i] = 5;
+        }
         if (stop_after == 1) return 0;
 
         if (threads == 1) {
@@ -535,10 +546,11 @@ int ggo_set_layer(void* h, const char* name, const float* src) {
     std::memcpy(o->layers[k].data(), src, o->layers[k].size() * sizeof(float));
     return 0;
 }
-// returns number of points in the output cloud; labels (npts bytes), out_cloud (npts records)
-// and out_index (npts u32: input index of every output point, reference order) may be NULL.
+// returns number of points in the output cloud; labels (npts bytes), out_cloud (npts records),
+// out_index (npts u32: input index of every output point, reference order) and classes (npts bytes: the class of
+// every input point, as filter_cloud above numbers them) may be NULL.
 long ggo_filter_cloud(void* h, const void* pts, size_t npts, const float* origin3, double base_z, int threads,
-                      int stop_after, uint8_t* labels, void* out_cloud, uint32_t* out_index) {
+                      int stop_after, uint8_t* labels, void* out_cloud, uint32_t* out_index, uint8_t* classes) {
     auto* o = static_cast<ggo::Oracle*>(h);
     if (!o->have_map) return -1;
     ggo::Point origin{};
@@ -546,7 +558,7 @@ long ggo_filter_cloud(void* h, const void* pts, size_t npts, const float* origin
     origin.y = origin3[1];
     origin.z = origin3[2];
     return static_cast<long>(o->filter_cloud(static_cast<const ggo::Point*>(pts), npts, origin, base_z, threads, stop_after,
-                                             labels, static_cast<ggo::Point*>(out_cloud), out_index));
+                                             labels, static_cast<ggo::Point*>(out_cloud), out_index, classes));
 }
 // Isolated pieces for known-answer tests.
 void ggo_interpolate_cell(void* h, int x, int y) {

@@ -40,7 +40,8 @@ def terrain_image(ground, points_raw):
     s = np.zeros((n, n), np.float32)
     for di in (-1, 0, 1):
         for dj in (-1, 0, 1):
-            s[1:-1, 1:-1] += points_raw[1 + di:n - 1 + di, 1 + dj:n - 1 + dj]   # exact small integers: order free
+            # integers; near 2^24 their fp32 sum rounds and depends on the order, but not on which side of 27 it lies
+            s[1:-1, 1:-1] += points_raw[1 + di:n - 1 + di, 1 + dj:n - 1 + dj]
     img[1:-1, 1:-1, 1] = (s[1:-1, 1:-1] >= 27).astype(np.float32)   # border cells: the reference reads out of bounds; defined as 0
     return img
 

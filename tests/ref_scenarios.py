@@ -587,6 +587,23 @@ def outlier_priors(make, rec, which):
         scan(m, rec, c.cloud(), c.origin, 0.0, c.name, layers=("points", "ground", "groundpatch", "minGroundHeight", "variance"))
 
 
+# ---- cells past 2^24 points and scans across the tile edges of the output order (tests/large_clouds.py) ---------------
+def crowded_cells(make, rec):
+    """Piles of 2^24 + 2 and 2^24 + 3 ignored points in one cell (the reference's float counts of "pointsRaw" and "points"
+    stop at 2^24), each on a fresh small map, and a scan of TILE_EDGE + 1 points after an ordinary one."""
+    import large_clouds as lc
+
+    for count, how in ((lc.FLOAT_STOP + 2, "ring"), (lc.FLOAT_STOP + 3, "near")):
+        m = make(*lc.PILE_GEOMETRY)
+        m.init_map(0.0, 0.0, 0.0)
+        pts, org, _, _ = lc.pile(count, how)
+        scan(m, rec, pts, org, 0.0, f"pile {count} {how}", cloud=False)
+    m = make(*lc.BOUNDARY_GEOMETRY)
+    m.init_map(0.0, 0.0, 0.0)
+    scan(m, rec, *lc.prior_scan(), 0.0, "prior")
+    scan(m, rec, *lc.boundary_cloud(lc.TILE_EDGE + 1), 0.0, f"{lc.TILE_EDGE + 1} points")
+
+
 SCENARIOS = {
     "expected_points_table": (expected_points_table, [()]),
     "cfg1_cfg2_64_beam_300": (cfg1_cfg2_64_beam_300, [()]),
@@ -606,6 +623,7 @@ SCENARIOS = {
     "nonfinite_confidence": (nonfinite_confidence, [()]),
     "detect_planes": (detect_planes, [(n,) for n in DETECT_SIZES]),
     "outlier_priors": (outlier_priors, [(w,) for w in OUTLIER_SIZES]),
+    "crowded_cells": (crowded_cells, [()]),
 }
 
 

@@ -96,6 +96,12 @@ def test_outlier_priors(which):
     rs.run("outlier_priors", rs.Oracle, which)
 
 
+def test_crowded_cells():
+    """Cells of 2^24 + 2 and 2^24 + 3 points, where the reference's float counts have stopped, and a scan whose output
+    order spans two tiles of the CUDA path's output scan (tests/large_clouds.py), on the oracle port."""
+    rs.run("crowded_cells", rs.Oracle)
+
+
 def test_reference_threading_as_shipped_runs():
     """thread_count = 8 (the shipped default: 8 insert + 4 patch-detection threads) is racy and therefore not a parity
     target; it must still run and label nearly everything like the reference's sequential execution (stored in
