@@ -210,6 +210,44 @@ class StepDesc(C.Structure):
     ]
 
 
+class StepReadouts(C.Structure):
+    """gg_step_readouts: the read-out calls of a step plan's step 4 (gg_step_plan_create_with_readouts); zero = not run."""
+
+    _fields_ = [
+        ("n_layer_names", C.c_int),
+        ("layer_names", C.c_void_p),
+        ("layers", C.c_void_p),
+        ("n_image_names", C.c_int),
+        ("image_names", C.c_void_p),
+        ("images", C.c_void_p),
+        ("image_ranges", C.c_void_p),
+        ("terrain_images", C.c_void_p),
+        ("n_sample_names", C.c_int),
+        ("sample_names", C.c_void_p),
+        ("samples", C.c_void_p),
+        ("sample_mode", C.c_int),
+        ("point_info", C.c_void_p),
+        ("eval_counts", C.c_void_p),
+    ]
+
+
+class PlanReadouts:
+    """The read-out tensors of a step plan (StepPlan.readouts), rewritten by every replay; None where not asked for.
+    Each has the shape and layout of the standalone method's result:
+      layers        : float32 [count, n_names, N, N] with column-major planes (get_layers_to_device)
+      images, ranges: uint8 [count, n_names, N, N] and float32 [count, n_names, 2] (layer_images_to_device)
+      terrain       : float32 [count, N, N, 3] (terrain_images_to_device)
+      positions     : the CUDA position tensors the plan reads at every replay (write the next step's positions into them)
+      samples, cells: per slot float32 [n_names, n] and int32 [n] (sample_layers_to_device)
+      codes, height : per slot int32 / float32 [n], n the scan's capacity; the first last_scan_points entries are
+                      written (point_info_to_device)
+      tallies       : int64 [count, 1024, 2], to which every replay adds its tallies (eval_counts_to_device(out=))"""
+
+    def __init__(self):
+        self.layers = self.images = self.ranges = self.terrain = None
+        self.positions = self.samples = self.cells = self.codes = self.height = self.tallies = None
+
+
 class DeviceOutputs:
     """What GroundGridB200.run_scans_to_device returns: per-scan views into flat CUDA tensors.
       labels[k] : uint8 [n_k], the labels of every input point (None unless asked for)
@@ -242,13 +280,15 @@ class StepPlan:
                             torch.cuda.graph capture it adds the step to the captured graph
       outputs             : DeviceOutputs of the step (allocated at capacity), rewritten by every replay
       moved               : int32 [count] dev_moved of the roll, or None
+      readouts            : PlanReadouts of the step's read-outs (all None for a plan without them)
       kernels             : kernel launches per replay
       close()             : gg_step_plan_destroy (waits for the device); the slots accept every call again
     The plan keeps its input and output tensors alive; write the next step's inputs into them (e.g. with copy_) on the
     stream before launching."""
 
-    def __init__(self, owner, p, outputs, moved, keep):
+    def __init__(self, owner, p, outputs, moved, keep, readouts=None):
         self._owner, self._p, self.outputs, self.moved, self._keep = owner, p, outputs, moved, keep
+        self.readouts = readouts if readouts is not None else PlanReadouts()
         owner._plans.add(self)
 
     def launch(self, stream=None):
@@ -343,6 +383,7 @@ def load(build_if_missing=True):
         "gg_step_plan_create": (i, [vp, C.POINTER(StepDesc), C.POINTER(vp)]),
         "gg_init_maps_from_device": (i, [vp, i, vp, C.POINTER(DeviceResets), vp]),
         "gg_step_plan_create_with_resets": (i, [vp, C.POINTER(StepDesc), C.POINTER(DeviceResets), C.POINTER(vp)]),
+        "gg_step_plan_create_with_readouts": (i, [vp, C.POINTER(StepDesc), C.POINTER(DeviceResets), C.POINTER(StepReadouts), C.POINTER(vp)]),
         "gg_step_plan_launch": (i, [vp, vp]),
         "gg_step_plan_kernels": (i, [vp]),
         "gg_step_plan_destroy": (i, [vp]),
@@ -750,7 +791,22 @@ class GroundGridB200:
         if mode not in SAMPLE_MODES:
             raise ValueError(f"mode must be one of {list(SAMPLE_MODES)}")
         L = len(names)
-        q = np.zeros(max(1, len(slots)), POSITIONS_DTYPE)
+        q, ns = self._position_sets(torch, dev, positions)
+        if out is not None:
+            if len(out) != len(slots):
+                raise ValueError("out needs one tensor per slot")
+            out = [self._stream_out(torch, dev, current, stream, o, (L, n), torch.float32, f"out[{k}]") for k, (o, n) in enumerate(zip(out, ns))]
+        out, cell = self._sample_outputs(torch, dev, stream, q, ns, L, out, cells)
+        if stream != current:
+            for p in positions:
+                p.record_stream(stream)
+        self.sample_layers_to_device_ptrs(slots, q[:len(slots)], names, mode, stream.cuda_stream or None)
+        return (out, cell) if cells else out
+
+    @staticmethod
+    def _position_sets(torch, dev, positions):
+        """(POSITIONS_DTYPE array with data, n, point_step and offsets of each set of positions, the sets' sizes)."""
+        q = np.zeros(max(1, len(positions)), POSITIONS_DTYPE)
         ns = []
         for k, p in enumerate(positions):
             if p.dtype != torch.float32 or p.device != dev or p.dim() != 2 or p.shape[1] < 2 or (p.shape[0] > 1 and p.stride(1) != 1):
@@ -761,15 +817,17 @@ class GroundGridB200:
                 raise ValueError(f"positions[{k}]: a row stride of {p.stride(0)} elements is no record layout")
             ns.append(n)
             q["data"][k], q["n"][k], q["point_step"][k], q["off_x"][k], q["off_y"][k] = p.data_ptr() if n else 0, n, step, 0, 4
+        return q, ns
+
+    @staticmethod
+    def _sample_outputs(torch, dev, stream, q, ns, L, out, cells):
+        """The lookup results of sets of ns[k] positions: `out` (or float32 [L, n] tensors allocated on `stream`) and, with
+        `cells`, int32 [n] tensors; their addresses are written into q.  Returns (out, cells or None)."""
         total = sum(ns)
         if out is None:
             with torch.cuda.stream(stream):
                 flat = torch.empty(L * total, dtype=torch.float32, device=dev)
             out = [t.view(L, n) for t, n in zip(torch.split(flat, [L * n for n in ns]), ns)]
-        else:
-            if len(out) != len(slots):
-                raise ValueError("out needs one tensor per slot")
-            out = [self._stream_out(torch, dev, current, stream, o, (L, n), torch.float32, f"out[{k}]") for k, (o, n) in enumerate(zip(out, ns))]
         cell = None
         if cells:
             with torch.cuda.stream(stream):
@@ -778,11 +836,7 @@ class GroundGridB200:
             if n:
                 q["dst"][k] = out[k].data_ptr()
                 q["cell"][k] = cell[k].data_ptr() if cells else 0
-        if stream != current:
-            for p in positions:
-                p.record_stream(stream)
-        self.sample_layers_to_device_ptrs(slots, q[:len(slots)], names, mode, stream.cuda_stream or None)
-        return (out, cell) if cells else out
+        return out, cell
 
     def layer_images_to_device_ptrs(self, slots, names, dst_ptr, range_ptr, stream_ptr):
         """gg_layer_images_to_device with raw device addresses: dst_ptr uint8 [count][n_names][N][N] (row-major planes),
@@ -1051,7 +1105,9 @@ class GroundGridB200:
 
     def step_plan(self, slots, clouds=None, payloads=None, point_step=32, field_offsets=(0, 4, 8, 16, 20), T=None, origins="device",
                   base_z=None, counts=None, xy=None, T_base_from_map=None, pose_origins=None, pose_base_z=None, moved=False, labels=True,
-                  select="nonground", index=False, reset_xyz=None, reset_mask=None):
+                  select="nonground", index=False, reset_xyz=None, reset_mask=None, layers=None, layer_images=None, terrain_images=False,
+                  samples=None, sample_names=("ground", "groundpatch"), sample_mode="nearest", sample_cells=False, point_info=None,
+                  tallies=None):
         """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
         Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
         pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
@@ -1070,6 +1126,16 @@ class GroundGridB200:
           labels, select, index : the outputs, as in run_scans_to_device
           reset_xyz, reset_mask : CUDA float64 [count, 3] and int32 [count] (or None: every slot) as in
                      init_maps_from_device, read at every replay; reset_mask without reset_xyz is an error
+        Read-outs: with any of these the step ends with a step 4 of read-out calls (gg_step_plan_create_with_readouts),
+        whose results land in plan.readouts (PlanReadouts) at every replay:
+          layers       : layer names, as get_layers_to_device
+          layer_images : layer names, as layer_images_to_device
+          terrain_images : True: terrain_images_to_device (needs the full layers)
+          samples      : one CUDA position tensor per slot, as sample_layers_to_device(positions); the plan looks up what
+                         they hold at each replay, and their row counts are fixed capacities.  sample_names,
+                         sample_mode and sample_cells are that call's names, mode and cells
+          point_info   : ("codes", "height"), either or both: point_info_to_device into buffers of the scans' capacities
+          tallies      : int64 CUDA tensor [count, 1024, 2] to which every replay adds its tallies (eval_counts_to_device(out=))
         Returns a StepPlan.  Until it is closed the slots are bound to it (see the C header)."""
         import torch
 
@@ -1143,15 +1209,79 @@ class GroundGridB200:
         d.outs = ptrs.ctypes.data
         d.select = sel
         d.dev_counts = out.counts.data_ptr() if out.counts is not None else None
+        ro, ro_c = self._plan_readouts(torch_, dev, stream, slots, n, keep, layers, layer_images, terrain_images, samples, sample_names,
+                                       sample_mode, sample_cells, point_info, tallies)
         p = C.c_void_p()
-        if reset_xyz is None:
-            if reset_mask is not None:
-                raise ValueError("reset_mask needs reset_xyz")
+        if reset_mask is not None and reset_xyz is None:
+            raise ValueError("reset_mask needs reset_xyz")
+        r = None if reset_xyz is None else DeviceResets(dptr(reset_xyz, torch.float64, (count, 3), "reset_xyz"),
+                                                        dptr(reset_mask, torch.int32, (count,), "reset_mask"))
+        if ro_c is not None:
+            _check(self._l.gg_step_plan_create_with_readouts(self._h, C.byref(d), None if r is None else C.byref(r), C.byref(ro_c), C.byref(p)))
+        elif r is None:
             _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
         else:
-            r = DeviceResets(dptr(reset_xyz, torch.float64, (count, 3), "reset_xyz"), dptr(reset_mask, torch.int32, (count,), "reset_mask"))
             _check(self._l.gg_step_plan_create_with_resets(self._h, C.byref(d), C.byref(r), C.byref(p)))
-        return StepPlan(self, p, out, mv, keep)
+        return StepPlan(self, p, out, mv, keep, ro)
+
+    def _plan_readouts(self, torch, dev, stream, slots, n, keep, layers, layer_images, terrain_images, samples, sample_names, sample_mode,
+                       sample_cells, point_info, tallies):
+        """step_plan's read-outs: (PlanReadouts with tensors allocated on `stream`, their StepReadouts or None for none).
+        n[k] is scan k's capacity."""
+        ro, r = PlanReadouts(), StepReadouts()
+        count, N = len(slots), self.n
+        given = False
+        with torch.cuda.stream(stream):
+            if layers:
+                _, r.n_layer_names, nm = self._layer_batch_args(slots, layers)
+                ro.layers = torch.empty((count, len(layers), N, N), dtype=torch.float32, device=dev).transpose(-1, -2)
+                r.layer_names, r.layers = C.cast(nm, C.c_void_p), ro.layers.data_ptr()
+                keep.append(nm)
+                given = True
+            if layer_images:
+                _, r.n_image_names, nm = self._layer_batch_args(slots, layer_images)
+                ro.images = torch.empty((count, len(layer_images), N, N), dtype=torch.uint8, device=dev)
+                ro.ranges = torch.empty((count, len(layer_images), 2), dtype=torch.float32, device=dev)
+                r.image_names, r.images, r.image_ranges = C.cast(nm, C.c_void_p), ro.images.data_ptr(), ro.ranges.data_ptr()
+                keep.append(nm)
+                given = True
+            if terrain_images:
+                ro.terrain = torch.empty((count, N, N, 3), dtype=torch.float32, device=dev)
+                r.terrain_images = ro.terrain.data_ptr()
+                given = True
+            if samples is not None:
+                if len(samples) != count:
+                    raise ValueError("samples needs one position tensor per slot")
+                if sample_mode not in SAMPLE_MODES:
+                    raise ValueError(f"sample_mode must be one of {list(SAMPLE_MODES)}")
+                q, ns = self._position_sets(torch, dev, samples)
+                ro.positions = list(samples)
+                ro.samples, ro.cells = self._sample_outputs(torch, dev, stream, q, ns, len(sample_names), None, sample_cells)
+                _, r.n_sample_names, nm = self._layer_batch_args(slots, sample_names)
+                r.sample_names, r.samples, r.sample_mode = C.cast(nm, C.c_void_p), q.ctypes.data, SAMPLE_MODES[sample_mode]
+                keep += [q, nm]
+                given = True
+            if point_info:
+                fields = (point_info,) if isinstance(point_info, str) else tuple(point_info)
+                if not set(fields) <= {"codes", "height"}:
+                    raise ValueError('point_info takes "codes", "height" or both')
+                o = np.zeros(max(1, count), POINT_INFO_DTYPE)
+                for field, dtype in (("codes", torch.int32), ("height", torch.float32)):
+                    if field in fields:
+                        views = list(torch.split(torch.empty(int(sum(n)), dtype=dtype, device=dev), list(n)))
+                        o[field][:count] = [t.data_ptr() if m else 0 for t, m in zip(views, n)]
+                        setattr(ro, field, views)
+                r.point_info = o.ctypes.data
+                keep.append(o)
+                given = True
+        if tallies is not None:
+            shape = (count, 1024, 2)
+            if tuple(tallies.shape) != shape or tallies.dtype != torch.int64 or tallies.device != dev or not tallies.is_contiguous():
+                raise ValueError(f"tallies must be a contiguous int64 tensor {shape} on {dev}")
+            ro.tallies = tallies
+            r.eval_counts = tallies.data_ptr()
+            given = True
+        return ro, (r if given else None)
 
     # shared by run_scans_to_device / run_cloud_msgs_to_device / run_merged_cloud_msgs_to_device
     def _device_call(self, select, index, stream):

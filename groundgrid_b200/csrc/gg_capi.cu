@@ -294,18 +294,19 @@ struct SlotState {
 };
 
 // While gg_step_plan_create records a step, run_groups takes its staging entries from here instead of the ring: per stream
-// group with slots in the plan one block of kStepCalls * per_call[g] records (one entry per call of the step), each record array
-// (SlotParams, OutDest, UnpackDesc, PoseBits) contiguous in the block.  The records are filled in the host image; the
-// plan keeps a pristine device copy of it, and each replay first restores the working block of every group from it
-// (the pose and staging kernels patch the working records in place).  Nothing is committed from the host and no ring
-// event is recorded: the launches go to the recorder's capture streams.
-constexpr int kStepCalls = 4;   // calls of a recorded step: resets, counts, poses, scans
+// group with slots in the plan one block of calls * per_call[g] records (one entry per call the step records), each record
+// array (SlotParams, OutDest, UnpackDesc, QueryDesc, PointInfoDest, PoseBits) contiguous in the block.  The records are
+// filled in the host image; the plan keeps a pristine device copy of it, and each replay first restores the working block
+// of every group from it (the pose and staging kernels patch the working records in place).  Nothing is committed from
+// the host and no ring event is recorded: the launches go to the recorder's capture streams.
 struct PlanRecorder {
     struct Block {
         size_t at = 0, bytes = 0;                    // byte range of the group's block in the image
-        size_t params = 0, dest = 0, unpack = 0, bits = 0;   // byte offsets of its arrays in the image
+        size_t params = 0, dest = 0, unpack = 0, query = 0, pinfo = 0, bits = 0;   // byte offsets of its arrays in the image
         int per_call = 0, next = 0;                  // records per entry; records handed out
+        int calls = 0;                               // entries the block holds
         int first = 0;                               // index of the group's first record over all blocks
+        int scan = -1;                               // index in the block of the scan call's first record
     };
     Block blk[kStreams];
     cudaStream_t streams[kStreams] = {};             // capture branch of each group with slots in the plan
@@ -529,7 +530,7 @@ struct Staging {
     // While a step is recorded: the next entry of group g's block (PlanRecorder).
     int acquire_recorded(gg_handle h, int g) {
         PlanRecorder::Block& b = h->rec->blk[g];
-        if (b.next + b.per_call > kStepCalls * b.per_call) return fail(GG_E_STATE, "stream group %d: more entries than a recorded step holds", g);
+        if (b.next + b.per_call > b.calls * b.per_call) return fail(GG_E_STATE, "stream group %d: more entries than a recorded step holds", g);
         const int at = b.next;
         b.next += b.per_call;
         unsigned char *host = h->rec->host.data(), *dev = h->rec->work;
@@ -539,9 +540,13 @@ struct Staging {
         ddest = reinterpret_cast<gg::OutDest*>(dev + b.dest) + at;
         hunpack = reinterpret_cast<gg::UnpackDesc*>(host + b.unpack) + at;
         dunpack = reinterpret_cast<gg::UnpackDesc*>(dev + b.unpack) + at;
+        hquery = reinterpret_cast<gg::QueryDesc*>(host + b.query) + at;
+        dquery = reinterpret_cast<gg::QueryDesc*>(dev + b.query) + at;
+        hpinfo = reinterpret_cast<gg::PointInfoDest*>(host + b.pinfo) + at;
+        dpinfo = reinterpret_cast<gg::PointInfoDest*>(dev + b.pinfo) + at;
         hbits = reinterpret_cast<int*>(host + b.bits) + at;
         dbits = reinterpret_cast<int*>(dev + b.bits) + at;
-        return GG_OK;   // no query sets or point-info destinations: no call of a step uses them
+        return GG_OK;
     }
     int commit(cudaStream_t st) const {
         GG_CUDA(cudaMemcpyAsync(dp, hp, (size_t)m * sizeof(gg::SlotParams), cudaMemcpyHostToDevice, st));
@@ -2779,12 +2784,34 @@ int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_device_resets* 
     return GG_OK;
 }
 
-// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_resets): per branch the restore of
+// Which calls of step 4 a plan's read-outs give (gg_step_plan_create_with_readouts): a call runs when any of its
+// fields is set, and then checks them as it always does.
+struct ReadoutCalls {
+    bool layers = false, images = false, terrain = false, samples = false, point_info = false, eval = false;
+    explicit ReadoutCalls(const gg_step_readouts* o) {
+        if (!o) return;
+        layers = o->n_layer_names || o->layer_names || o->layers;
+        images = o->n_image_names || o->image_names || o->images || o->image_ranges;
+        terrain = o->terrain_images != nullptr;
+        samples = o->n_sample_names || o->sample_names || o->samples;
+        point_info = o->point_info != nullptr;
+        eval = o->eval_counts != nullptr;
+    }
+    int count() const { return layers + images + terrain + samples + point_info + eval; }
+};
+
+// The calls a plan's step records: the resets, counts and poses when given, the scans, and the read-outs.
+int step_calls(const gg_step_desc& d, const gg_device_resets* resets, const gg_step_readouts* readouts) {
+    const gg_device_poses& q = d.poses;
+    return (resets != nullptr) + (d.dev_n_points != nullptr) + (q.xy || q.T_base_from_map || q.origin || q.base_z) + 1 + ReadoutCalls(readouts).count();
+}
+
+// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_readouts): per branch the restore of
 // its records and, where a payload takes a device transform, the transform staging; then the step's calls, the resets
-// (when given) first.
-int record_step(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, const std::vector<int>& slots, const std::vector<char>& T_group,
-                cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
-    const PlanRecorder& r = *h->rec;
+// (when given) first and the read-outs last.
+int record_step(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, const gg_step_readouts* readouts, const std::vector<int>& slots,
+                const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
+    PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
         const PlanRecorder::Block& b = r.blk[g];
@@ -2792,21 +2819,33 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
         GG_CUDA(cudaStreamWaitEvent(st, fork, 0));
         GG_CUDA(cudaMemcpyAsync(p->work + b.at, p->pristine + b.at, b.bytes, cudaMemcpyDeviceToDevice, st));
         if (T_group[g])
-            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.unpack), p->dev_T + b.first, kStepCalls * b.per_call, st);
+            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.unpack), p->dev_T + b.first, b.calls * b.per_call, st);
     }
     int rc;
+    const int n = d.count;
+    const int* sl = slots.data();
     const gg_device_poses& q = d.poses;
-    if (resets && (rc = gg_init_maps_from_device(h, d.count, slots.data(), resets, root))) return rc;
-    if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, d.count, slots.data(), d.dev_n_points, root))) return rc;
-    if ((q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, d.count, slots.data(), &q, d.dev_moved, root)))
-        return rc;
-    if (d.dev_points) return gg_run_scans_to_device(h, d.count, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root);
-    return gg_run_cloud_msgs_to_device(h, d.count, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
+    if (resets && (rc = gg_init_maps_from_device(h, n, sl, resets, root))) return rc;
+    if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
+    if ((q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, n, sl, &q, d.dev_moved, root))) return rc;
+    rc = d.dev_points ? gg_run_scans_to_device(h, n, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root)
+                      : gg_run_cloud_msgs_to_device(h, n, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
+    if (rc) return rc;
+    for (int g : p->groups) r.blk[g].scan = r.blk[g].next - r.blk[g].per_call;   // the payload records k_stage_transforms patches
+    const ReadoutCalls c(readouts);
+    const gg_step_readouts o = readouts ? *readouts : gg_step_readouts{};
+    if (c.layers && (rc = gg_get_layers_to_device(h, n, sl, o.n_layer_names, o.layer_names, o.layers, root))) return rc;
+    if (c.images && (rc = gg_layer_images_to_device(h, n, sl, o.n_image_names, o.image_names, o.images, o.image_ranges, root))) return rc;
+    if (c.terrain && (rc = gg_terrain_images_to_device(h, n, sl, o.terrain_images, root))) return rc;
+    if (c.samples && (rc = gg_sample_layers_to_device(h, n, sl, o.samples, o.n_sample_names, o.sample_names, o.sample_mode, root))) return rc;
+    if (c.point_info && (rc = gg_point_info_to_device(h, n, sl, o.point_info, root))) return rc;
+    if (c.eval && (rc = gg_eval_counts_to_device(h, n, sl, o.eval_counts, root))) return rc;
+    return GG_OK;
 }
 
 // Everything the recorded kernels address that the step's calls would allocate on first use, and the spiral's shared
 // memory opt-in: a recording may not allocate, and the View it records must not change afterwards.
-int prepare_recording(gg_handle h) {
+int prepare_recording(gg_handle h, const gg_step_readouts* readouts) {
     const size_t S = (size_t)h->n_slots;
     int rc;
     if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
@@ -2816,6 +2855,11 @@ int prepare_recording(gg_handle h) {
     if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
     if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
     if ((rc = ensure_out_cloud(h))) return rc;
+    const ReadoutCalls c(readouts);
+    if (c.images && (rc = ensure_image_partials(h))) return rc;
+    if (c.point_info && !h->d_pinfo && (rc = dev_alloc(h, &h->d_pinfo, (size_t)kRing * S))) return rc;
+    if (c.point_info && !h->h_pinfo)
+        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * kRing * S, cudaHostAllocDefault));
     if (gg::prepare_scan_pipeline(h->view)) return fail(GG_E_CUDA, "spiral shared-memory opt-in: %s", cudaGetErrorString(cudaGetLastError()));
     return GG_OK;
 }
@@ -2823,8 +2867,8 @@ int prepare_recording(gg_handle h) {
 // gg_step_plan_create after check_step_desc and prepare_recording: lays out the record blocks, seeds the positions,
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
-int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, gg_step_plan p) {
-    const int count = d.count;
+int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, const gg_step_readouts* readouts, gg_step_plan p) {
+    const int count = d.count, calls = step_calls(d, resets, readouts);
     std::vector<int>& slots = p->slots;
     slots.resize(count);
     for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
@@ -2840,14 +2884,18 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
             }
         if (c == 0) continue;
         PlanRecorder::Block& b = rec.blk[g];
+        const size_t m = (size_t)calls * c;
         b.per_call = c;
+        b.calls = calls;
         b.first = rec.records;
-        rec.records += kStepCalls * c;
+        rec.records += (int)m;
         b.at = b.params = at;
-        b.dest = at = align16(at + kStepCalls * c * sizeof(gg::SlotParams));
-        b.unpack = at = align16(at + kStepCalls * c * sizeof(gg::OutDest));
-        b.bits = at = align16(at + kStepCalls * c * sizeof(gg::UnpackDesc));
-        at = align16(at + kStepCalls * c * sizeof(int));
+        b.dest = at = align16(at + m * sizeof(gg::SlotParams));
+        b.unpack = at = align16(at + m * sizeof(gg::OutDest));
+        b.query = at = align16(at + m * sizeof(gg::UnpackDesc));
+        b.pinfo = at = align16(at + m * sizeof(gg::QueryDesc));
+        b.bits = at = align16(at + m * sizeof(gg::PointInfoDest));
+        at = align16(at + m * sizeof(int));
         b.bytes = at - b.at;
         p->groups.push_back(g);
     }
@@ -2891,7 +2939,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, resets, slots, T_group, root, fork, p);
+        rc = record_step(h, d, resets, readouts, slots, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -2920,7 +2968,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
     std::vector<const double*> T_rec(rec.records, nullptr);
     for (int g : p->groups) {
         const PlanRecorder::Block& b = rec.blk[g];
-        int j = b.first + b.next - b.per_call;   // the scan call's entry is the group's last
+        int j = b.first + b.scan;
         for (int i = 0; i < count; ++i)
             if (stream_index(h, slots[i]) == g) T_rec[j++] = d.dev_T_map_from_frame ? d.dev_T_map_from_frame[i] : nullptr;
     }
@@ -2935,16 +2983,21 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
 int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out) { return gg_step_plan_create_with_resets(h, desc, nullptr, out); }
 
 int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out) {
+    return gg_step_plan_create_with_readouts(h, desc, resets, nullptr, out);
+}
+
+int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, const gg_step_readouts* readouts,
+                                      gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
     if (!h || !desc) return fail(GG_E_ARG, "null argument");
     int rc;
     if ((rc = check_step_desc(h, *desc, resets))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
-    if ((rc = prepare_recording(h))) return rc;
+    if ((rc = prepare_recording(h, readouts))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, resets, p))) {
+    if ((rc = record_plan(h, *desc, resets, readouts, p))) {
         free_plan(p);
         return rc;
     }

@@ -504,7 +504,8 @@ int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out
  * order, then steps 1-3 as above.  Every replay is bit-identical to that four-call sequence run with the buffers'
  * contents at replay time (resets->xyz and resets->mask are read at replay time, so the mask may change every step).
  * resets NULL is exactly gg_step_plan_create.  Validation: what gg_step_plan_create validates, what
- * gg_init_maps_from_device validates, and GG_E_ARG for resets without xyz.  The plan adds one kernel per stream group. */
+ * gg_init_maps_from_device validates, and GG_E_ARG for resets without xyz.  The plan adds one kernel per stream group.
+ * gg_step_plan_create_with_readouts (below, after gg_sample_layers_to_device) adds a step 4 of read-outs. */
 int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out);
 int gg_step_plan_launch(gg_step_plan plan, void* stream);
 int gg_step_plan_kernels(gg_step_plan plan);   /* kernels per replay */
@@ -777,6 +778,43 @@ typedef struct gg_positions {
 } gg_positions;
 int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const gg_positions* queries, int n_names, const char* const* names,
                                int mode, void* stream);
+
+/* ---- step plan read-outs: what a replayed step writes into caller memory besides its scan outputs ----
+ * A plan created with read-outs has a step 4 after step 3 (gg_step_plan_create): these calls, in this order, over the
+ * plan's slots in desc->scans order, each only when one of its fields is set (nonzero / non-NULL):
+ *   1. gg_get_layers_to_device(n_layer_names, layer_names, layers)
+ *   2. gg_layer_images_to_device(n_image_names, image_names, images, image_ranges)
+ *   3. gg_terrain_images_to_device(terrain_images)
+ *   4. gg_sample_layers_to_device(samples, n_sample_names, sample_names, sample_mode)
+ *   5. gg_point_info_to_device(point_info)
+ *   6. gg_eval_counts_to_device(eval_counts)
+ * Every replay is bit-identical to the plan's step followed by that call sequence, run with the buffers' contents at
+ * replay time.  What gg_step_plan_create_with_readouts reads, and when:
+ *   - the host arrays (layer_names, image_names, sample_names, samples[count], point_info[count]) and sample_mode are
+ *     read at creation and may be freed afterwards;
+ *   - every DEVICE address (layers, images, image_ranges, terrain_images, samples[k].data / dst / cell,
+ *     point_info[k].codes / height, eval_counts) is fixed for the plan's life, and the memory behind it is read or
+ *     written at replay time: positions written into samples[k].data before a launch are the ones that replay looks
+ *     up, and eval_counts grows by one step's tallies per replay;
+ *   - samples[k].n is a fixed capacity: every row gets a value, the caller ignores the rows it does not need;
+ *   - after GG_SCAN_DEVICE_COUNT scans, point_info destinations are sized for the scans' capacities, and each replay
+ *     writes only the first u entries (u the count the scan used), as the standalone call does.
+ * readouts NULL, or a gg_step_readouts with every field zero, is exactly gg_step_plan_create_with_resets.
+ * Validation: what gg_step_plan_create_with_resets validates, and what the six calls validate, with the same codes (the
+ * calls run while the step is recorded, after the slots' state the scans leave).  A rejected plan leaves no plan, no
+ * bound slot, the slots' host state and gg_kernel_launches unchanged.  Creation also allocates what the read-outs
+ * allocate on first use (the image range scratch, the point-info staging).  The bound-slot rules, gg_step_plan_launch
+ * and gg_step_plan_destroy are those of every plan; the read-outs change no slot state. */
+typedef struct gg_step_readouts {
+    int n_layer_names;  const char* const* layer_names;  float* layers;                       /* gg_get_layers_to_device */
+    int n_image_names;  const char* const* image_names;  uint8_t* images; float* image_ranges;  /* gg_layer_images_to_device */
+    float* terrain_images;                                                                    /* gg_terrain_images_to_device */
+    int n_sample_names; const char* const* sample_names; const gg_positions* samples; int sample_mode;  /* gg_sample_layers_to_device */
+    const gg_point_info* point_info;                                                          /* gg_point_info_to_device */
+    uint64_t* eval_counts;                                                                    /* gg_eval_counts_to_device */
+} gg_step_readouts;
+int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets,
+                                      const gg_step_readouts* readouts, gg_step_plan* out);
 
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
