@@ -170,6 +170,8 @@ SCAN_DESC_DTYPE = np.dtype({"names": ["slot", "flags", "n_points", "origin", "ba
                                         ScanDesc.base_z.offset], "itemsize": C.sizeof(ScanDesc)})
 SCAN_DEVICE_POSE = 1   # GG_SCAN_DEVICE_POSE: the scan's origin / base_z come from the slot's device scan pose
 SCAN_DEVICE_COUNT = 2  # GG_SCAN_DEVICE_COUNT: n_points is the capacity; the scan runs on the slot's stored device count
+SCAN_DEVICE_PART_COUNTS = 4  # GG_SCAN_DEVICE_PART_COUNTS: merged scans only; each part's n_points is its capacity and the part
+                             # runs on the slot's stored part count
 
 
 class DevicePoses(C.Structure):
@@ -207,6 +209,18 @@ class StepDesc(C.Structure):
         ("outs", C.c_void_p),
         ("select", C.c_uint),
         ("dev_counts", C.c_void_p),
+    ]
+
+
+class StepParts(C.Structure):
+    """gg_step_parts: the parts of a step plan whose step is a merged scan (gg_step_plan_create_with_parts)."""
+
+    _fields_ = [
+        ("n_parts", C.c_void_p),
+        ("parts", C.c_void_p),
+        ("dev_T_map_from_part", C.c_void_p),
+        ("dev_part_counts", C.c_void_p),
+        ("parts_per_slot", C.c_int),
     ]
 
 
@@ -380,10 +394,13 @@ def load(build_if_missing=True):
         "gg_update_poses_from_device": (i, [vp, i, vp, C.POINTER(DevicePoses), vp, vp]),
         "gg_last_scan_points": (i, [vp, i, C.POINTER(sz)]),
         "gg_set_point_counts_from_device": (i, [vp, i, vp, vp, vp]),
+        "gg_set_part_counts_from_device": (i, [vp, i, vp, i, vp, vp]),
         "gg_step_plan_create": (i, [vp, C.POINTER(StepDesc), C.POINTER(vp)]),
         "gg_init_maps_from_device": (i, [vp, i, vp, C.POINTER(DeviceResets), vp]),
         "gg_step_plan_create_with_resets": (i, [vp, C.POINTER(StepDesc), C.POINTER(DeviceResets), C.POINTER(vp)]),
         "gg_step_plan_create_with_readouts": (i, [vp, C.POINTER(StepDesc), C.POINTER(DeviceResets), C.POINTER(StepReadouts), C.POINTER(vp)]),
+        "gg_step_plan_create_with_parts": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(StepReadouts),
+                                               C.POINTER(vp)]),
         "gg_step_plan_launch": (i, [vp, vp]),
         "gg_step_plan_kernels": (i, [vp]),
         "gg_step_plan_destroy": (i, [vp]),
@@ -649,6 +666,32 @@ class GroundGridB200:
             with torch.cuda.stream(stream):
                 counts = counts.reshape(-1).to(torch.int32).contiguous()
         self.set_point_counts_from_device_ptrs(slots, counts.data_ptr() if count else None, stream.cuda_stream or None)
+
+    def set_part_counts_from_device_ptrs(self, slots, parts_per_slot, counts_ptr, stream_ptr):
+        """gg_set_part_counts_from_device with a raw device address (int32 [count, parts_per_slot]); stream_ptr None = the
+        legacy default stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        _check(self._l.gg_set_part_counts_from_device(self._h, len(sl), _ptr(sl), int(parts_per_slot), counts_ptr, stream_ptr))
+
+    def set_part_counts_from_device(self, slots, counts, stream=None):
+        """The per-part point counts of the slots' next merged scans from a CUDA tensor (gg_set_part_counts_from_device):
+        merged scans run with device_counts=True use them.
+          counts : int32 [count, P] (int64 is converted on `stream`, without a host wait), on this handle's device; entry
+                   [k, p] is the count of part p of slots[k], P (1 ... MAX_CLOUD_PARTS) the most parts such a scan may have
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        The call returns without waiting for the device; `counts` may be freed or overwritten right after it when it
+        belongs to `stream` (another stream's tensor is marked in use on `stream`).  A count outside [0, capacity] runs
+        the part empty."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count = len(slots)
+        if counts.device != dev or counts.dim() != 2 or counts.shape[0] != count or counts.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"counts must be an int32 or int64 tensor [{count}, parts] on {dev}")
+        if stream != current:
+            counts.record_stream(stream)
+        if counts.dtype != torch.int32 or not counts.is_contiguous():
+            with torch.cuda.stream(stream):
+                counts = counts.to(torch.int32).contiguous()
+        self.set_part_counts_from_device_ptrs(slots, counts.shape[1], counts.data_ptr() if count else None, stream.cuda_stream or None)
 
     def init_maps_from_device_ptrs(self, slots, xyz_ptr, mask_ptr, stream_ptr):
         """gg_init_maps_from_device with raw device addresses (ints, or None for NULL); stream_ptr None = the legacy
@@ -1073,7 +1116,7 @@ class GroundGridB200:
                                                           stream_ptr))
 
     def run_merged_cloud_msgs_to_device(self, payloads, point_step, field_offsets, T, slots, origins, base_z, labels=True,
-                                        select="nonground", index=False, stream=None):
+                                        select="nonground", index=False, stream=None, device_counts=False):
         """Scans made of several sensor_msgs/PointCloud2 payloads each (a multi-LiDAR rig), in caller-owned CUDA memory:
         every part is unpacked and transformed to the map frame on the device, the parts of a scan are concatenated in
         order in the slot's buffer, and the merged scans then run like run_scans_to_device
@@ -1085,6 +1128,8 @@ class GroundGridB200:
           T             : lookupTransform("map", frame_id) as a 3x4, one for every part or nested [k][p]; None: the part
                           is already in the map frame
         origins (one cloudOrigin per merged scan), base_z, labels, select, index and stream as in run_scans_to_device.
+          device_counts : each payload's length is its part's capacity, and each part runs on the slot's stored part count
+                          (set_part_counts_from_device, GG_SCAN_DEVICE_PART_COUNTS); the outputs are allocated at capacity
         Each payload may be freed right after the call when it was allocated on `stream` (other streams' payloads are
         marked in use on `stream`).  Returns DeviceOutputs."""
         torch, dev, stream, sel = self._device_call(select, index, stream)
@@ -1097,6 +1142,8 @@ class GroundGridB200:
         first = np.cumsum(n_parts) - n_parts
         n = [int(parts["n_points"][b:b + m].sum()) for b, m in zip(first, n_parts)]
         descs = self._device_descs(slots, n, origins, base_z)
+        if device_counts:
+            descs["flags"] |= SCAN_DEVICE_PART_COUNTS
         out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, [c for scan in payloads for c in scan])
         self.run_merged_cloud_msgs_to_device_ptrs(descs, n_parts, parts, ptrs, sel, out.counts.data_ptr() if out.counts is not None else None,
                                                   stream.cuda_stream or None)
@@ -1107,18 +1154,24 @@ class GroundGridB200:
                   base_z=None, counts=None, xy=None, T_base_from_map=None, pose_origins=None, pose_base_z=None, moved=False, labels=True,
                   select="nonground", index=False, reset_xyz=None, reset_mask=None, layers=None, layer_images=None, terrain_images=False,
                   samples=None, sample_names=("ground", "groundpatch"), sample_mode="nearest", sample_cells=False, point_info=None,
-                  tallies=None):
+                  tallies=None, parts=None, part_counts=None):
         """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
         Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
         pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
         its inputs are given, and every replay is bit-identical to it run on the tensors' contents at replay time.  With
         reset_xyz the step starts with init_maps_from_device(reset_xyz, reset_mask) (gg_step_plan_create_with_resets).
-          clouds / payloads : exactly one: contiguous CUDA tensors as in run_scans_to_device / run_cloud_msgs_to_device;
-                              their lengths are the scans' capacities
-          point_step, field_offsets : the payloads' layout (one value or one per scan)
+          clouds / payloads / parts : exactly one: contiguous CUDA tensors as in run_scans_to_device /
+                              run_cloud_msgs_to_device, or nested [scan][part] as in run_merged_cloud_msgs_to_device (the
+                              step's scan is then that call, gg_step_plan_create_with_parts); their lengths are the
+                              scans' (or parts') capacities
+          point_step, field_offsets : the payloads' layout (one value or one per scan; with parts one value or nested [k][p])
           T        : payloads only.  None (map frame); a CUDA float64 tensor [count, 12] (or [count, 3, 4]) or a list of
                      CUDA float64 [12] tensors / None: lookupTransform("map", frame_id) read at every replay; a numpy
-                     [count, 3, 4] or a list of numpy 3x4 / None: fixed host transforms
+                     [count, 3, 4] or a list of numpy 3x4 / None: fixed host transforms.  With parts: one value or nested
+                     [k][p] of those entries, or a CUDA float64 tensor [count, P, 12] (or [count, P, 3, 4]) read at every
+                     replay
+          part_counts : parts only.  CUDA int32 [count, P] or None: the parts' point counts, read at every replay
+                     (set_part_counts_from_device, GG_SCAN_DEVICE_PART_COUNTS)
           origins  : "device" (the slots' device scan poses, GG_SCAN_DEVICE_POSE) or host [count][3] with base_z
           counts   : CUDA int32 [count] or None: the scans' point counts, read at every replay (GG_SCAN_DEVICE_COUNT)
           xy, T_base_from_map, pose_origins, pose_base_z : CUDA tensors as in update_poses_from_device, or None
@@ -1141,8 +1194,10 @@ class GroundGridB200:
 
         torch_, dev, stream, sel = self._device_call(select, index, None)
         count = len(slots)
-        if (clouds is None) == (payloads is None):
-            raise ValueError("give exactly one of clouds and payloads")
+        if (clouds is not None) + (payloads is not None) + (parts is not None) != 1:
+            raise ValueError("give exactly one of clouds, payloads and parts")
+        if part_counts is not None and parts is None:
+            raise ValueError("part_counts needs parts")
         keep = []
 
         def dptr(t, dtype, shape, name):
@@ -1155,7 +1210,10 @@ class GroundGridB200:
 
         d = StepDesc()
         d.count = count
-        if clouds is not None:
+        sp = None
+        if parts is not None:
+            n, sp = self._plan_parts(torch, dev, parts, point_step, field_offsets, T, part_counts, keep, dptr)
+        elif clouds is not None:
             n = []
             for c in clouds:
                 nbytes = c.numel() * c.element_size()
@@ -1196,6 +1254,8 @@ class GroundGridB200:
                 if tp.any():
                     d.dev_T_map_from_frame = tp.ctypes.data
         descs = self._device_descs(slots, n, origins, base_z, counts is not None)
+        if part_counts is not None:
+            descs["flags"] |= SCAN_DEVICE_PART_COUNTS
         sl = np.ascontiguousarray(slots, np.int32)
         keep += [descs, sl]
         d.scans = descs.ctypes.data
@@ -1216,13 +1276,57 @@ class GroundGridB200:
             raise ValueError("reset_mask needs reset_xyz")
         r = None if reset_xyz is None else DeviceResets(dptr(reset_xyz, torch.float64, (count, 3), "reset_xyz"),
                                                         dptr(reset_mask, torch.int32, (count,), "reset_mask"))
-        if ro_c is not None:
+        if sp is not None:
+            _check(self._l.gg_step_plan_create_with_parts(self._h, C.byref(d), C.byref(sp), None if r is None else C.byref(r),
+                                                          None if ro_c is None else C.byref(ro_c), C.byref(p)))
+        elif ro_c is not None:
             _check(self._l.gg_step_plan_create_with_readouts(self._h, C.byref(d), None if r is None else C.byref(r), C.byref(ro_c), C.byref(p)))
         elif r is None:
             _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
         else:
             _check(self._l.gg_step_plan_create_with_resets(self._h, C.byref(d), C.byref(r), C.byref(p)))
         return StepPlan(self, p, out, mv, keep, ro)
+
+    @staticmethod
+    def _plan_parts(torch, dev, parts, point_step, field_offsets, T, part_counts, keep, dptr):
+        """step_plan's merged scans: (capacity of each scan, StepParts).  Host arrays and the tensors go to keep."""
+        count = len(parts)
+        m = [len(scan) for scan in parts]
+        for scan in parts:
+            for c in scan:
+                if c.device != dev or not c.is_contiguous():
+                    raise ValueError(f"parts must be contiguous tensors on {dev}")
+        if isinstance(T, torch.Tensor):
+            T3 = T.reshape(count, -1, 12)
+            T = [[T3[k, q] for q in range(mk)] for k, mk in enumerate(m)]
+        dev_T = np.zeros(max(1, sum(m)), np.uint64)
+        if isinstance(T, (list, tuple)) and any(isinstance(t, torch.Tensor) for scan in T if isinstance(scan, (list, tuple)) for t in scan):
+            if len(T) != count or any(len(scan) != mk for scan, mk in zip(T, m)):
+                raise ValueError("T must be nested [scan][part] like the parts")
+            host, at = [], 0
+            for scan in T:
+                row = []
+                for t in scan:
+                    if isinstance(t, torch.Tensor):
+                        dev_T[at] = dptr(t, torch.float64, (12,), "T")
+                        t = None
+                    row.append(t)
+                    at += 1
+                host.append(row)
+            T = host
+        n_parts, arr, Tarr = cloud_parts([[c.numel() * c.element_size() for c in scan] for scan in parts],
+                                         [[c.data_ptr() for c in scan] for scan in parts], point_step, field_offsets, T)
+        first = np.cumsum(n_parts) - n_parts
+        n = [int(arr["n_points"][b:b + mk].sum()) for b, mk in zip(first, n_parts)]
+        arr = np.ascontiguousarray(arr)
+        keep += [parts, n_parts, arr, Tarr, dev_T]   # host transforms: read by gg_step_plan_create_with_parts
+        sp = StepParts(n_parts.ctypes.data, arr.ctypes.data, dev_T.ctypes.data if dev_T.any() else None, None, 0)
+        if part_counts is not None:
+            if part_counts.dim() != 2:
+                raise ValueError("part_counts must be a CUDA int32 tensor [count, parts]")
+            sp.dev_part_counts = dptr(part_counts, torch.int32, (count, part_counts.shape[1]), "part_counts")
+            sp.parts_per_slot = part_counts.shape[1]
+        return n, sp
 
     def _plan_readouts(self, torch, dev, stream, slots, n, keep, layers, layer_images, terrain_images, samples, sample_names, sample_mode,
                        sample_cells, point_info, tallies):

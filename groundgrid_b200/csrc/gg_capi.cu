@@ -291,10 +291,14 @@ struct SlotState {
     // gg_set_point_counts_from_device
     bool stored_count = false;      // the device holds a stored count of the slot (GG_SCAN_DEVICE_COUNT scans may run)
     bool device_count = false;      // n_points / scan_points are the last scan's capacity: its count lives in CountTables::last
+    // gg_set_part_counts_from_device: parts_per_slot of the latest call, 0: no part counts stored since gg_init_map
+    // (GG_SCAN_DEVICE_PART_COUNTS scans may run with up to that many parts)
+    int stored_parts = 0;
 };
 
 // While gg_step_plan_create records a step, run_groups takes its staging entries from here instead of the ring: per stream
-// group with slots in the plan one block of calls * per_call[g] records (one entry per call the step records), each record
+// group with slots in the plan one block of calls * per_call[g] records (one entry per call the step records, and one per
+// part round of a merged scan), each record
 // array (SlotParams, OutDest, UnpackDesc, QueryDesc, PointInfoDest, PoseBits) contiguous in the block.  The records are
 // filled in the host image; the plan keeps a pristine device copy of it, and each replay first restores the working block
 // of every group from it (the pose and staging kernels patch the working records in place).  Nothing is committed from
@@ -307,6 +311,8 @@ struct PlanRecorder {
         int calls = 0;                               // entries the block holds
         int first = 0;                               // index of the group's first record over all blocks
         int scan = -1;                               // index in the block of the scan call's first record
+        int part[GG_MAX_CLOUD_PARTS];                // ... of part round p's first record (merged scans), -1: no round
+        Block() { std::fill(part, part + GG_MAX_CLOUD_PARTS, -1); }
     };
     Block blk[kStreams];
     cudaStream_t streams[kStreams] = {};             // capture branch of each group with slots in the plan
@@ -603,9 +609,10 @@ struct SlotList {
 
 // The checks of every call on a list of slots, in this order: at most n_slots entries, then per entry a slot in range,
 // no slot twice (the scans of a batch run concurrently), an initialised map (unless need_map is false) and, for a list of
-// scans, at most pcap points and (with `clouds`) a cloud for every non-empty scan.  h->seen_scratch is free again when it
-// returns, so a checked call may run checked sub-batches.
-int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* clouds = nullptr, bool need_map = true) {
+// scans, at most pcap points and (with `clouds`) a cloud for every non-empty scan.  GG_SCAN_DEVICE_PART_COUNTS is only
+// accepted with `merged` (gg_run_merged_cloud_msgs_to_device).  h->seen_scratch is free again when it returns, so a checked
+// call may run checked sub-batches.
+int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* clouds = nullptr, bool need_map = true, bool merged = false) {
     if (count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", count, h->n_slots);
     std::vector<unsigned char>& seen = h->seen_scratch;
     seen.assign((size_t)h->n_slots, 0);
@@ -620,6 +627,11 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
             return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_POSE without a device scan pose since gg_init_map", slot);
         if ((slots.scans[i].flags & GG_SCAN_DEVICE_COUNT) && !h->slots[slot].stored_count)
             return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_COUNT without a stored count since gg_init_map", slot);
+        if (slots.scans[i].flags & GG_SCAN_DEVICE_PART_COUNTS) {
+            if (!merged) return fail(GG_E_ARG, "scan %d: GG_SCAN_DEVICE_PART_COUNTS is only for gg_run_merged_cloud_msgs_to_device", i);
+            if (!h->slots[slot].stored_parts)
+                return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_PART_COUNTS without stored part counts since gg_init_map", slot);
+        }
         const size_t n = slots.scans[i].n_points;
         if (n > h->pcap) return fail(GG_E_ARG, "slot %d: %zu points exceed capacity %zu", slot, n, h->pcap);
         if (clouds && n && !clouds[i]) return fail(GG_E_ARG, "scan %d: null cloud", i);
@@ -644,7 +656,8 @@ int check_host_counts(int count, const gg_scan_desc* scans) {
 // host wait but the flow control of the staging ring.
 // Poses: when fill staged slot positions (e.position), a record of a slot whose position is device-owned, or of a scan
 // flagged GG_SCAN_DEVICE_POSE, is patched from the device tables by k_stage_poses right after the copy.  Counts: a scan
-// flagged GG_SCAN_DEVICE_COUNT takes its count from the slot's stored one; when fill staged last-scan counts (e.count),
+// flagged GG_SCAN_DEVICE_COUNT takes its count from the slot's stored one (a merged scan flagged
+// GG_SCAN_DEVICE_PART_COUNTS takes its parts' counts in launch_part_rounds); when fill staged last-scan counts (e.count),
 // a non-empty record of a slot whose last count is device-owned takes that count.  Without such records (every all-host
 // flow) nothing more is copied or launched.
 template <typename Fill, typename Launch>
@@ -664,10 +677,12 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
                     if (h->slots[slots[i]].device_position) bits |= gg::POSE_POSITION;
                     if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_POSE)) bits |= gg::POSE_ORIGIN;
                     if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_COUNT)) bits |= gg::POSE_COUNT;
+                    if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_PART_COUNTS)) bits |= gg::POSE_PART_COUNTS;
                 }
                 if (e.count && h->slots[slots[i]].device_count && e.hp[e.m].n_points > 0) bits |= gg::POSE_LAST_COUNT;
                 e.hbits[e.m] = bits;
-                if (bits) e.stage = e.pose_bits = true;
+                if (bits) e.pose_bits = true;
+                if (bits & ~gg::POSE_PART_COUNTS) e.stage = true;   // POSE_PART_COUNTS is k_stage_parts' (launch_part_rounds)
             }
             e.max_points = std::max(e.max_points, e.hp[e.m].n_points);
             ++e.m;
@@ -748,43 +763,66 @@ struct CallerOutputs {
     const int* part_base = nullptr;
 };
 
-// A staging entry per part round is taken while the group's scan entry is held, so the rounds of one group never
-// wrap the ring onto it.
+// The part rounds of a group hold their staging entries together, while the group's scan entry is held, so they never
+// wrap the ring onto one another or onto it.
 static_assert(GG_MAX_CLOUD_PARTS < kRing, "the part rounds of a group must fit in the staging ring");
 
 // The part rounds of the merged scans in the scan entry `e` (e.hp[j].pos = the scan's position in the call), on the
-// group's stream `st`: round p is one launch of the unpack kernel over part p of every scan of the group that has a
-// non-empty one, each landing in its slot's buffer after the scan's parts before p.  Each round takes its own staging
-// entry.  Returns the number of launches, or a negative error code.
+// group's stream `st`: round p is one launch of the unpack kernel over part p of every scan of the group, record j of its
+// staging entry being part p of the entry's scan j (n_points 0 when the scan has no such part), each landing in its
+// slot's buffer after the scan's parts before p.  A round with no part to read is not launched.  When scans of the entry
+// take device part counts (POSE_PART_COUNTS), k_stage_parts resolves their round records once every round's entry is
+// copied, before the first round.  While a step is recorded the rounds' entries come from the group's block.  Returns
+// the number of launches, or a negative error code.
 int launch_part_rounds(gg_handle h, const Staging& e, const CallerOutputs& c, cudaStream_t st) {
     int rounds = 0, n = 0, rc;
-    for (int j = 0; j < e.m; ++j) rounds = std::max(rounds, c.n_parts[e.hp[j].pos]);
+    bool resolve = false;
+    for (int j = 0; j < e.m; ++j) {
+        rounds = std::max(rounds, c.n_parts[e.hp[j].pos]);
+        resolve = resolve || (e.hbits && (e.hbits[j] & gg::POSE_PART_COUNTS));
+    }
+    const int g = stream_index(h, e.hp[0].slot);
+    Staging r[GG_MAX_CLOUD_PARTS];
+    gg::PartRounds pr{};
     for (int p = 0; p < rounds; ++p) {
-        Staging r;
+        bool used = false;
         for (int j = 0; j < e.m; ++j) {
             const int k = e.hp[j].pos;
-            if (p >= c.n_parts[k]) continue;
-            const gg_cloud_part* part = c.parts + c.part_base[k];
-            if (part[p].n_points == 0) continue;
-            if (r.m == 0 && (rc = r.acquire(h))) return rc;
-            gg::SlotParams& sp = r.hp[r.m];
+            used = used || (p < c.n_parts[k] && c.parts[c.part_base[k] + p].n_points > 0);
+        }
+        if (!used) continue;
+        Staging& q = r[p];
+        if ((rc = h->rec ? q.acquire_recorded(h, g) : q.acquire(h))) return rc;
+        if (h->rec) h->rec->blk[g].part[p] = h->rec->blk[g].next - h->rec->blk[g].per_call;
+        for (q.m = 0; q.m < e.m; ++q.m) {
+            const int k = e.hp[q.m].pos;
+            gg::SlotParams& sp = q.hp[q.m];
             std::memset(&sp, 0, sizeof(sp));
-            sp.slot = e.hp[j].slot;
+            sp.slot = e.hp[q.m].slot;
+            if (p >= c.n_parts[k]) {
+                std::memset(&q.hunpack[q.m], 0, sizeof(gg::UnpackDesc));
+                continue;
+            }
+            const gg_cloud_part* part = c.parts + c.part_base[k];
             sp.n_points = (int)part[p].n_points;
             const gg_cloud_msg& msg = part[p].msg;
-            fill_unpack(r.hunpack[r.m], msg.data, msg.point_step, msg.field_offsets, msg.T_map_from_frame);
+            fill_unpack(q.hunpack[q.m], msg.data, msg.point_step, msg.field_offsets, msg.T_map_from_frame);
             size_t first = 0;
-            for (int q = 0; q < p; ++q) first += part[q].n_points;
-            r.hunpack[r.m].first = (int)first;
-            r.max_points = std::max(r.max_points, sp.n_points);
-            ++r.m;
+            for (int b = 0; b < p; ++b) first += part[b].n_points;
+            q.hunpack[q.m].first = (int)first;
+            q.max_points = std::max(q.max_points, sp.n_points);
         }
-        if (r.m == 0) continue;
-        r.unpack = true;
-        if ((rc = r.commit(st))) return rc;
-        n += gg::launch_unpack(h->view, r.dp, r.dunpack, r.m, r.max_points, st, h->prof);
+        q.unpack = true;
+        if (!h->rec && (rc = q.commit(st))) return rc;
+        pr.params[p] = q.dp;
+        pr.descs[p] = q.dunpack;
+    }
+    if (resolve) n += gg::launch_stage_parts(h->counts, e.dp, e.dbits, e.m, pr, st, h->prof);
+    for (int p = 0; p < rounds; ++p) {
+        if (r[p].m == 0) continue;
+        n += gg::launch_unpack(h->view, r[p].dp, r[p].dunpack, r[p].m, r[p].max_points, st, h->prof);
         GG_CUDA(cudaGetLastError());
-        if ((rc = r.release(h, st))) return rc;
+        if (!h->rec && (rc = r[p].release(h, st))) return rc;
     }
     return n;
 }
@@ -796,7 +834,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
                       const float* const* packed_ptrs = nullptr, uint8_t* labels_base = nullptr, const CallerOutputs* caller = nullptr) {
     if (count <= 0) return GG_OK;
     int rc;
-    if ((rc = check_slots(h, count, scans))) return rc;
+    if ((rc = check_slots(h, count, scans, nullptr, true, caller && caller->parts))) return rc;
     gg::View view = h->view;
     if (labels_base) view.labels = labels_base;
     // count + scan passes when counts are wanted; the write pass when any scan of the group wants labels, index or cloud
@@ -837,7 +875,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         s.scan_points = d.n_points;
         s.moved_since_scan = false;
         s.device_rolled = false;
-        s.device_count = (d.flags & GG_SCAN_DEVICE_COUNT) != 0;   // a host-count scan makes the count host-owned again
+        s.device_count = (d.flags & (GG_SCAN_DEVICE_COUNT | GG_SCAN_DEVICE_PART_COUNTS)) != 0;   // a host-count scan makes the count host-owned again
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) {
@@ -1579,7 +1617,7 @@ int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_des
                                        const gg_scan_outputs* outs, unsigned select, int32_t* dev_counts, void* stream) {
     if (!h || !scans || (count > 0 && (!n_parts || !parts))) return fail(GG_E_ARG, "null argument");
     int rc;
-    if ((rc = check_host_counts(count, scans))) return rc;   // per-part device counts would need device part offsets
+    if ((rc = check_host_counts(count, scans))) return rc;   // device counts are per part here (GG_SCAN_DEVICE_PART_COUNTS)
     if ((rc = check_outputs(outs, -1, select, dev_counts))) return rc;
     std::vector<int>& base = h->part_base;
     base.assign((size_t)std::max(count, 0), 0);
@@ -1599,6 +1637,10 @@ int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_des
         }
         if (n != scans[i].n_points) return fail(GG_E_ARG, "scan %d: its parts hold %zu points, its n_points is %zu", i, n, scans[i].n_points);
         next += m;
+        // a flagged scan's parts need stored counts (slot range and the rest: check_slots)
+        const int slot = scans[i].slot;
+        if ((scans[i].flags & GG_SCAN_DEVICE_PART_COUNTS) && slot >= 0 && slot < h->n_slots && h->slots[slot].stored_parts && m > h->slots[slot].stored_parts)
+            return fail(GG_E_STATE, "scan %d: %d parts, but slot %d has stored counts for %d", i, m, slot, h->slots[slot].stored_parts);
         // as in gg_run_cloud_msgs_to_device, outputs may overlap the scan's own parts: every part is consumed before the
         // scan's first kernel on the same stream
         if ((rc = check_outputs(outs, i, select, dev_counts))) return rc;
@@ -1918,7 +1960,7 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
                                            "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve", "k_store_counts",
-                                           "k_reset_maps"};
+                                           "k_reset_maps", "k_stage_parts", "k_store_part_counts"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2686,6 +2728,42 @@ int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, co
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
+// Part counts from device memory: per stream group one k_store_part_counts over the group's slots.
+int gg_set_part_counts_from_device(gg_handle h, int count, const int* slots, int parts_per_slot, const int32_t* dev_part_counts, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0) return GG_OK;
+    if (!slots || !dev_part_counts) return fail(GG_E_ARG, "null argument");
+    if (parts_per_slot < 1 || parts_per_slot > GG_MAX_CLOUD_PARTS)
+        return fail(GG_E_ARG, "parts_per_slot %d not in [1, %d]", parts_per_slot, GG_MAX_CLOUD_PARTS);
+    if (reinterpret_cast<uintptr_t>(dev_part_counts) % alignof(int32_t)) return fail(GG_E_ARG, "dev_part_counts is not 4-byte aligned");
+    const gg::View& v = h->view;
+    if (ranges_overlap(dev_part_counts, (size_t)count * parts_per_slot * sizeof(int32_t), v.layers,
+                       (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float)))
+        return fail(GG_E_ARG, "dev_part_counts overlaps the handle's layers");
+    int rc;
+    if ((rc = check_slots(h, count, slots))) return rc;
+    GG_CUDA(cudaSetDevice(h->device));
+    // the device tables and the staging of the per-record bits, on first use (a handle that never asks has none)
+    const size_t S = (size_t)h->n_slots;
+    if (!h->counts.parts && (rc = dev_alloc(h, &h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
+    if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
+    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
+    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    auto fill = [&](int i, Staging& e) {
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        h->slots[slots[i]].stored_parts = parts_per_slot;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) {
+        return gg::launch_store_part_counts(h->counts, e.dp, e.m, dev_part_counts, parts_per_slot, st, h->prof);
+    };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
 // Map resets from device memory: per stream group one k_reset_maps over the group's slots.  The host cannot see the mask,
 // so every slot of the call leaves it in the same state: a device-owned position (k_reset_maps seeds the host-owned
 // positions of masked-off slots), the stored scan pose and count kept, the last scan's outputs still readable, and its
@@ -2756,31 +2834,48 @@ void free_plan(gg_step_plan p) {
 }
 
 // What gg_step_plan_create checks beyond the step's calls (those check their own arguments while the step is recorded).
-int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets) {
+int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets) {
     if (resets && !resets->xyz) return fail(GG_E_ARG, "resets without xyz");
     if (d.count <= 0) return fail(GG_E_ARG, "a step plan needs count > 0 scans, got %d", d.count);
     if (!d.scans) return fail(GG_E_ARG, "null scans");
     if (d.count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", d.count, h->n_slots);
-    if (!d.dev_points == !d.msgs) return fail(GG_E_ARG, "a step plan takes exactly one of dev_points and msgs");
-    if (d.dev_T_map_from_frame && !d.msgs) return fail(GG_E_ARG, "dev_T_map_from_frame needs msgs");
+    if (parts) {
+        if (d.dev_points || d.msgs || d.dev_T_map_from_frame || d.dev_n_points)
+            return fail(GG_E_ARG, "a step plan with parts takes no dev_points, msgs, dev_T_map_from_frame or dev_n_points");
+        if (!parts->n_parts || !parts->parts) return fail(GG_E_ARG, "null n_parts or parts");
+    } else {
+        if (!d.dev_points == !d.msgs) return fail(GG_E_ARG, "a step plan takes exactly one of dev_points and msgs");
+        if (d.dev_T_map_from_frame && !d.msgs) return fail(GG_E_ARG, "dev_T_map_from_frame needs msgs");
+    }
     int rc;
     for (int i = 0; i < d.count; ++i) {
         const int slot = d.scans[i].slot;
         if ((rc = check_slot(h, slot))) return rc;
         if (h->slot_plan[slot]) return fail(GG_E_STATE, "slot %d is already bound to a step plan", slot);
+        if (parts && (parts->n_parts[i] < 0 || parts->n_parts[i] > GG_MAX_CLOUD_PARTS))
+            return fail(GG_E_ARG, "scan %d: %d parts, not in [0, %d]", i, parts->n_parts[i], GG_MAX_CLOUD_PARTS);
     }
-    if (!d.dev_T_map_from_frame) return GG_OK;
+    // the device transforms: per payload (msgs) or per part, each with its host transform
+    std::vector<std::pair<const double*, const double*>> dev_host;
+    if (parts && parts->dev_T_map_from_part) {
+        for (int i = 0, at = 0; i < d.count; at += parts->n_parts[i++])
+            for (int q = 0; q < parts->n_parts[i]; ++q) dev_host.push_back({parts->dev_T_map_from_part[at + q], parts->parts[at + q].msg.T_map_from_frame});
+    } else if (!parts && d.dev_T_map_from_frame) {
+        for (int k = 0; k < d.count; ++k) dev_host.push_back({d.dev_T_map_from_frame[k], d.msgs[k].T_map_from_frame});
+    }
+    const char* what = parts ? "part" : "scan";   // k below counts the parts over all scans, or the scans
+    const char* name = parts ? "dev_T_map_from_part" : "dev_T_map_from_frame";
     std::vector<uintptr_t> ts;
-    for (int k = 0; k < d.count; ++k) {
-        const uintptr_t t = reinterpret_cast<uintptr_t>(d.dev_T_map_from_frame[k]);
+    for (size_t k = 0; k < dev_host.size(); ++k) {
+        const uintptr_t t = reinterpret_cast<uintptr_t>(dev_host[k].first);
         if (!t) continue;
-        if (t % alignof(double)) return fail(GG_E_ARG, "scan %d: dev_T_map_from_frame is not 8-byte aligned", k);
-        if (d.msgs[k].T_map_from_frame) return fail(GG_E_ARG, "scan %d: both a device and a host T_map_from_frame", k);
+        if (t % alignof(double)) return fail(GG_E_ARG, "%s %zu: %s is not 8-byte aligned", what, k, name);
+        if (dev_host[k].second) return fail(GG_E_ARG, "%s %zu: both a device and a host T_map_from_frame", what, k);
         ts.push_back(t);
     }
     std::sort(ts.begin(), ts.end());
     for (size_t j = 1; j < ts.size(); ++j)
-        if (ts[j] < ts[j - 1] + 12 * sizeof(double)) return fail(GG_E_ARG, "two dev_T_map_from_frame entries overlap");
+        if (ts[j] < ts[j - 1] + 12 * sizeof(double)) return fail(GG_E_ARG, "two %s entries overlap", name);
     return GG_OK;
 }
 
@@ -2800,17 +2895,18 @@ struct ReadoutCalls {
     int count() const { return layers + images + terrain + samples + point_info + eval; }
 };
 
-// The calls a plan's step records: the resets, counts and poses when given, the scans, and the read-outs.
-int step_calls(const gg_step_desc& d, const gg_device_resets* resets, const gg_step_readouts* readouts) {
+// The calls a plan's step records: the resets, counts (or part counts) and poses when given, the scans, and the read-outs.
+int step_calls(const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_step_readouts* readouts) {
     const gg_device_poses& q = d.poses;
-    return (resets != nullptr) + (d.dev_n_points != nullptr) + (q.xy || q.T_base_from_map || q.origin || q.base_z) + 1 + ReadoutCalls(readouts).count();
+    return (resets != nullptr) + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) + (q.xy || q.T_base_from_map || q.origin || q.base_z) +
+           1 + ReadoutCalls(readouts).count();
 }
 
 // The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_readouts): per branch the restore of
 // its records and, where a payload takes a device transform, the transform staging; then the step's calls, the resets
 // (when given) first and the read-outs last.
-int record_step(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, const gg_step_readouts* readouts, const std::vector<int>& slots,
-                const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
+int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_step_readouts* readouts,
+                const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
     PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
@@ -2827,11 +2923,19 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
     const gg_device_poses& q = d.poses;
     if (resets && (rc = gg_init_maps_from_device(h, n, sl, resets, root))) return rc;
     if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
+    if (parts && parts->dev_part_counts && (rc = gg_set_part_counts_from_device(h, n, sl, parts->parts_per_slot, parts->dev_part_counts, root)))
+        return rc;
     if ((q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, n, sl, &q, d.dev_moved, root))) return rc;
-    rc = d.dev_points ? gg_run_scans_to_device(h, n, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root)
-                      : gg_run_cloud_msgs_to_device(h, n, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
-    if (rc) return rc;
-    for (int g : p->groups) r.blk[g].scan = r.blk[g].next - r.blk[g].per_call;   // the payload records k_stage_transforms patches
+    if (parts) {
+        // the part rounds remember their own records (PlanRecorder::Block::part)
+        rc = gg_run_merged_cloud_msgs_to_device(h, n, d.scans, parts->n_parts, parts->parts, d.outs, d.select, d.dev_counts, root);
+        if (rc) return rc;
+    } else {
+        rc = d.dev_points ? gg_run_scans_to_device(h, n, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root)
+                          : gg_run_cloud_msgs_to_device(h, n, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
+        if (rc) return rc;
+        for (int g : p->groups) r.blk[g].scan = r.blk[g].next - r.blk[g].per_call;   // the payload records k_stage_transforms patches
+    }
     const ReadoutCalls c(readouts);
     const gg_step_readouts o = readouts ? *readouts : gg_step_readouts{};
     if (c.layers && (rc = gg_get_layers_to_device(h, n, sl, o.n_layer_names, o.layer_names, o.layers, root))) return rc;
@@ -2852,6 +2956,7 @@ int prepare_recording(gg_handle h, const gg_step_readouts* readouts) {
     if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
     if (!h->counts.stored && (rc = dev_alloc(h, &h->counts.stored, S))) return rc;
     if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
+    if (!h->counts.parts && (rc = dev_alloc(h, &h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
     if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
     if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
     if ((rc = ensure_out_cloud(h))) return rc;
@@ -2867,26 +2972,34 @@ int prepare_recording(gg_handle h, const gg_step_readouts* readouts) {
 // gg_step_plan_create after check_step_desc and prepare_recording: lays out the record blocks, seeds the positions,
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
-int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* resets, const gg_step_readouts* readouts, gg_step_plan p) {
-    const int count = d.count, calls = step_calls(d, resets, readouts);
+int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_step_readouts* readouts,
+                gg_step_plan p) {
+    const int count = d.count, calls = step_calls(d, parts, resets, readouts);
     std::vector<int>& slots = p->slots;
     slots.resize(count);
     for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
+    // with parts: index in parts->parts of each scan's first part
+    std::vector<int> base(count, 0);
+    for (int i = 1; parts && i < count; ++i) base[i] = base[i - 1] + parts->n_parts[i - 1];
     PlanRecorder rec;
     std::vector<char> T_group(kStreams, 0);
     size_t at = 0;
     for (int g = 0; g < h->n_streams; ++g) {
-        int c = 0;
+        int c = 0, rounds = 0;   // the group's scans, and the part rounds of its merged scans (one entry each at most)
         for (int i = 0; i < count; ++i)
             if (stream_index(h, slots[i]) == g) {
                 ++c;
                 if (d.dev_T_map_from_frame && d.dev_T_map_from_frame[i]) T_group[g] = 1;
+                if (!parts) continue;
+                rounds = std::max(rounds, parts->n_parts[i]);
+                for (int q = 0; parts->dev_T_map_from_part && q < parts->n_parts[i]; ++q)
+                    if (parts->dev_T_map_from_part[base[i] + q]) T_group[g] = 1;
             }
         if (c == 0) continue;
         PlanRecorder::Block& b = rec.blk[g];
-        const size_t m = (size_t)calls * c;
+        const size_t m = (size_t)(calls + rounds) * c;
         b.per_call = c;
-        b.calls = calls;
+        b.calls = calls + rounds;
         b.first = rec.records;
         rec.records += (int)m;
         b.at = b.params = at;
@@ -2903,7 +3016,8 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
     GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->pristine), at));
     GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->work), at));
     rec.work = p->work;
-    if (d.dev_T_map_from_frame) GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->dev_T), (size_t)rec.records * sizeof(double*)));
+    const bool dev_T = d.dev_T_map_from_frame || (parts && parts->dev_T_map_from_part);
+    if (dev_T) GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->dev_T), (size_t)rec.records * sizeof(double*)));
 
     // the slots' stream groups are idle from here on: nothing in flight reads or writes what is seeded below
     for (int g : p->groups) GG_CUDA(cudaStreamSynchronize(h->streams[g]));
@@ -2939,7 +3053,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, resets, readouts, slots, T_group, root, fork, p);
+        rc = record_step(h, d, parts, resets, readouts, slots, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -2964,13 +3078,19 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_device_resets* rese
     if (rc) return rc;
     for (int j = 0; j < count; ++j) h->slots[slots[j]].device_position = true;
 
-    // the records as recorded, the caller transforms of the payload records, and the executable graph
+    // the records as recorded, the caller transforms of the payload records (row j of the scan entry, or of part round q's
+    // entry, is the group's j-th scan), and the executable graph
     std::vector<const double*> T_rec(rec.records, nullptr);
     for (int g : p->groups) {
         const PlanRecorder::Block& b = rec.blk[g];
-        int j = b.first + b.scan;
-        for (int i = 0; i < count; ++i)
-            if (stream_index(h, slots[i]) == g) T_rec[j++] = d.dev_T_map_from_frame ? d.dev_T_map_from_frame[i] : nullptr;
+        int j = 0;
+        for (int i = 0; i < count; ++i) {
+            if (stream_index(h, slots[i]) != g) continue;
+            if (!parts && d.dev_T_map_from_frame) T_rec[b.first + b.scan + j] = d.dev_T_map_from_frame[i];
+            for (int q = 0; parts && parts->dev_T_map_from_part && q < parts->n_parts[i]; ++q)
+                if (b.part[q] >= 0) T_rec[b.first + b.part[q] + j] = parts->dev_T_map_from_part[base[i] + q];
+            ++j;
+        }
     }
     GG_CUDA(cudaMemcpy(p->pristine, rec.host.data(), at, cudaMemcpyHostToDevice));
     if (p->dev_T) GG_CUDA(cudaMemcpy(p->dev_T, T_rec.data(), T_rec.size() * sizeof(double*), cudaMemcpyHostToDevice));
@@ -2988,16 +3108,21 @@ int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const
 
 int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, const gg_step_readouts* readouts,
                                       gg_step_plan* out) {
+    return gg_step_plan_create_with_parts(h, desc, nullptr, resets, readouts, out);
+}
+
+int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                   const gg_step_readouts* readouts, gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
     if (!h || !desc) return fail(GG_E_ARG, "null argument");
     int rc;
-    if ((rc = check_step_desc(h, *desc, resets))) return rc;
+    if ((rc = check_step_desc(h, *desc, parts, resets))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     if ((rc = prepare_recording(h, readouts))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, resets, readouts, p))) {
+    if ((rc = record_plan(h, *desc, parts, resets, readouts, p))) {
         free_plan(p);
         return rc;
     }

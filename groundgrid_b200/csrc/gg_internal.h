@@ -181,7 +181,7 @@ constexpr int OUT_TILE = 1024;
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
     K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_STAGE_POSES, K_POSE_RESOLVE,
-    K_STORE_COUNTS, K_RESET_MAPS,
+    K_STORE_COUNTS, K_RESET_MAPS, K_STAGE_PARTS, K_STORE_PART_COUNTS,
     K_NUM
 };
 
@@ -472,6 +472,8 @@ enum PoseBits : int {
     POSE_COUNT = 4,      // a scan of GG_SCAN_DEVICE_COUNT: n_points (staged: the capacity) from the slot's stored count,
                          // 0 when that is outside [0, capacity); the result also goes to the slot's last count
     POSE_LAST_COUNT = 8, // n_points from the slot's last count (the count of its last scan is device-owned)
+    POSE_PART_COUNTS = 16,  // a merged scan of GG_SCAN_DEVICE_PART_COUNTS: k_stage_parts (not k_stage_poses) resolves
+                            // its parts' counts and offsets from the slot's stored part counts
 };
 // The handle's per-slot device tables (allocated on the first gg_update_poses_from_device).
 struct PoseTables {
@@ -482,12 +484,31 @@ struct PoseTables {
 struct CountTables {
     int32_t* stored;     // [n_slots] the latest count gg_set_point_counts_from_device stored, as the caller gave it
     int32_t* last;       // [n_slots] the count the slot's last GG_SCAN_DEVICE_COUNT scan ran on
+    int32_t* parts;      // [n_slots][GG_MAX_CLOUD_PARTS] the latest part counts gg_set_part_counts_from_device stored
+                         // (allocated on its first call)
 };
 // Patches the `count` records of batch whose bits ask for it from the tables; runs after the entry's copy and before
 // the kernels that read it.
 int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof);
 // One thread per record: the count of batch[j] (at dev_n[batch[j].pos]) into the slot's entry of c.stored.
 int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof);
+// One thread per record: the parts_per_slot part counts of batch[j] (at dev_n[batch[j].pos * parts_per_slot]) into the
+// slot's row of c.parts.
+int launch_store_part_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, int parts_per_slot, cudaStream_t st,
+                             Profiler* prof);
+// The part rounds of one scan entry of gg_run_merged_cloud_msgs_to_device: record j of round p's entry is part p of the
+// entry's scan j (n_points = the part's capacity, 0 without one; descs[j].first = the capacities before it).  Null: the
+// round has no part to read and is not launched.
+struct PartRounds {
+    SlotParams* params[GG_MAX_CLOUD_PARTS];
+    UnpackDesc* descs[GG_MAX_CLOUD_PARTS];
+};
+// One thread per record of the scan entry whose bits hold POSE_PART_COUNTS: per part p the count u_p = v_p if
+// 0 <= v_p <= capacity, else 0 (v_p: the slot's stored part count), written into round p's record with the offset
+// u_0 + ... + u_{p-1}; the scan record's n_points and the slot's last count become the sum.  Runs after the entries'
+// copies and before the rounds.
+int launch_stage_parts(const CountTables& c, SlotParams* batch, const int* bits, int count, const PartRounds& rounds, cudaStream_t st,
+                       Profiler* prof);
 // The poses of one gg_update_poses_from_device call (entry batch[j].pos of each array); null xy: no roll, null origin:
 // no scan pose.
 struct DevicePoses {

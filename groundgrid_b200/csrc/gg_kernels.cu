@@ -2377,6 +2377,46 @@ __global__ void __launch_bounds__(POSE_THREADS) k_store_counts(CountTables c, co
     c.stored[p.slot] = dev_n[p.pos];
 }
 
+// Part counts from device memory (gg_set_part_counts_from_device): record j stores the caller's part counts of its slot,
+// as given; k_stage_parts applies the capacity rule per part when a scan uses them.
+__global__ void __launch_bounds__(POSE_THREADS) k_store_part_counts(CountTables c, const SlotParams* __restrict__ batch, int count,
+                                                                    const int32_t* __restrict__ dev_n, int parts_per_slot) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count) return;
+    const SlotParams& p = batch[j];
+    int32_t* dst = c.parts + (size_t)p.slot * GG_MAX_CLOUD_PARTS;
+    const int32_t* src = dev_n + (size_t)p.pos * parts_per_slot;
+    for (int q = 0; q < parts_per_slot; ++q) dst[q] = src[q];
+}
+
+// A merged scan of GG_SCAN_DEVICE_PART_COUNTS (record j of a scan entry): the rule of k_stage_poses' POSE_COUNT applied
+// to each part, with the parts landing back to back.  Round records staged with the part's capacity; a capacity of 0
+// (no such part, or an empty one) is never read and gives 0 whatever was stored.
+__global__ void __launch_bounds__(POSE_THREADS) k_stage_parts(CountTables c, SlotParams* __restrict__ batch, const int* __restrict__ bits, int count,
+                                                              PartRounds r) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count || !(bits[j] & POSE_PART_COUNTS)) return;
+    SlotParams& p = batch[j];
+    const int32_t* stored = c.parts + (size_t)p.slot * GG_MAX_CLOUD_PARTS;
+    int first = 0;   // <= the scan's capacity <= max_points: no overflow
+#pragma unroll 1
+    for (int q = 0; q < GG_MAX_CLOUD_PARTS; ++q) {
+        if (!r.params[q]) continue;
+        SlotParams& sp = r.params[q][j];
+        const int cap = sp.n_points;
+        int u = 0;
+        if (cap > 0) {
+            const int v = stored[q];
+            u = (v >= 0 && v <= cap) ? v : 0;
+        }
+        sp.n_points = u;
+        r.descs[q][j].first = first;
+        first += u;
+    }
+    p.n_points = first;
+    c.last[p.slot] = first;
+}
+
 // Step plans (gg_step_plan_create): record j of a replay's working UnpackDescs takes its sensor-to-map transform from
 // the caller's device memory, read at replay time; the copy is bitwise, so k_unpack_transform computes what it computes
 // for the same doubles staged from the host.
@@ -2747,6 +2787,18 @@ int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* ba
 
 int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof) {
     GG_LAUNCH(K_STORE_COUNTS, k_store_counts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(c, batch, count, dev_n));
+    return 1;
+}
+
+int launch_store_part_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, int parts_per_slot, cudaStream_t st,
+                             Profiler* prof) {
+    GG_LAUNCH(K_STORE_PART_COUNTS, k_store_part_counts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(c, batch, count, dev_n, parts_per_slot));
+    return 1;
+}
+
+int launch_stage_parts(const CountTables& c, SlotParams* batch, const int* bits, int count, const PartRounds& rounds, cudaStream_t st,
+                       Profiler* prof) {
+    GG_LAUNCH(K_STAGE_PARTS, k_stage_parts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(c, batch, bits, count, rounds));
     return 1;
 }
 

@@ -86,9 +86,13 @@ typedef struct gg_handle_s* gg_handle;
  *             instead of this descriptor;
  *             GG_SCAN_DEVICE_COUNT: n_points is the scan's capacity and the scan runs on the slot's stored device count
  *             (gg_set_point_counts_from_device);
+ *             GG_SCAN_DEVICE_PART_COUNTS: gg_run_merged_cloud_msgs_to_device only (every other call rejects it with
+ *             GG_E_ARG): each part's n_points is its capacity and the part runs on the slot's stored part count
+ *             (gg_set_part_counts_from_device);
  *             the other bits are reserved and ignored (pass 0)                */
 #define GG_SCAN_DEVICE_POSE 1
 #define GG_SCAN_DEVICE_COUNT 2
+#define GG_SCAN_DEVICE_PART_COUNTS 4
 typedef struct gg_scan_desc {
     int slot;
     int flags;
@@ -539,10 +543,70 @@ typedef struct gg_cloud_part {
  * count == 0 returns GG_OK and enqueues nothing.  GG_E_ARG, with nothing enqueued: what gg_run_cloud_msgs_to_device
  * rejects (GG_E_STATE for a map not initialised); null n_parts or parts with count > 0; n_parts[k] < 0 or
  * > GG_MAX_CLOUD_PARTS; scans[k].n_points other than the sum of its parts' n_points; per part the layout rules of
- * gg_upload_cloud_msg (the error text names the scan and the part). */
+ * gg_upload_cloud_msg (the error text names the scan and the part).
+ * Device part counts (GG_SCAN_DEVICE_PART_COUNTS on scans[k]): each part's n_points is that part's CAPACITY c_p (the
+ *   payload must be readable for the records the part uses), and scans[k].n_points is still the sum of the capacities
+ *   (<= max_points).  With v_p the latest part count stored for the slot in its stream order
+ *   (gg_set_part_counts_from_device), part p uses u_p = v_p if 0 <= v_p <= c_p, else u_p = 0 -- the rule of
+ *   GG_SCAN_DEVICE_COUNT applied per part, without clamping -- and lands from record u_0 + ... + u_{p-1} on; the scan
+ *   runs on U = u_0 + u_1 + ...  Everything (labels, of which only the first U are written, index, cloud, dev_counts,
+ *   layers, gg_get_output, point info, tallies, gg_last_scan_points) is bit-identical to the same call with host counts
+ *   and parts of n_points = u_p on the same first u_p records of each payload.  Nothing past c_p of a payload is read;
+ *   a part with c_p == 0 is never read and its stored count is ignored.  After the scan the slot's last-scan count U is
+ *   device-owned, with every rule of GG_SCAN_DEVICE_COUNT (gg_set_point_counts_from_device) for the calls that need it
+ *   on the host; outputs and point-info destinations are sized for the capacity.  The flag combines with
+ *   GG_SCAN_DEVICE_POSE.  GG_E_STATE, with nothing enqueued: a flagged scan of a slot with no part counts stored since its
+ *   gg_init_map, or with more parts than the parts_per_slot last stored for the slot.  GG_SCAN_DEVICE_COUNT stays
+ *   GG_E_ARG here, with or without the flag. */
 int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scans, const int* n_parts,
                                        const gg_cloud_part* parts, const gg_scan_outputs* outs, unsigned select,
                                        int32_t* dev_counts, void* stream);
+
+/* The part counts of the slots' next merged scans, read from DEVICE memory, for rigs whose per-sensor counts change
+ * every sweep (drop-outs, range gates) and are known only on the GPU (a GPU packet decoder).
+ *   dev_part_counts : int32 [count][parts_per_slot], 4-byte aligned, on the handle's device; entry [k][p] becomes the
+ *                     stored count of part p of slots[k] for every later GG_SCAN_DEVICE_PART_COUNTS scan of the slot,
+ *                     until the next call stores another.  Values are stored as given, not validated.
+ *   parts_per_slot  : 1 ... GG_MAX_CLOUD_PARTS; a flagged scan of the slot may have up to this many parts.
+ *   stream          : the contract of gg_set_point_counts_from_device: the work starts after everything already enqueued
+ *                     on `stream` and on the slots' stream groups, nothing waits on the host except the flow control of
+ *                     the parameter staging ring, and the counts are consumed by the first kernel of each stream group,
+ *                     so they may be freed or refilled on `stream` right after the call.
+ * The part-count table and the count table of gg_set_point_counts_from_device are independent.  gg_init_map forgets the
+ * stored part counts; gg_init_maps_from_device keeps them.
+ * count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle, slots or dev_part_counts; count > n_slots; a slot out of range or repeated; parts_per_slot
+ *              out of range; dev_part_counts not 4-byte aligned or overlapping the handle's layers
+ *   GG_E_STATE a slot whose map is not initialised */
+int gg_set_part_counts_from_device(gg_handle h, int count, const int* slots, int parts_per_slot, const int32_t* dev_part_counts,
+                                   void* stream);
+
+/* A step plan whose step is a merged scan (a multi-LiDAR rig in a CUDA graph).  Scan k of desc->scans owns the next
+ * n_parts[k] entries of `parts`.  The step is, by definition, this sequence over the plan's slots in desc->scans order:
+ *   0. gg_init_maps_from_device(resets), if resets is given;
+ *   1. gg_set_part_counts_from_device(parts_per_slot, dev_part_counts), if dev_part_counts is given;
+ *   2. gg_update_poses_from_device(desc->poses, desc->dev_moved), if any pose pointer is given;
+ *   3. gg_run_merged_cloud_msgs_to_device(desc->scans, n_parts, parts, desc->outs, desc->select, desc->dev_counts);
+ *      part p with a non-NULL dev_T_map_from_part entry is transformed with the 12 doubles found there AT REPLAY TIME,
+ *      bit-identical to passing them as its host T_map_from_frame (which must then be NULL);
+ *   4. the read-outs, as in gg_step_plan_create_with_readouts.
+ * Every replay is bit-identical to that sequence run on the buffers' contents at replay time.  desc->dev_points,
+ * desc->msgs, desc->dev_T_map_from_frame and desc->dev_n_points must be NULL (GG_E_ARG).  parts NULL is exactly
+ * gg_step_plan_create_with_readouts.  Everything else is what the recorded calls and gg_step_plan_create validate, with
+ * the same codes, plus GG_E_ARG for null n_parts or parts, an n_parts[k] outside [0, GG_MAX_CLOUD_PARTS], and a
+ * dev_T_map_from_part entry that is misaligned, overlaps another or goes with a non-NULL host T_map_from_frame.  A
+ * rejected plan leaves no plan, no bound slot, and the slots' state and gg_kernel_launches unchanged.  Bound slots,
+ * gg_step_plan_launch, gg_step_plan_kernels and gg_step_plan_destroy are those of every plan. */
+typedef struct gg_step_parts {
+    const int* n_parts;                        /* host [count], 0 ... GG_MAX_CLOUD_PARTS */
+    const gg_cloud_part* parts;                /* host [sum n_parts], scan k's after scan k-1's; msg.data = DEVICE payloads
+                                                  at fixed addresses; n_points = capacity for flagged scans */
+    const double* const* dev_T_map_from_part;  /* NULL or host [sum n_parts] of DEVICE pointers (12 doubles, 8-byte
+                                                  aligned, pairwise disjoint) or NULL entries */
+    const int32_t* dev_part_counts;            /* DEVICE [count][parts_per_slot] or NULL: step 1 */
+    int parts_per_slot;
+} gg_step_parts;
+/* gg_step_plan_create_with_parts is declared after gg_step_plan_create_with_readouts, below. */
 
 /* The host-memory form, as gg_upload_cloud_msg is for gg_run_cloud_msgs_to_device: the n_parts payloads in HOST memory
  * are copied to the device, unpacked and transformed into the slot's cloud buffer back to back (part p from record
@@ -815,6 +879,9 @@ typedef struct gg_step_readouts {
 } gg_step_readouts;
 int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets,
                                       const gg_step_readouts* readouts, gg_step_plan* out);
+/* A step plan whose step 3 is a merged scan: see gg_step_parts (after gg_run_merged_cloud_msgs_to_device). */
+int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
+                                   const gg_device_resets* resets, const gg_step_readouts* readouts, gg_step_plan* out);
 
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
