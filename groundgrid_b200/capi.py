@@ -194,6 +194,16 @@ class DeviceResets(C.Structure):
     ]
 
 
+class DeviceConfigs(C.Structure):
+    """gg_device_configs: device addresses of the configurations and the mask of gg_set_slot_configs_from_device (None =
+    NULL)."""
+
+    _fields_ = [
+        ("cfg", C.c_void_p),
+        ("mask", C.c_void_p),
+    ]
+
+
 class StepDesc(C.Structure):
     """gg_step_desc: the fixed batch and caller device buffers of a step plan (gg_step_plan_create)."""
 
@@ -401,6 +411,9 @@ def load(build_if_missing=True):
         "gg_step_plan_create_with_readouts": (i, [vp, C.POINTER(StepDesc), C.POINTER(DeviceResets), C.POINTER(StepReadouts), C.POINTER(vp)]),
         "gg_step_plan_create_with_parts": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(StepReadouts),
                                                C.POINTER(vp)]),
+        "gg_set_slot_configs_from_device": (i, [vp, i, vp, C.POINTER(DeviceConfigs), vp]),
+        "gg_step_plan_create_with_configs": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(DeviceConfigs),
+                                                 C.POINTER(StepReadouts), C.POINTER(vp)]),
         "gg_step_plan_launch": (i, [vp, vp]),
         "gg_step_plan_kernels": (i, [vp]),
         "gg_step_plan_destroy": (i, [vp]),
@@ -502,6 +515,39 @@ def default_config():
     return cfg
 
 
+def config_tensor(configs, device="cuda"):
+    """uint8 tensor [n, sizeof(gg_config)] holding `configs` (a list of Config objects, or dicts of the fields that differ
+    from the defaults) in the gg_config layout, on `device`: the input of set_configs_from_device and of a step plan's
+    configs.  config_field gives typed views of its fields."""
+    import torch
+
+    rows = []
+    for c in configs:
+        if not isinstance(c, Config):
+            d, c = c, default_config()
+            for k, v in d.items():
+                if not hasattr(c, k):
+                    raise KeyError(k)
+                setattr(c, k, v)
+        rows.append(np.frombuffer(bytes(c), np.uint8))
+    a = np.stack(rows) if rows else np.zeros((0, C.sizeof(Config)), np.uint8)
+    return torch.from_numpy(a.copy()).to(device)
+
+
+def config_field(t, name):
+    """The `name` field of every row of a config_tensor as a strided view ([n], int32 or float64), so that the field can be
+    written in place on the GPU: config_field(t, "outlier_tolerance").uniform_(0.05, 0.3)."""
+    import torch
+
+    if t.dtype != torch.uint8 or t.dim() != 2 or t.shape[1] != C.sizeof(Config) or not t.is_contiguous():
+        raise ValueError("t must be a contiguous uint8 tensor [n, sizeof(gg_config)] (config_tensor)")
+    ctype = dict(Config._fields_)[name]
+    off = getattr(Config, name).offset
+    if ctype is C.c_int:
+        return t.view(torch.int32)[:, off // 4]
+    return t.view(torch.float64)[:, off // 8]
+
+
 def host_geometry_constants(dimension_m, resolution, full_layers=False):
     """{name: value} of the geometry constants the kernels get (gg::Const)."""
     out = np.zeros(len(GEOMETRY_CONSTANTS), np.float64)
@@ -576,7 +622,8 @@ class GroundGridB200:
             _check(self._l.gg_set_slot_config(self._h, int(slot), C.byref(cfg)))
 
     def get_config(self, slot=None):
-        """The handle-wide configuration (slot=None) or the one a slot runs with."""
+        """The handle-wide configuration (slot=None) or the one a slot runs with (on a device-configured slot: the stored
+        configuration, after a wait for the slot's work)."""
         cfg = Config()
         if slot is None:
             _check(self._l.gg_get_config(self._h, C.byref(cfg)))
@@ -724,6 +771,39 @@ class GroundGridB200:
                 t.record_stream(stream)
             ptrs.append(t.data_ptr() if count else None)
         self.init_maps_from_device_ptrs(slots, ptrs[0], ptrs[1], stream.cuda_stream or None)
+
+    def set_configs_from_device_ptrs(self, slots, cfg_ptr, mask_ptr, stream_ptr):
+        """gg_set_slot_configs_from_device with raw device addresses (ints, or None for NULL); stream_ptr None = the legacy
+        default stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        c = DeviceConfigs(cfg_ptr, mask_ptr)
+        _check(self._l.gg_set_slot_configs_from_device(self._h, len(sl), _ptr(sl), C.byref(c), stream_ptr))
+
+    def set_configs_from_device(self, slots, cfgs, mask=None, stream=None):
+        """set_config(slot=...) for the slots a device mask picks, with configurations in GPU memory
+        (gg_set_slot_configs_from_device).
+          cfgs   : uint8 [count, sizeof(gg_config)] (config_tensor), one configuration per slot
+          mask   : int32 [count], nonzero = reconfigure slots[k]; None = every slot
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        Every tensor must be contiguous on this handle's device.  The call returns without waiting for the device; the
+        tensors may be freed or refilled right after it when they belong to `stream` (others are marked in use on
+        `stream`).  Afterwards every slot of the call is device-configured, reconfigured or not: get_config(slot) waits
+        for the slot's work and returns the stored configuration (see the C header)."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count = len(slots)
+        ptrs = []
+        for name, t, dtype, shape in (("cfgs", cfgs, torch.uint8, (count, C.sizeof(Config))), ("mask", mask, torch.int32, (count,))):
+            if t is None:
+                ptrs.append(None)
+                continue
+            if t.dtype != dtype or t.device != dev or not t.is_contiguous() or t.numel() != int(np.prod(shape)) or (count and t.shape[0] != count):
+                raise ValueError(f"{name} must be a contiguous {dtype} tensor {shape} on {dev}")
+            if stream != current:
+                t.record_stream(stream)
+            ptrs.append(t.data_ptr() if count else None)
+        if cfgs is None and count:
+            raise ValueError("cfgs is required")
+        self.set_configs_from_device_ptrs(slots, ptrs[0], ptrs[1], stream.cuda_stream or None)
 
     def position(self, slot=0):
         xy = np.zeros(2, np.float64)
@@ -1154,7 +1234,7 @@ class GroundGridB200:
                   base_z=None, counts=None, xy=None, T_base_from_map=None, pose_origins=None, pose_base_z=None, moved=False, labels=True,
                   select="nonground", index=False, reset_xyz=None, reset_mask=None, layers=None, layer_images=None, terrain_images=False,
                   samples=None, sample_names=("ground", "groundpatch"), sample_mode="nearest", sample_cells=False, point_info=None,
-                  tallies=None, parts=None, part_counts=None):
+                  tallies=None, parts=None, part_counts=None, configs=None, config_mask=None):
         """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
         Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
         pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
@@ -1179,6 +1259,10 @@ class GroundGridB200:
           labels, select, index : the outputs, as in run_scans_to_device
           reset_xyz, reset_mask : CUDA float64 [count, 3] and int32 [count] (or None: every slot) as in
                      init_maps_from_device, read at every replay; reset_mask without reset_xyz is an error
+          configs, config_mask : CUDA uint8 [count, sizeof(gg_config)] (config_tensor) and int32 [count] (or None: every
+                     slot) as in set_configs_from_device, read at every replay: the step then starts with that call
+                     (gg_step_plan_create_with_configs), and the slots are device-configured from the plan's creation;
+                     config_mask without configs is an error
         Read-outs: with any of these the step ends with a step 4 of read-out calls (gg_step_plan_create_with_readouts),
         whose results land in plan.readouts (PlanReadouts) at every replay:
           layers       : layer names, as get_layers_to_device
@@ -1276,7 +1360,13 @@ class GroundGridB200:
             raise ValueError("reset_mask needs reset_xyz")
         r = None if reset_xyz is None else DeviceResets(dptr(reset_xyz, torch.float64, (count, 3), "reset_xyz"),
                                                         dptr(reset_mask, torch.int32, (count,), "reset_mask"))
-        if sp is not None:
+        if config_mask is not None and configs is None:
+            raise ValueError("config_mask needs configs")
+        if configs is not None:
+            cc = DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"), dptr(config_mask, torch.int32, (count,), "config_mask"))
+            _check(self._l.gg_step_plan_create_with_configs(self._h, C.byref(d), None if sp is None else C.byref(sp), None if r is None else C.byref(r),
+                                                            C.byref(cc), None if ro_c is None else C.byref(ro_c), C.byref(p)))
+        elif sp is not None:
             _check(self._l.gg_step_plan_create_with_parts(self._h, C.byref(d), C.byref(sp), None if r is None else C.byref(r),
                                                           None if ro_c is None else C.byref(ro_c), C.byref(p)))
         elif ro_c is not None:

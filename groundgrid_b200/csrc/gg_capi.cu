@@ -294,6 +294,9 @@ struct SlotState {
     // gg_set_part_counts_from_device: parts_per_slot of the latest call, 0: no part counts stored since gg_init_map
     // (GG_SCAN_DEVICE_PART_COUNTS scans may run with up to that many parts)
     int stored_parts = 0;
+    // gg_set_slot_configs_from_device: the slot's configuration lives in the device tables (ConfigTables, its private
+    // detect table); gg_init_map keeps it, gg_set_slot_config / gg_set_config make the slot host-configured again
+    bool device_config = false;
 };
 
 // While gg_step_plan_create records a step, run_groups takes its staging entries from here instead of the ring: per stream
@@ -361,6 +364,8 @@ struct gg_handle_s {
     int* d_pose_bits = nullptr;
     gg::PoseTables poses{};                // per-slot device positions and scan poses (first gg_update_poses_from_device)
     gg::CountTables counts{};              // per-slot device point counts (first gg_set_point_counts_from_device)
+    gg::ConfigTables configs{};            // per-slot device configurations (first gg_set_slot_configs_from_device)
+    std::vector<float4*> config_tab;       // per slot: its private detect table (allocated when it is first device-configured)
     cudaEvent_t ring_ev[kRing] = {};
     cudaEvent_t caller_in = nullptr;            // gg_run_scans_to_device: recorded on the caller's stream, awaited by the groups
     cudaEvent_t caller_out[kStreams] = {};      // ... recorded by each group after its outputs, awaited by the caller's stream
@@ -503,6 +508,7 @@ struct Staging {
     bool query = false;          // ... and the QueryDesc records
     bool pinfo = false;          // ... and the PointInfoDest records
     bool pose_bits = false;      // ... and the PoseBits of the records
+    bool config = false;         // the records carry a configuration (run_groups then patches device-owned ones on the device)
     bool position = false;       // fill staged slot positions (run_groups then patches device-owned ones on the device)
     bool count = false;          // fill staged last-scan counts (run_groups then takes device-owned ones on the device)
     bool stage = false;          // some record takes its position, scan pose or count from the device tables (k_stage_poses)
@@ -658,8 +664,10 @@ int check_host_counts(int count, const gg_scan_desc* scans) {
 // flagged GG_SCAN_DEVICE_POSE, is patched from the device tables by k_stage_poses right after the copy.  Counts: a scan
 // flagged GG_SCAN_DEVICE_COUNT takes its count from the slot's stored one (a merged scan flagged
 // GG_SCAN_DEVICE_PART_COUNTS takes its parts' counts in launch_part_rounds); when fill staged last-scan counts (e.count),
-// a non-empty record of a slot whose last count is device-owned takes that count.  Without such records (every all-host
-// flow) nothing more is copied or launched.
+// a non-empty record of a slot whose last count is device-owned takes that count.  Configurations: when fill staged
+// configurations (e.config), a record of a device-configured slot takes its constants from the device table (its
+// detect_tab, the slot's private table, is staged by fill_params).  Without such records (every all-host flow) nothing
+// more is copied or launched.
 template <typename Fill, typename Launch>
 int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t caller, Fill&& fill, Launch&& launch) {
     int rc;
@@ -671,7 +679,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
             if (stream_index(h, slots[i]) != g) continue;
             if (e.m == 0 && (rc = h->rec ? e.acquire_recorded(h, g) : e.acquire(h))) return rc;
             work |= fill(i, e);
-            if ((e.position || e.count) && e.hbits) {
+            if ((e.position || e.count || e.config) && e.hbits) {
                 int bits = 0;
                 if (e.position) {
                     if (h->slots[slots[i]].device_position) bits |= gg::POSE_POSITION;
@@ -680,6 +688,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
                     if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_PART_COUNTS)) bits |= gg::POSE_PART_COUNTS;
                 }
                 if (e.count && h->slots[slots[i]].device_count && e.hp[e.m].n_points > 0) bits |= gg::POSE_LAST_COUNT;
+                if (e.config && h->slots[slots[i]].device_config) bits |= gg::POSE_CONFIG;
                 e.hbits[e.m] = bits;
                 if (bits) e.pose_bits = true;
                 if (bits & ~gg::POSE_PART_COUNTS) e.stage = true;   // POSE_PART_COUNTS is k_stage_parts' (launch_part_rounds)
@@ -692,7 +701,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
         cudaStream_t st = h->rec ? h->rec->streams[g] : h->streams[g];
         if (work) {
             if (!h->rec && (rc = e.commit(st))) return rc;
-            if (e.stage) h->launches += gg::launch_stage_poses(h->poses, h->counts, e.dp, e.dbits, e.m, st, h->prof);
+            if (e.stage) h->launches += gg::launch_stage_poses(h->poses, h->counts, h->configs.cfg, e.dp, e.dbits, e.m, st, h->prof);
             if (fenced) GG_CUDA(cudaStreamWaitEvent(st, h->caller_in, 0));
             const int n = launch(e, st);
             if (n < 0) return n;
@@ -734,8 +743,8 @@ void fill_params(gg_handle h, const gg_scan_desc& d, gg::SlotParams& p, const gg
     const SlotState& s = h->slots[d.slot];
     std::memset(&p, 0, sizeof(p));
     const int var = h->variants.variant_of(d.slot);
-    p.cfg = h->variants.constants(var);
-    p.detect_tab = h->variant_tab[var];
+    p.cfg = h->variants.constants(var);   // a device-configured slot's constants are patched on the device (POSE_CONFIG)
+    p.detect_tab = s.device_config ? h->config_tab[d.slot] : h->variant_tab[var];
     p.px = s.px;
     p.py = s.py;
     p.ox = d.origin[0];
@@ -845,6 +854,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         const float* packed = packed_ptrs ? packed_ptrs[i] : nullptr;
         fill_params(h, d, e.hp[e.m], dev_points ? dev_points[i] : nullptr, packed);
         e.position = true;
+        e.config = true;
         if (caller) {
             if (e.m == 0) write = false;
             gg::OutDest& od = e.hdest[e.m];
@@ -993,6 +1003,7 @@ int run_phase(gg_handle h, int slot, double base_z, Launch&& launch) {
         d.base_z = base_z;
         fill_params(h, d, e.hp[0], h->slots[slot].src);
         e.position = true;
+        e.config = true;
         return true;
     };
     return run_groups(h, 1, &slot, false, nullptr, fill, launch);
@@ -1043,6 +1054,58 @@ int take_count_back(gg_handle h, int slot) {
     GG_CUDA(cudaStreamSynchronize(st));
     s.n_points = s.scan_points = (size_t)u;
     s.device_count = false;
+    return GG_OK;
+}
+
+// The configuration of a device-configured slot as the caller gave it, once the slot's stream group has finished what is
+// enqueued (a host wait).  The slot stays device-configured.
+int read_device_config(gg_handle h, int slot, gg_config* cfg) {
+    GG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream_of(h, slot);
+    GG_CUDA(cudaMemcpyAsync(cfg, h->configs.raw + slot, sizeof(gg_config), cudaMemcpyDeviceToHost, st));
+    GG_CUDA(cudaStreamSynchronize(st));
+    return GG_OK;
+}
+
+// The constants the single-cell calls pass by value: the slot's variant, or for a device-configured slot the derivation
+// of its stored configuration (read back with a host wait; derive_config is the function k_store_configs runs).
+int slot_constants(gg_handle h, int slot, gg::CfgConst* kc) {
+    if (!h->slots[slot].device_config) {
+        *kc = h->variants.constants(h->variants.variant_of(slot));
+        return GG_OK;
+    }
+    gg_config c;
+    int rc = read_device_config(h, slot, &c);
+    if (rc) return rc;
+    gg::derive_config(c, *kc);
+    return GG_OK;
+}
+
+// The configuration tables, the staging of the per-record bits and the private detect table of each of `slots`, on
+// first use (a handle that never asks has none).  Step plans call it before recording, which may not allocate.
+int ensure_config_tables(gg_handle h, int count, const int* slots) {
+    const size_t S = (size_t)h->n_slots;
+    int rc;
+    if (!h->configs.raw && (rc = dev_alloc(h, &h->configs.raw, S))) return rc;
+    if (!h->configs.cfg && (rc = dev_alloc(h, &h->configs.cfg, S))) return rc;
+    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
+    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    if (h->config_tab.empty()) h->config_tab.assign(S, nullptr);
+    for (int i = 0; i < count; ++i)
+        if (!h->config_tab[slots[i]] && (rc = dev_alloc(h, &h->config_tab[slots[i]], (size_t)h->view.k.N2))) return rc;
+    return GG_OK;
+}
+
+// A host-configured slot that becomes device-configured: its entries of the tables and its private detect table take its
+// current host configuration, on the slot's stream, so that a record the mask leaves alone runs as before.  Nothing in
+// flight reads them: they are the slot's only while it is device-configured, and it was not.
+int seed_device_config(gg_handle h, int slot) {
+    cudaStream_t st = stream_of(h, slot);
+    const gg::CfgConst& kc = h->variants.constants(h->variants.variant_of(slot));
+    GG_CUDA(cudaMemcpyAsync(h->configs.raw + slot, &h->slot_cfg[slot], sizeof(gg_config), cudaMemcpyHostToDevice, st));
+    GG_CUDA(cudaMemcpyAsync(h->configs.cfg + slot, &kc, sizeof(kc), cudaMemcpyHostToDevice, st));
+    h->launches += gg::launch_build_detect_table(h->view, kc, h->config_tab[slot], st);
+    GG_CUDA(cudaGetLastError());
     return GG_OK;
 }
 
@@ -1311,6 +1374,7 @@ int gg_set_config(gg_handle h, const gg_config* cfg) {
     if (rc) return rc;
     h->cfg = *cfg;
     h->slot_cfg.assign((size_t)h->n_slots, *cfg);
+    for (SlotState& s : h->slots) s.device_config = false;
     gg::CfgConst kc;
     gg::derive_config(*cfg, kc);
     h->variants.reset(h->n_slots, kc);   // every slot on variant 0; nothing reads the others any more
@@ -1356,6 +1420,7 @@ int gg_set_slot_config(gg_handle h, int slot, const gg_config* cfg) {
         }
     }
     h->slot_cfg[slot] = *cfg;
+    h->slots[slot].device_config = false;
     return GG_OK;
 }
 
@@ -1363,6 +1428,7 @@ int gg_get_slot_config(gg_handle h, int slot, gg_config* cfg) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
     if (!cfg) return fail(GG_E_ARG, "null argument");
+    if (h->slots[slot].device_config) return read_device_config(h, slot, cfg);
     *cfg = h->slot_cfg[slot];
     return GG_OK;
 }
@@ -1373,7 +1439,9 @@ int gg_init_map(gg_handle h, int slot, double x, double y, double z) {
     if ((rc = take_position_back(h, slot))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
     SlotState& s = h->slots[slot];
+    const bool device_config = s.device_config;   // the map starts over, the configuration stays
     s = SlotState();
+    s.device_config = device_config;
     s.px = x;
     s.py = y;
     s.have_map = true;
@@ -1848,8 +1916,10 @@ int gg_interpolate_cell(gg_handle h, int slot, int x, int y) {
     if (rc) return rc;
     const int N = h->view.k.N;
     if (x < 1 || y < 1 || x >= N - 1 || y >= N - 1) return fail(GG_E_ARG, "cell (%d, %d) has no 3x3 neighbourhood", x, y);
+    gg::CfgConst kc;
+    if ((rc = slot_constants(h, slot, &kc))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
-    h->launches += gg::launch_interpolate_cell(h->view, h->variants.constants(h->variants.variant_of(slot)), slot, x, y, stream_of(h, slot));
+    h->launches += gg::launch_interpolate_cell(h->view, kc, slot, x, y, stream_of(h, slot));
     GG_CUDA(cudaGetLastError());
     return GG_OK;
 }
@@ -1862,9 +1932,10 @@ int gg_detect_ground_patch(gg_handle h, int slot, int patch_size, int i, int j) 
     if (i < H || j < H || i >= N - H || j >= N - H) return fail(GG_E_ARG, "cell (%d, %d) has no %dx%d neighbourhood", i, j, patch_size, patch_size);
     int points = gg::L_COUNT;
     if ((rc = layer_index(h, slot, "points", &points))) return rc;
+    gg::CfgConst kc;
+    if ((rc = slot_constants(h, slot, &kc))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
-    h->launches += gg::launch_detect_cell(h->view, h->variants.constants(h->variants.variant_of(slot)), slot, patch_size, i, j, points,
-                                          stream_of(h, slot));
+    h->launches += gg::launch_detect_cell(h->view, kc, slot, patch_size, i, j, points, stream_of(h, slot));
     GG_CUDA(cudaGetLastError());
     return GG_OK;
 }
@@ -1960,7 +2031,8 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_roll_commit", "k_out_count",     "k_out_scan",         "k_out_write",     "k_unpack_transform",
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
                                            "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve", "k_store_counts",
-                                           "k_reset_maps", "k_stage_parts", "k_store_part_counts"};
+                                           "k_reset_maps", "k_stage_parts", "k_store_part_counts", "k_store_configs",
+                                           "k_rebuild_detect_tables"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2811,6 +2883,46 @@ int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
+// Configurations from device memory: per stream group one k_store_configs and one k_rebuild_detect_tables over the group's
+// slots.  The host cannot see the mask, so every slot of the call leaves it device-configured.
+int gg_set_slot_configs_from_device(gg_handle h, int count, const int* slots, const gg_device_configs* configs, void* stream) {
+    if (!h) return fail(GG_E_ARG, "null handle");
+    if (count < 0) return fail(GG_E_ARG, "negative count");
+    if (count == 0) return GG_OK;
+    if (!slots || !configs || !configs->cfg) return fail(GG_E_ARG, "null argument");
+    const gg_device_configs& in = *configs;
+    if (reinterpret_cast<uintptr_t>(in.cfg) % alignof(double)) return fail(GG_E_ARG, "cfg is not 8-byte aligned");
+    if (reinterpret_cast<uintptr_t>(in.mask) % alignof(int32_t)) return fail(GG_E_ARG, "mask is not 4-byte aligned");
+    const gg::View& v = h->view;
+    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    if (ranges_overlap(in.cfg, (size_t)count * sizeof(gg_config), v.layers, arena_bytes) ||
+        ranges_overlap(in.mask, (size_t)count * sizeof(int32_t), v.layers, arena_bytes))
+        return fail(GG_E_ARG, "cfg or mask overlaps the handle's layers");
+    int rc;
+    if ((rc = check_slots(h, count, slots, nullptr, false))) return rc;
+    // a plan's records of a host-configured slot carry its configuration by value
+    for (int i = 0; i < count; ++i)
+        if (h->slot_plan[slots[i]] && !h->slots[slots[i]].device_config)
+            return fail(GG_E_STATE, "slot %d is bound to a step plan recorded while it was host-configured", slots[i]);
+    GG_CUDA(cudaSetDevice(h->device));
+    if ((rc = ensure_config_tables(h, count, slots))) return rc;
+    for (int i = 0; i < count; ++i)
+        if (!h->slots[slots[i]].device_config && (rc = seed_device_config(h, slots[i]))) return rc;
+    auto fill = [&](int i, Staging& e) {
+        gg::SlotParams& p = e.hp[e.m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slots[i];
+        p.pos = i;
+        p.detect_tab = h->config_tab[slots[i]];
+        h->slots[slots[i]].device_config = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) {
+        return gg::launch_store_configs(h->view, h->configs, e.dp, e.m, in.cfg, in.mask, st, h->prof);
+    };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
 int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
@@ -2834,8 +2946,9 @@ void free_plan(gg_step_plan p) {
 }
 
 // What gg_step_plan_create checks beyond the step's calls (those check their own arguments while the step is recorded).
-int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets) {
+int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs) {
     if (resets && !resets->xyz) return fail(GG_E_ARG, "resets without xyz");
+    if (configs && !configs->cfg) return fail(GG_E_ARG, "configs without cfg");
     if (d.count <= 0) return fail(GG_E_ARG, "a step plan needs count > 0 scans, got %d", d.count);
     if (!d.scans) return fail(GG_E_ARG, "null scans");
     if (d.count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", d.count, h->n_slots);
@@ -2895,18 +3008,20 @@ struct ReadoutCalls {
     int count() const { return layers + images + terrain + samples + point_info + eval; }
 };
 
-// The calls a plan's step records: the resets, counts (or part counts) and poses when given, the scans, and the read-outs.
-int step_calls(const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_step_readouts* readouts) {
+// The calls a plan's step records: the configurations, resets, counts (or part counts) and poses when given, the scans,
+// and the read-outs.
+int step_calls(const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
+               const gg_step_readouts* readouts) {
     const gg_device_poses& q = d.poses;
-    return (resets != nullptr) + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) + (q.xy || q.T_base_from_map || q.origin || q.base_z) +
+    return (configs != nullptr) + (resets != nullptr) + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) + (q.xy || q.T_base_from_map || q.origin || q.base_z) +
            1 + ReadoutCalls(readouts).count();
 }
 
-// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_readouts): per branch the restore of
-// its records and, where a payload takes a device transform, the transform staging; then the step's calls, the resets
-// (when given) first and the read-outs last.
-int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_step_readouts* readouts,
-                const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
+// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_configs): per branch the restore of
+// its records and, where a payload takes a device transform, the transform staging; then the step's calls, the
+// configurations and the resets (when given) first and the read-outs last.
+int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
+                const gg_step_readouts* readouts, const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
     PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
@@ -2921,6 +3036,7 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     const int n = d.count;
     const int* sl = slots.data();
     const gg_device_poses& q = d.poses;
+    if (configs && (rc = gg_set_slot_configs_from_device(h, n, sl, configs, root))) return rc;
     if (resets && (rc = gg_init_maps_from_device(h, n, sl, resets, root))) return rc;
     if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
     if (parts && parts->dev_part_counts && (rc = gg_set_part_counts_from_device(h, n, sl, parts->parts_per_slot, parts->dev_part_counts, root)))
@@ -2949,7 +3065,7 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
 
 // Everything the recorded kernels address that the step's calls would allocate on first use, and the spiral's shared
 // memory opt-in: a recording may not allocate, and the View it records must not change afterwards.
-int prepare_recording(gg_handle h, const gg_step_readouts* readouts) {
+int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_configs* configs, const gg_step_readouts* readouts) {
     const size_t S = (size_t)h->n_slots;
     int rc;
     if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
@@ -2965,6 +3081,11 @@ int prepare_recording(gg_handle h, const gg_step_readouts* readouts) {
     if (c.point_info && !h->d_pinfo && (rc = dev_alloc(h, &h->d_pinfo, (size_t)kRing * S))) return rc;
     if (c.point_info && !h->h_pinfo)
         GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * kRing * S, cudaHostAllocDefault));
+    if (configs) {
+        std::vector<int> slots(d.count);
+        for (int i = 0; i < d.count; ++i) slots[i] = d.scans[i].slot;
+        if ((rc = ensure_config_tables(h, d.count, slots.data()))) return rc;
+    }
     if (gg::prepare_scan_pipeline(h->view)) return fail(GG_E_CUDA, "spiral shared-memory opt-in: %s", cudaGetErrorString(cudaGetLastError()));
     return GG_OK;
 }
@@ -2972,9 +3093,9 @@ int prepare_recording(gg_handle h, const gg_step_readouts* readouts) {
 // gg_step_plan_create after check_step_desc and prepare_recording: lays out the record blocks, seeds the positions,
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
-int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_step_readouts* readouts,
-                gg_step_plan p) {
-    const int count = d.count, calls = step_calls(d, parts, resets, readouts);
+int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
+                const gg_step_readouts* readouts, gg_step_plan p) {
+    const int count = d.count, calls = step_calls(d, parts, resets, configs, readouts);
     std::vector<int>& slots = p->slots;
     slots.resize(count);
     for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
@@ -3037,6 +3158,19 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         }
         s.device_position = true;
     }
+    // with configurations, the slots become device-configured here (seeded, as a standalone call seeds them), so the
+    // recorded call has nothing to seed; a rejected plan takes the seed launches back with the state
+    const uint64_t seed_launches = h->launches;
+    for (int j = 0; configs && j < count; ++j) {
+        SlotState& s = h->slots[slots[j]];
+        if (s.device_config) continue;
+        if (int rc = seed_device_config(h, slots[j])) {
+            restore();
+            h->launches = seed_launches;
+            return rc;
+        }
+        s.device_config = true;
+    }
 
     cudaStream_t root = nullptr;
     cudaEvent_t fork = nullptr;
@@ -3053,7 +3187,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, parts, resets, readouts, slots, T_group, root, fork, p);
+        rc = record_step(h, d, parts, resets, configs, readouts, slots, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -3073,10 +3207,17 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         p->after.resize(count);
         for (int j = 0; j < count; ++j) p->after[j] = h->slots[slots[j]];
     }
-    // the recording ran nothing: the slots keep their state, with the seeded positions device-owned on success
+    // the recording ran nothing: the slots keep their state, with the seeded positions device-owned (and, with
+    // configurations, the slots device-configured) on success
     restore();
-    if (rc) return rc;
-    for (int j = 0; j < count; ++j) h->slots[slots[j]].device_position = true;
+    if (rc) {
+        h->launches = seed_launches;
+        return rc;
+    }
+    for (int j = 0; j < count; ++j) {
+        h->slots[slots[j]].device_position = true;
+        if (configs) h->slots[slots[j]].device_config = true;
+    }
 
     // the records as recorded, the caller transforms of the payload records (row j of the scan entry, or of part round q's
     // entry, is the group's j-th scan), and the executable graph
@@ -3113,16 +3254,21 @@ int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, con
 
 int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
                                    const gg_step_readouts* readouts, gg_step_plan* out) {
+    return gg_step_plan_create_with_configs(h, desc, parts, resets, nullptr, readouts, out);
+}
+
+int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                     const gg_device_configs* configs, const gg_step_readouts* readouts, gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
     if (!h || !desc) return fail(GG_E_ARG, "null argument");
     int rc;
-    if ((rc = check_step_desc(h, *desc, parts, resets))) return rc;
+    if ((rc = check_step_desc(h, *desc, parts, resets, configs))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
-    if ((rc = prepare_recording(h, readouts))) return rc;
+    if ((rc = prepare_recording(h, *desc, configs, readouts))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, parts, resets, readouts, p))) {
+    if ((rc = record_plan(h, *desc, parts, resets, configs, readouts, p))) {
         free_plan(p);
         return rc;
     }

@@ -51,35 +51,6 @@ void derive_geometry(double dimension_m, float resolution, unsigned flags, Const
     k.res_sq = (double)k.res_f * (double)k.res_f;
 }
 
-// The constants of one configuration (GroundSegmentation::setConfig, GroundGrid::setConfig).
-void derive_config(const gg_config& c, CfgConst& k) {
-    std::memset(&k, 0, sizeof(k));
-    k.max_ring = c.max_ring;
-    k.pc_var_thresh_f = (float)c.point_count_cell_variance_threshold;
-    k.min_outlier_conf = c.min_outlier_detection_ground_confidence;
-    k.outlier_tol = c.outlier_tolerance;
-    k.gp_thresh = c.ground_patch_detection_minimum_point_count_threshold;
-    k.df_sq = c.distance_factor * c.distance_factor;
-    k.mdf_sq = c.minimum_distance_factor * c.minimum_distance_factor;
-    const double m10 = c.minimum_distance_factor * 10;
-    k.mdf10_sq = m10 * m10;
-    k.psc_sq = c.patch_size_change_distance * c.patch_size_change_distance;
-    k.occ_factor = c.occupied_cells_point_count_factor;
-    k.occ_factor2 = c.occupied_cells_point_count_factor * 2.0f;
-    k.dec_factor = c.occupied_cells_decrease_factor;
-    k.lab_fac = c.minimum_distance_factor * 5;
-    k.lab_thres = c.miminum_point_height_threshold;
-    k.lab_obs = c.minimum_point_height_obstacle_threshold;
-    // decay_confidence (gg_kernels.cu): o - o / dec_factor, floored at 0.001.  For factors >= 1 the exact value
-    // o * (1 - 1/F) grows with o, so if the floor value 0.001f itself decays to clearly below 0.001, every
-    // confidence <= 0.001f ends on the floor as well (rounding errors are ~1e-19, the margin asked for is 1e-6).
-    {
-        const double o = (double)0.001f;
-        const double dec = o - o / k.dec_factor;
-        k.decay_floor_ok = (k.dec_factor >= 1.0 && dec < 0.000999) ? 1 : 0;
-    }
-}
-
 void ConfigRegistry::reset(int n_slots, const CfgConst& k) {
     for (Variant& v : vars_) v.refs = 0;
     if (vars_.empty()) vars_.push_back(Variant{});

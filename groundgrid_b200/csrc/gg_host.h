@@ -9,7 +9,6 @@ namespace gg {
 int cells_per_side(double dimension_m, float resolution);
 void build_expected_points(int n, std::vector<float>& table);
 void derive_geometry(double dimension_m, float resolution, unsigned flags, Const& k);
-void derive_config(const gg_config& c, CfgConst& k);
 
 // Configuration variants of a handle.  Slots whose derived constants are identical share one variant (one
 // constants record and one detect table on the device), so device memory grows with the number of distinct

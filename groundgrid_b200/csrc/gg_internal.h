@@ -181,7 +181,7 @@ constexpr int OUT_TILE = 1024;
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
     K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_STAGE_POSES, K_POSE_RESOLVE,
-    K_STORE_COUNTS, K_RESET_MAPS, K_STAGE_PARTS, K_STORE_PART_COUNTS,
+    K_STORE_COUNTS, K_RESET_MAPS, K_STAGE_PARTS, K_STORE_PART_COUNTS, K_STORE_CONFIGS, K_REBUILD_DETECT,
     K_NUM
 };
 
@@ -312,6 +312,35 @@ __host__ __device__ __forceinline__ double pose_div(double a, double b) {
 #else
     return a / b;
 #endif
+}
+
+// ---- the constants of one configuration (GroundSegmentation::setConfig, GroundGrid::setConfig) ----
+// One derivation for the host (gg_set_slot_config, gg_set_config) and the device (k_store_configs), with the same
+// correctly rounded fp64 operations, so both produce the same 120 bytes for the same gg_config.
+__host__ __device__ __forceinline__ void derive_config(const gg_config& c, CfgConst& k) {
+    k.max_ring = c.max_ring;
+    k.pc_var_thresh_f = (float)c.point_count_cell_variance_threshold;
+    k.min_outlier_conf = c.min_outlier_detection_ground_confidence;
+    k.outlier_tol = c.outlier_tolerance;
+    k.gp_thresh = c.ground_patch_detection_minimum_point_count_threshold;
+    k.df_sq = pose_mul(c.distance_factor, c.distance_factor);
+    k.mdf_sq = pose_mul(c.minimum_distance_factor, c.minimum_distance_factor);
+    const double m10 = pose_mul(c.minimum_distance_factor, 10.0);
+    k.mdf10_sq = pose_mul(m10, m10);
+    k.psc_sq = pose_mul(c.patch_size_change_distance, c.patch_size_change_distance);
+    k.occ_factor = c.occupied_cells_point_count_factor;
+    k.occ_factor2 = pose_mul(c.occupied_cells_point_count_factor, (double)2.0f);
+    k.dec_factor = c.occupied_cells_decrease_factor;
+    k.lab_fac = pose_mul(c.minimum_distance_factor, 5.0);
+    k.lab_thres = c.miminum_point_height_threshold;
+    k.lab_obs = c.minimum_point_height_obstacle_threshold;
+    // decay_confidence: o - o / dec_factor, floored at 0.001.  For factors >= 1 the exact value o * (1 - 1/F) grows
+    // with o, so if the floor value 0.001f itself decays to clearly below 0.001, every confidence <= 0.001f ends on the
+    // floor as well (rounding errors are ~1e-19, the margin asked for is 1e-6).
+    const double o = (double)0.001f;
+    const double dec = pose_sub(o, pose_div(o, k.dec_factor));
+    k.decay_floor_ok = (k.dec_factor >= 1.0 && dec < 0.000999) ? 1 : 0;
+    k.reserved = 0;
 }
 
 // ---- confidence decay of the spiral sweep (interpolate_cell :463-464), shared by every spiral path ----
@@ -474,6 +503,13 @@ enum PoseBits : int {
     POSE_LAST_COUNT = 8, // n_points from the slot's last count (the count of its last scan is device-owned)
     POSE_PART_COUNTS = 16,  // a merged scan of GG_SCAN_DEVICE_PART_COUNTS: k_stage_parts (not k_stage_poses) resolves
                             // its parts' counts and offsets from the slot's stored part counts
+    POSE_CONFIG = 32,    // cfg from the slot's entry of ConfigTables::cfg (the slot is device-configured; its detect_tab
+                         // is staged from the host: the slot's private table)
+};
+// The handle's per-slot configurations from device memory (allocated on the first gg_set_slot_configs_from_device).
+struct ConfigTables {
+    gg_config* raw;      // [n_slots] the configuration as the caller gave it (gg_get_slot_config returns it)
+    CfgConst* cfg;       // [n_slots] its derived constants
 };
 // The handle's per-slot device tables (allocated on the first gg_update_poses_from_device).
 struct PoseTables {
@@ -489,7 +525,15 @@ struct CountTables {
 };
 // Patches the `count` records of batch whose bits ask for it from the tables; runs after the entry's copy and before
 // the kernels that read it.
-int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof);
+int launch_stage_poses(const PoseTables& t, const CountTables& c, const CfgConst* cfgs, SlotParams* batch, const int* bits, int count,
+                       cudaStream_t st, Profiler* prof);
+// Configurations from device memory (gg_set_slot_configs_from_device), two launches on one staging entry whose record j
+// carries slot, pos and detect_tab (the slot's private table).  k_store_configs, one thread per record: unless mask (may
+// be null) is zero at pos, cfg[pos] goes to the slot's entry of t.raw and its derivation (derive_config) to t.cfg; the
+// record's n_points becomes 1 if it was reconfigured, else 0.  k_rebuild_detect_tables, a grid of (cells, records):
+// each reconfigured record's detect table is rebuilt from t.cfg; the blocks of the other records exit after one load.
+int launch_store_configs(const View& v, const ConfigTables& t, SlotParams* batch, int count, const gg_config* cfg, const int32_t* mask,
+                         cudaStream_t st, Profiler* prof);
 // One thread per record: the count of batch[j] (at dev_n[batch[j].pos]) into the slot's entry of c.stored.
 int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof);
 // One thread per record: the parts_per_slot part counts of batch[j] (at dev_n[batch[j].pos * parts_per_slot]) into the

@@ -792,11 +792,10 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
 //   y: variance threshold (:369)      z: expectedPoints      w: flags
 constexpr int DTF_S5 = 1, DTF_FAR = 2, DTF_INNER = 4;
 
-__global__ void k_build_detect_table(View v, const CfgConst kc, float4* __restrict__ tab) {
+// The table entry of one cell (cell < N2); k_build_detect_table and k_rebuild_detect_tables share it.
+__device__ __forceinline__ float4 detect_table_entry(const View& v, const CfgConst& kc, int cell) {
     const Const& k = v.k;
     const int N = k.N;
-    const int cell = blockIdx.x * blockDim.x + threadIdx.x;
-    if (cell >= k.N2) return;
     const int i = cell % N, j = cell / N;
     const double di = __dsub_rn((double)i, (double)N / 2.0), dj = __dsub_rn((double)j, (double)N / 2.0);
     const float sqdist = (float)__dmul_rn(__dadd_rn(__dmul_rn(di, di), __dmul_rn(dj, dj)), k.res_sq);  // :332,356
@@ -815,7 +814,25 @@ __global__ void k_build_detect_table(View v, const CfgConst kc, float4* __restri
     const double a = __dmul_rn((double)sqdist, kc.df_sq);
     const double m = (a < kc.mdf_sq) ? kc.mdf_sq : a;
     const float vt = (float)((kc.mdf10_sq < m) ? kc.mdf10_sq : m);
-    tab[cell] = make_float4(__double2float_ru(need), vt, e, __int_as_float(flags));
+    return make_float4(__double2float_ru(need), vt, e, __int_as_float(flags));
+}
+
+__global__ void k_build_detect_table(View v, const CfgConst kc, float4* __restrict__ tab) {
+    const int cell = blockIdx.x * blockDim.x + threadIdx.x;
+    if (cell >= v.k.N2) return;
+    tab[cell] = detect_table_entry(v, kc, cell);
+}
+
+// The detect tables of the records k_store_configs reconfigured (gg_set_slot_configs_from_device): block (x, y) builds
+// cells [x * 256, x * 256 + 256) of record y's table from the slot's derived constants.
+__global__ void __launch_bounds__(256) k_rebuild_detect_tables(View v, const CfgConst* __restrict__ cfgs, const SlotParams* __restrict__ batch) {
+    const SlotParams& p = batch[blockIdx.y];
+    if (!p.n_points) return;   // masked off: the slot keeps its configuration and its table
+    const int cell = blockIdx.x * 256 + threadIdx.x;
+    if (cell >= v.k.N2) return;
+    // the slot's private table (gg_capi.cu:ensure_config_tables); the record only carries it as the read-only pointer
+    // the pipeline kernels take
+    const_cast<float4*>(p.detect_tab)[cell] = detect_table_entry(v, cfgs[p.slot], cell);
 }
 
 // returns true when (g, c) changed
@@ -2302,13 +2319,14 @@ constexpr int POSE_THREADS = 128;
 
 // A staging entry's records take the slot's device-owned position and / or its device scan pose, and their point count
 // from the count tables, after the entry's copy and before the kernels that read them (the same stream).
-__global__ void __launch_bounds__(POSE_THREADS) k_stage_poses(PoseTables t, CountTables c, SlotParams* __restrict__ batch, const int* __restrict__ bits,
-                                                              int count) {
+__global__ void __launch_bounds__(POSE_THREADS) k_stage_poses(PoseTables t, CountTables c, const CfgConst* __restrict__ cfgs,
+                                                              SlotParams* __restrict__ batch, const int* __restrict__ bits, int count) {
     const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
     if (j >= count) return;
     const int b = bits[j];
     if (!b) return;
     SlotParams& p = batch[j];
+    if (b & POSE_CONFIG) p.cfg = cfgs[p.slot];
     if (b & POSE_COUNT) {
         // the staged n_points is the scan's capacity: a count outside [0, capacity] runs the scan empty, never clamped
         const int v = c.stored[p.slot];
@@ -2387,6 +2405,23 @@ __global__ void __launch_bounds__(POSE_THREADS) k_store_part_counts(CountTables 
     int32_t* dst = c.parts + (size_t)p.slot * GG_MAX_CLOUD_PARTS;
     const int32_t* src = dev_n + (size_t)p.pos * parts_per_slot;
     for (int q = 0; q < parts_per_slot; ++q) dst[q] = src[q];
+}
+
+// Configurations from device memory (gg_set_slot_configs_from_device): record j stores the caller's configuration of its
+// slot, unless the mask is zero there, as given and derived; its n_points tells k_rebuild_detect_tables whether it did.
+__global__ void __launch_bounds__(POSE_THREADS) k_store_configs(ConfigTables t, SlotParams* __restrict__ batch, int count,
+                                                                const gg_config* __restrict__ cfg, const int32_t* __restrict__ mask) {
+    const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
+    if (j >= count) return;
+    SlotParams& p = batch[j];
+    const int on = !mask || mask[p.pos] != 0;
+    p.n_points = on;
+    if (!on) return;
+    const gg_config c = cfg[p.pos];
+    t.raw[p.slot] = c;
+    CfgConst k;
+    derive_config(c, k);
+    t.cfg[p.slot] = k;
 }
 
 // A merged scan of GG_SCAN_DEVICE_PART_COUNTS (record j of a scan entry): the rule of k_stage_poses' POSE_COUNT applied
@@ -2780,9 +2815,17 @@ int launch_point_info(const View& v, const SlotParams* batch, const PointInfoDes
     return 1;
 }
 
-int launch_stage_poses(const PoseTables& t, const CountTables& c, SlotParams* batch, const int* bits, int count, cudaStream_t st, Profiler* prof) {
-    GG_LAUNCH(K_STAGE_POSES, k_stage_poses<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(t, c, batch, bits, count));
+int launch_stage_poses(const PoseTables& t, const CountTables& c, const CfgConst* cfgs, SlotParams* batch, const int* bits, int count,
+                       cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_STAGE_POSES, k_stage_poses<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(t, c, cfgs, batch, bits, count));
     return 1;
+}
+
+int launch_store_configs(const View& v, const ConfigTables& t, SlotParams* batch, int count, const gg_config* cfg, const int32_t* mask,
+                         cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_STORE_CONFIGS, k_store_configs<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(t, batch, count, cfg, mask));
+    GG_LAUNCH(K_REBUILD_DETECT, k_rebuild_detect_tables<<<dim3(cdiv(v.k.N2, 256), count), 256, 0, st>>>(v, t.cfg, batch));
+    return 2;
 }
 
 int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof) {

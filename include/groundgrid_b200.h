@@ -277,6 +277,54 @@ typedef struct gg_device_resets {
  * _wait) first. */
 int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_device_resets* resets, void* stream);
 
+/* ---- configurations from caller GPU memory ----
+ * gg_set_slot_config for the slots a DEVICE mask picks, with configurations read from DEVICE memory, ordered on the
+ * caller's stream.  For callers that choose configurations on the GPU (a simulator that randomises perception parameters
+ * per episode, a population-based parameter search scored with gg_eval_counts_to_device, a GPU classifier that picks
+ * thresholds per terrain), which would otherwise read them back to the host and, inside a step plan, destroy and
+ * re-record the plan.  Entry k of both arrays belongs to slots[k]. */
+typedef struct gg_device_configs {
+    const gg_config* cfg;   /* DEVICE [count], 8-byte aligned: the new configuration of slots[k] (the gg_config layout, 104 bytes) */
+    const int32_t* mask;    /* DEVICE [count] or NULL, 4-byte aligned: nonzero = reconfigure slots[k]; NULL = every slot */
+} gg_device_configs;
+
+/* Effect: for each k with mask[k] != 0 (every k when mask is NULL), slot slots[k] runs with cfg[k] from its next launch
+ *   in its stream order on: every later result of the slot -- labels, index, cloud, dev_counts, every layer
+ *   (GG_FLAG_FULL_LAYERS layers included), gg_get_output, point info, tallies -- is bit-identical to gg_set_slot_config(
+ *   slots[k], &cfg[k]) at the same point of the slot's stream.  A slot whose mask entry is zero keeps the configuration it
+ *   had.  Values are not validated, as in gg_set_slot_config (NaN, infinities, negative values and INT_MAX behave as
+ *   there); thread_count and groundpatch_detection_minimum_threshold are stored and not used.  The constants are derived
+ *   on the device by the function the host uses, and each reconfigured slot's per-cell detect table is rebuilt there.
+ * stream: cudaStream_t; NULL is the legacy default stream.  The contract of gg_init_maps_from_device: the work starts
+ *   after everything already enqueued on `stream` and on the stream groups of the slots, work enqueued on `stream`
+ *   afterwards sees the new configurations, and nothing waits on the host except the flow control of the parameter
+ *   staging ring.  cfg and mask are consumed by the first kernel of each stream group, so a stream-ordered allocator may
+ *   free or refill them on `stream` right after the call.
+ * Host state afterwards -- the host cannot see the mask, so it is the same for every slot of the call, reconfigured or
+ *   not: the slot is DEVICE-CONFIGURED.
+ *   - Every launch that reads a configuration (gg_filter_cloud[_batch[_begin]], gg_run_scans[_device],
+ *     gg_run_scans_to_device, gg_run_cloud_msgs_to_device, gg_run_merged_cloud_msgs_to_device, the per-phase entries)
+ *     takes the slot's constants from the device in stream order, and its detect table from a table private to the slot.
+ *   - gg_get_slot_config waits on the host for the slot's stream group and returns the stored gg_config bytes as the
+ *     caller gave them; gg_detect_ground_patch and gg_interpolate_cell wait the same way and run with the stored
+ *     configuration.  The slot stays device-configured.
+ *   - gg_set_slot_config makes the slot host-configured again, and gg_set_config makes every slot so.
+ *   - gg_init_map and gg_init_maps_from_device keep the configuration.
+ * Memory: the first call allocates 224 bytes per slot of the handle, and each slot's first call 16 * N * N bytes for its
+ * private detect table (slots with equal device configurations do not share tables).  A slot's first call also copies
+ * its current host configuration into its entries and builds its table (one kernel, on the slot's stream), so a slot the
+ * mask leaves alone runs as before.
+ * Slots bound to a step plan: accepted when the slot was device-configured when the plan was created (the plan's records
+ * then read the configuration at replay); GG_E_STATE otherwise, since the plan's records carry it by value.
+ * No map is needed.  count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued and every slot's
+ * state and gg_kernel_launches unchanged:
+ *   GG_E_ARG   null handle, slots, configs or cfg; count > n_slots; a slot out of range or repeated; cfg not 8-byte or mask
+ *              not 4-byte aligned; cfg or mask overlapping the handle's layers
+ *   GG_E_STATE a slot bound to a plan that does not read configurations at replay
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_set_slot_configs_from_device(gg_handle h, int count, const int* slots, const gg_device_configs* configs, void* stream);
+
 /* A whole step -- resets, counts, poses and scans -- recorded once and replayed from caller GPU memory: see the step plans
  * (gg_step_plan_create) after gg_run_cloud_msgs_to_device. */
 
@@ -882,6 +930,22 @@ int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, con
 /* A step plan whose step 3 is a merged scan: see gg_step_parts (after gg_run_merged_cloud_msgs_to_device). */
 int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                    const gg_device_resets* resets, const gg_step_readouts* readouts, gg_step_plan* out);
+/* A step plan whose step starts with the slots' configurations: gg_set_slot_configs_from_device(configs) over the plan's
+ * slots in desc->scans order, then steps 0-4 as in gg_step_plan_create_with_parts (parts may be NULL: then
+ * desc->dev_points / msgs as in gg_step_plan_create_with_readouts).  Every replay is bit-identical to that call sequence
+ * run on the buffers' contents at replay time: configs->cfg and configs->mask are read at replay time, so both may change
+ * every step.  configs NULL is exactly gg_step_plan_create_with_parts.  With configs the plan's slots become
+ * device-configured at creation (seeded with their current configurations, as a first standalone call seeds them).
+ * Bound slots: a plan's records of a slot that is device-configured at creation read the slot's configuration at every
+ * replay, with or without configs, so a standalone gg_set_slot_configs_from_device on such a bound slot is accepted and
+ * reaches the plan's next replay; on a slot that was host-configured at creation it is GG_E_STATE.  gg_set_slot_config and
+ * gg_set_config stay refused on bound slots.  Validation: what gg_step_plan_create_with_parts validates, what
+ * gg_set_slot_configs_from_device validates, and GG_E_ARG for configs without cfg.  A rejected plan leaves no plan, no
+ * bound slot, no device-configured slot, and the slots' state and gg_kernel_launches unchanged.  The config stage adds
+ * two kernels per stream group. */
+int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
+                                     const gg_device_resets* resets, const gg_device_configs* configs,
+                                     const gg_step_readouts* readouts, gg_step_plan* out);
 
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
