@@ -17,6 +17,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "gg_host.h"
@@ -324,12 +325,29 @@ struct PlanRecorder {
     int records = 0;                                 // records over all blocks
 };
 
-// A caller's device byte range [begin, end) of one query set: its positions (input) or one of its outputs.
+// A caller's device byte range [begin, end), non-empty: an input or an output of entry `set` of a call (a buffer, a query
+// set, a slot, a scan or part).
 struct ByteRange {
     uintptr_t begin, end;
     int set;
     bool output;
 };
+
+// The rule for a call's caller ranges: an output overlaps no other range, inputs may overlap each other.  Returns the
+// first offending pair found, earlier start first, or two nulls.  Sorted by start, a range
+// overlaps an earlier one iff it starts below the largest end among them, so one sweep keeps the farthest-reaching range
+// and the farthest-reaching output.  Sorts `ranges`.
+std::pair<const ByteRange*, const ByteRange*> find_overlap(std::vector<ByteRange>& ranges) {
+    std::sort(ranges.begin(), ranges.end(), [](const ByteRange& a, const ByteRange& b) { return a.begin < b.begin; });
+    const ByteRange *far_any = nullptr, *far_out = nullptr;
+    for (const ByteRange& r : ranges) {
+        const ByteRange* o = r.output ? far_any : far_out;
+        if (o && o->end > r.begin) return {o, &r};
+        if (!far_any || r.end > far_any->end) far_any = &r;
+        if (r.output && (!far_out || r.end > far_out->end)) far_out = &r;
+    }
+    return {nullptr, nullptr};
+}
 
 }  // namespace
 
@@ -359,8 +377,8 @@ struct gg_handle_s {
     gg::QueryDesc* h_query = nullptr;    // terrain lookups: query sets of the entry's slots, same shape as h_ring / d_ring
     gg::QueryDesc* d_query = nullptr;
     gg::PointInfoDest* h_pinfo = nullptr;  // point classes and heights: destinations of the entry's slots, same shape
-    gg::PointInfoDest* d_pinfo = nullptr;  // (both allocated on first use)
-    int* h_pose_bits = nullptr;            // gg::PoseBits of the entry's records, same shape (allocated with `poses`)
+    gg::PointInfoDest* d_pinfo = nullptr;  // (both allocated on first use: ensure_tables)
+    int* h_pose_bits = nullptr;            // gg::PoseBits of the entry's records, same shape (allocated on first use)
     int* d_pose_bits = nullptr;
     gg::PoseTables poses{};                // per-slot device positions and scan poses (first gg_update_poses_from_device)
     gg::CountTables counts{};              // per-slot device point counts (first gg_set_point_counts_from_device)
@@ -375,9 +393,8 @@ struct gg_handle_s {
     std::vector<void*> dev_allocs;
     std::vector<unsigned char> seen_scratch;  // duplicate-slot check of the batch calls (check_slots)
     std::vector<int> part_base;               // gg_run_merged_cloud_msgs_to_device: index in `parts` of each scan's first part
-    std::vector<ByteRange> range_scratch;     // gg_sample_layers_to_device: the overlap check of the sets' ranges
+    std::vector<ByteRange> range_scratch;     // the overlap checks of the batched calls (find_overlap)
     int sched_levels = 0, sched_visits = 0, sched_max = 0;
-    bool out_cloud_ready = false;
     // f1: device copy of a PointCloud2 payload, one buffer per stream group (the copy and the unpack kernel of a slot
     // run on the slot's stream; stream order then keeps two slots of one group from overwriting each other's payload)
     unsigned char* d_raw[kStreams] = {};
@@ -533,9 +550,9 @@ struct Staging {
         dunpack = h->d_unpack + at;
         hquery = h->h_query + at;
         dquery = h->d_query + at;
-        hpinfo = h->h_pinfo ? h->h_pinfo + at : nullptr;   // allocated on the first gg_point_info_to_device
+        hpinfo = h->h_pinfo ? h->h_pinfo + at : nullptr;   // allocated on first use (ensure_tables)
         dpinfo = h->d_pinfo ? h->d_pinfo + at : nullptr;
-        hbits = h->h_pose_bits ? h->h_pose_bits + at : nullptr;   // allocated on the first gg_update_poses_from_device
+        hbits = h->h_pose_bits ? h->h_pose_bits + at : nullptr;
         dbits = h->d_pose_bits ? h->d_pose_bits + at : nullptr;
         return GG_OK;
     }
@@ -559,6 +576,14 @@ struct Staging {
         hbits = reinterpret_cast<int*>(host + b.bits) + at;
         dbits = reinterpret_cast<int*>(dev + b.bits) + at;
         return GG_OK;
+    }
+    // The next record (hp[m]), zeroed, for `slot` at position `pos` in the call.
+    gg::SlotParams& record(int slot, int pos) {
+        gg::SlotParams& p = hp[m];
+        std::memset(&p, 0, sizeof(p));
+        p.slot = slot;
+        p.pos = pos;
+        return p;
     }
     int commit(cudaStream_t st) const {
         GG_CUDA(cudaMemcpyAsync(dp, hp, (size_t)m * sizeof(gg::SlotParams), cudaMemcpyHostToDevice, st));
@@ -739,9 +764,9 @@ int build_variant(gg_handle h, int id, cudaStream_t st) {
     return GG_OK;
 }
 
+// The record of scan d; p is zeroed and names d.slot (Staging::record).
 void fill_params(gg_handle h, const gg_scan_desc& d, gg::SlotParams& p, const gg_point* src, const float* packed = nullptr) {
     const SlotState& s = h->slots[d.slot];
-    std::memset(&p, 0, sizeof(p));
     const int var = h->variants.variant_of(d.slot);
     p.cfg = h->variants.constants(var);   // a device-configured slot's constants are patched on the device (POSE_CONFIG)
     p.detect_tab = s.device_config ? h->config_tab[d.slot] : h->variant_tab[var];
@@ -752,7 +777,6 @@ void fill_params(gg_handle h, const gg_scan_desc& d, gg::SlotParams& p, const gg
     p.oz = d.origin[2];
     p.base_z_f = (float)d.base_z;  // ggl(c, c) = ps.point.z (double -> float), GroundSegmentation.cpp:411
     p.n_points = (int)d.n_points;
-    p.slot = d.slot;
     p.src = src ? src : h->view.points + (size_t)d.slot * h->pcap;
     p.packed = packed;
 }
@@ -805,9 +829,7 @@ int launch_part_rounds(gg_handle h, const Staging& e, const CallerOutputs& c, cu
         if (h->rec) h->rec->blk[g].part[p] = h->rec->blk[g].next - h->rec->blk[g].per_call;
         for (q.m = 0; q.m < e.m; ++q.m) {
             const int k = e.hp[q.m].pos;
-            gg::SlotParams& sp = q.hp[q.m];
-            std::memset(&sp, 0, sizeof(sp));
-            sp.slot = e.hp[q.m].slot;
+            gg::SlotParams& sp = q.record(e.hp[q.m].slot, k);
             if (p >= c.n_parts[k]) {
                 std::memset(&q.hunpack[q.m], 0, sizeof(gg::UnpackDesc));
                 continue;
@@ -852,7 +874,7 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
     auto fill = [&](int i, Staging& e) {
         const gg_scan_desc& d = scans[i];
         const float* packed = packed_ptrs ? packed_ptrs[i] : nullptr;
-        fill_params(h, d, e.hp[e.m], dev_points ? dev_points[i] : nullptr, packed);
+        fill_params(h, d, e.record(d.slot, i), dev_points ? dev_points[i] : nullptr, packed);
         e.position = true;
         e.config = true;
         if (caller) {
@@ -873,7 +895,6 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
                 fill_unpack(e.hunpack[e.m], msg.data, msg.point_step, msg.field_offsets, msg.T_map_from_frame);
                 e.unpack = true;
             }
-            if (caller->parts) e.hp[e.m].pos = i;
         }
         SlotState& s = h->slots[d.slot];
         s.n_points = d.n_points;
@@ -929,11 +950,40 @@ bool encode_layer_map(gg_handle h) {
     return r == CUDA_SUCCESS;
 }
 
-int ensure_out_cloud(gg_handle h) {
-    if (h->out_cloud_ready) return GG_OK;
-    int rc = dev_alloc(h, &h->view.out_cloud, (size_t)h->n_slots * h->pcap);
-    if (rc) return rc;
-    h->out_cloud_ready = true;
+// The buffers a handle allocates the first time a call needs them, so a handle that never makes the call has none.  Step
+// plans allocate the union of what their calls need before recording (prepare_recording), since a recording may not
+// allocate.
+enum Tables : unsigned {
+    T_POSES = 1u << 0,          // PoseTables: device positions and scan poses
+    T_STORED_COUNTS = 1u << 1,  // CountTables::stored
+    T_LAST_COUNTS = 1u << 2,    // CountTables::last
+    T_PART_COUNTS = 1u << 3,    // CountTables::parts
+    T_POSE_BITS = 1u << 4,      // staging of the records' PoseBits, device and pinned
+    T_OUT_CLOUD = 1u << 5,      // the output cloud of gg_get_output
+    T_IMAGE_RANGES = 1u << 6,   // per-block range scratch of the layer images (launch_layer_images)
+    T_POINT_INFO = 1u << 7,     // staging of the PointInfoDest records, device and pinned
+    T_CONFIGS = 1u << 8,        // ConfigTables (the private detect tables: ensure_config_tables)
+};
+
+// Makes the handle's device current and allocates the buffers of `need` that are missing.
+int ensure_tables(gg_handle h, unsigned need) {
+    GG_CUDA(cudaSetDevice(h->device));
+    const size_t S = (size_t)h->n_slots, R = (size_t)kRing * S;
+    auto dev = [&](auto** p, size_t n) { return *p ? GG_OK : dev_alloc(h, p, n); };
+    int rc;
+    if ((need & T_POSES) && ((rc = dev(&h->poses.position, S)) || (rc = dev(&h->poses.scan_pose, S)))) return rc;
+    if ((need & T_STORED_COUNTS) && (rc = dev(&h->counts.stored, S))) return rc;
+    if ((need & T_LAST_COUNTS) && (rc = dev(&h->counts.last, S))) return rc;
+    if ((need & T_PART_COUNTS) && (rc = dev(&h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
+    if ((need & T_POSE_BITS) && (rc = dev(&h->d_pose_bits, R))) return rc;
+    if ((need & T_POSE_BITS) && !h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * R, cudaHostAllocDefault));
+    if ((need & T_OUT_CLOUD) && (rc = dev(&h->view.out_cloud, S * h->pcap))) return rc;
+    if ((need & T_IMAGE_RANGES) && (rc = dev(&h->d_img_part, S * gg::L_NUM * ((h->view.k.N2 + gg::IMG_RANGE_CELLS - 1) / gg::IMG_RANGE_CELLS))))
+        return rc;
+    if ((need & T_POINT_INFO) && (rc = dev(&h->d_pinfo, R))) return rc;
+    if ((need & T_POINT_INFO) && !h->h_pinfo)
+        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * R, cudaHostAllocDefault));
+    if ((need & T_CONFIGS) && ((rc = dev(&h->configs.raw, S)) || (rc = dev(&h->configs.cfg, S)))) return rc;
     return GG_OK;
 }
 
@@ -943,11 +993,9 @@ int run_output_on(gg_handle h, int slot, bool want_cloud) {
     if (want_cloud && s.packed_input)
         return fail(GG_E_STATE, "slot %d: the output cloud needs the 32-byte records on the device (use gg_filter_cloud or GG_HOST_PACK=0)", slot);
     int rc;
-    if (want_cloud && (rc = ensure_out_cloud(h))) return rc;
+    if (want_cloud && (rc = ensure_tables(h, T_OUT_CLOUD))) return rc;
     auto fill = [&](int, Staging& e) {
-        gg::SlotParams& p = e.hp[0];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slot;
+        gg::SlotParams& p = e.record(slot, 0);
         p.n_points = (int)s.n_points;
         p.src = s.src ? s.src : h->view.points + (size_t)slot * h->pcap;
         gg::OutDest& od = e.hdest[0];
@@ -978,11 +1026,7 @@ template <typename Launch>
 int enqueue_slot_batch(gg_handle h, int count, const int* slots, void* stream, Launch&& launch) {
     GG_CUDA(cudaSetDevice(h->device));
     auto fill = [&](int i, Staging& e) {
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
-        p.points_layer = points_layer(h, slots[i]);
+        e.record(slots[i], i).points_layer = points_layer(h, slots[i]);
         return true;
     };
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
@@ -1001,7 +1045,7 @@ int run_phase(gg_handle h, int slot, double base_z, Launch&& launch) {
         d.slot = slot;
         d.n_points = h->slots[slot].n_points;
         d.base_z = base_z;
-        fill_params(h, d, e.hp[0], h->slots[slot].src);
+        fill_params(h, d, e.record(slot, 0), h->slots[slot].src);
         e.position = true;
         e.config = true;
         return true;
@@ -1084,13 +1128,9 @@ int slot_constants(gg_handle h, int slot, gg::CfgConst* kc) {
 // The configuration tables, the staging of the per-record bits and the private detect table of each of `slots`, on
 // first use (a handle that never asks has none).  Step plans call it before recording, which may not allocate.
 int ensure_config_tables(gg_handle h, int count, const int* slots) {
-    const size_t S = (size_t)h->n_slots;
     int rc;
-    if (!h->configs.raw && (rc = dev_alloc(h, &h->configs.raw, S))) return rc;
-    if (!h->configs.cfg && (rc = dev_alloc(h, &h->configs.cfg, S))) return rc;
-    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
-    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
-    if (h->config_tab.empty()) h->config_tab.assign(S, nullptr);
+    if ((rc = ensure_tables(h, T_CONFIGS | T_POSE_BITS))) return rc;
+    if (h->config_tab.empty()) h->config_tab.assign((size_t)h->n_slots, nullptr);
     for (int i = 0; i < count; ++i)
         if (!h->config_tab[slots[i]] && (rc = dev_alloc(h, &h->config_tab[slots[i]], (size_t)h->view.k.N2))) return rc;
     return GG_OK;
@@ -1462,8 +1502,7 @@ int gg_update_pose_batch(gg_handle h, int count, const int* slots, const double*
     GG_CUDA(cudaSetDevice(h->device));
     auto fill = [&](int i, Staging& e) {
         SlotState& s = h->slots[slots[i]];
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
+        gg::SlotParams& p = e.record(slots[i], i);
         gg::move_map(h->view.k.res, s.px, s.py, xy[2 * i], xy[2 * i + 1], p.shift_i, p.shift_j);
         p.px = s.px;
         p.py = s.py;
@@ -1472,7 +1511,6 @@ int gg_update_pose_batch(gg_handle h, int count, const int* slots, const double*
         p.t21 = t[9];
         p.t22 = t[10];
         p.t23 = t[11];
-        p.slot = slots[i];
         const bool mv = p.shift_i != 0 || p.shift_j != 0;   // else: "We havent moved so we have nothing to do", GroundGrid.cpp:136-137
         if (moved) moved[i] = mv ? 1 : 0;
         if (mv) s.moved_since_scan = true;
@@ -1544,6 +1582,13 @@ namespace {
 bool ranges_overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
     const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
     return a && b && a_bytes && b_bytes && x < y + b_bytes && y < x + a_bytes;
+}
+
+// Whether a caller's device range overlaps the handle's layer arena (the kernels of the batched calls read and write the
+// layers concurrently with the caller's buffers).
+bool overlaps_layers(gg_handle h, const void* p, size_t bytes) {
+    const gg::View& v = h->view;
+    return ranges_overlap(p, bytes, v.layers, (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float));
 }
 
 // The output rules of gg_run_scans_to_device and gg_run_cloud_msgs_to_device: for the call, known select bits and an
@@ -1618,9 +1663,7 @@ int upload_parts(gg_handle h, int slot, int n_parts, const gg_cloud_part* parts)
         const size_t part_bytes = part.n_points * (size_t)part.msg.point_step;
         if (part_bytes) GG_CUDA(cudaMemcpyAsync(h->d_raw[sg] + at, part.msg.data, part_bytes, cudaMemcpyHostToDevice, st));
         auto fill = [&](int, Staging& e) {
-            std::memset(&e.hp[0], 0, sizeof(gg::SlotParams));
-            e.hp[0].slot = slot;
-            e.hp[0].n_points = (int)part.n_points;
+            e.record(slot, 0).n_points = (int)part.n_points;
             fill_unpack(e.hunpack[0], h->d_raw[sg] + at, part.msg.point_step, part.msg.field_offsets, part.msg.T_map_from_frame);
             e.hunpack[0].first = (int)n_points;
             e.unpack = true;
@@ -1723,43 +1766,49 @@ int gg_run_merged_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_des
 }
 
 namespace {
-// A caller-owned device buffer of a batched slot call.
+// A caller-owned argument of a batched slot call: a device buffer of `bytes` bytes, or (bytes 0) a host descriptor that
+// is only checked for null.
 struct CallerBuf {
+    // Two buffers are compared only when at least one of them is an OUTPUT.  An INPUT_ANYWHERE is an input that is not
+    // checked against the layer arena either (the poses of gg_update_poses_from_device).
+    enum Role { OUTPUT, INPUT, INPUT_ANYWHERE };
     const void* p;
     size_t bytes;
     size_t align;
     bool required;     // false: may be null
     const char* what;
+    Role role = OUTPUT;
 };
 
-// The validation shared by the batched calls on a set of slots and layer names (gg_get_layers_to_device,
-// gg_set_layers_from_device, gg_layer_images_to_device, gg_terrain_images_to_device), in this order: the handle, the
-// counts (count == 0 or n_names == 0 is a valid call with nothing to do: GG_OK, and the caller enqueues nothing), null
-// arguments, at most L_NUM names, each buffer (aligned, outside the layer arena, disjoint from the other buffers),
-// the slot checks of check_slots, `n_names` distinct names resolved as gg_get_layer
-// resolves them ("points" per slot, as LAYER_POINTS at *points_at; "expectedPoints" is not a layer of a slot).
-// A call without layer names (gg_eval_counts_to_device) passes list == nullptr: n_names and names are then ignored.
+// The validation shared by the batched calls on a set of slots (and layer names), in this order: the handle, the counts
+// (count == 0 or n_names == 0 is a valid call with nothing to do: GG_OK, and the caller enqueues nothing), null
+// arguments, at most L_NUM names, each buffer (aligned, outside the layer arena unless INPUT_ANYWHERE), the overlaps
+// between buffers (find_overlap), the slot checks of check_slots (with need_map), `n_names` distinct names resolved as
+// gg_get_layer resolves them ("points" per slot, as LAYER_POINTS at *points_at; "expectedPoints" is not a layer of a
+// slot).  A call without layer names passes list == nullptr: n_names and names are then ignored.
 int check_slot_batch(gg_handle h, int count, const int* slots, int n_names, const char* const* names, std::initializer_list<CallerBuf> bufs,
-                     gg::LayerList* list, int* points_at) {
+                     gg::LayerList* list, int* points_at, bool need_map = true) {
     const bool named = list != nullptr;
     if (!h) return fail(GG_E_ARG, "null handle");
     if (count < 0 || (named && n_names < 0)) return fail(GG_E_ARG, "negative count");
     if (count == 0 || (named && n_names == 0)) return GG_OK;
     if (!slots || (named && !names)) return fail(GG_E_ARG, "null argument");
     for (const CallerBuf& b : bufs)
-        if (b.required && !b.p) return fail(GG_E_ARG, "null argument");
+        if (b.required && !b.p) return fail(GG_E_ARG, "null %s", b.what);
     if (named && n_names > gg::L_NUM) return fail(GG_E_ARG, "%d layer names, at most %d", n_names, (int)gg::L_NUM);
-    const gg::View& v = h->view;
-    const size_t arena = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    std::vector<ByteRange>& ranges = h->range_scratch;
+    ranges.clear();
     for (const CallerBuf& b : bufs) {
         if (!b.p) continue;
         if (reinterpret_cast<uintptr_t>(b.p) % b.align) return fail(GG_E_ARG, "%s is not %zu-byte aligned", b.what, b.align);
-        if (ranges_overlap(b.p, b.bytes, v.layers, arena)) return fail(GG_E_ARG, "%s overlaps the handle's layers", b.what);
-        for (const CallerBuf& o : bufs)
-            if (&o < &b && o.p && ranges_overlap(b.p, b.bytes, o.p, o.bytes)) return fail(GG_E_ARG, "%s overlaps %s", b.what, o.what);
+        if (b.role != CallerBuf::INPUT_ANYWHERE && overlaps_layers(h, b.p, b.bytes)) return fail(GG_E_ARG, "%s overlaps the handle's layers", b.what);
+        const uintptr_t at = reinterpret_cast<uintptr_t>(b.p);
+        if (b.bytes) ranges.push_back({at, at + b.bytes, (int)(&b - bufs.begin()), b.role == CallerBuf::OUTPUT});
     }
+    const auto bad = find_overlap(ranges);
+    if (bad.first) return fail(GG_E_ARG, "%s overlaps %s", bufs.begin()[bad.second->set].what, bufs.begin()[bad.first->set].what);
     int rc;
-    if ((rc = check_slots(h, count, slots))) return rc;
+    if ((rc = check_slots(h, count, slots, nullptr, need_map))) return rc;
     if (!named) return GG_OK;
     list->n = n_names;
     for (int l = 0; l < n_names; ++l) {
@@ -1776,14 +1825,6 @@ int check_slot_batch(gg_handle h, int count, const int* slots, int n_names, cons
         }
     }
     return GG_OK;
-}
-
-// Per-block range scratch of the layer images (launch_layer_images), allocated on first use.
-int ensure_image_partials(gg_handle h) {
-    if (h->d_img_part) return GG_OK;
-    GG_CUDA(cudaSetDevice(h->device));
-    const size_t n = (size_t)h->n_slots * gg::L_NUM * ((h->view.k.N2 + gg::IMG_RANGE_CELLS - 1) / gg::IMG_RANGE_CELLS);
-    return dev_alloc(h, &h->d_img_part, n);
 }
 
 int layer_images(gg_handle h, int count, const int* slots, const gg::LayerList& list, uint8_t* dst, float* dev_range, void* stream) {
@@ -1812,10 +1853,7 @@ int eval_counts(gg_handle h, int count, const int* slots, unsigned long long* ds
     for (int i = 0; i < count; ++i) max_points = std::max(max_points, (int)h->slots[slots[i]].n_points);
     auto fill = [&](int i, Staging& e) {
         const SlotState& s = h->slots[slots[i]];
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
+        gg::SlotParams& p = e.record(slots[i], i);
         p.n_points = (int)s.n_points;
         p.src = s.src ? s.src : h->view.points + (size_t)slots[i] * h->pcap;
         p.packed = s.packed_input;
@@ -1858,7 +1896,7 @@ int gg_layer_image_u8(gg_handle h, int slot, const char* name, uint8_t* dst, flo
         if ((rc = dev_alloc(h, &h->d_image_u8, n))) return rc;
         if ((rc = dev_alloc(h, &h->d_minmax, 2))) return rc;
     }
-    if ((rc = ensure_image_partials(h))) return rc;
+    if ((rc = ensure_tables(h, T_IMAGE_RANGES))) return rc;
     cudaStream_t st = stream_of(h, slot);
     if ((rc = layer_images(h, 1, &slot, list, h->d_image_u8, h->d_minmax, st))) return rc;
     float range[2];
@@ -1880,7 +1918,7 @@ int gg_layer_images_to_device(gg_handle h, int count, const int* slots, int n_na
                                &list, &points_at)) ||
         count == 0 || n_names == 0)
         return rc;
-    if ((rc = ensure_image_partials(h))) return rc;
+    if ((rc = ensure_tables(h, T_IMAGE_RANGES))) return rc;
     return layer_images(h, count, slots, list, dst, dev_range, stream);
 }
 
@@ -2581,12 +2619,10 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
                                int mode, void* stream) {
     gg::LayerList list{};
     int points_at = -1, rc;
-    if ((rc = check_slot_batch(h, count, slots, n_names, names, {}, &list, &points_at)) || count == 0 || n_names == 0) return rc;
-    if (!queries) return fail(GG_E_ARG, "null queries");
+    if ((rc = check_slot_batch(h, count, slots, n_names, names, {{queries, 0, 1, true, "queries"}}, &list, &points_at)) || count == 0 ||
+        n_names == 0)
+        return rc;
     if (mode != GG_SAMPLE_NEAREST && mode != GG_SAMPLE_LINEAR) return fail(GG_E_ARG, "unknown sample mode %d", mode);
-    const gg::View& v = h->view;
-    const void* arena = v.layers;
-    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
     std::vector<ByteRange>& ranges = h->range_scratch;
     ranges.clear();
     size_t total = 0;
@@ -2601,35 +2637,25 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
         if (reinterpret_cast<uintptr_t>(q.data) % 4 || reinterpret_cast<uintptr_t>(q.dst) % 4 || reinterpret_cast<uintptr_t>(q.cell) % 4)
             return fail(GG_E_ARG, "set %d: data, dst or cell is not 4-byte aligned", k);
         const size_t dst_bytes = (size_t)n_names * q.n * sizeof(float), cell_bytes = q.n * sizeof(int32_t);
-        if (ranges_overlap(q.dst, dst_bytes, arena, arena_bytes) || ranges_overlap(q.cell, cell_bytes, arena, arena_bytes))
-            return fail(GG_E_ARG, "set %d: an output overlaps the handle's layers", k);
+        if (overlaps_layers(h, q.dst, dst_bytes) || overlaps_layers(h, q.cell, cell_bytes)) return fail(GG_E_ARG, "set %d: an output overlaps the handle's layers", k);
         const uintptr_t data = reinterpret_cast<uintptr_t>(q.data), dst = reinterpret_cast<uintptr_t>(q.dst);
         ranges.push_back({data, data + q.n * (size_t)q.point_step, k, false});
         ranges.push_back({dst, dst + dst_bytes, k, true});
         if (q.cell) ranges.push_back({reinterpret_cast<uintptr_t>(q.cell), reinterpret_cast<uintptr_t>(q.cell) + cell_bytes, k, true});
         total += q.n;
     }
-    // Outputs must not overlap any range; inputs may share memory.  Sorted by start, a range overlaps an earlier one iff
-    // it starts below the largest end among them, so one sweep keeps the farthest-reaching range and the farthest output.
-    std::sort(ranges.begin(), ranges.end(), [](const ByteRange& a, const ByteRange& b) { return a.begin < b.begin; });
-    const ByteRange *far_any = nullptr, *far_out = nullptr;
-    for (const ByteRange& r : ranges) {
-        const ByteRange* o = r.output ? far_any : far_out;
-        if (o && o->end > r.begin)
-            return fail(GG_E_ARG, "set %d: %s overlaps %s of set %d", r.set, r.output ? "an output" : "the positions",
-                        o->output ? "an output" : "the positions", o->set);
-        if (!far_any || r.end > far_any->end) far_any = &r;
-        if (r.output && (!far_out || r.end > far_out->end)) far_out = &r;
+    const auto bad = find_overlap(ranges);
+    if (bad.first) {
+        const ByteRange &o = *bad.first, &r = *bad.second;
+        return fail(GG_E_ARG, "set %d: %s overlaps %s of set %d", r.set, r.output ? "an output" : "the positions", o.output ? "an output" : "the positions",
+                    o.set);
     }
     if (total == 0) return GG_OK;
     GG_CUDA(cudaSetDevice(h->device));
     auto fill = [&](int i, Staging& e) {
         const gg_positions& q = queries[i];
         const SlotState& s = h->slots[slots[i]];
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
+        gg::SlotParams& p = e.record(slots[i], i);
         p.points_layer = points_layer(h, slots[i]);
         p.px = s.px;
         p.py = s.py;
@@ -2654,15 +2680,8 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
 
 // Point classes and heights: one k_point_info per stream group with something to write.
 int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_point_info* outs, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0) return GG_OK;
-    if (!slots || !outs) return fail(GG_E_ARG, "null argument");
     int rc;
-    if ((rc = check_slots(h, count, slots))) return rc;
-    const gg::View& v = h->view;
-    const void* arena = v.layers;
-    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr, {{outs, 0, 1, true, "outs"}}, nullptr, nullptr)) || count == 0) return rc;
     std::vector<ByteRange>& ranges = h->range_scratch;
     ranges.clear();
     for (int k = 0; k < count; ++k) {
@@ -2678,32 +2697,19 @@ int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_p
         const size_t bytes = s.scan_points * sizeof(uint32_t);
         for (const void* p : {static_cast<const void*>(o.codes), static_cast<const void*>(o.height)}) {
             if (!p || !bytes) continue;
-            if (ranges_overlap(p, bytes, arena, arena_bytes)) return fail(GG_E_ARG, "slot %d: an output overlaps the handle's layers", slot);
+            if (overlaps_layers(h, p, bytes)) return fail(GG_E_ARG, "slot %d: an output overlaps the handle's layers", slot);
             ranges.push_back({reinterpret_cast<uintptr_t>(p), reinterpret_cast<uintptr_t>(p) + bytes, k, true});
         }
     }
-    // every range is an output: sorted by start, a range overlaps an earlier one iff it starts below their largest end
-    std::sort(ranges.begin(), ranges.end(), [](const ByteRange& a, const ByteRange& b) { return a.begin < b.begin; });
-    const ByteRange* far = nullptr;
-    for (const ByteRange& r : ranges) {
-        if (far && far->end > r.begin) return fail(GG_E_ARG, "an output of slot %d overlaps an output of slot %d", slots[r.set], slots[far->set]);
-        if (!far || r.end > far->end) far = &r;
-    }
+    const auto bad = find_overlap(ranges);
+    if (bad.first) return fail(GG_E_ARG, "an output of slot %d overlaps an output of slot %d", slots[bad.second->set], slots[bad.first->set]);
     if (ranges.empty()) return GG_OK;
-    GG_CUDA(cudaSetDevice(h->device));
-    // the staging of the destinations, parallel to the ring, on first use (a handle that never asks has none)
-    if (!h->d_pinfo && (rc = dev_alloc(h, &h->d_pinfo, (size_t)kRing * h->n_slots))) return rc;
-    if (!h->h_pinfo)
-        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * kRing * h->n_slots, cudaHostAllocDefault));
+    if ((rc = ensure_tables(h, T_POINT_INFO))) return rc;
     auto fill = [&](int i, Staging& e) {
         const SlotState& s = h->slots[slots[i]];
         const gg_point_info& o = outs[i];
         const bool write = s.scan_points > 0 && (o.codes || o.height);
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
-        p.n_points = write ? (int)s.scan_points : 0;
+        e.record(slots[i], i).n_points = write ? (int)s.scan_points : 0;
         gg::PointInfoDest& d = e.hpinfo[e.m];
         d.codes = o.codes;
         d.height = o.height;
@@ -2718,41 +2724,28 @@ int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_p
 // Poses from device memory: per stream group one k_pose_resolve over the group's slots, then (with xy) the roll kernels
 // on the same staging entry.
 int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const gg_device_poses* poses, int32_t* dev_moved, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0) return GG_OK;
-    if (!slots || !poses) return fail(GG_E_ARG, "null argument");
+    const gg_device_poses in = poses ? *poses : gg_device_poses{};
+    const size_t n = (size_t)count;
     int rc;
-    if ((rc = check_slots(h, count, slots))) return rc;
-    const gg_device_poses& in = *poses;
+    // the poses are not checked against the layers
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr,
+                               {{poses, 0, 1, true, "poses"},
+                                {dev_moved, n * sizeof(int32_t), alignof(int32_t), false, "dev_moved", CallerBuf::OUTPUT},
+                                {in.xy, n * 2 * sizeof(double), alignof(double), false, "xy", CallerBuf::INPUT_ANYWHERE},
+                                {in.T_base_from_map, n * 12 * sizeof(double), alignof(double), false, "T_base_from_map", CallerBuf::INPUT_ANYWHERE},
+                                {in.origin, n * 3 * sizeof(float), alignof(float), false, "origin", CallerBuf::INPUT_ANYWHERE},
+                                {in.base_z, n * sizeof(double), alignof(double), false, "base_z", CallerBuf::INPUT_ANYWHERE}},
+                               nullptr, nullptr)) ||
+        count == 0)
+        return rc;
     if (!in.xy != !in.T_base_from_map) return fail(GG_E_ARG, "xy and T_base_from_map must both be given or both be NULL");
     if (!in.origin != !in.base_z) return fail(GG_E_ARG, "origin and base_z must both be given or both be NULL");
-    auto misaligned = [](const void* p, size_t a) { return reinterpret_cast<uintptr_t>(p) % a != 0; };
-    if (misaligned(in.xy, 8) || misaligned(in.T_base_from_map, 8) || misaligned(in.base_z, 8))
-        return fail(GG_E_ARG, "xy, T_base_from_map or base_z is not 8-byte aligned");
-    if (misaligned(in.origin, 4) || misaligned(dev_moved, 4)) return fail(GG_E_ARG, "origin or dev_moved is not 4-byte aligned");
-    const size_t n = (size_t)count, moved_bytes = n * sizeof(int32_t);
-    const gg::View& v = h->view;
-    if (ranges_overlap(dev_moved, moved_bytes, v.layers, (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float)))
-        return fail(GG_E_ARG, "dev_moved overlaps the handle's layers");
-    if (ranges_overlap(dev_moved, moved_bytes, in.xy, n * 2 * sizeof(double)) || ranges_overlap(dev_moved, moved_bytes, in.T_base_from_map, n * 12 * sizeof(double)) ||
-        ranges_overlap(dev_moved, moved_bytes, in.origin, n * 3 * sizeof(float)) || ranges_overlap(dev_moved, moved_bytes, in.base_z, n * sizeof(double)))
-        return fail(GG_E_ARG, "dev_moved overlaps the poses");
     if (!in.xy && !in.origin) return GG_OK;
-    GG_CUDA(cudaSetDevice(h->device));
-    // the device tables and the staging of the pose bits, on first use (a handle that never asks has none)
-    const size_t S = (size_t)h->n_slots;
-    if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
-    if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
-    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
-    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    if ((rc = ensure_tables(h, T_POSES | T_POSE_BITS))) return rc;
     const gg::DevicePoses dp{in.xy, in.T_base_from_map, in.origin, in.base_z, dev_moved};
     auto fill = [&](int i, Staging& e) {
         SlotState& s = h->slots[slots[i]];
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
+        gg::SlotParams& p = e.record(slots[i], i);
         p.px = s.px;   // the position k_pose_resolve starts from, unless the device table holds it
         p.py = s.py;
         e.hbits[e.m] = s.device_position ? gg::POSE_POSITION : 0;
@@ -2771,28 +2764,15 @@ int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const 
 
 // Point counts from device memory: per stream group one k_store_counts over the group's slots.
 int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_n_points, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0) return GG_OK;
-    if (!slots || !dev_n_points) return fail(GG_E_ARG, "null argument");
-    if (reinterpret_cast<uintptr_t>(dev_n_points) % alignof(int32_t)) return fail(GG_E_ARG, "dev_n_points is not 4-byte aligned");
-    const gg::View& v = h->view;
-    if (ranges_overlap(dev_n_points, (size_t)count * sizeof(int32_t), v.layers, (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float)))
-        return fail(GG_E_ARG, "dev_n_points overlaps the handle's layers");
     int rc;
-    if ((rc = check_slots(h, count, slots))) return rc;
-    GG_CUDA(cudaSetDevice(h->device));
-    // the device tables and the staging of the per-record bits, on first use (a handle that never asks has none)
-    const size_t S = (size_t)h->n_slots;
-    if (!h->counts.stored && (rc = dev_alloc(h, &h->counts.stored, S))) return rc;
-    if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
-    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
-    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr,
+                               {{dev_n_points, (size_t)count * sizeof(int32_t), alignof(int32_t), true, "dev_n_points", CallerBuf::INPUT}}, nullptr,
+                               nullptr)) ||
+        count == 0)
+        return rc;
+    if ((rc = ensure_tables(h, T_STORED_COUNTS | T_LAST_COUNTS | T_POSE_BITS))) return rc;
     auto fill = [&](int i, Staging& e) {
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
+        e.record(slots[i], i);
         h->slots[slots[i]].stored_count = true;
         return true;
     };
@@ -2802,31 +2782,18 @@ int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, co
 
 // Part counts from device memory: per stream group one k_store_part_counts over the group's slots.
 int gg_set_part_counts_from_device(gg_handle h, int count, const int* slots, int parts_per_slot, const int32_t* dev_part_counts, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0) return GG_OK;
-    if (!slots || !dev_part_counts) return fail(GG_E_ARG, "null argument");
-    if (parts_per_slot < 1 || parts_per_slot > GG_MAX_CLOUD_PARTS)
+    // before the buffer's size is taken from it (a call with count == 0 is accepted whatever it says)
+    if (count > 0 && (parts_per_slot < 1 || parts_per_slot > GG_MAX_CLOUD_PARTS))
         return fail(GG_E_ARG, "parts_per_slot %d not in [1, %d]", parts_per_slot, GG_MAX_CLOUD_PARTS);
-    if (reinterpret_cast<uintptr_t>(dev_part_counts) % alignof(int32_t)) return fail(GG_E_ARG, "dev_part_counts is not 4-byte aligned");
-    const gg::View& v = h->view;
-    if (ranges_overlap(dev_part_counts, (size_t)count * parts_per_slot * sizeof(int32_t), v.layers,
-                       (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float)))
-        return fail(GG_E_ARG, "dev_part_counts overlaps the handle's layers");
+    const size_t bytes = (size_t)count * parts_per_slot * sizeof(int32_t);
     int rc;
-    if ((rc = check_slots(h, count, slots))) return rc;
-    GG_CUDA(cudaSetDevice(h->device));
-    // the device tables and the staging of the per-record bits, on first use (a handle that never asks has none)
-    const size_t S = (size_t)h->n_slots;
-    if (!h->counts.parts && (rc = dev_alloc(h, &h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
-    if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
-    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
-    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr, {{dev_part_counts, bytes, alignof(int32_t), true, "dev_part_counts", CallerBuf::INPUT}},
+                               nullptr, nullptr)) ||
+        count == 0)
+        return rc;
+    if ((rc = ensure_tables(h, T_LAST_COUNTS | T_PART_COUNTS | T_POSE_BITS))) return rc;
     auto fill = [&](int i, Staging& e) {
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
+        e.record(slots[i], i);
         h->slots[slots[i]].stored_parts = parts_per_slot;
         return true;
     };
@@ -2841,34 +2808,21 @@ int gg_set_part_counts_from_device(gg_handle h, int count, const int* slots, int
 // positions of masked-off slots), the stored scan pose and count kept, the last scan's outputs still readable, and its
 // point info refused until the next scan, as after a device roll.
 int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_device_resets* resets, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0) return GG_OK;
-    if (!slots || !resets || !resets->xyz) return fail(GG_E_ARG, "null argument");
-    const gg_device_resets& in = *resets;
-    if (reinterpret_cast<uintptr_t>(in.xyz) % alignof(double)) return fail(GG_E_ARG, "xyz is not 8-byte aligned");
-    if (reinterpret_cast<uintptr_t>(in.mask) % alignof(int32_t)) return fail(GG_E_ARG, "mask is not 4-byte aligned");
-    const gg::View& v = h->view;
-    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
-    if (ranges_overlap(in.xyz, (size_t)count * 3 * sizeof(double), v.layers, arena_bytes) ||
-        ranges_overlap(in.mask, (size_t)count * sizeof(int32_t), v.layers, arena_bytes))
-        return fail(GG_E_ARG, "xyz or mask overlaps the handle's layers");
+    const gg_device_resets in = resets ? *resets : gg_device_resets{};
+    const size_t n = (size_t)count;
     int rc;
     // without a mask every slot gets a map, so a slot needs none beforehand
-    if ((rc = check_slots(h, count, slots, nullptr, in.mask != nullptr))) return rc;
-    GG_CUDA(cudaSetDevice(h->device));
-    // the device tables and the staging of the pose bits, on first use (a handle that never asks has none)
-    const size_t S = (size_t)h->n_slots;
-    if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
-    if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
-    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
-    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr,
+                               {{resets, 0, 1, true, "resets"},
+                                {in.xyz, n * 3 * sizeof(double), alignof(double), true, "xyz", CallerBuf::INPUT},
+                                {in.mask, n * sizeof(int32_t), alignof(int32_t), false, "mask", CallerBuf::INPUT}},
+                               nullptr, nullptr, in.mask != nullptr)) ||
+        count == 0)
+        return rc;
+    if ((rc = ensure_tables(h, T_POSES | T_POSE_BITS))) return rc;
     auto fill = [&](int i, Staging& e) {
         SlotState& s = h->slots[slots[i]];
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
+        gg::SlotParams& p = e.record(slots[i], i);
         p.px = s.px;   // what a masked-off record seeds into the table, unless the table already holds the position
         p.py = s.py;
         e.hbits[e.m] = s.device_position ? gg::POSE_POSITION : 0;
@@ -2886,34 +2840,25 @@ int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_
 // Configurations from device memory: per stream group one k_store_configs and one k_rebuild_detect_tables over the group's
 // slots.  The host cannot see the mask, so every slot of the call leaves it device-configured.
 int gg_set_slot_configs_from_device(gg_handle h, int count, const int* slots, const gg_device_configs* configs, void* stream) {
-    if (!h) return fail(GG_E_ARG, "null handle");
-    if (count < 0) return fail(GG_E_ARG, "negative count");
-    if (count == 0) return GG_OK;
-    if (!slots || !configs || !configs->cfg) return fail(GG_E_ARG, "null argument");
-    const gg_device_configs& in = *configs;
-    if (reinterpret_cast<uintptr_t>(in.cfg) % alignof(double)) return fail(GG_E_ARG, "cfg is not 8-byte aligned");
-    if (reinterpret_cast<uintptr_t>(in.mask) % alignof(int32_t)) return fail(GG_E_ARG, "mask is not 4-byte aligned");
-    const gg::View& v = h->view;
-    const size_t arena_bytes = (size_t)h->n_slots * v.n_layers * v.k.N2 * sizeof(float);
-    if (ranges_overlap(in.cfg, (size_t)count * sizeof(gg_config), v.layers, arena_bytes) ||
-        ranges_overlap(in.mask, (size_t)count * sizeof(int32_t), v.layers, arena_bytes))
-        return fail(GG_E_ARG, "cfg or mask overlaps the handle's layers");
+    const gg_device_configs in = configs ? *configs : gg_device_configs{};
+    const size_t n = (size_t)count;
     int rc;
-    if ((rc = check_slots(h, count, slots, nullptr, false))) return rc;
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr,
+                               {{configs, 0, 1, true, "configs"},
+                                {in.cfg, n * sizeof(gg_config), alignof(double), true, "cfg", CallerBuf::INPUT},
+                                {in.mask, n * sizeof(int32_t), alignof(int32_t), false, "mask", CallerBuf::INPUT}},
+                               nullptr, nullptr, false)) ||
+        count == 0)
+        return rc;
     // a plan's records of a host-configured slot carry its configuration by value
     for (int i = 0; i < count; ++i)
         if (h->slot_plan[slots[i]] && !h->slots[slots[i]].device_config)
             return fail(GG_E_STATE, "slot %d is bound to a step plan recorded while it was host-configured", slots[i]);
-    GG_CUDA(cudaSetDevice(h->device));
     if ((rc = ensure_config_tables(h, count, slots))) return rc;
     for (int i = 0; i < count; ++i)
         if (!h->slots[slots[i]].device_config && (rc = seed_device_config(h, slots[i]))) return rc;
     auto fill = [&](int i, Staging& e) {
-        gg::SlotParams& p = e.hp[e.m];
-        std::memset(&p, 0, sizeof(p));
-        p.slot = slots[i];
-        p.pos = i;
-        p.detect_tab = h->config_tab[slots[i]];
+        e.record(slots[i], i).detect_tab = h->config_tab[slots[i]];
         h->slots[slots[i]].device_config = true;
         return true;
     };
@@ -2978,17 +2923,16 @@ int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_step_parts* par
     }
     const char* what = parts ? "part" : "scan";   // k below counts the parts over all scans, or the scans
     const char* name = parts ? "dev_T_map_from_part" : "dev_T_map_from_frame";
-    std::vector<uintptr_t> ts;
+    std::vector<ByteRange> ts;   // every transform counts as an output: none may overlap another
     for (size_t k = 0; k < dev_host.size(); ++k) {
         const uintptr_t t = reinterpret_cast<uintptr_t>(dev_host[k].first);
         if (!t) continue;
         if (t % alignof(double)) return fail(GG_E_ARG, "%s %zu: %s is not 8-byte aligned", what, k, name);
         if (dev_host[k].second) return fail(GG_E_ARG, "%s %zu: both a device and a host T_map_from_frame", what, k);
-        ts.push_back(t);
+        ts.push_back({t, t + 12 * sizeof(double), (int)k, true});
     }
-    std::sort(ts.begin(), ts.end());
-    for (size_t j = 1; j < ts.size(); ++j)
-        if (ts[j] < ts[j - 1] + 12 * sizeof(double)) return fail(GG_E_ARG, "two %s entries overlap", name);
+    const auto bad = find_overlap(ts);
+    if (bad.first) return fail(GG_E_ARG, "the %s entries of %s %d and %s %d overlap", name, what, bad.first->set, what, bad.second->set);
     return GG_OK;
 }
 
@@ -3066,21 +3010,14 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
 // Everything the recorded kernels address that the step's calls would allocate on first use, and the spiral's shared
 // memory opt-in: a recording may not allocate, and the View it records must not change afterwards.
 int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_configs* configs, const gg_step_readouts* readouts) {
-    const size_t S = (size_t)h->n_slots;
-    int rc;
-    if (!h->poses.position && (rc = dev_alloc(h, &h->poses.position, S))) return rc;
-    if (!h->poses.scan_pose && (rc = dev_alloc(h, &h->poses.scan_pose, S))) return rc;
-    if (!h->counts.stored && (rc = dev_alloc(h, &h->counts.stored, S))) return rc;
-    if (!h->counts.last && (rc = dev_alloc(h, &h->counts.last, S))) return rc;
-    if (!h->counts.parts && (rc = dev_alloc(h, &h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
-    if (!h->d_pose_bits && (rc = dev_alloc(h, &h->d_pose_bits, (size_t)kRing * S))) return rc;
-    if (!h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * kRing * S, cudaHostAllocDefault));
-    if ((rc = ensure_out_cloud(h))) return rc;
+    // the tables of the poses, counts and part counts whether or not the step records those calls (record_plan seeds the
+    // positions), and the output cloud
+    unsigned need = T_POSES | T_STORED_COUNTS | T_LAST_COUNTS | T_PART_COUNTS | T_POSE_BITS | T_OUT_CLOUD;
     const ReadoutCalls c(readouts);
-    if (c.images && (rc = ensure_image_partials(h))) return rc;
-    if (c.point_info && !h->d_pinfo && (rc = dev_alloc(h, &h->d_pinfo, (size_t)kRing * S))) return rc;
-    if (c.point_info && !h->h_pinfo)
-        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * kRing * S, cudaHostAllocDefault));
+    if (c.images) need |= T_IMAGE_RANGES;
+    if (c.point_info) need |= T_POINT_INFO;
+    int rc;
+    if ((rc = ensure_tables(h, need))) return rc;
     if (configs) {
         std::vector<int> slots(d.count);
         for (int i = 0; i < d.count; ++i) slots[i] = d.scans[i].slot;

@@ -406,3 +406,8 @@ def test_rejections_enqueue_nothing(monkeypatch):
     for s in range(B):
         assert np.array_equal(g.layer("groundpatch", slot=s), before[s]), f"slot {s}: layers changed"
         assert bytes(g.get_config(slot=s)) == cfgs[s], f"slot {s}: configuration changed"
+    # inputs may share memory: a mask inside cfg is accepted (its nonzero words reconfigure the slots)
+    n1 = g.kernel_launches
+    g.set_configs_from_device_ptrs([0, 1], ct.data_ptr(), ct.data_ptr() + 8, None)
+    assert g.kernel_launches > n1
+    assert bytes(g.get_config(slot=1)) == cfg_bytes(CFGS[1])

@@ -423,6 +423,11 @@ def test_rejections_enqueue_nothing_and_state_rules():
     g.run_scans(g.make_descs([0], [len(pts)], "device", None))
     g.point_info_to_device([0])
     g.synchronize()
+    # inputs may share memory: poses whose arrays overlap each other are accepted
+    before = g.kernel_launches
+    assert call(1, [2], (full[0], full[1], full[1] + 8, full[0])) == 0
+    assert g.kernel_launches > before
+    g.synchronize()
 
 
 def test_launch_counts(monkeypatch):

@@ -412,3 +412,7 @@ def test_rejections_enqueue_nothing(monkeypatch):
     assert call() == 0
     assert g.kernel_launches == before + len({s * GROUPS // B for s in (0, 3, 5)})
     g.synchronize()
+    # inputs may share memory: a mask inside xyz is accepted (its zero words reset no slot)
+    assert call(mask=rx.data_ptr() + 8) == 0
+    assert g.kernel_launches == before + 2 * len({s * GROUPS // B for s in (0, 3, 5)})
+    g.synchronize()
