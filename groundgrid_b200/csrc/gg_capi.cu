@@ -1295,6 +1295,10 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
             GG_TRY(dev_upload(h, &w.ph_end, plan.ph_end));
             GG_TRY(dev_upload(h, &w.ph_cell0, plan.ph_cell0));
             GG_TRY(dev_upload(h, &w.cell_home, sk.cell_home));
+            GG_TRY(dev_upload(h, &w.home_irr, sk.home_irr));
+            w.home_words = sk.home_words;
+            w.K = sk.K;
+            std::memcpy(w.off, sk.off, sizeof(sk.off));
             const uint32_t* d_irr = nullptr;
             GG_TRY(dev_upload(h, &d_irr, plan.irr_blocks, 16));
             float2* d_sk = nullptr;

@@ -308,6 +308,16 @@ void build_spiral_skew(int n, const std::vector<int>& level_start, const std::ve
         for (int s = 0; s < 4; ++s) add_home(c, c, slot(s, -1, -3 + off[s]));  // centre: virtual ring -1
     }
     auto homes = [&](int x, int y) { return &t.cell_home[((size_t)x + (size_t)y * n) * 4]; };
+    // the cells whose homes the closed form does not give (k_detect stores those from cell_home)
+    std::memcpy(t.off, off, sizeof(off));
+    t.home_words = (n + 31) / 32;
+    t.home_irr.assign((size_t)n * t.home_words, 0u);
+    for (int y = 0; y < n; ++y)
+        for (int x = 0; x < n; ++x) {
+            const int* h = homes(x, y);
+            if (h[0] != skew_regular_home(n, K, t.KP, t.rows, t.row0, t.off, x, y) || h[1] >= 0)
+                t.home_irr[(size_t)y * t.home_words + x / 32] |= 1u << (x % 32);
+        }
 
     // neighbour slot candidates + offset statistics -> the regular pattern of each side
     std::vector<std::vector<std::pair<int, int>>> stat(36);  // (offset, count), small
@@ -714,6 +724,38 @@ int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* 
     if (cell_home) std::memcpy(cell_home, t.cell_home.data(), t.cell_home.size() * sizeof(int));
     if (irr_level_start) std::memcpy(irr_level_start, t.irr_level_start.data(), t.irr_level_start.size() * sizeof(int));
     if (irr_recs && irr_cap_words >= (int)t.irr_recs.size()) std::memcpy(irr_recs, t.irr_recs.data(), t.irr_recs.size() * sizeof(uint32_t));
+    return 1;
+}
+
+int gg_host_skew_homes(int n, int* homes, int* n_table) {
+    std::vector<int> ls;
+    std::vector<uint32_t> vs;
+    gg::build_spiral_schedule(n, ls, vs);
+    gg::SkewTables t;
+    gg::build_spiral_skew(n, ls, vs, t);
+    if (!t.ok) return 0;
+    gg::SkewView w;
+    std::memset(&w, 0, sizeof(w));
+    w.cell_home = t.cell_home.data();
+    w.home_irr = t.home_irr.data();
+    w.home_words = t.home_words;
+    w.K = t.K;
+    w.KP = t.KP;
+    w.rows = t.rows;
+    w.row0 = t.row0;
+    std::memcpy(w.off, t.off, sizeof(t.off));
+    int table = 0;
+    for (int y = 0; y < n; ++y)
+        for (int x = 0; x < n; ++x) {
+            const int4 h = gg::skew_home(w, n, x, y);
+            int* o = homes + ((size_t)x + (size_t)y * n) * 4;
+            o[0] = h.x;
+            o[1] = h.y;
+            o[2] = h.z;
+            o[3] = h.w;
+            table += (t.home_irr[(size_t)y * t.home_words + x / 32] >> (x % 32)) & 1u;
+        }
+    *n_table = table;
     return 1;
 }
 

@@ -55,6 +55,9 @@ struct SkewTables {
     std::vector<int> lane_begin, lane_end;   // [lanes] level range [begin, end) of the lane's regular run
     std::vector<int> lane_cell0;             // [lanes] cell (x + y * n) of the first regular visit; the lane then steps by +n, +1, -n, -1 (side 0..3)
     std::vector<int> cell_home;          // [n * n * 4] slots holding a copy of the cell (-1 padded; [0] first visit, [1] second visit)
+    int off[4] = {0, 0, 0, 0};           // first level of ring k on side s: 3 k + off[s] (gg_internal.h:skew_regular_home)
+    int home_words = 0;                  // ceil(n / 32)
+    std::vector<uint32_t> home_irr;      // [n][home_words] bit per cell: its cell_home entry is not {skew_regular_home, -1, -1, -1}
     std::vector<int> irr_level_start;    // [levels + 1] CSR over levels
     std::vector<uint32_t> irr_recs;      // 16 words per irregular visit: own, nb[9], recents01, recents23, mirror, lane, cell, pad
     int max_irr_per_level = 0;
@@ -100,6 +103,9 @@ int gg_host_pack_cloud(const gg_point* src, size_t n, unsigned char* dst);
 int gg_host_packer_selftest(int threads, int n_jobs, size_t n_points, int ring_slots, int rounds, int lag);
 int gg_host_spiral_plan(int n, float resolution, int* out);
 int gg_host_spiral_skew(int n, int* header, int* pattern, int* lane_begin, int* lane_end, int* cell_home, int* irr_level_start, uint32_t* irr_recs, int irr_cap_words);
+// homes[n * n * 4]: the slots k_detect stores each cell to (gg_internal.h:skew_home), n_table: how many cells it reads
+// from the homes table; 0 when the map has no skewed layout
+int gg_host_skew_homes(int n, int* homes, int* n_table);
 int gg_host_decay_confidence(const gg_config* cfg, const float* occ, size_t n, float* out);
 int gg_host_skew_visit_confidence(const float* d, const float* occ, size_t n, float* out);
 int gg_host_outlier_walk(double dimension_m, float resolution, const double* pos_xy, const float* G, const float* C, double thr, double tol,

@@ -131,7 +131,53 @@ struct SkewView {
     int irr_max, irr_chunks;
     int KP, rows, row0, lanes, levels;
     int pattern[36];
+    // Homes of the cells (skew_home): bit x % 32 of home_irr[y * home_words + x / 32] is set for a cell whose homes in
+    // cell_home are not the single slot skew_regular_home derives (ring corners, lane ends, the centre, the border)
+    const uint32_t* home_irr;   // [N][home_words]
+    int home_words;             // ceil(N / 32)
+    int K;                      // rings 0 .. K - 1 are swept, ring K is the border they read
+    int off[4];                 // first level of ring k on side s: 3 k + off[s]
 };
+
+// The slot cell (x, y) of an n x n map would take in the skewed layout if its lane visited it once, one level per cell
+// (gg_host.cpp:build_spiral_skew): ring k = Chebyshev distance from the centre cell c minus one, side and position j along
+// the side as the sequential sweep walks them, level 3 k + off[side] + j.  -1 outside rings 0 .. K.
+__host__ __device__ __forceinline__ int skew_regular_home(int n, int K, int KP, int rows, int row0, const int* off, int x, int y) {
+    const int c = n / 2 - 1;
+    const int ax = x > c ? x - c : c - x, ay = y > c ? y - c : c - y;
+    const int k = (ax > ay ? ax : ay) - 1;
+    if (k < 0 || k > K) return -1;
+    const int p = c - 1 - k, q = c + 1 + k;
+    int s, j;
+    if (x == p && y < q) {
+        s = 0;   // (p, p + j)
+        j = y - p;
+    } else if (y == p && x < q) {
+        s = 1;   // (p + j, p)
+        j = x - p;
+    } else if (x == q) {
+        s = 2;   // (q, q - j)
+        j = q - y;
+    } else {
+        s = 3;   // (q - j, q)
+        j = q - x;
+    }
+    return (s * rows + 3 * k + off[s] + j + row0) * KP + k + 1;
+}
+
+// The homes of cell (x, y) of an n x n map: what cell_home holds for it (-1 padded), read from there only for the cells
+// home_irr marks.  k_detect stores every cell through it; gg_host_skew_homes runs it on the host.
+__host__ __device__ __forceinline__ int4 skew_home(const SkewView& w, int n, int x, int y) {
+    if ((w.home_irr[y * w.home_words + (x >> 5)] >> (x & 31)) & 1u) {
+#ifdef __CUDA_ARCH__
+        return __ldg(reinterpret_cast<const int4*>(w.cell_home) + x + y * n);
+#else
+        const int* h = w.cell_home + 4 * ((size_t)x + (size_t)y * n);
+        return make_int4(h[0], h[1], h[2], h[3]);
+#endif
+    }
+    return make_int4(skew_regular_home(n, w.K, w.KP, w.rows, w.row0, w.off, x, y), -1, -1, -1);
+}
 
 // Pointers / strides of the handle's device arena, passed to kernels by value.
 struct View {

@@ -759,11 +759,12 @@ constexpr int DT_R = DT_Y + 2 * DT_H;   // 12
 
 // the confidence decay of interpolate_cell (:464) is gg_internal.h:decay_confidence
 
-// Fused into k_detect: every cell is copied to its home slot(s) as soon as its final G, C are known.
-__device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams& sp, int cell, int x, int y, float g, float c, bool far) {
+// Fused into k_detect: every cell is copied to its home slot(s) as soon as its final G, C are known.  The slot is
+// derived from (x, y) (gg_internal.h:skew_home); the homes table is read for the few cells the closed form misses,
+// whose bits share one word per tile row of a warp.
+__device__ __forceinline__ void skew_store_homes(const View& v, const SlotParams& sp, int4 home, int x, int y, float g, float c, bool far) {
     const Const& k = v.k;
     const CfgConst& kc = sp.cfg;
-    const int4 home = __ldg(reinterpret_cast<const int4*>(v.skew.cell_home) + cell);
     if (home.x < 0) return;
     const int cidx = k.N / 2 - 1;
     if (x == cidx && y == cidx) {  // spiral_ground_interpolation :405,411 (the normal layers get it in k_spiral_skew)
@@ -783,6 +784,62 @@ __device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams&
     }
     if (home.z >= 0) SK[home.z] = gc;
     if (home.w >= 0) SK[home.w] = gc;
+}
+__device__ __forceinline__ void skew_store_cell(const View& v, const SlotParams& sp, int x, int y, float g, float c, bool far) {
+    skew_store_homes(v, sp, skew_home(v.skew, v.k.N, x, y), x, y, g, c, far);
+}
+
+// The same stores for a whole DT_X x DT_Y tile (every thread of the CTA calls it), written in an order that keeps a
+// warp's stores on few sectors.  Slot (side, level, k) and (side, level, k + 1) hold cells one step apart along
+// (x, y) +- (4, 1) on sides 1 and 3 and +- (1, 4) on sides 0 and 2.  Cells with one home pass their (G, C, decay, slot)
+// through stage[] to the thread that stores them: in the upper and lower quarters of the map a group of eight lanes takes
+// the cells (u + 4 r mod 32, r), r = 0 .. 7 -- up to eight consecutive slots --, in the left and right quarters a pair of
+// lanes takes (u, r) and (u + 1 mod 32, r + 4).  Cells with several homes (ring corners, the centre) store their own.
+__device__ __forceinline__ void skew_store_tile(const View& v, const SlotParams& sp, float4* stage, bool live, int x, int y, float g, float c,
+                                                bool far) {
+    const int N = v.k.N;
+    const int cidx = N / 2 - 1;
+    int slot = -1;
+    float d = SKEW_NEAR;
+    if (live) {
+        const int4 home = skew_home(v.skew, N, x, y);
+        if (home.x >= 0) {
+            if (x == cidx && y == cidx) {   // as skew_store_homes
+                g = sp.base_z_f;
+                c = 1.0f;
+            }
+            if (far) d = decay_confidence(sp.cfg, c);
+            slot = home.x;
+            if (home.y >= 0) {   // the other homes of a ring corner or of the centre
+                float2* SK = v.skew.sk + (size_t)sp.slot * v.skew.slots;
+                const float2 gc = make_float2(g, c);
+                SK[home.y] = gc;
+                v.skew.sd[(size_t)sp.slot * v.skew.slots + home.y] = far ? decay_confidence(sp.cfg, d) : SKEW_NEAR;
+                if (home.z >= 0) SK[home.z] = gc;
+                if (home.w >= 0) SK[home.w] = gc;
+            }
+        }
+    }
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    const int ax = abs(x - tx + DT_X / 2 - cidx), ay = abs(y - ty + DT_Y / 2 - cidx);   // from the tile's centre
+    const int lane = tx, w = ty;
+    int lx, ly;
+    if (ay > ax) {   // sides 1 and 3
+        ly = lane & 7;
+        lx = (w * 4 + (lane >> 3) + 4 * ly) & (DT_X - 1);
+    } else {         // sides 0 and 2
+        const int h = lane & 1;
+        ly = (w >> 1) + 4 * h;
+        lx = ((w & 1) * 16 + (lane >> 1) + h) & (DT_X - 1);
+    }
+    stage[ty * DT_X + tx] = make_float4(g, c, d, __int_as_float(slot));
+    __syncthreads();
+    const float4 e = stage[ly * DT_X + lx];
+    const int sl = __float_as_int(e.w);
+    if (sl >= 0) {
+        v.skew.sk[(size_t)sp.slot * v.skew.slots + sl] = make_float2(e.x, e.y);
+        v.skew.sd[(size_t)sp.slot * v.skew.slots + sl] = e.z;
+    }
 }
 
 // Per-cell quantities of detect_ground_patches that depend only on the grid and the configuration, computed
@@ -959,7 +1016,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const Slot
         }
     }
     if (v.skew.sk) {
-        skew_store_cell(v, sp, cell, i, j, g, c, (flags & DTF_FAR) != 0);
+        skew_store_cell(v, sp, i, j, g, c, (flags & DTF_FAR) != 0);
     } else if (v.spiral_recs) {
         // Decayed confidence for the spiral sweep, taken off its sequential critical path: the
         // confidence of a cell only changes at its own visit(s), so decay(C) after patch
@@ -1107,6 +1164,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
                                                              int count_layer, bool recompute) {
     __shared__ DetectTile s;
     __shared__ __align__(8) uint64_t s_bar[2];
+    __shared__ float4 s_stage[DT_X * DT_Y];   // skew_store_tile
     const SlotParams& sp = batch[blockIdx.z];
     const Const& k = v.k;
     const CfgConst& kc = sp.cfg;
@@ -1139,6 +1197,9 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
         // every thread is past the previous tile (barrier at the end of the loop body): its stage may be refilled
         if (tid == 0 && kk + 1 < n_tiles) issue(kk + 1);
         const DetectRaw& raw = s.raw[kk & 1];
+        // the tile loops' positions are recomputed per tile rather than kept in registers across it
+        int tile_tid = tid;
+        asm volatile("" : "+r"(tile_tid));
         // own cell (overlaps the tile transfer)
         const int j = (tile0 + kk) * DT_Y + ty;
         const bool live = i < N && j < N;
@@ -1154,7 +1215,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
         mbar_wait(&s_bar[kk & 1], (uint32_t)((kk >> 1) & 1));
         if (recompute) {   // :323 on the tile: V holds m2 (see k_detect_ldg); outside the map 0 / FLT_MIN = 0, as before
             DetectRaw& rw = s.raw[kk & 1];
-            for (int p = tid; p < DT_R * DT_WT; p += DT_X * DT_Y) {
+            for (int p = tile_tid; p < DT_R * DT_WT; p += DT_X * DT_Y) {
                 const int row = p / DT_WT, col = p % DT_WT;
                 rw.V[row][col] = __fdiv_rn(rw.V[row][col], __fadd_rn(rw.P[row][col], FLT_MIN));
             }
@@ -1167,7 +1228,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
         // (only columns 0 .. 35 are ever the first row of a window: col + 4 <= 39 stays inside the tile, no bounds tests;
         // together they read every entry of the tile, so they also tell whether all its counts are small integers)
         bool exact = true;
-        for (int p = tid; p < DT_R * DT_WC; p += DT_X * DT_Y) {
+        for (int p = tile_tid; p < DT_R * DT_WC; p += DT_X * DT_Y) {
             const int row = p / DT_WC, col = p % DT_WC;   // row = j index of the tile, col = i index
             float a[5];
 #pragma unroll
@@ -1205,7 +1266,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
             // stage B: products, pairs, triples and column minima
             // (products are needed up to column 37 -- the last row of the right-most window --, pairs up to 36, the rest up
             // to 35; reads of columns 40 / 41 for those two extra columns stay inside this struct and feed unused entries)
-            for (int p = tid; p < DT_R * DT_WB; p += DT_X * DT_Y) {
+            for (int p = tile_tid; p < DT_R * DT_WB; p += DT_X * DT_Y) {
                 const int row = p / DT_WB, col = p % DT_WB;
                 float qv[3], qm[3], m[5];
 #pragma unroll
@@ -1257,21 +1318,19 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
                 }
             }
         }
-        if (live) {
-            if (changed) {
-                L0[L_GROUND * N2 + cell] = g;
-                L0[L_GROUNDPATCH * N2 + cell] = c;
-            }
-            if (v.skew.sk) {
-                skew_store_cell(v, sp, cell, i, j, g, c, (flags & DTF_FAR) != 0);
-            } else if (v.spiral_recs) {
-                const float d1 = decay_confidence(kc, c);
-                float* D1 = v.roll_scratch + (size_t)sp.slot * 2 * k.N2;
-                D1[cell] = d1;
-                if (i == j) D1[k.N2 + cell] = decay_confidence(kc, d1);
-            }
+        if (live && changed) {
+            L0[L_GROUND * N2 + cell] = g;
+            L0[L_GROUNDPATCH * N2 + cell] = c;
         }
-        __syncthreads();   // the derived arrays and this stage are free again
+        if (v.skew.sk) {
+            skew_store_tile(v, sp, s_stage, live, i, j, g, c, (flags & DTF_FAR) != 0);
+        } else if (live && v.spiral_recs) {
+            const float d1 = decay_confidence(kc, c);
+            float* D1 = v.roll_scratch + (size_t)sp.slot * 2 * k.N2;
+            D1[cell] = d1;
+            if (i == j) D1[k.N2 + cell] = decay_confidence(kc, d1);
+        }
+        __syncthreads();   // the derived arrays, this stage and s_stage are free again
     }
 }
 
