@@ -300,23 +300,43 @@ struct SlotState {
     bool device_config = false;
 };
 
+// Where the record arrays of `records` staging records start in a buffer: SlotParams, OutDest, UnpackDesc, QueryDesc,
+// PointInfoDest and PoseBits (an int), one after the other, each at a 16-byte boundary.  The parameter ring and a step
+// plan's blocks are both laid out by record_layout, so record i of every array is found the same way in either.
+struct RecordLayout {
+    size_t params, dest, unpack, query, pinfo, bits;   // byte offsets of the arrays
+    size_t bytes;                                      // size of the buffer, a multiple of 16
+};
+
+RecordLayout record_layout(size_t records) {
+    auto align16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    RecordLayout l;
+    l.params = 0;
+    l.dest = align16(l.params + records * sizeof(gg::SlotParams));
+    l.unpack = align16(l.dest + records * sizeof(gg::OutDest));
+    l.query = align16(l.unpack + records * sizeof(gg::UnpackDesc));
+    l.pinfo = align16(l.query + records * sizeof(gg::QueryDesc));
+    l.bits = align16(l.pinfo + records * sizeof(gg::PointInfoDest));
+    l.bytes = align16(l.bits + records * sizeof(int));
+    return l;
+}
+
 // While gg_step_plan_create records a step, run_groups takes its staging entries from here instead of the ring: per stream
 // group with slots in the plan one block of calls * per_call[g] records (one entry per call the step records, and one per
-// part round of a merged scan), each record
-// array (SlotParams, OutDest, UnpackDesc, QueryDesc, PointInfoDest, PoseBits) contiguous in the block.  The records are
+// part round of a merged scan), laid out by record_layout.  The records are
 // filled in the host image; the plan keeps a pristine device copy of it, and each replay first restores the working block
 // of every group from it (the pose and staging kernels patch the working records in place).  Nothing is committed from
 // the host and no ring event is recorded: the launches go to the recorder's capture streams.
 struct PlanRecorder {
     struct Block {
-        size_t at = 0, bytes = 0;                    // byte range of the group's block in the image
-        size_t params = 0, dest = 0, unpack = 0, query = 0, pinfo = 0, bits = 0;   // byte offsets of its arrays in the image
+        size_t at = 0;                               // byte offset of the group's block in the image
         int per_call = 0, next = 0;                  // records per entry; records handed out
         int calls = 0;                               // entries the block holds
         int first = 0;                               // index of the group's first record over all blocks
         int scan = -1;                               // index in the block of the scan call's first record
         int part[GG_MAX_CLOUD_PARTS];                // ... of part round p's first record (merged scans), -1: no round
         Block() { std::fill(part, part + GG_MAX_CLOUD_PARTS, -1); }
+        RecordLayout layout() const { return record_layout((size_t)calls * per_call); }
     };
     Block blk[kStreams];
     cudaStream_t streams[kStreams] = {};             // capture branch of each group with slots in the plan
@@ -367,19 +387,11 @@ struct gg_handle_s {
     cudaStream_t streams[kStreams] = {};
     bool own_streams = true;
     int n_streams = kStreams;
-    // parameter staging ring: pinned host copy + device copy per entry
-    gg::SlotParams* h_ring = nullptr;
-    gg::SlotParams* d_ring = nullptr;
-    gg::OutDest* h_dest = nullptr;   // output destinations of the entry's scans, same shape as h_ring / d_ring
-    gg::OutDest* d_dest = nullptr;
-    gg::UnpackDesc* h_unpack = nullptr;  // PointCloud2 payloads of the entry's scans, same shape as h_ring / d_ring
-    gg::UnpackDesc* d_unpack = nullptr;
-    gg::QueryDesc* h_query = nullptr;    // terrain lookups: query sets of the entry's slots, same shape as h_ring / d_ring
-    gg::QueryDesc* d_query = nullptr;
-    gg::PointInfoDest* h_pinfo = nullptr;  // point classes and heights: destinations of the entry's slots, same shape
-    gg::PointInfoDest* d_pinfo = nullptr;  // (both allocated on first use: ensure_tables)
-    int* h_pose_bits = nullptr;            // gg::PoseBits of the entry's records, same shape (allocated on first use)
-    int* d_pose_bits = nullptr;
+    // parameter staging ring: kRing entries of n_slots records, pinned on the host with a device copy; entry pos holds
+    // records [pos * n_slots, (pos + 1) * n_slots) of each array
+    unsigned char* h_ring = nullptr;
+    unsigned char* d_ring = nullptr;
+    RecordLayout ring_layout{};            // record_layout(kRing * n_slots)
     gg::PoseTables poses{};                // per-slot device positions and scan poses (first gg_update_poses_from_device)
     gg::CountTables counts{};              // per-slot device point counts (first gg_set_point_counts_from_device)
     gg::ConfigTables configs{};            // per-slot device configurations (first gg_set_slot_configs_from_device)
@@ -513,9 +525,9 @@ int layer_index(gg_handle h, int slot, const char* name, int* idx) {
     return fail(GG_E_LAYER, "unknown layer '%s'", name);
 }
 
-// One entry of the parameter staging ring: the SlotParams of up to n_slots scans and, in arrays parallel to them, their
-// output destinations (OutDest), PointCloud2 payloads (UnpackDesc), query sets (QueryDesc) and point-info destinations
-// (PointInfoDest), each pinned on the host with a device copy.
+// One entry of the parameter staging ring (or of a recorded step's block): the SlotParams of up to n_slots scans and, in
+// arrays parallel to them, their output destinations (OutDest), PointCloud2 payloads (UnpackDesc), query sets
+// (QueryDesc), point-info destinations (PointInfoDest) and PoseBits, each on the host with a device copy.
 struct Staging {
     int pos = 0;                 // position in the ring
     int m = 0;                   // records filled
@@ -536,45 +548,34 @@ struct Staging {
     gg::PointInfoDest *hpinfo = nullptr, *dpinfo = nullptr;
     int *hbits = nullptr, *dbits = nullptr;
 
+    // The entry whose first record is record `first` of the buffers at `host` and `dev`, laid out by `l`.
+    void bind(unsigned char* host, unsigned char* dev, const RecordLayout& l, size_t first) {
+        bind_array(hp, dp, host, dev, l.params, first);
+        bind_array(hdest, ddest, host, dev, l.dest, first);
+        bind_array(hunpack, dunpack, host, dev, l.unpack, first);
+        bind_array(hquery, dquery, host, dev, l.query, first);
+        bind_array(hpinfo, dpinfo, host, dev, l.pinfo, first);
+        bind_array(hbits, dbits, host, dev, l.bits, first);
+    }
+    template <typename T>
+    static void bind_array(T*& hq, T*& dq, unsigned char* host, unsigned char* dev, size_t offset, size_t first) {
+        hq = reinterpret_cast<T*>(host + offset) + first;
+        dq = reinterpret_cast<T*>(dev + offset) + first;
+    }
     // Reserve the next entry (waits only if the ring wrapped onto an in-flight entry).
     int acquire(gg_handle h) {
         pos = h->ring_pos;
         h->ring_pos = (pos + 1) % kRing;
         if (h->ring_used[pos]) GG_CUDA(cudaEventSynchronize(h->ring_ev[pos]));
-        const size_t at = (size_t)pos * h->n_slots;
-        hp = h->h_ring + at;
-        dp = h->d_ring + at;
-        hdest = h->h_dest + at;
-        ddest = h->d_dest + at;
-        hunpack = h->h_unpack + at;
-        dunpack = h->d_unpack + at;
-        hquery = h->h_query + at;
-        dquery = h->d_query + at;
-        hpinfo = h->h_pinfo ? h->h_pinfo + at : nullptr;   // allocated on first use (ensure_tables)
-        dpinfo = h->d_pinfo ? h->d_pinfo + at : nullptr;
-        hbits = h->h_pose_bits ? h->h_pose_bits + at : nullptr;
-        dbits = h->d_pose_bits ? h->d_pose_bits + at : nullptr;
+        bind(h->h_ring, h->d_ring, h->ring_layout, (size_t)pos * h->n_slots);
         return GG_OK;
     }
     // While a step is recorded: the next entry of group g's block (PlanRecorder).
     int acquire_recorded(gg_handle h, int g) {
         PlanRecorder::Block& b = h->rec->blk[g];
         if (b.next + b.per_call > b.calls * b.per_call) return fail(GG_E_STATE, "stream group %d: more entries than a recorded step holds", g);
-        const int at = b.next;
+        bind(h->rec->host.data() + b.at, h->rec->work + b.at, b.layout(), (size_t)b.next);
         b.next += b.per_call;
-        unsigned char *host = h->rec->host.data(), *dev = h->rec->work;
-        hp = reinterpret_cast<gg::SlotParams*>(host + b.params) + at;
-        dp = reinterpret_cast<gg::SlotParams*>(dev + b.params) + at;
-        hdest = reinterpret_cast<gg::OutDest*>(host + b.dest) + at;
-        ddest = reinterpret_cast<gg::OutDest*>(dev + b.dest) + at;
-        hunpack = reinterpret_cast<gg::UnpackDesc*>(host + b.unpack) + at;
-        dunpack = reinterpret_cast<gg::UnpackDesc*>(dev + b.unpack) + at;
-        hquery = reinterpret_cast<gg::QueryDesc*>(host + b.query) + at;
-        dquery = reinterpret_cast<gg::QueryDesc*>(dev + b.query) + at;
-        hpinfo = reinterpret_cast<gg::PointInfoDest*>(host + b.pinfo) + at;
-        dpinfo = reinterpret_cast<gg::PointInfoDest*>(dev + b.pinfo) + at;
-        hbits = reinterpret_cast<int*>(host + b.bits) + at;
-        dbits = reinterpret_cast<int*>(dev + b.bits) + at;
         return GG_OK;
     }
     // The next record (hp[m]), zeroed, for `slot` at position `pos` in the call.
@@ -704,7 +705,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
             if (stream_index(h, slots[i]) != g) continue;
             if (e.m == 0 && (rc = h->rec ? e.acquire_recorded(h, g) : e.acquire(h))) return rc;
             work |= fill(i, e);
-            if ((e.position || e.count || e.config) && e.hbits) {
+            if (e.position || e.count || e.config) {
                 int bits = 0;
                 if (e.position) {
                     if (h->slots[slots[i]].device_position) bits |= gg::POSE_POSITION;
@@ -805,14 +806,15 @@ static_assert(GG_MAX_CLOUD_PARTS < kRing, "the part rounds of a group must fit i
 // staging entry being part p of the entry's scan j (n_points 0 when the scan has no such part), each landing in its
 // slot's buffer after the scan's parts before p.  A round with no part to read is not launched.  When scans of the entry
 // take device part counts (POSE_PART_COUNTS), k_stage_parts resolves their round records once every round's entry is
-// copied, before the first round.  While a step is recorded the rounds' entries come from the group's block.  Returns
+// copied, before the first round (the bits are those run_groups wrote for e: run_scans_grouped stages positions, so every
+// record of a scan entry has them).  While a step is recorded the rounds' entries come from the group's block.  Returns
 // the number of launches, or a negative error code.
 int launch_part_rounds(gg_handle h, const Staging& e, const CallerOutputs& c, cudaStream_t st) {
     int rounds = 0, n = 0, rc;
     bool resolve = false;
     for (int j = 0; j < e.m; ++j) {
         rounds = std::max(rounds, c.n_parts[e.hp[j].pos]);
-        resolve = resolve || (e.hbits && (e.hbits[j] & gg::POSE_PART_COUNTS));
+        resolve = resolve || (e.hbits[j] & gg::POSE_PART_COUNTS);
     }
     const int g = stream_index(h, e.hp[0].slot);
     Staging r[GG_MAX_CLOUD_PARTS];
@@ -950,39 +952,32 @@ bool encode_layer_map(gg_handle h) {
     return r == CUDA_SUCCESS;
 }
 
-// The buffers a handle allocates the first time a call needs them, so a handle that never makes the call has none.  Step
-// plans allocate the union of what their calls need before recording (prepare_recording), since a recording may not
-// allocate.
+// The device buffers a handle allocates the first time a call needs them, so a handle that never makes the call has none
+// (the staging records are all allocated with the ring, in gg_create).  Step plans allocate the union of what their calls
+// need before recording (prepare_recording), since a recording may not allocate.
 enum Tables : unsigned {
     T_POSES = 1u << 0,          // PoseTables: device positions and scan poses
     T_STORED_COUNTS = 1u << 1,  // CountTables::stored
     T_LAST_COUNTS = 1u << 2,    // CountTables::last
     T_PART_COUNTS = 1u << 3,    // CountTables::parts
-    T_POSE_BITS = 1u << 4,      // staging of the records' PoseBits, device and pinned
-    T_OUT_CLOUD = 1u << 5,      // the output cloud of gg_get_output
-    T_IMAGE_RANGES = 1u << 6,   // per-block range scratch of the layer images (launch_layer_images)
-    T_POINT_INFO = 1u << 7,     // staging of the PointInfoDest records, device and pinned
-    T_CONFIGS = 1u << 8,        // ConfigTables (the private detect tables: ensure_config_tables)
+    T_OUT_CLOUD = 1u << 4,      // the output cloud of gg_get_output
+    T_IMAGE_RANGES = 1u << 5,   // per-block range scratch of the layer images (launch_layer_images)
+    T_CONFIGS = 1u << 6,        // ConfigTables (the private detect tables: ensure_config_tables)
 };
 
 // Makes the handle's device current and allocates the buffers of `need` that are missing.
 int ensure_tables(gg_handle h, unsigned need) {
     GG_CUDA(cudaSetDevice(h->device));
-    const size_t S = (size_t)h->n_slots, R = (size_t)kRing * S;
+    const size_t S = (size_t)h->n_slots;
     auto dev = [&](auto** p, size_t n) { return *p ? GG_OK : dev_alloc(h, p, n); };
     int rc;
     if ((need & T_POSES) && ((rc = dev(&h->poses.position, S)) || (rc = dev(&h->poses.scan_pose, S)))) return rc;
     if ((need & T_STORED_COUNTS) && (rc = dev(&h->counts.stored, S))) return rc;
     if ((need & T_LAST_COUNTS) && (rc = dev(&h->counts.last, S))) return rc;
     if ((need & T_PART_COUNTS) && (rc = dev(&h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
-    if ((need & T_POSE_BITS) && (rc = dev(&h->d_pose_bits, R))) return rc;
-    if ((need & T_POSE_BITS) && !h->h_pose_bits) GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pose_bits), sizeof(int) * R, cudaHostAllocDefault));
     if ((need & T_OUT_CLOUD) && (rc = dev(&h->view.out_cloud, S * h->pcap))) return rc;
     if ((need & T_IMAGE_RANGES) && (rc = dev(&h->d_img_part, S * gg::L_NUM * ((h->view.k.N2 + gg::IMG_RANGE_CELLS - 1) / gg::IMG_RANGE_CELLS))))
         return rc;
-    if ((need & T_POINT_INFO) && (rc = dev(&h->d_pinfo, R))) return rc;
-    if ((need & T_POINT_INFO) && !h->h_pinfo)
-        GG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pinfo), sizeof(gg::PointInfoDest) * R, cudaHostAllocDefault));
     if ((need & T_CONFIGS) && ((rc = dev(&h->configs.raw, S)) || (rc = dev(&h->configs.cfg, S)))) return rc;
     return GG_OK;
 }
@@ -1125,11 +1120,11 @@ int slot_constants(gg_handle h, int slot, gg::CfgConst* kc) {
     return GG_OK;
 }
 
-// The configuration tables, the staging of the per-record bits and the private detect table of each of `slots`, on
-// first use (a handle that never asks has none).  Step plans call it before recording, which may not allocate.
+// The configuration tables and the private detect table of each of `slots`, on first use (a handle that never asks has
+// none).  Step plans call it before recording, which may not allocate.
 int ensure_config_tables(gg_handle h, int count, const int* slots) {
     int rc;
-    if ((rc = ensure_tables(h, T_CONFIGS | T_POSE_BITS))) return rc;
+    if ((rc = ensure_tables(h, T_CONFIGS))) return rc;
     if (h->config_tab.empty()) h->config_tab.assign((size_t)h->n_slots, nullptr);
     for (int i = 0; i < count; ++i)
         if (!h->config_tab[slots[i]] && (rc = dev_alloc(h, &h->config_tab[slots[i]], (size_t)h->view.k.N2))) return rc;
@@ -1340,14 +1335,9 @@ int gg_create(double dimension_m, float resolution, int device, int n_slots, siz
         h->n_streams = std::max(1, std::min(std::min(want, kStreams), n_slots));
         for (int i = 0; i < h->n_streams; ++i) GG_CUDA_TRY(cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
     }
-    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_ring), sizeof(gg::SlotParams) * kRing * S, cudaHostAllocDefault));
-    GG_TRY(dev_alloc(h, &h->d_ring, (size_t)kRing * S));
-    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_dest), sizeof(gg::OutDest) * kRing * S, cudaHostAllocDefault));
-    GG_TRY(dev_alloc(h, &h->d_dest, (size_t)kRing * S));
-    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_unpack), sizeof(gg::UnpackDesc) * kRing * S, cudaHostAllocDefault));
-    GG_TRY(dev_alloc(h, &h->d_unpack, (size_t)kRing * S));
-    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_query), sizeof(gg::QueryDesc) * kRing * S, cudaHostAllocDefault));
-    GG_TRY(dev_alloc(h, &h->d_query, (size_t)kRing * S));
+    h->ring_layout = record_layout((size_t)kRing * S);
+    GG_CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->h_ring), h->ring_layout.bytes, cudaHostAllocDefault));
+    GG_TRY(dev_alloc(h, &h->d_ring, h->ring_layout.bytes));
     for (int i = 0; i < kRing; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->ring_ev[i], cudaEventDisableTiming));
     GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_in, cudaEventDisableTiming));
     for (int i = 0; i < kStreams; ++i) GG_CUDA_TRY(cudaEventCreateWithFlags(&h->caller_out[i], cudaEventDisableTiming));
@@ -1383,11 +1373,6 @@ int gg_destroy(gg_handle h) {
     if (h->copy_out) cudaStreamDestroy(h->copy_out);
     for (void* p : h->dev_allocs) cudaFree(p);
     if (h->h_ring) cudaFreeHost(h->h_ring);
-    if (h->h_dest) cudaFreeHost(h->h_dest);
-    if (h->h_unpack) cudaFreeHost(h->h_unpack);
-    if (h->h_query) cudaFreeHost(h->h_query);
-    if (h->h_pinfo) cudaFreeHost(h->h_pinfo);
-    if (h->h_pose_bits) cudaFreeHost(h->h_pose_bits);
     for (int i = 0; i < kRing; ++i)
         if (h->ring_ev[i]) cudaEventDestroy(h->ring_ev[i]);
     if (h->own_streams)
@@ -2708,7 +2693,7 @@ int gg_point_info_to_device(gg_handle h, int count, const int* slots, const gg_p
     const auto bad = find_overlap(ranges);
     if (bad.first) return fail(GG_E_ARG, "an output of slot %d overlaps an output of slot %d", slots[bad.second->set], slots[bad.first->set]);
     if (ranges.empty()) return GG_OK;
-    if ((rc = ensure_tables(h, T_POINT_INFO))) return rc;
+    GG_CUDA(cudaSetDevice(h->device));
     auto fill = [&](int i, Staging& e) {
         const SlotState& s = h->slots[slots[i]];
         const gg_point_info& o = outs[i];
@@ -2745,7 +2730,7 @@ int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const 
     if (!in.xy != !in.T_base_from_map) return fail(GG_E_ARG, "xy and T_base_from_map must both be given or both be NULL");
     if (!in.origin != !in.base_z) return fail(GG_E_ARG, "origin and base_z must both be given or both be NULL");
     if (!in.xy && !in.origin) return GG_OK;
-    if ((rc = ensure_tables(h, T_POSES | T_POSE_BITS))) return rc;
+    if ((rc = ensure_tables(h, T_POSES))) return rc;
     const gg::DevicePoses dp{in.xy, in.T_base_from_map, in.origin, in.base_z, dev_moved};
     auto fill = [&](int i, Staging& e) {
         SlotState& s = h->slots[slots[i]];
@@ -2774,7 +2759,7 @@ int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, co
                                nullptr)) ||
         count == 0)
         return rc;
-    if ((rc = ensure_tables(h, T_STORED_COUNTS | T_LAST_COUNTS | T_POSE_BITS))) return rc;
+    if ((rc = ensure_tables(h, T_STORED_COUNTS | T_LAST_COUNTS))) return rc;
     auto fill = [&](int i, Staging& e) {
         e.record(slots[i], i);
         h->slots[slots[i]].stored_count = true;
@@ -2795,7 +2780,7 @@ int gg_set_part_counts_from_device(gg_handle h, int count, const int* slots, int
                                nullptr, nullptr)) ||
         count == 0)
         return rc;
-    if ((rc = ensure_tables(h, T_LAST_COUNTS | T_PART_COUNTS | T_POSE_BITS))) return rc;
+    if ((rc = ensure_tables(h, T_LAST_COUNTS | T_PART_COUNTS))) return rc;
     auto fill = [&](int i, Staging& e) {
         e.record(slots[i], i);
         h->slots[slots[i]].stored_parts = parts_per_slot;
@@ -2823,7 +2808,7 @@ int gg_init_maps_from_device(gg_handle h, int count, const int* slots, const gg_
                                nullptr, nullptr, in.mask != nullptr)) ||
         count == 0)
         return rc;
-    if ((rc = ensure_tables(h, T_POSES | T_POSE_BITS))) return rc;
+    if ((rc = ensure_tables(h, T_POSES))) return rc;
     auto fill = [&](int i, Staging& e) {
         SlotState& s = h->slots[slots[i]];
         gg::SlotParams& p = e.record(slots[i], i);
@@ -2883,8 +2868,6 @@ int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
 
 // ---- step plans -------------------------------------------------------------------------------
 namespace {
-size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
-
 void free_plan(gg_step_plan p) {
     if (p->exec) cudaGraphExecDestroy(p->exec);
     if (p->graph) cudaGraphDestroy(p->graph);
@@ -2974,11 +2957,12 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
         const PlanRecorder::Block& b = r.blk[g];
+        const RecordLayout l = b.layout();
         cudaStream_t st = r.streams[g];
         GG_CUDA(cudaStreamWaitEvent(st, fork, 0));
-        GG_CUDA(cudaMemcpyAsync(p->work + b.at, p->pristine + b.at, b.bytes, cudaMemcpyDeviceToDevice, st));
+        GG_CUDA(cudaMemcpyAsync(p->work + b.at, p->pristine + b.at, l.bytes, cudaMemcpyDeviceToDevice, st));
         if (T_group[g])
-            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.unpack), p->dev_T + b.first, b.calls * b.per_call, st);
+            h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.at + l.unpack), p->dev_T + b.first, b.calls * b.per_call, st);
     }
     int rc;
     const int n = d.count;
@@ -3016,10 +3000,8 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
 int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_configs* configs, const gg_step_readouts* readouts) {
     // the tables of the poses, counts and part counts whether or not the step records those calls (record_plan seeds the
     // positions), and the output cloud
-    unsigned need = T_POSES | T_STORED_COUNTS | T_LAST_COUNTS | T_PART_COUNTS | T_POSE_BITS | T_OUT_CLOUD;
-    const ReadoutCalls c(readouts);
-    if (c.images) need |= T_IMAGE_RANGES;
-    if (c.point_info) need |= T_POINT_INFO;
+    unsigned need = T_POSES | T_STORED_COUNTS | T_LAST_COUNTS | T_PART_COUNTS | T_OUT_CLOUD;
+    if (ReadoutCalls(readouts).images) need |= T_IMAGE_RANGES;
     int rc;
     if ((rc = ensure_tables(h, need))) return rc;
     if (configs) {
@@ -3059,19 +3041,12 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
             }
         if (c == 0) continue;
         PlanRecorder::Block& b = rec.blk[g];
-        const size_t m = (size_t)(calls + rounds) * c;
         b.per_call = c;
         b.calls = calls + rounds;
         b.first = rec.records;
-        rec.records += (int)m;
-        b.at = b.params = at;
-        b.dest = at = align16(at + m * sizeof(gg::SlotParams));
-        b.unpack = at = align16(at + m * sizeof(gg::OutDest));
-        b.query = at = align16(at + m * sizeof(gg::UnpackDesc));
-        b.pinfo = at = align16(at + m * sizeof(gg::QueryDesc));
-        b.bits = at = align16(at + m * sizeof(gg::PointInfoDest));
-        at = align16(at + m * sizeof(int));
-        b.bytes = at - b.at;
+        rec.records += b.calls * b.per_call;
+        b.at = at;
+        at += b.layout().bytes;
         p->groups.push_back(g);
     }
     rec.host.assign(at, 0);

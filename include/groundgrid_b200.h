@@ -915,7 +915,7 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
  * Validation: what gg_step_plan_create_with_resets validates, and what the six calls validate, with the same codes (the
  * calls run while the step is recorded, after the slots' state the scans leave).  A rejected plan leaves no plan, no
  * bound slot, the slots' host state and gg_kernel_launches unchanged.  Creation also allocates what the read-outs
- * allocate on first use (the image range scratch, the point-info staging).  The bound-slot rules, gg_step_plan_launch
+ * allocate on first use (the image range scratch).  The bound-slot rules, gg_step_plan_launch
  * and gg_step_plan_destroy are those of every plan; the read-outs change no slot state. */
 typedef struct gg_step_readouts {
     int n_layer_names;  const char* const* layer_names;  float* layers;                       /* gg_get_layers_to_device */
