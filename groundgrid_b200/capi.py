@@ -331,7 +331,10 @@ class StepPlan:
         if getattr(self, "_p", None):
             p, self._p = self._p, None
             self._owner._plans.discard(self)
-            _check(self._owner._l.gg_step_plan_destroy(p))
+            # a plan collected in one cycle with its handle may find the handle closed already: gg_destroy destroyed it
+            # (the handle's weak set of plans is emptied before either finaliser runs)
+            if self._owner._h:
+                _check(self._owner._l.gg_step_plan_destroy(p))
 
     def __del__(self):
         try:

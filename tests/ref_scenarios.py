@@ -89,6 +89,22 @@ class Recorder:
         return self.got
 
 
+class Folded:
+    """Takes the values of one case in place of a Recorder and hands the Recorder ONE digest of them (of their keys and
+    digests, in order) under `key`: for scenarios of many cases, where a digest per value would make the stored file
+    large.  A mismatch names the case; the tests that compare the CUDA path with the oracle value by value name the
+    value."""
+
+    def __init__(self, rec, key):
+        self.rec, self.key, self.parts = rec, key, []
+
+    def __call__(self, key, value):
+        self.parts.append(f"{key}:{digest(np.asarray(value))}")
+
+    def done(self):
+        self.rec(self.key, np.frombuffer("\n".join(self.parts).encode(), np.uint8))
+
+
 # ---- implementations ------------------------------------------------------------------------------------------------
 class Reference:
     """oracle/_ref: the reference's own sources."""
@@ -604,6 +620,63 @@ def crowded_cells(make, rec):
     scan(m, rec, *lc.boundary_cloud(lc.TILE_EDGE + 1), 0.0, f"{lc.TILE_EDGE + 1} points")
 
 
+# ---- every configuration field at the ends of its range and beyond (tests/config_limits.py) -----------------------------
+def near_returns(count, seed, radius=3.3):
+    """`count` returns on the ground within `radius` m (< sqrt(12) m) of the sensor at the origin, on rings 0 .. 31: points
+    filter_cloud ignores for the statistics and still labels."""
+    rng = np.random.default_rng(seed)
+    r = np.sqrt(rng.uniform(0.01, radius * radius, count))
+    a = rng.uniform(-np.pi, np.pi, count)
+    pts = np.zeros(count, synth.POINT_DTYPE)
+    pts["x"], pts["y"] = (r * np.cos(a)).astype(np.float32), (r * np.sin(a)).astype(np.float32)
+    pts["z"] = rng.uniform(-0.1, 0.6, count).astype(np.float32)
+    pts["ring"] = rng.integers(0, 32, count)
+    return pts
+
+
+def config_limits_stream(n, scans=3):
+    """The scans of config_limits on an N x N map: (ego x, y, yaw, base_z, points, origin) per scan; every scan after the
+    first follows a roll with yaw and a pitched base frame and has points pushed below the ground."""
+    dim, _ = DENSE_GEOMETRY[n]
+    scene = synth.make_scene(seed=70 + n, n_boxes=8, rmin=3.0, rmax=0.4 * dim)
+    out = []
+    for k in range(scans):
+        ex, ey, yaw = 0.9 * k, -0.6 * k, 0.15 * k
+        pts, org = synth.lidar_scan(scene, (ex, ey), yaw, beams=32, az_steps=512, seed=7000 + 10 * n + k)
+        near = near_returns(300, 7100 + 10 * n + k)
+        near["x"] += np.float32(org[0])
+        near["y"] += np.float32(org[1])
+        pts = np.concatenate([pts, near]).astype(synth.POINT_DTYPE)   # concatenate drops the padding of the records
+        if k:
+            push_below_ground(pts, 500, 7200 + 10 * n + k)
+        out.append((ex, ey, yaw, 0.02 * k, pts, org))
+    return out
+
+
+def config_limits(make, rec, n):
+    """Every case of tests/config_limits.py on a fresh N x N map (N = 100: the TMA detection and the skewed spiral; N = 101:
+    the plain-load detection on an odd map): three scans with a roll in between; the roll's moved flag and position, and
+    labels, output order and cloud and all eleven layers after every scan, folded into one digest per case."""
+    import config_limits as cl
+
+    dim, res = DENSE_GEOMETRY[n]
+    stream = config_limits_stream(n)
+    for name, cfg in cl.CASES.items():
+        m = make(dim, res)
+        assert m.n == n
+        m.set_config(**cfg)
+        m.init_map(0.0, 0.0, 0.0)
+        case = Folded(rec, name)
+        for k, (ex, ey, yaw, base_z, pts, org) in enumerate(stream):
+            if k:
+                q, t = base_from_map_qt(ex, ey, yaw, base_z, pitch=0.02)
+                update(m, case, ex, ey, q, t, f"roll {k}", layers=())
+            scan(m, case, pts, org, base_z, f"scan {k}")
+            if name == "minimum_distance_factor=0.0":   # cells of one point have variance 0: the label tolerance is 0 / 0
+                assert ((m.layer("pointsRaw") == 1) & (m.layer("variance") == 0)).sum() > 100
+        case.done()
+
+
 SCENARIOS = {
     "expected_points_table": (expected_points_table, [()]),
     "cfg1_cfg2_64_beam_300": (cfg1_cfg2_64_beam_300, [()]),
@@ -624,6 +697,7 @@ SCENARIOS = {
     "detect_planes": (detect_planes, [(n,) for n in DETECT_SIZES]),
     "outlier_priors": (outlier_priors, [(w,) for w in OUTLIER_SIZES]),
     "crowded_cells": (crowded_cells, [()]),
+    "config_limits": (config_limits, [(n,) for n in DENSE_GEOMETRY]),
 }
 
 
