@@ -204,6 +204,51 @@ class DeviceConfigs(C.Structure):
     ]
 
 
+SNAPSHOT_MAGIC = 0x534D4747   # GG_SNAPSHOT_MAGIC ("GGMS")
+SNAPSHOT_VERSION = 1          # GG_SNAPSHOT_VERSION
+
+
+class MapSnapshot(C.Structure):
+    """gg_map_snapshot: the 64-byte header of a map snapshot record; "ground" follows at byte 64 and "groundpatch" at
+    64 + 4 * N2p (N2p = N * N rounded up to a multiple of 4), both column-major."""
+
+    _fields_ = [
+        ("magic", C.c_uint32),
+        ("version", C.c_uint32),
+        ("cells_per_side", C.c_int32),
+        ("resolution", C.c_float),
+        ("position", C.c_double * 2),
+        ("reserved", C.c_uint32 * 8),
+    ]
+
+
+def snapshot_bytes(n):
+    """The size of one snapshot record of an n x n map: 64 + 8 * N2p, N2p = n * n rounded up to a multiple of 4."""
+    return C.sizeof(MapSnapshot) + 8 * ((n * n + 3) // 4 * 4)
+
+
+class MapRestore(C.Structure):
+    """gg_map_restore: device addresses of the snapshot pool, the index and the status of gg_restore_maps_from_device
+    (None = NULL)."""
+
+    _fields_ = [
+        ("pool", C.c_void_p),
+        ("n_pool", C.c_int),
+        ("index", C.c_void_p),
+        ("status", C.c_void_p),
+    ]
+
+
+class StepSnapshots(C.Structure):
+    """gg_step_snapshots: a step plan's restore (step 3) and save (step 8) stages (gg_step_plan_create_with_snapshots)."""
+
+    _fields_ = [
+        ("restore", MapRestore),
+        ("save", C.c_void_p),
+        ("save_mask", C.c_void_p),
+    ]
+
+
 class StepDesc(C.Structure):
     """gg_step_desc: the fixed batch and caller device buffers of a step plan (gg_step_plan_create)."""
 
@@ -305,6 +350,8 @@ class StepPlan:
       outputs             : DeviceOutputs of the step (allocated at capacity), rewritten by every replay
       moved               : int32 [count] dev_moved of the roll, or None
       readouts            : PlanReadouts of the step's read-outs (all None for a plan without them)
+      restore_status      : int32 [count] status of the step's restore, or None
+      saved               : uint8 [count, snapshot_bytes] records of the step's save, or None
       kernels             : kernel launches per replay
       close()             : gg_step_plan_destroy (waits for the device); the slots accept every call again
     The plan keeps its input and output tensors alive; write the next step's inputs into them (e.g. with copy_) on the
@@ -313,6 +360,7 @@ class StepPlan:
     def __init__(self, owner, p, outputs, moved, keep, readouts=None):
         self._owner, self._p, self.outputs, self.moved, self._keep = owner, p, outputs, moved, keep
         self.readouts = readouts if readouts is not None else PlanReadouts()
+        self.restore_status = self.saved = None
         owner._plans.add(self)
 
     def launch(self, stream=None):
@@ -417,6 +465,11 @@ def load(build_if_missing=True):
         "gg_set_slot_configs_from_device": (i, [vp, i, vp, C.POINTER(DeviceConfigs), vp]),
         "gg_step_plan_create_with_configs": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(DeviceConfigs),
                                                  C.POINTER(StepReadouts), C.POINTER(vp)]),
+        "gg_map_snapshot_bytes": (sz, [vp]),
+        "gg_save_maps_to_device": (i, [vp, i, vp, vp, vp, vp]),
+        "gg_restore_maps_from_device": (i, [vp, i, vp, C.POINTER(MapRestore), vp]),
+        "gg_step_plan_create_with_snapshots": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(DeviceConfigs),
+                                                   C.POINTER(StepSnapshots), C.POINTER(StepReadouts), C.POINTER(vp)]),
         "gg_step_plan_launch": (i, [vp, vp]),
         "gg_step_plan_kernels": (i, [vp]),
         "gg_step_plan_destroy": (i, [vp]),
@@ -807,6 +860,83 @@ class GroundGridB200:
         if cfgs is None and count:
             raise ValueError("cfgs is required")
         self.set_configs_from_device_ptrs(slots, ptrs[0], ptrs[1], stream.cuda_stream or None)
+
+    @property
+    def snapshot_bytes(self):
+        """Bytes of one map snapshot record of this handle (gg_map_snapshot_bytes)."""
+        return int(self._l.gg_map_snapshot_bytes(self._h))
+
+    def save_maps_to_device_ptrs(self, slots, dst_ptr, mask_ptr, stream_ptr):
+        """gg_save_maps_to_device with raw device addresses (ints, or None for NULL); stream_ptr None = the legacy default
+        stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        _check(self._l.gg_save_maps_to_device(self._h, len(sl), _ptr(sl), dst_ptr, mask_ptr, stream_ptr))
+
+    def save_maps_to_device(self, slots, mask=None, out=None, stream=None):
+        """Snapshots of the maps of `slots` -- "ground", "groundpatch" and the map position -- as one uint8 CUDA tensor
+        [count, snapshot_bytes] (gg_save_maps_to_device); record k starts with a MapSnapshot header.
+          mask   : int32 [count] or None: a record whose entry is zero is left untouched (a new `out` starts zeroed then)
+          out    : uint8 [count, snapshot_bytes] to fill instead of a new tensor (contiguous, 16-byte aligned)
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        The call returns without waiting for the device; work enqueued on `stream` afterwards sees the records.  The
+        slots' state does not change."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count, rb = len(slots), self.snapshot_bytes
+        if out is None:
+            with torch.cuda.stream(stream):
+                out = (torch.zeros if mask is not None else torch.empty)((count, rb), dtype=torch.uint8, device=dev)
+        elif out.dtype != torch.uint8 or out.device != dev or not out.is_contiguous() or tuple(out.shape) != (count, rb):
+            raise ValueError(f"out must be a contiguous uint8 tensor {(count, rb)} on {dev}")
+        elif stream != current:
+            out.record_stream(stream)
+        mask_ptr = None
+        if mask is not None:
+            if mask.dtype != torch.int32 or mask.device != dev or not mask.is_contiguous() or mask.numel() != count:
+                raise ValueError(f"mask must be a contiguous int32 tensor ({count},) on {dev}")
+            if stream != current:
+                mask.record_stream(stream)
+            mask_ptr = mask.data_ptr() if count else None
+        self.save_maps_to_device_ptrs(slots, out.data_ptr() if count else None, mask_ptr, stream.cuda_stream or None)
+        return out
+
+    def restore_maps_from_device_ptrs(self, slots, pool_ptr, n_pool, index_ptr, status_ptr, stream_ptr):
+        """gg_restore_maps_from_device with raw device addresses (ints, or None for NULL); stream_ptr None = the legacy
+        default stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        r = MapRestore(pool_ptr, int(n_pool), index_ptr, status_ptr)
+        _check(self._l.gg_restore_maps_from_device(self._h, len(sl), _ptr(sl), C.byref(r), stream_ptr))
+
+    def restore_maps_from_device(self, slots, pool, index=None, status=False, stream=None):
+        """Restores slots[k] from snapshot pool[index[k]] (gg_restore_maps_from_device): "ground", "groundpatch" and the
+        map position as saved, every other layer as init_map starts it.
+          pool   : uint8 CUDA tensor [n_pool, snapshot_bytes] (save_maps_to_device records, or their bytes from a file)
+          index  : int32 [count] or None (= k): an index outside [0, n_pool) leaves the slot untouched
+          status : True: also return an int32 [count] tensor, 1 restored, 0 index out of range, -1 record rejected
+                   (another map size or resolution, or not a snapshot)
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        Every slot needs a map already.  The call returns without waiting for the device; afterwards every slot of the
+        call has a device-owned position and refuses point_info_to_device until its next scan, restored or not."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count, rb = len(slots), self.snapshot_bytes
+        if pool.dtype != torch.uint8 or pool.device != dev or not pool.is_contiguous() or pool.dim() != 2 or pool.shape[1] != rb:
+            raise ValueError(f"pool must be a contiguous uint8 tensor [n_pool, {rb}] on {dev}")
+        if index is not None and (index.dtype != torch.int32 or index.device != dev or not index.is_contiguous() or index.numel() != count):
+            raise ValueError(f"index must be a contiguous int32 tensor ({count},) on {dev}")
+        ptrs = []
+        for t in (pool, index):
+            if t is None:
+                ptrs.append(None)
+                continue
+            if stream != current:
+                t.record_stream(stream)
+            ptrs.append(t.data_ptr() if t.numel() else None)
+        st = None
+        if status:
+            with torch.cuda.stream(stream):
+                st = torch.empty(count, dtype=torch.int32, device=dev)
+        self.restore_maps_from_device_ptrs(slots, ptrs[0], pool.shape[0], ptrs[1], st.data_ptr() if st is not None and count else None,
+                                           stream.cuda_stream or None)
+        return st
 
     def position(self, slot=0):
         xy = np.zeros(2, np.float64)
@@ -1237,7 +1367,8 @@ class GroundGridB200:
                   base_z=None, counts=None, xy=None, T_base_from_map=None, pose_origins=None, pose_base_z=None, moved=False, labels=True,
                   select="nonground", index=False, reset_xyz=None, reset_mask=None, layers=None, layer_images=None, terrain_images=False,
                   samples=None, sample_names=("ground", "groundpatch"), sample_mode="nearest", sample_cells=False, point_info=None,
-                  tallies=None, parts=None, part_counts=None, configs=None, config_mask=None):
+                  tallies=None, parts=None, part_counts=None, configs=None, config_mask=None, restore_pool=None, restore_index=None,
+                  restore_status=False, save=None, save_mask=None):
         """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
         Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
         pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
@@ -1266,6 +1397,11 @@ class GroundGridB200:
                      slot) as in set_configs_from_device, read at every replay: the step then starts with that call
                      (gg_step_plan_create_with_configs), and the slots are device-configured from the plan's creation;
                      config_mask without configs is an error
+          restore_pool, restore_index, restore_status : CUDA uint8 [n_pool, snapshot_bytes], int32 [count] (or None: k)
+                     and True for plan.restore_status, as in restore_maps_from_device, read at every replay: the step then
+                     restores after the resets and before the counts (gg_step_plan_create_with_snapshots)
+          save, save_mask : True (a new tensor) or a CUDA uint8 [count, snapshot_bytes], and int32 [count] (or None: every
+                     slot), as in save_maps_to_device: the step then ends with that call, into plan.saved
         Read-outs: with any of these the step ends with a step 4 of read-out calls (gg_step_plan_create_with_readouts),
         whose results land in plan.readouts (PlanReadouts) at every replay:
           layers       : layer names, as get_layers_to_device
@@ -1365,7 +1501,32 @@ class GroundGridB200:
                                                         dptr(reset_mask, torch.int32, (count,), "reset_mask"))
         if config_mask is not None and configs is None:
             raise ValueError("config_mask needs configs")
-        if configs is not None:
+        if (restore_index is not None or restore_status) and restore_pool is None:
+            raise ValueError("restore_index and restore_status need restore_pool")
+        if save_mask is not None and save is None:
+            raise ValueError("save_mask needs save")
+        snap, rstatus, saved = None, None, None
+        if restore_pool is not None or save is not None:
+            snap = StepSnapshots()
+            rb = self.snapshot_bytes
+            if restore_pool is not None:
+                if restore_pool.dim() != 2 or restore_pool.shape[1] != rb:
+                    raise ValueError(f"restore_pool must be a CUDA uint8 tensor [n_pool, {rb}]")
+                rstatus = torch.empty(count, dtype=torch.int32, device=dev) if restore_status else None
+                snap.restore = MapRestore(dptr(restore_pool, torch.uint8, tuple(restore_pool.shape), "restore_pool"), restore_pool.shape[0],
+                                          dptr(restore_index, torch.int32, (count,), "restore_index"),
+                                          rstatus.data_ptr() if rstatus is not None else None)
+            if save is not None:
+                saved = torch.zeros((count, rb), dtype=torch.uint8, device=dev) if save is True else save
+                snap.save = dptr(saved, torch.uint8, (count, rb), "save")
+                snap.save_mask = dptr(save_mask, torch.int32, (count,), "save_mask")
+        if snap is not None:
+            cc = None if configs is None else DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"),
+                                                            dptr(config_mask, torch.int32, (count,), "config_mask"))
+            _check(self._l.gg_step_plan_create_with_snapshots(self._h, C.byref(d), None if sp is None else C.byref(sp),
+                                                              None if r is None else C.byref(r), None if cc is None else C.byref(cc),
+                                                              C.byref(snap), None if ro_c is None else C.byref(ro_c), C.byref(p)))
+        elif configs is not None:
             cc = DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"), dptr(config_mask, torch.int32, (count,), "config_mask"))
             _check(self._l.gg_step_plan_create_with_configs(self._h, C.byref(d), None if sp is None else C.byref(sp), None if r is None else C.byref(r),
                                                             C.byref(cc), None if ro_c is None else C.byref(ro_c), C.byref(p)))
@@ -1378,7 +1539,9 @@ class GroundGridB200:
             _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
         else:
             _check(self._l.gg_step_plan_create_with_resets(self._h, C.byref(d), C.byref(r), C.byref(p)))
-        return StepPlan(self, p, out, mv, keep, ro)
+        plan = StepPlan(self, p, out, mv, keep, ro)
+        plan.restore_status, plan.saved = rstatus, saved
+        return plan
 
     @staticmethod
     def _plan_parts(torch, dev, parts, point_step, field_offsets, T, part_counts, keep, dptr):

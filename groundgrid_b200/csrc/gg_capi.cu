@@ -2059,7 +2059,7 @@ const char* gg_profile_kernel_name(int id) {
                                            "k_terrain_image", "k_eval_counts", "k_layer_copy", "k_layer_range", "k_layer_image",
                                            "k_sample_layers", "k_point_info", "k_stage_poses", "k_pose_resolve", "k_store_counts",
                                            "k_reset_maps", "k_stage_parts", "k_store_part_counts", "k_store_configs",
-                                           "k_rebuild_detect_tables"};
+                                           "k_rebuild_detect_tables", "k_reset_maps_restore", "k_save_maps"};
     return (id >= 0 && id < gg::K_NUM) ? names[id] : "";
 }
 
@@ -2857,6 +2857,78 @@ int gg_set_slot_configs_from_device(gg_handle h, int count, const int* slots, co
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
+size_t gg_map_snapshot_bytes(gg_handle h) { return h ? gg::snapshot_bytes(h->view.k.N2) : 0; }
+
+namespace {
+// The handle's float resolution bitwise (a snapshot's header carries it, and a restore compares it).
+uint32_t resolution_bits(gg_handle h) {
+    uint32_t b;
+    std::memcpy(&b, &h->resolution, sizeof(b));
+    return b;
+}
+}  // namespace
+
+// Map snapshots: per stream group one k_save_maps over the group's slots.  Each record stages the host position and,
+// for a device-owned one, POSE_POSITION: the kernel then reads the table, so nothing waits on the host.  No slot state
+// changes.
+int gg_save_maps_to_device(gg_handle h, int count, const int* slots, void* dst, const int32_t* mask, void* stream) {
+    const size_t n = (size_t)count;
+    int rc;
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr,
+                               {{dst, h ? n * gg::snapshot_bytes(h->view.k.N2) : 0, 16, true, "dst"},
+                                {mask, n * sizeof(int32_t), alignof(int32_t), false, "mask", CallerBuf::INPUT}},
+                               nullptr, nullptr)) ||
+        count == 0)
+        return rc;
+    GG_CUDA(cudaSetDevice(h->device));
+    const gg::SnapshotDest out{static_cast<unsigned char*>(dst), mask, resolution_bits(h)};
+    auto fill = [&](int i, Staging& e) {
+        const SlotState& s = h->slots[slots[i]];
+        gg::SlotParams& p = e.record(slots[i], i);
+        p.px = s.px;
+        p.py = s.py;
+        e.hbits[e.m] = s.device_position ? gg::POSE_POSITION : 0;
+        e.pose_bits = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_save_maps(h->view, h->poses, e.dp, e.dbits, e.m, out, st, h->prof); };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
+// Map restores: per stream group one k_reset_maps<.., RESTORE> over the group's slots.  The host cannot see the index
+// or the records, so every slot of the call leaves it as gg_init_maps_from_device with a mask leaves it: a device-owned
+// position (the kernel seeds the host-owned positions of slots it leaves untouched), and its point info refused until
+// the next scan.
+int gg_restore_maps_from_device(gg_handle h, int count, const int* slots, const gg_map_restore* r, void* stream) {
+    const gg_map_restore in = r ? *r : gg_map_restore{};
+    const size_t n = (size_t)count;
+    if (count > 0 && in.n_pool < 0) return fail(GG_E_ARG, "n_pool %d is negative", in.n_pool);
+    const size_t pool_bytes = (h && in.n_pool > 0) ? (size_t)in.n_pool * gg::snapshot_bytes(h->view.k.N2) : 0;
+    int rc;
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr,
+                               {{r, 0, 1, true, "r"},
+                                {in.pool, pool_bytes, 16, in.n_pool > 0, "pool", CallerBuf::INPUT},
+                                {in.index, n * sizeof(int32_t), alignof(int32_t), false, "index", CallerBuf::INPUT},
+                                {in.status, n * sizeof(int32_t), alignof(int32_t), false, "status", CallerBuf::OUTPUT}},
+                               nullptr, nullptr)) ||
+        count == 0)
+        return rc;
+    if ((rc = ensure_tables(h, T_POSES))) return rc;
+    const gg::SnapshotPool pool{static_cast<const unsigned char*>(in.pool), in.index, in.status, in.n_pool, resolution_bits(h)};
+    auto fill = [&](int i, Staging& e) {
+        SlotState& s = h->slots[slots[i]];
+        gg::SlotParams& p = e.record(slots[i], i);
+        p.px = s.px;   // what an untouched record seeds into the table, unless the table already holds the position
+        p.py = s.py;
+        e.hbits[e.m] = s.device_position ? gg::POSE_POSITION : 0;
+        e.pose_bits = true;
+        s.device_position = s.device_rolled = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_restore_maps(h->view, h->poses, e.dp, e.dbits, e.m, pool, st, h->prof); };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
 int gg_last_scan_points(gg_handle h, int slot, size_t* n_points) {
     int rc = check_slot(h, slot);
     if (rc) return rc;
@@ -2939,20 +3011,32 @@ struct ReadoutCalls {
     int count() const { return layers + images + terrain + samples + point_info + eval; }
 };
 
-// The calls a plan's step records: the configurations, resets, counts (or part counts) and poses when given, the scans,
-// and the read-outs.
+// Which snapshot stages a plan's step records (gg_step_plan_create_with_snapshots): the restore when any field of
+// snaps->restore is set, the save when save or save_mask is; each call then checks its arguments as it always does.
+struct SnapshotCalls {
+    bool restore = false, save = false;
+    explicit SnapshotCalls(const gg_step_snapshots* s) {
+        if (!s) return;
+        restore = s->restore.pool || s->restore.n_pool || s->restore.index || s->restore.status;
+        save = s->save || s->save_mask;
+    }
+};
+
+// The calls a plan's step records: the configurations, resets, restore, counts (or part counts) and poses when given, the
+// scans, the read-outs, and the save when given.
 int step_calls(const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-               const gg_step_readouts* readouts) {
+               const gg_step_snapshots* snaps, const gg_step_readouts* readouts) {
     const gg_device_poses& q = d.poses;
-    return (configs != nullptr) + (resets != nullptr) + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) + (q.xy || q.T_base_from_map || q.origin || q.base_z) +
-           1 + ReadoutCalls(readouts).count();
+    const SnapshotCalls sc(snaps);
+    return (configs != nullptr) + (resets != nullptr) + sc.restore + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) +
+           (q.xy || q.T_base_from_map || q.origin || q.base_z) + 1 + ReadoutCalls(readouts).count() + sc.save;
 }
 
-// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_configs): per branch the restore of
+// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_snapshots): per branch the restore of
 // its records and, where a payload takes a device transform, the transform staging; then the step's calls, the
-// configurations and the resets (when given) first and the read-outs last.
+// configurations, the resets and the restore (when given) first, then the read-outs, and the save (when given) last.
 int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-                const gg_step_readouts* readouts, const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
+                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
     PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
@@ -2970,6 +3054,8 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     const gg_device_poses& q = d.poses;
     if (configs && (rc = gg_set_slot_configs_from_device(h, n, sl, configs, root))) return rc;
     if (resets && (rc = gg_init_maps_from_device(h, n, sl, resets, root))) return rc;
+    const SnapshotCalls sc(snaps);
+    if (sc.restore && (rc = gg_restore_maps_from_device(h, n, sl, &snaps->restore, root))) return rc;
     if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
     if (parts && parts->dev_part_counts && (rc = gg_set_part_counts_from_device(h, n, sl, parts->parts_per_slot, parts->dev_part_counts, root)))
         return rc;
@@ -2992,6 +3078,7 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     if (c.samples && (rc = gg_sample_layers_to_device(h, n, sl, o.samples, o.n_sample_names, o.sample_names, o.sample_mode, root))) return rc;
     if (c.point_info && (rc = gg_point_info_to_device(h, n, sl, o.point_info, root))) return rc;
     if (c.eval && (rc = gg_eval_counts_to_device(h, n, sl, o.eval_counts, root))) return rc;
+    if (sc.save && (rc = gg_save_maps_to_device(h, n, sl, snaps->save, snaps->save_mask, root))) return rc;
     return GG_OK;
 }
 
@@ -3017,8 +3104,8 @@ int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_config
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
 int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-                const gg_step_readouts* readouts, gg_step_plan p) {
-    const int count = d.count, calls = step_calls(d, parts, resets, configs, readouts);
+                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, gg_step_plan p) {
+    const int count = d.count, calls = step_calls(d, parts, resets, configs, snaps, readouts);
     std::vector<int>& slots = p->slots;
     slots.resize(count);
     for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
@@ -3103,7 +3190,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, parts, resets, configs, readouts, slots, T_group, root, fork, p);
+        rc = record_step(h, d, parts, resets, configs, snaps, readouts, slots, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -3175,6 +3262,12 @@ int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const 
 
 int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
                                      const gg_device_configs* configs, const gg_step_readouts* readouts, gg_step_plan* out) {
+    return gg_step_plan_create_with_snapshots(h, desc, parts, resets, configs, nullptr, readouts, out);
+}
+
+int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                       const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
+                                       gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
     if (!h || !desc) return fail(GG_E_ARG, "null argument");
@@ -3184,7 +3277,7 @@ int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, cons
     if ((rc = prepare_recording(h, *desc, configs, readouts))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, parts, resets, configs, readouts, p))) {
+    if ((rc = record_plan(h, *desc, parts, resets, configs, snaps, readouts, p))) {
         free_plan(p);
         return rc;
     }

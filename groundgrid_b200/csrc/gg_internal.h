@@ -227,7 +227,7 @@ constexpr int OUT_TILE = 1024;
 enum KernelId : int {
     K_RASTERIZE = 0, K_CELL_TILES, K_CELL_PLACE, K_SCATTER, K_CELL_STATS, K_DETECT, K_SPIRAL, K_LABEL, K_ROLL_GATHER, K_ROLL_COMMIT, K_OUT_COUNT, K_OUT_SCAN,
     K_OUT_WRITE, K_UNPACK, K_TERRAIN, K_EVAL, K_LAYER_COPY, K_LAYER_RANGE, K_LAYER_IMAGE, K_SAMPLE, K_POINT_INFO, K_STAGE_POSES, K_POSE_RESOLVE,
-    K_STORE_COUNTS, K_RESET_MAPS, K_STAGE_PARTS, K_STORE_PART_COUNTS, K_STORE_CONFIGS, K_REBUILD_DETECT,
+    K_STORE_COUNTS, K_RESET_MAPS, K_STAGE_PARTS, K_STORE_PART_COUNTS, K_STORE_CONFIGS, K_REBUILD_DETECT, K_RESTORE_MAPS, K_SAVE_MAPS,
     K_NUM
 };
 
@@ -618,6 +618,35 @@ int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, c
 // masked-off record whose bits lack POSE_POSITION seeds its staged px / py into the table instead.
 int launch_reset_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const double* xyz, const int32_t* mask,
                       cudaStream_t st, Profiler* prof);
+// Map snapshots (gg_save_maps_to_device, gg_restore_maps_from_device): records of snapshot_bytes(N2p) bytes, the
+// gg_map_snapshot header followed by "ground" at byte 64 and "groundpatch" at 64 + 4 * n2p.
+constexpr int SNAPSHOT_HEADER = 64;
+static_assert(sizeof(gg_map_snapshot) == SNAPSHOT_HEADER, "gg_map_snapshot is the 64-byte header of a snapshot");
+__host__ __device__ constexpr int snapshot_cells(int N2) { return (N2 + 3) & ~3; }
+__host__ __device__ constexpr size_t snapshot_bytes(int N2) { return SNAPSHOT_HEADER + (size_t)8 * snapshot_cells(N2); }
+struct SnapshotPool {
+    const unsigned char* records;  // [n_pool][snapshot_bytes]
+    const int32_t* index;          // [count] or null (= pos)
+    int32_t* status;               // [count] or null
+    int n_pool;
+    uint32_t res_bits;             // the handle's float resolution, bitwise
+};
+struct SnapshotDest {
+    unsigned char* records;        // [count][snapshot_bytes]
+    const int32_t* mask;           // [count] or null
+    uint32_t res_bits;
+};
+// Restore: the snapshot-taking instantiation of k_reset_maps.  Record j takes "ground" and "groundpatch" from the pool
+// record index[pos] (pos when index is null), every other layer starts as k_init_map starts it, and the record's position
+// goes to the table; status[pos] = 1.  An index outside [0, n_pool) (status 0) or a record whose header does not match
+// the handle (status -1) leaves the slot untouched, and a host-owned position (bits lack POSE_POSITION) is seeded from the
+// staged px / py, as a masked-off reset seeds it.
+int launch_restore_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const SnapshotPool& pool,
+                        cudaStream_t st, Profiler* prof);
+// Save (k_save_maps): record j writes the header (position from the table when bits hold POSE_POSITION, else the staged
+// px / py) and both planes of its slot into records[pos], unless mask is zero at pos.
+int launch_save_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const SnapshotDest& dst,
+                     cudaStream_t st, Profiler* prof);
 
 // ---- step plans (gg_step_plan_create) ----
 // One thread per record: descs[j] takes the 12 doubles at T[j] as its transform (transform = 1) when T[j] is given, and

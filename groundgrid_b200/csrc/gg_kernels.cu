@@ -2564,46 +2564,135 @@ int launch_init_map(const View& v, int slot, float z, cudaStream_t st) {
 // with all of a slot's layers in flight at once.  A masked-off record costs one mask load per block; its block 0 seeds
 // a host-owned position into the table, as k_pose_resolve does, since the host counts the slot's position as
 // device-owned afterwards.
+// RESTORE (gg_restore_maps_from_device) takes the map from a snapshot instead of a pose: "ground" and "groundpatch"
+// from the pool record, the other layers as k_init_map starts them (their values do not depend on z), the record's
+// position.  Every block checks the record's header itself, so a rejected record costs one 16-byte load per block;
+// block 0 writes the position and the status.  xyz and mask are not read, and the reset instantiations do not read
+// `pool`.
 constexpr int RESET_THREADS = 256;
 constexpr int RESET_VEC = 4;
 constexpr int RESET_CELLS = RESET_THREADS * RESET_VEC;
 
-template <bool VEC>
+template <bool VEC, bool RESTORE>
 __global__ void __launch_bounds__(RESET_THREADS) k_reset_maps(View v, PoseTables t, const SlotParams* __restrict__ batch, const int* __restrict__ bits,
-                                                              const double* __restrict__ xyz, const int32_t* __restrict__ mask) {
+                                                              const double* __restrict__ xyz, const int32_t* __restrict__ mask, SnapshotPool pool) {
     const int j = blockIdx.y;
     const SlotParams& p = batch[j];
     const int k = p.pos;
     const bool first = blockIdx.x == 0 && threadIdx.x == 0;
-    if (mask && mask[k] == 0) {
-        if (first && !(bits[j] & POSE_POSITION)) t.position[p.slot] = make_double2(p.px, p.py);
-        return;
+    const float* planes = nullptr;   // RESTORE: the record's "ground", then "groundpatch" at + n2p
+    if constexpr (RESTORE) {
+        const int idx = pool.index ? pool.index[k] : k;
+        int status = 0;
+        if (idx >= 0 && idx < pool.n_pool) {
+            const unsigned char* rec = pool.records + (size_t)idx * snapshot_bytes(v.k.N2);
+            const uint4 h = __ldg(reinterpret_cast<const uint4*>(rec));   // magic, version, cells_per_side, resolution
+            status = (h.x == GG_SNAPSHOT_MAGIC && h.y == GG_SNAPSHOT_VERSION && (int)h.z == v.k.N && h.w == pool.res_bits) ? 1 : -1;
+            planes = reinterpret_cast<const float*>(rec + SNAPSHOT_HEADER);
+            if (status == 1 && first) t.position[p.slot] = __ldg(reinterpret_cast<const double2*>(rec + 16));
+        }
+        if (first && pool.status) pool.status[k] = status;
+        if (status != 1) {
+            if (first && !(bits[j] & POSE_POSITION)) t.position[p.slot] = make_double2(p.px, p.py);
+            return;
+        }
+    } else {
+        if (mask && mask[k] == 0) {
+            if (first && !(bits[j] & POSE_POSITION)) t.position[p.slot] = make_double2(p.px, p.py);
+            return;
+        }
     }
     const int s = p.slot;
-    const float z = __double2float_rn(xyz[3 * k + 2]);
-    if (first) t.position[s] = make_double2(xyz[3 * k], xyz[3 * k + 1]);
+    const float z = RESTORE ? 0.0f : __double2float_rn(xyz[3 * k + 2]);
+    if (!RESTORE && first) t.position[s] = make_double2(xyz[3 * k], xyz[3 * k + 1]);
     const int N2 = v.k.N2;
     float* base = v.layer(s, 0);
     const int nl = v.n_layers;
     if (VEC) {
         const int c = blockIdx.x * RESET_CELLS + threadIdx.x * RESET_VEC;
         if (c >= N2) return;
+        float4 g, gp;   // RESTORE: both planes' loads in flight before the stores (N2p == N2 here)
+        if constexpr (RESTORE) {
+            g = __ldg(reinterpret_cast<const float4*>(planes + c));
+            gp = __ldg(reinterpret_cast<const float4*>(planes + N2 + c));
+        }
 #pragma unroll
         for (int l = 0; l < L_NUM; ++l) {
             if (l >= nl) break;
             const float f = init_value(l, z);
-            *reinterpret_cast<float4*>(base + (size_t)l * N2 + c) = make_float4(f, f, f, f);
+            float4 q = make_float4(f, f, f, f);
+            if constexpr (RESTORE) {
+                if (l == L_GROUND) q = g;
+                if (l == L_GROUNDPATCH) q = gp;
+            }
+            *reinterpret_cast<float4*>(base + (size_t)l * N2 + c) = q;
         }
     } else {
         const int c0 = blockIdx.x * RESET_CELLS + threadIdx.x;
+        if constexpr (RESTORE) {
+            const int n2p = snapshot_cells(N2);
 #pragma unroll
-        for (int l = 0; l < L_NUM; ++l) {
+            for (int u = 0; u < RESET_VEC; ++u) {
+                const int c = c0 + u * RESET_THREADS;
+                if (c < N2) {
+                    base[(size_t)L_GROUND * N2 + c] = __ldg(planes + c);
+                    base[(size_t)L_GROUNDPATCH * N2 + c] = __ldg(planes + n2p + c);
+                }
+            }
+        }
+#pragma unroll
+        for (int l = RESTORE ? L_OBSTACLES : 0; l < L_NUM; ++l) {
             if (l >= nl) break;
             const float f = init_value(l, z);
 #pragma unroll
             for (int u = 0; u < RESET_VEC; ++u) {
                 const int c = c0 + u * RESET_THREADS;
                 if (c < N2) base[(size_t)l * N2 + c] = f;
+            }
+        }
+    }
+}
+
+// Map snapshots (gg_save_maps_to_device): block (x, j) copies cells [x * RESET_CELLS, (x + 1) * RESET_CELLS) of both
+// planes of record j's slot into its snapshot, the padding cells past N2 as 0; threads 0-3 of block 0 write the header
+// (position from the table when the slot's position is device-owned).  16-byte loads and stores when N2 % 4 == 0 (the
+// layers and the record's planes are then 16-byte aligned), plain ones otherwise.  A masked-off record costs one mask
+// load per block.
+template <bool VEC>
+__global__ void __launch_bounds__(RESET_THREADS) k_save_maps(View v, PoseTables t, const SlotParams* __restrict__ batch, const int* __restrict__ bits,
+                                                             SnapshotDest dst) {
+    const int j = blockIdx.y;
+    const SlotParams& p = batch[j];
+    const int k = p.pos;
+    if (dst.mask && dst.mask[k] == 0) return;
+    const int N2 = v.k.N2, n2p = snapshot_cells(N2);
+    unsigned char* rec = dst.records + (size_t)k * snapshot_bytes(N2);
+    if (blockIdx.x == 0 && threadIdx.x < 4) {
+        uint4 h = make_uint4(0u, 0u, 0u, 0u);   // threads 2, 3: reserved
+        if (threadIdx.x == 0) h = make_uint4(GG_SNAPSHOT_MAGIC, GG_SNAPSHOT_VERSION, (uint32_t)v.k.N, dst.res_bits);
+        if (threadIdx.x == 1) {
+            const double2 q = (bits[j] & POSE_POSITION) ? t.position[p.slot] : make_double2(p.px, p.py);
+            h = make_uint4(__double2loint(q.x), __double2hiint(q.x), __double2loint(q.y), __double2hiint(q.y));
+        }
+        reinterpret_cast<uint4*>(rec)[threadIdx.x] = h;
+    }
+    const float* base = v.layer(p.slot, 0);
+    float* out = reinterpret_cast<float*>(rec + SNAPSHOT_HEADER);
+    if (VEC) {
+        const int c = blockIdx.x * RESET_CELLS + threadIdx.x * RESET_VEC;
+        if (c >= N2) return;
+        const float4 g = __ldg(reinterpret_cast<const float4*>(base + c));
+        const float4 gp = __ldg(reinterpret_cast<const float4*>(base + N2 + c));
+        *reinterpret_cast<float4*>(out + c) = g;
+        *reinterpret_cast<float4*>(out + N2 + c) = gp;
+    } else {
+        const int c0 = blockIdx.x * RESET_CELLS + threadIdx.x;
+#pragma unroll
+        for (int u = 0; u < RESET_VEC; ++u) {
+            const int c = c0 + u * RESET_THREADS;
+            if (c < n2p) {
+                out[c] = c < N2 ? __ldg(base + c) : 0.0f;
+                out[n2p + c] = c < N2 ? __ldg(base + N2 + c) : 0.0f;
             }
         }
     }
@@ -2942,10 +3031,31 @@ int launch_pose_resolve(const View& v, const PoseTables& t, SlotParams* batch, c
 int launch_reset_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const double* xyz, const int32_t* mask,
                       cudaStream_t st, Profiler* prof) {
     const dim3 grid(cdiv(v.k.N2, RESET_CELLS), count);
+    const SnapshotPool none{};
     if (v.k.N2 % RESET_VEC == 0)
-        GG_LAUNCH(K_RESET_MAPS, k_reset_maps<true><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, xyz, mask));
+        GG_LAUNCH(K_RESET_MAPS, k_reset_maps<true, false><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, xyz, mask, none));
     else
-        GG_LAUNCH(K_RESET_MAPS, k_reset_maps<false><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, xyz, mask));
+        GG_LAUNCH(K_RESET_MAPS, k_reset_maps<false, false><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, xyz, mask, none));
+    return 1;
+}
+
+int launch_restore_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const SnapshotPool& pool,
+                        cudaStream_t st, Profiler* prof) {
+    const dim3 grid(cdiv(v.k.N2, RESET_CELLS), count);
+    if (v.k.N2 % RESET_VEC == 0)
+        GG_LAUNCH(K_RESTORE_MAPS, k_reset_maps<true, true><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, nullptr, nullptr, pool));
+    else
+        GG_LAUNCH(K_RESTORE_MAPS, k_reset_maps<false, true><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, nullptr, nullptr, pool));
+    return 1;
+}
+
+int launch_save_maps(const View& v, const PoseTables& t, const SlotParams* batch, const int* bits, int count, const SnapshotDest& dst,
+                     cudaStream_t st, Profiler* prof) {
+    const dim3 grid(cdiv(snapshot_cells(v.k.N2), RESET_CELLS), count);
+    if (v.k.N2 % RESET_VEC == 0)
+        GG_LAUNCH(K_SAVE_MAPS, k_save_maps<true><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, dst));
+    else
+        GG_LAUNCH(K_SAVE_MAPS, k_save_maps<false><<<grid, RESET_THREADS, 0, st>>>(v, t, batch, bits, dst));
     return 1;
 }
 

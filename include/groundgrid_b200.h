@@ -325,6 +325,76 @@ typedef struct gg_device_configs {
  * _wait) first. */
 int gg_set_slot_configs_from_device(gg_handle h, int count, const int* slots, const gg_device_configs* configs, void* stream);
 
+/* ---- map snapshots in caller GPU memory ----
+ * The state a stream carries from scan to scan -- "ground", "groundpatch" and the map position that
+ * GroundGrid::initGroundGrid (src/GroundGrid.cpp:50-80) starts and GroundGrid::update rolls; SURVEY.md section 5,
+ * checkpoint / resume: "dump/load G, C, position" -- saved from `count` slots into DEVICE records and restored from a
+ * DEVICE pool, ordered on the caller's stream.  For callers that checkpoint perception state on the GPU (a simulator's
+ * environment save / restore, episodes that start from a warmed-up map, rollouts that branch one slot into many, resume
+ * from a file or on another GPU), which would otherwise wait on the host per slot and could not run inside a step plan.
+ * A snapshot of one slot is a fixed-size record of gg_map_snapshot_bytes(h) bytes, 16-byte aligned: this 64-byte header,
+ * then "ground" at byte 64 and "groundpatch" at byte 64 + 4 * N2p (N2p = N * N rounded up to a multiple of 4), each
+ * column-major like gg_get_layer, with its padding floats 0: snapshots of equal states are byte-identical.  The
+ * configuration is not part of a snapshot (gg_set_slot_config / gg_set_slot_configs_from_device carry it). */
+#define GG_SNAPSHOT_MAGIC 0x534d4747u   /* "GGMS" */
+#define GG_SNAPSHOT_VERSION 1
+typedef struct gg_map_snapshot {       /* 64-byte header; the planes follow it */
+    uint32_t magic, version;
+    int32_t cells_per_side;            /* N of the handle that wrote it */
+    float resolution;                  /* the handle's float resolution, bit for bit */
+    double position[2];                /* map position as exact doubles (device- or host-owned, whichever is current) */
+    uint32_t reserved[8];              /* written as 0 */
+} gg_map_snapshot;
+size_t gg_map_snapshot_bytes(gg_handle h);   /* 64 + 8 * N2p; 0 for a null handle */
+
+/* Record k of dst ([count][gg_map_snapshot_bytes], DEVICE, 16-byte aligned) receives the header and both planes of
+ *   slots[k] at that point of the slot's stream, plane bits unchanged (NaN payloads and -0 included), unless mask (DEVICE
+ *   int32 [count] or NULL, 4-byte aligned) is zero at k: that record is left untouched.  The position is taken from the
+ *   device position table when it is device-owned and from the host otherwise, so the call never waits on the host.  No
+ *   slot state changes.
+ * stream: cudaStream_t; NULL is the legacy default stream.  The contract of gg_get_layers_to_device: the work starts after
+ *   everything already enqueued on `stream` and on the stream groups of the slots, work enqueued on `stream` afterwards
+ *   sees the records complete, and nothing waits on the host except the flow control of the parameter staging ring.
+ * count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued and gg_kernel_launches unchanged:
+ *   GG_E_ARG   null handle, slots or dst; count > n_slots; a slot out of range or repeated; dst not 16-byte or mask not
+ *              4-byte aligned; dst overlapping the handle's layers or the mask; mask overlapping the handle's layers
+ *   GG_E_STATE a slot whose map is not initialised */
+int gg_save_maps_to_device(gg_handle h, int count, const int* slots, void* dst, const int32_t* mask, void* stream);
+
+typedef struct gg_map_restore {
+    const void* pool;      /* DEVICE [n_pool][gg_map_snapshot_bytes], 16-byte aligned (NULL allowed when n_pool == 0) */
+    int n_pool;
+    const int32_t* index;  /* DEVICE [count] or NULL (= k), 4-byte aligned: slots[k] is restored from pool[index[k]] when
+                              0 <= index[k] < n_pool */
+    int32_t* status;       /* DEVICE [count] or NULL, 4-byte aligned: 1 restored, 0 index out of range (untouched), -1 record
+                              rejected (untouched) */
+} gg_map_restore;
+
+/* Effect: slots[k] whose index names a record of the pool ends up bit-identical to gg_init_map(slots[k], px, py, any z)
+ *   followed by gg_set_layer("ground") and gg_set_layer("groundpatch") with the record's planes, run at the same point
+ *   of the slot's stream: every layer (GG_FLAG_FULL_LAYERS layers included) and the map position (px, py) as exact
+ *   doubles.  An index outside [0, n_pool) leaves the slot untouched, and so does a record whose magic or version is
+ *   not this header's, whose cells_per_side is not the handle's N or whose resolution bits are not the handle's: one bad
+ *   record must not fail a batch (status -1).  Many slots may restore the same record.
+ * stream: the contract of gg_init_maps_from_device: the work starts after everything already enqueued on `stream` and on
+ *   the stream groups of the slots, work enqueued on `stream` afterwards sees the restore and the status, nothing waits
+ *   on the host except the flow control of the parameter staging ring, and the pool and index are consumed by the first
+ *   kernel of each stream group, so a stream-ordered allocator may free or refill them on `stream` right after the call.
+ * Host state afterwards -- the host cannot see the index, so it is that of gg_init_maps_from_device with a mask, for every
+ *   slot of the call, restored or not: the map position is device-owned (the host calls listed at gg_get_map_position
+ *   wait for it); the stored device scan pose, point count and part counts are kept; the last scan's outputs stay
+ *   readable; gg_point_info_to_device is GG_E_STATE until the slot's next scan.  Slots bound to a step plan are accepted.
+ * Every slot must already have a map: to resume into a fresh handle, run gg_init_map or gg_init_maps_from_device (mask
+ *   NULL) first, in the same step plan if need be.
+ * count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued and gg_kernel_launches unchanged:
+ *   GG_E_ARG   null handle, slots or r; null pool with n_pool > 0; n_pool < 0; count > n_slots; a slot out of range or
+ *              repeated; pool not 16-byte, index or status not 4-byte aligned; pool, index or status overlapping the
+ *              handle's layers; status overlapping the pool or the index
+ *   GG_E_STATE a slot whose map is not initialised
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_restore_maps_from_device(gg_handle h, int count, const int* slots, const gg_map_restore* r, void* stream);
+
 /* A whole step -- resets, counts, poses and scans -- recorded once and replayed from caller GPU memory: see the step plans
  * (gg_step_plan_create) after gg_run_cloud_msgs_to_device. */
 
@@ -816,6 +886,7 @@ int gg_set_map_position(gg_handle h, int slot, double x, double y);
  * Later scans of a slot read what gg_set_layers_from_device wrote.  Moving a stream to another slot, handle or GPU:
  * gg_init_map at the old slot's map position, gg_set_slot_config with its configuration, then import "ground" and
  * "groundpatch" (the only layers a scan reads from the previous one): the slot then continues bit-identically.
+ * gg_save_maps_to_device / gg_restore_maps_from_device do the same without a host wait (the configuration aside).
  * count == 0 or n_names == 0 enqueues nothing and returns GG_OK.  Rejected with nothing enqueued:
  *   GG_E_ARG   null handle; null slots / names / buffer; count > n_slots; a slot out of range or repeated; a name
  *              repeated; n_names > 12; a buffer not 4-byte aligned or overlapping the handle's layers (e.g. a
@@ -946,6 +1017,28 @@ int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const 
 int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                      const gg_device_resets* resets, const gg_device_configs* configs,
                                      const gg_step_readouts* readouts, gg_step_plan* out);
+/* A step plan that also restores and saves map snapshots (gg_restore_maps_from_device, gg_save_maps_to_device).  The step
+ * is, by definition, this call sequence over the plan's slots in desc->scans order, each stage only when it is given:
+ *   1. gg_set_slot_configs_from_device(configs);
+ *   2. gg_init_maps_from_device(resets);
+ *   3. gg_restore_maps_from_device(&snaps->restore), when any field of snaps->restore is set;
+ *   4. the counts (or part counts), 5. the poses and 6. the scan, as in gg_step_plan_create_with_configs;
+ *   7. the read-outs;
+ *   8. gg_save_maps_to_device(snaps->save, snaps->save_mask), when either is set.
+ * Every replay is bit-identical to that sequence run on the buffers' contents at replay time: the pool, the index, the
+ * save mask and the slots' planes are read, and the status and the saved records written, at replay time.  A restore and
+ * a save on the same pool in one plan are allowed; the stage order defines them.  snaps NULL is exactly
+ * gg_step_plan_create_with_configs.  Validation: what gg_step_plan_create_with_configs validates and what the two calls
+ * validate, with the same codes.  A rejected plan leaves no plan, no bound slot, and the slots' state and
+ * gg_kernel_launches unchanged.  Each snapshot stage adds one kernel per stream group. */
+typedef struct gg_step_snapshots {
+    gg_map_restore restore;      /* step 3 */
+    void* save;                  /* step 8: DEVICE [count][gg_map_snapshot_bytes] or NULL */
+    const int32_t* save_mask;    /* DEVICE [count] or NULL */
+} gg_step_snapshots;
+int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
+                                       const gg_device_resets* resets, const gg_device_configs* configs,
+                                       const gg_step_snapshots* snaps, const gg_step_readouts* readouts, gg_step_plan* out);
 
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
