@@ -172,6 +172,7 @@ SCAN_DEVICE_POSE = 1   # GG_SCAN_DEVICE_POSE: the scan's origin / base_z come fr
 SCAN_DEVICE_COUNT = 2  # GG_SCAN_DEVICE_COUNT: n_points is the capacity; the scan runs on the slot's stored device count
 SCAN_DEVICE_PART_COUNTS = 4  # GG_SCAN_DEVICE_PART_COUNTS: merged scans only; each part's n_points is its capacity and the part
                              # runs on the slot's stored part count
+SCAN_DEVICE_MASK = 8   # GG_SCAN_DEVICE_MASK: the scan runs only if the slot's stored device scan mask is nonzero; else it is skipped
 
 
 class DevicePoses(C.Structure):
@@ -470,6 +471,9 @@ def load(build_if_missing=True):
         "gg_restore_maps_from_device": (i, [vp, i, vp, C.POINTER(MapRestore), vp]),
         "gg_step_plan_create_with_snapshots": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(DeviceConfigs),
                                                    C.POINTER(StepSnapshots), C.POINTER(StepReadouts), C.POINTER(vp)]),
+        "gg_set_scan_masks_from_device": (i, [vp, i, vp, vp, vp]),
+        "gg_step_plan_create_with_scan_masks": (i, [vp, C.POINTER(StepDesc), C.POINTER(StepParts), C.POINTER(DeviceResets), C.POINTER(DeviceConfigs),
+                                                    C.POINTER(StepSnapshots), C.POINTER(StepReadouts), vp, C.POINTER(vp)]),
         "gg_step_plan_launch": (i, [vp, vp]),
         "gg_step_plan_kernels": (i, [vp]),
         "gg_step_plan_destroy": (i, [vp]),
@@ -769,6 +773,31 @@ class GroundGridB200:
             with torch.cuda.stream(stream):
                 counts = counts.reshape(-1).to(torch.int32).contiguous()
         self.set_point_counts_from_device_ptrs(slots, counts.data_ptr() if count else None, stream.cuda_stream or None)
+
+    def set_scan_masks_from_device_ptrs(self, slots, mask_ptr, stream_ptr):
+        """gg_set_scan_masks_from_device with a raw device address (int32 [count]); stream_ptr None = the legacy default
+        stream."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        _check(self._l.gg_set_scan_masks_from_device(self._h, len(sl), _ptr(sl), mask_ptr, stream_ptr))
+
+    def set_scan_masks_from_device(self, slots, mask, stream=None):
+        """Which of the slots' next scans run, from a CUDA tensor (gg_set_scan_masks_from_device): scans run with
+        device_masks=True run where the slot's mask is nonzero and are skipped where it is 0 (the map, position and stored
+        inputs stay untouched, no output is written but a zero count, and the slot's last scan becomes an empty one).
+          mask   : int32 [count] (int64 or bool is converted on `stream`, without a host wait), on this handle's device
+          stream : torch.cuda.Stream the work is ordered on (default: the current stream).
+        The call returns without waiting for the device; `mask` may be freed or overwritten right after it when it belongs
+        to `stream` (another stream's tensor is marked in use on `stream`)."""
+        torch, dev, current, stream = self._layer_stream(stream)
+        count = len(slots)
+        if mask.device != dev or mask.numel() != count or mask.dtype not in (torch.int32, torch.int64, torch.bool):
+            raise ValueError(f"mask must be an int32, int64 or bool tensor of {count} entries on {dev}")
+        if stream != current:
+            mask.record_stream(stream)
+        if mask.dtype != torch.int32 or not mask.is_contiguous():
+            with torch.cuda.stream(stream):
+                mask = mask.reshape(-1).to(torch.int32).contiguous()
+        self.set_scan_masks_from_device_ptrs(slots, mask.data_ptr() if count else None, stream.cuda_stream or None)
 
     def set_part_counts_from_device_ptrs(self, slots, parts_per_slot, counts_ptr, stream_ptr):
         """gg_set_part_counts_from_device with a raw device address (int32 [count, parts_per_slot]); stream_ptr None = the
@@ -1216,14 +1245,17 @@ class GroundGridB200:
     def run_scans(self, descs, stop_after=0):
         _check(self._l.gg_run_scans(self._h, len(descs), descs, stop_after))
 
-    def run_scans_device(self, descs, dev_ptrs, stop_after=0, device_counts=False):
+    def run_scans_device(self, descs, dev_ptrs, stop_after=0, device_counts=False, device_masks=False):
         """dev_ptrs: device addresses (ints) of the per-scan clouds (32-byte records).  device_counts: flag every scan
-        GG_SCAN_DEVICE_COUNT (its n_points is then the capacity; set_point_counts_from_device stores the counts)."""
-        if device_counts and isinstance(descs, np.ndarray):
-            descs["flags"] |= SCAN_DEVICE_COUNT
-        elif device_counts:
+        GG_SCAN_DEVICE_COUNT (its n_points is then the capacity; set_point_counts_from_device stores the counts).
+        device_masks: flag every scan GG_SCAN_DEVICE_MASK (it runs only where set_scan_masks_from_device stored a nonzero
+        mask)."""
+        flags = (SCAN_DEVICE_COUNT if device_counts else 0) | (SCAN_DEVICE_MASK if device_masks else 0)
+        if flags and isinstance(descs, np.ndarray):
+            descs["flags"] |= flags
+        elif flags:
             for d in descs:
-                d.flags |= SCAN_DEVICE_COUNT
+                d.flags |= flags
         pp = (C.c_void_p * len(descs))(*dev_ptrs)
         _check(self._l.gg_run_scans_device(self._h, len(descs), _ptr(descs) if isinstance(descs, np.ndarray) else descs, pp, stop_after))
 
@@ -1238,7 +1270,7 @@ class GroundGridB200:
         _check(self._l.gg_run_scans_to_device(self._h, count, d, _ptr(pp), _ptr(op), int(select), counts_ptr, stream_ptr))
 
     def run_scans_to_device(self, clouds, slots, origins, base_z, labels=True, select="nonground", index=False, stream=None,
-                            device_counts=False):
+                            device_counts=False, device_masks=False):
         """One scan per slot on caller-owned CUDA tensors, results left in new CUDA tensors (gg_run_scans_to_device).
           clouds : contiguous CUDA tensors of 32-byte point records (e.g. float32 [n, 8] or uint8 [n * 32]), 16-byte aligned
           origins: [count][3] sensor positions in the map frame; base_z: one value or one per scan.  origins="device"
@@ -1249,6 +1281,8 @@ class GroundGridB200:
           stream : torch.cuda.Stream the work is ordered on (default: the current stream); the outputs are allocated on it.
           device_counts : each cloud's length is the scan's capacity, and the scan runs on the slot's stored device count
                    (set_point_counts_from_device, GG_SCAN_DEVICE_COUNT); the outputs are allocated at capacity.
+          device_masks : every scan runs only where the slot's stored scan mask is nonzero (set_scan_masks_from_device,
+                   GG_SCAN_DEVICE_MASK); a skipped scan leaves its map untouched, writes none of its outputs and counts 0.
         The call returns without waiting for the device.  Work enqueued on `stream` afterwards sees complete outputs, and
         the inputs may be freed right after the call when they were allocated on `stream` (other streams' inputs are
         marked in use on `stream`).  Returns DeviceOutputs."""
@@ -1259,7 +1293,7 @@ class GroundGridB200:
             if c.device != dev or not c.is_contiguous() or nbytes % 32:
                 raise ValueError(f"clouds must be contiguous tensors of 32-byte records on {dev}")
             n.append(nbytes // 32)
-        descs = self._device_descs(slots, n, origins, base_z, device_counts)
+        descs = self._device_descs(slots, n, origins, base_z, device_counts, device_masks)
         out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, clouds)
         self.run_scans_to_device_ptrs(descs, [c.data_ptr() for c in clouds], ptrs, sel,
                                       out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
@@ -1290,7 +1324,7 @@ class GroundGridB200:
         _check(self._l.gg_run_cloud_msgs_to_device(self._h, count, d, _ptr(msgs), _ptr(op), int(select), counts_ptr, stream_ptr))
 
     def run_cloud_msgs_to_device(self, payloads, point_step, field_offsets, T, slots, origins, base_z, labels=True, select="nonground",
-                                 index=False, stream=None, device_counts=False):
+                                 index=False, stream=None, device_counts=False, device_masks=False):
         """One sensor_msgs/PointCloud2 payload per slot, in caller-owned CUDA memory, unpacked and transformed to the map frame
         on the device and then run like run_scans_to_device (gg_run_cloud_msgs_to_device).
           payloads      : contiguous CUDA tensors of any dtype whose byte size is a multiple of the scan's point_step
@@ -1299,8 +1333,8 @@ class GroundGridB200:
           field_offsets : byte offsets of x, y, z, intensity, ring (-1 absent), one 5-tuple or one per scan
           T             : None (every payload in the map frame), an array [count, 3, 4] of lookupTransform("map", frame_id), or
                           a list with None entries
-        origins, base_z, labels, select, index, stream and device_counts (each payload's length is then the capacity) as
-        in run_scans_to_device.  Each payload may be freed right after the call when it was allocated on `stream` (other
+        origins, base_z, labels, select, index, stream, device_counts (each payload's length is then the capacity) and
+        device_masks as in run_scans_to_device.  Each payload may be freed right after the call when it was allocated on `stream` (other
         streams' payloads are marked in use on `stream`).  Returns DeviceOutputs."""
         torch, dev, stream, sel = self._device_call(select, index, stream)
         count = len(payloads)
@@ -1311,7 +1345,7 @@ class GroundGridB200:
             if c.device != dev or not c.is_contiguous() or step <= 0 or nbytes % step:
                 raise ValueError(f"payloads must be contiguous tensors on {dev} whose byte size is a multiple of point_step")
             n.append(int(nbytes // step))
-        descs = self._device_descs(slots, n, origins, base_z, device_counts)
+        descs = self._device_descs(slots, n, origins, base_z, device_counts, device_masks)
         out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, payloads)
         self.run_cloud_msgs_to_device_ptrs(descs, [c.data_ptr() for c in payloads], steps, field_offsets, T, ptrs, sel,
                                            out.counts.data_ptr() if out.counts is not None else None, stream.cuda_stream or None)
@@ -1329,7 +1363,7 @@ class GroundGridB200:
                                                           stream_ptr))
 
     def run_merged_cloud_msgs_to_device(self, payloads, point_step, field_offsets, T, slots, origins, base_z, labels=True,
-                                        select="nonground", index=False, stream=None, device_counts=False):
+                                        select="nonground", index=False, stream=None, device_counts=False, device_masks=False):
         """Scans made of several sensor_msgs/PointCloud2 payloads each (a multi-LiDAR rig), in caller-owned CUDA memory:
         every part is unpacked and transformed to the map frame on the device, the parts of a scan are concatenated in
         order in the slot's buffer, and the merged scans then run like run_scans_to_device
@@ -1340,7 +1374,8 @@ class GroundGridB200:
           field_offsets : byte offsets of x, y, z, intensity, ring (-1 absent), one 5-tuple or nested [k][p]
           T             : lookupTransform("map", frame_id) as a 3x4, one for every part or nested [k][p]; None: the part
                           is already in the map frame
-        origins (one cloudOrigin per merged scan), base_z, labels, select, index and stream as in run_scans_to_device.
+        origins (one cloudOrigin per merged scan), base_z, labels, select, index, stream and device_masks as in
+        run_scans_to_device.
           device_counts : each payload's length is its part's capacity, and each part runs on the slot's stored part count
                           (set_part_counts_from_device, GG_SCAN_DEVICE_PART_COUNTS); the outputs are allocated at capacity
         Each payload may be freed right after the call when it was allocated on `stream` (other streams' payloads are
@@ -1354,7 +1389,7 @@ class GroundGridB200:
                                            [[c.data_ptr() for c in scan] for scan in payloads], point_step, field_offsets, T)
         first = np.cumsum(n_parts) - n_parts
         n = [int(parts["n_points"][b:b + m].sum()) for b, m in zip(first, n_parts)]
-        descs = self._device_descs(slots, n, origins, base_z)
+        descs = self._device_descs(slots, n, origins, base_z, device_masks=device_masks)
         if device_counts:
             descs["flags"] |= SCAN_DEVICE_PART_COUNTS
         out, ptrs = self._device_outputs(torch, dev, stream, n, labels, sel, index, [c for scan in payloads for c in scan])
@@ -1368,7 +1403,7 @@ class GroundGridB200:
                   select="nonground", index=False, reset_xyz=None, reset_mask=None, layers=None, layer_images=None, terrain_images=False,
                   samples=None, sample_names=("ground", "groundpatch"), sample_mode="nearest", sample_cells=False, point_info=None,
                   tallies=None, parts=None, part_counts=None, configs=None, config_mask=None, restore_pool=None, restore_index=None,
-                  restore_status=False, save=None, save_mask=None):
+                  restore_status=False, save=None, save_mask=None, scan_mask=None):
         """One step of a fixed batch recorded once as a CUDA graph and replayed from these tensors (gg_step_plan_create).
         Its step is the call sequence set_point_counts_from_device(counts) -> update_poses_from_device(xy, T_base_from_map,
         pose_origins, pose_base_z) -> run_scans_to_device(clouds) / run_cloud_msgs_to_device(payloads), each part only when
@@ -1402,6 +1437,9 @@ class GroundGridB200:
                      restores after the resets and before the counts (gg_step_plan_create_with_snapshots)
           save, save_mask : True (a new tensor) or a CUDA uint8 [count, snapshot_bytes], and int32 [count] (or None: every
                      slot), as in save_maps_to_device: the step then ends with that call, into plan.saved
+          scan_mask : CUDA int32 [count] or None: which scans run, read at every replay.  The step then stores it with
+                     set_scan_masks_from_device just before the counts, and every scan is flagged device_masks
+                     (gg_step_plan_create_with_scan_masks)
         Read-outs: with any of these the step ends with a step 4 of read-out calls (gg_step_plan_create_with_readouts),
         whose results land in plan.readouts (PlanReadouts) at every replay:
           layers       : layer names, as get_layers_to_device
@@ -1476,7 +1514,7 @@ class GroundGridB200:
                 keep += [tp, Tarr]
                 if tp.any():
                     d.dev_T_map_from_frame = tp.ctypes.data
-        descs = self._device_descs(slots, n, origins, base_z, counts is not None)
+        descs = self._device_descs(slots, n, origins, base_z, counts is not None, scan_mask is not None)
         if part_counts is not None:
             descs["flags"] |= SCAN_DEVICE_PART_COUNTS
         sl = np.ascontiguousarray(slots, np.int32)
@@ -1520,7 +1558,14 @@ class GroundGridB200:
                 saved = torch.zeros((count, rb), dtype=torch.uint8, device=dev) if save is True else save
                 snap.save = dptr(saved, torch.uint8, (count, rb), "save")
                 snap.save_mask = dptr(save_mask, torch.int32, (count,), "save_mask")
-        if snap is not None:
+        if scan_mask is not None:
+            cc = None if configs is None else DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"),
+                                                            dptr(config_mask, torch.int32, (count,), "config_mask"))
+            _check(self._l.gg_step_plan_create_with_scan_masks(self._h, C.byref(d), None if sp is None else C.byref(sp),
+                                                               None if r is None else C.byref(r), None if cc is None else C.byref(cc),
+                                                               None if snap is None else C.byref(snap), None if ro_c is None else C.byref(ro_c),
+                                                               dptr(scan_mask, torch.int32, (count,), "scan_mask"), C.byref(p)))
+        elif snap is not None:
             cc = None if configs is None else DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"),
                                                             dptr(config_mask, torch.int32, (count,), "config_mask"))
             _check(self._l.gg_step_plan_create_with_snapshots(self._h, C.byref(d), None if sp is None else C.byref(sp),
@@ -1657,13 +1702,15 @@ class GroundGridB200:
         return torch, dev, (torch.cuda.current_stream(dev) if stream is None else stream), sel
 
     @staticmethod
-    def _device_descs(slots, n, origins, base_z, device_counts=False):
+    def _device_descs(slots, n, origins, base_z, device_counts=False, device_masks=False):
         count = len(n)
         descs = np.zeros(count, SCAN_DESC_DTYPE)
         descs["slot"] = np.asarray(slots, np.int32)
         descs["n_points"] = n
         if device_counts:   # n is the capacity; the slots' stored device counts (set_point_counts_from_device)
             descs["flags"] = SCAN_DEVICE_COUNT
+        if device_masks:    # the slots' stored scan masks (set_scan_masks_from_device)
+            descs["flags"] |= SCAN_DEVICE_MASK
         if isinstance(origins, str) and origins == "device":   # the slots' device scan poses (update_poses_from_device)
             descs["flags"] |= SCAN_DEVICE_POSE
             return descs

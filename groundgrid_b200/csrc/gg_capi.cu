@@ -295,6 +295,9 @@ struct SlotState {
     // gg_set_part_counts_from_device: parts_per_slot of the latest call, 0: no part counts stored since gg_init_map
     // (GG_SCAN_DEVICE_PART_COUNTS scans may run with up to that many parts)
     int stored_parts = 0;
+    // gg_set_scan_masks_from_device: the device holds a stored scan mask of the slot (GG_SCAN_DEVICE_MASK scans may run);
+    // gg_init_map forgets it, gg_init_maps_from_device and gg_restore_maps_from_device keep it
+    bool stored_mask = false;
     // gg_set_slot_configs_from_device: the slot's configuration lives in the device tables (ConfigTables, its private
     // detect table); gg_init_map keeps it, gg_set_slot_config / gg_set_config make the slot host-configured again
     bool device_config = false;
@@ -659,6 +662,8 @@ int check_slots(gg_handle h, int count, SlotList slots, const gg_point* const* c
             return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_POSE without a device scan pose since gg_init_map", slot);
         if ((slots.scans[i].flags & GG_SCAN_DEVICE_COUNT) && !h->slots[slot].stored_count)
             return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_COUNT without a stored count since gg_init_map", slot);
+        if ((slots.scans[i].flags & GG_SCAN_DEVICE_MASK) && !h->slots[slot].stored_mask)
+            return fail(GG_E_STATE, "slot %d: GG_SCAN_DEVICE_MASK without a stored scan mask since gg_init_map", slot);
         if (slots.scans[i].flags & GG_SCAN_DEVICE_PART_COUNTS) {
             if (!merged) return fail(GG_E_ARG, "scan %d: GG_SCAN_DEVICE_PART_COUNTS is only for gg_run_merged_cloud_msgs_to_device", i);
             if (!h->slots[slot].stored_parts)
@@ -679,6 +684,14 @@ int check_host_counts(int count, const gg_scan_desc* scans) {
     return GG_OK;
 }
 
+// The calls whose labels land on the host (gg_run_scans, gg_filter_cloud_batch[_begin]) reject GG_SCAN_DEVICE_MASK: the
+// host reads every scan's labels back, and cannot know which scans ran.
+int check_host_labels(int count, const gg_scan_desc* scans) {
+    for (int i = 0; i < count; ++i)
+        if (scans[i].flags & GG_SCAN_DEVICE_MASK) return fail(GG_E_ARG, "scan %d: GG_SCAN_DEVICE_MASK on a call whose labels land on the host", i);
+    return GG_OK;
+}
+
 // Every launch of a batch goes through here.  Per stream group with scans in the batch, on the group's stream: one
 // staging entry, fill(i, entry) for each of the group's scans i (it fills record entry.m and returns whether the record
 // needs the device), the copy of the entry, launch(entry, stream) (returns the number of kernels it launched, or a
@@ -689,7 +702,8 @@ int check_host_counts(int count, const gg_scan_desc* scans) {
 // Poses: when fill staged slot positions (e.position), a record of a slot whose position is device-owned, or of a scan
 // flagged GG_SCAN_DEVICE_POSE, is patched from the device tables by k_stage_poses right after the copy.  Counts: a scan
 // flagged GG_SCAN_DEVICE_COUNT takes its count from the slot's stored one (a merged scan flagged
-// GG_SCAN_DEVICE_PART_COUNTS takes its parts' counts in launch_part_rounds); when fill staged last-scan counts (e.count),
+// GG_SCAN_DEVICE_PART_COUNTS takes its parts' counts in launch_part_rounds), and a scan flagged GG_SCAN_DEVICE_MASK is
+// skipped when the slot's stored mask is 0 (k_stage_parts sees the skip too); when fill staged last-scan counts (e.count),
 // a non-empty record of a slot whose last count is device-owned takes that count.  Configurations: when fill staged
 // configurations (e.config), a record of a device-configured slot takes its constants from the device table (its
 // detect_tab, the slot's private table, is staged by fill_params).  Without such records (every all-host flow) nothing
@@ -712,6 +726,7 @@ int run_groups(gg_handle h, int count, SlotList slots, bool fenced, cudaStream_t
                     if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_POSE)) bits |= gg::POSE_ORIGIN;
                     if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_COUNT)) bits |= gg::POSE_COUNT;
                     if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_PART_COUNTS)) bits |= gg::POSE_PART_COUNTS;
+                    if (slots.scans && (slots.scans[i].flags & GG_SCAN_DEVICE_MASK)) bits |= gg::POSE_MASK;
                 }
                 if (e.count && h->slots[slots[i]].device_count && e.hp[e.m].n_points > 0) bits |= gg::POSE_LAST_COUNT;
                 if (e.config && h->slots[slots[i]].device_config) bits |= gg::POSE_CONFIG;
@@ -805,8 +820,8 @@ static_assert(GG_MAX_CLOUD_PARTS < kRing, "the part rounds of a group must fit i
 // group's stream `st`: round p is one launch of the unpack kernel over part p of every scan of the group, record j of its
 // staging entry being part p of the entry's scan j (n_points 0 when the scan has no such part), each landing in its
 // slot's buffer after the scan's parts before p.  A round with no part to read is not launched.  When scans of the entry
-// take device part counts (POSE_PART_COUNTS), k_stage_parts resolves their round records once every round's entry is
-// copied, before the first round (the bits are those run_groups wrote for e: run_scans_grouped stages positions, so every
+// take device part counts (POSE_PART_COUNTS) or may be skipped (POSE_MASK), k_stage_parts resolves their round records once
+// every round's entry is copied, before the first round (the bits are those run_groups wrote for e: run_scans_grouped stages positions, so every
 // record of a scan entry has them).  While a step is recorded the rounds' entries come from the group's block.  Returns
 // the number of launches, or a negative error code.
 int launch_part_rounds(gg_handle h, const Staging& e, const CallerOutputs& c, cudaStream_t st) {
@@ -814,7 +829,7 @@ int launch_part_rounds(gg_handle h, const Staging& e, const CallerOutputs& c, cu
     bool resolve = false;
     for (int j = 0; j < e.m; ++j) {
         rounds = std::max(rounds, c.n_parts[e.hp[j].pos]);
-        resolve = resolve || (e.hbits[j] & gg::POSE_PART_COUNTS);
+        resolve = resolve || (e.hbits[j] & (gg::POSE_PART_COUNTS | gg::POSE_MASK));
     }
     const int g = stream_index(h, e.hp[0].slot);
     Staging r[GG_MAX_CLOUD_PARTS];
@@ -908,7 +923,8 @@ int run_scans_grouped(gg_handle h, int count, const gg_scan_desc* scans, int sto
         s.scan_points = d.n_points;
         s.moved_since_scan = false;
         s.device_rolled = false;
-        s.device_count = (d.flags & (GG_SCAN_DEVICE_COUNT | GG_SCAN_DEVICE_PART_COUNTS)) != 0;   // a host-count scan makes the count host-owned again
+        // a host-count scan makes the count host-owned again; a masked scan's count is 0 or not, as only the device knows
+        s.device_count = (d.flags & (GG_SCAN_DEVICE_COUNT | GG_SCAN_DEVICE_PART_COUNTS | GG_SCAN_DEVICE_MASK)) != 0;
         return true;
     };
     auto launch = [&](const Staging& e, cudaStream_t st) {
@@ -963,6 +979,7 @@ enum Tables : unsigned {
     T_OUT_CLOUD = 1u << 4,      // the output cloud of gg_get_output
     T_IMAGE_RANGES = 1u << 5,   // per-block range scratch of the layer images (launch_layer_images)
     T_CONFIGS = 1u << 6,        // ConfigTables (the private detect tables: ensure_config_tables)
+    T_SCAN_MASKS = 1u << 7,     // CountTables::mask
 };
 
 // Makes the handle's device current and allocates the buffers of `need` that are missing.
@@ -975,6 +992,7 @@ int ensure_tables(gg_handle h, unsigned need) {
     if ((need & T_STORED_COUNTS) && (rc = dev(&h->counts.stored, S))) return rc;
     if ((need & T_LAST_COUNTS) && (rc = dev(&h->counts.last, S))) return rc;
     if ((need & T_PART_COUNTS) && (rc = dev(&h->counts.parts, S * GG_MAX_CLOUD_PARTS))) return rc;
+    if ((need & T_SCAN_MASKS) && (rc = dev(&h->counts.mask, S))) return rc;
     if ((need & T_OUT_CLOUD) && (rc = dev(&h->view.out_cloud, S * h->pcap))) return rc;
     if ((need & T_IMAGE_RANGES) && (rc = dev(&h->d_img_part, S * gg::L_NUM * ((h->view.k.N2 + gg::IMG_RANGE_CELLS - 1) / gg::IMG_RANGE_CELLS))))
         return rc;
@@ -1551,7 +1569,7 @@ int gg_run_scans(gg_handle h, int count, const gg_scan_desc* scans, int stop_aft
     if (!h || !scans) return fail(GG_E_ARG, "null argument");
     if (stop_after < 0 || stop_after > 3) return fail(GG_E_ARG, "stop_after must be 0..3");
     int rc;
-    if ((rc = check_host_counts(count, scans))) return rc;
+    if ((rc = check_host_counts(count, scans)) || (rc = check_host_labels(count, scans))) return rc;
     h->inputs_busy = true;
     GG_CUDA(cudaSetDevice(h->device));
     return run_scans_grouped(h, count, scans, stop_after);
@@ -2162,7 +2180,7 @@ int gg_filter_cloud_batch_begin(gg_handle h, int count, const gg_scan_desc* scan
     if (!h || !scans || !points) return fail(GG_E_ARG, "null argument");
     if (count < 0) return fail(GG_E_ARG, "negative count");
     int rc;
-    if ((rc = check_host_counts(count, scans))) return rc;
+    if ((rc = check_host_counts(count, scans)) || (rc = check_host_labels(count, scans))) return rc;
     if ((rc = check_slots(h, count, scans, points))) return rc;
     for (int i = 0; i < count; ++i)
         if ((rc = check_unbound(h, scans[i].slot, "gg_filter_cloud_batch[_begin]"))) return rc;
@@ -2765,7 +2783,25 @@ int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, co
         h->slots[slots[i]].stored_count = true;
         return true;
     };
-    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_store_counts(h->counts, e.dp, e.m, dev_n_points, st, h->prof); };
+    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_store_counts(h->counts.stored, e.dp, e.m, dev_n_points, st, h->prof); };
+    return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
+}
+
+// Scan masks from device memory: per stream group one k_store_counts over the group's slots, into the mask table.
+int gg_set_scan_masks_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_mask, void* stream) {
+    int rc;
+    if ((rc = check_slot_batch(h, count, slots, 0, nullptr, {{dev_mask, (size_t)count * sizeof(int32_t), alignof(int32_t), true, "dev_mask", CallerBuf::INPUT}},
+                               nullptr, nullptr)) ||
+        count == 0)
+        return rc;
+    // a flagged scan writes the slot's last count (k_stage_poses), so the table of last counts comes with the masks
+    if ((rc = ensure_tables(h, T_SCAN_MASKS | T_LAST_COUNTS))) return rc;
+    auto fill = [&](int i, Staging& e) {
+        e.record(slots[i], i);
+        h->slots[slots[i]].stored_mask = true;
+        return true;
+    };
+    auto launch = [&](const Staging& e, cudaStream_t st) { return gg::launch_store_counts(h->counts.mask, e.dp, e.m, dev_mask, st, h->prof); };
     return run_groups(h, count, slots, true, static_cast<cudaStream_t>(stream), fill, launch);
 }
 
@@ -3022,21 +3058,23 @@ struct SnapshotCalls {
     }
 };
 
-// The calls a plan's step records: the configurations, resets, restore, counts (or part counts) and poses when given, the
-// scans, the read-outs, and the save when given.
+// The calls a plan's step records: the configurations, resets, restore, scan masks, counts (or part counts) and poses when
+// given, the scans, the read-outs, and the save when given.
 int step_calls(const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-               const gg_step_snapshots* snaps, const gg_step_readouts* readouts) {
+               const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const int32_t* scan_mask) {
     const gg_device_poses& q = d.poses;
     const SnapshotCalls sc(snaps);
-    return (configs != nullptr) + (resets != nullptr) + sc.restore + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) +
+    return (configs != nullptr) + (resets != nullptr) + sc.restore + (scan_mask != nullptr) + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) +
            (q.xy || q.T_base_from_map || q.origin || q.base_z) + 1 + ReadoutCalls(readouts).count() + sc.save;
 }
 
-// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_snapshots): per branch the restore of
+// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_scan_masks): per branch the restore of
 // its records and, where a payload takes a device transform, the transform staging; then the step's calls, the
-// configurations, the resets and the restore (when given) first, then the read-outs, and the save (when given) last.
+// configurations, the resets, the restore and the scan masks (when given) first, then the read-outs, and the save (when
+// given) last.
 int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const std::vector<int>& slots, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
+                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const int32_t* scan_mask, const std::vector<int>& slots,
+                const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
     PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
@@ -3056,6 +3094,7 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     if (resets && (rc = gg_init_maps_from_device(h, n, sl, resets, root))) return rc;
     const SnapshotCalls sc(snaps);
     if (sc.restore && (rc = gg_restore_maps_from_device(h, n, sl, &snaps->restore, root))) return rc;
+    if (scan_mask && (rc = gg_set_scan_masks_from_device(h, n, sl, scan_mask, root))) return rc;
     if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
     if (parts && parts->dev_part_counts && (rc = gg_set_part_counts_from_device(h, n, sl, parts->parts_per_slot, parts->dev_part_counts, root)))
         return rc;
@@ -3085,9 +3124,9 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
 // Everything the recorded kernels address that the step's calls would allocate on first use, and the spiral's shared
 // memory opt-in: a recording may not allocate, and the View it records must not change afterwards.
 int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_configs* configs, const gg_step_readouts* readouts) {
-    // the tables of the poses, counts and part counts whether or not the step records those calls (record_plan seeds the
+    // the tables of the poses, counts, part counts and scan masks whether or not the step records those calls (record_plan seeds the
     // positions), and the output cloud
-    unsigned need = T_POSES | T_STORED_COUNTS | T_LAST_COUNTS | T_PART_COUNTS | T_OUT_CLOUD;
+    unsigned need = T_POSES | T_STORED_COUNTS | T_LAST_COUNTS | T_PART_COUNTS | T_SCAN_MASKS | T_OUT_CLOUD;
     if (ReadoutCalls(readouts).images) need |= T_IMAGE_RANGES;
     int rc;
     if ((rc = ensure_tables(h, need))) return rc;
@@ -3104,8 +3143,8 @@ int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_config
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
 int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, gg_step_plan p) {
-    const int count = d.count, calls = step_calls(d, parts, resets, configs, snaps, readouts);
+                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const int32_t* scan_mask, gg_step_plan p) {
+    const int count = d.count, calls = step_calls(d, parts, resets, configs, snaps, readouts, scan_mask);
     std::vector<int>& slots = p->slots;
     slots.resize(count);
     for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
@@ -3190,7 +3229,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, parts, resets, configs, snaps, readouts, slots, T_group, root, fork, p);
+        rc = record_step(h, d, parts, resets, configs, snaps, readouts, scan_mask, slots, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -3268,6 +3307,12 @@ int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, cons
 int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
                                        const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
                                        gg_step_plan* out) {
+    return gg_step_plan_create_with_scan_masks(h, desc, parts, resets, configs, snaps, readouts, nullptr, out);
+}
+
+int gg_step_plan_create_with_scan_masks(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                        const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
+                                        const int32_t* dev_scan_mask, gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
     if (!h || !desc) return fail(GG_E_ARG, "null argument");
@@ -3277,7 +3322,7 @@ int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, co
     if ((rc = prepare_recording(h, *desc, configs, readouts))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, parts, resets, configs, snaps, readouts, p))) {
+    if ((rc = record_plan(h, *desc, parts, resets, configs, snaps, readouts, dev_scan_mask, p))) {
         free_plan(p);
         return rc;
     }

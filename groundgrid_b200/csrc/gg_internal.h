@@ -90,6 +90,9 @@ struct SlotParams {
     // and the layer "points" names for the slot (LAYER_POINTS); appended, so the fields above keep their offsets
     int pos;
     int points_layer;
+    // a scan of GG_SCAN_DEVICE_MASK whose slot's stored mask is 0 (set by k_stage_poses, with n_points 0): every kernel
+    // of the scan returns at entry for it; appended, so the fields above keep their offsets
+    int skip;
 };
 
 // Per-scan destinations of the output kernels (launch_output).  They sit in the staging entry next to the scans'
@@ -551,6 +554,8 @@ enum PoseBits : int {
                             // its parts' counts and offsets from the slot's stored part counts
     POSE_CONFIG = 32,    // cfg from the slot's entry of ConfigTables::cfg (the slot is device-configured; its detect_tab
                          // is staged from the host: the slot's private table)
+    POSE_MASK = 64,      // a scan of GG_SCAN_DEVICE_MASK: skip = (the slot's stored mask == 0); a skipped scan runs on 0 points,
+                         // and the slot's last count becomes the scan's resolved count (0 when skipped)
 };
 // The handle's per-slot configurations from device memory (allocated on the first gg_set_slot_configs_from_device).
 struct ConfigTables {
@@ -568,6 +573,8 @@ struct CountTables {
     int32_t* last;       // [n_slots] the count the slot's last GG_SCAN_DEVICE_COUNT scan ran on
     int32_t* parts;      // [n_slots][GG_MAX_CLOUD_PARTS] the latest part counts gg_set_part_counts_from_device stored
                          // (allocated on its first call)
+    int32_t* mask;       // [n_slots] the latest scan mask gg_set_scan_masks_from_device stored, as the caller gave it
+                         // (allocated on its first call)
 };
 // Patches the `count` records of batch whose bits ask for it from the tables; runs after the entry's copy and before
 // the kernels that read it.
@@ -580,8 +587,9 @@ int launch_stage_poses(const PoseTables& t, const CountTables& c, const CfgConst
 // each reconfigured record's detect table is rebuilt from t.cfg; the blocks of the other records exit after one load.
 int launch_store_configs(const View& v, const ConfigTables& t, SlotParams* batch, int count, const gg_config* cfg, const int32_t* mask,
                          cudaStream_t st, Profiler* prof);
-// One thread per record: the count of batch[j] (at dev_n[batch[j].pos]) into the slot's entry of c.stored.
-int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof);
+// One thread per record: the count of batch[j] (at dev_n[batch[j].pos]) into the slot's entry of `table` (c.stored for
+// gg_set_point_counts_from_device, c.mask for gg_set_scan_masks_from_device).
+int launch_store_counts(int32_t* table, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof);
 // One thread per record: the parts_per_slot part counts of batch[j] (at dev_n[batch[j].pos * parts_per_slot]) into the
 // slot's row of c.parts.
 int launch_store_part_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, int parts_per_slot, cudaStream_t st,
@@ -595,8 +603,9 @@ struct PartRounds {
 };
 // One thread per record of the scan entry whose bits hold POSE_PART_COUNTS: per part p the count u_p = v_p if
 // 0 <= v_p <= capacity, else 0 (v_p: the slot's stored part count), written into round p's record with the offset
-// u_0 + ... + u_{p-1}; the scan record's n_points and the slot's last count become the sum.  Runs after the entries'
-// copies and before the rounds.
+// u_0 + ... + u_{p-1}; the scan record's n_points and the slot's last count become the sum.  A record that k_stage_poses
+// skipped (POSE_MASK) gets u_p = 0 for every part, so no part of it is unpacked.  Runs after k_stage_poses and the
+// entries' copies, and before the rounds.
 int launch_stage_parts(const CountTables& c, SlotParams* batch, const int* bits, int count, const PartRounds& rounds, cudaStream_t st,
                        Profiler* prof);
 // The poses of one gg_update_poses_from_device call (entry batch[j].pos of each array); null xy: no roll, null origin:

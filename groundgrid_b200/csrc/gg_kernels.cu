@@ -436,6 +436,7 @@ __device__ __forceinline__ void load_tile_counts(const unsigned long long* cnt64
 __global__ void __launch_bounds__(CT_THREADS) k_cell_tiles(View v, const SlotParams* __restrict__ batch) {
     __shared__ int s_cls[AGG_STRIDE];
     const SlotParams& sp = batch[blockIdx.y];
+    if (sp.skip) return;
     const int N2 = v.k.N2, tid = threadIdx.x, lane = tid & 31;
     if (tid < AGG_STRIDE) s_cls[tid] = 0;
     __syncthreads();
@@ -458,6 +459,7 @@ __global__ void __launch_bounds__(CT_THREADS) k_cell_place(View v, const SlotPar
     __shared__ int s_cur[AGG_STRIDE];   // worklist cursor of every class for this tile; [WL_CLASSES]: first segment start of the tile
     __shared__ int s_warp[CT_THREADS / 32];
     const SlotParams& sp = batch[blockIdx.y];
+    if (sp.skip) return;
     const int N2 = v.k.N2, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tiles = v.cell_tiles, tile = blockIdx.x;
     const int* agg = v.cell_agg + (size_t)sp.slot * tiles * AGG_STRIDE;
@@ -578,6 +580,7 @@ __device__ __forceinline__ float raw_count(int r) { return (float)min(r, 1 << 24
 template <bool FULL>
 __global__ void __launch_bounds__(CS_THREADS, FULL ? 2 : 4) k_cell_stats(View v, const SlotParams* __restrict__ batch) {
     const SlotParams& sp = batch[blockIdx.y];
+    if (sp.skip) return;   // a skipped scan: not even the per-scan resets
     const Const& k = v.k;
     const size_t coff = (size_t)sp.slot * k.N2;
     const int gt = blockIdx.x * CS_THREADS + threadIdx.x;
@@ -949,6 +952,7 @@ __device__ __forceinline__ bool detect_patch(const CfgConst& kc, const float (*s
 __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_ldg(View v, const SlotParams* __restrict__ batch, int count_layer, bool recompute) {
     __shared__ float sP[DT_R][DT_W], sPV[DT_R][DT_W], sPM[DT_R][DT_W], sM[DT_R][DT_W];
     const SlotParams& sp = batch[blockIdx.z];
+    if (sp.skip) return;
     const Const& k = v.k;
     const CfgConst& kc = sp.cfg;
     const int N = k.N;
@@ -1166,6 +1170,7 @@ __global__ void __launch_bounds__(DT_X* DT_Y, 5) k_detect_tma(View v, const Slot
     __shared__ __align__(8) uint64_t s_bar[2];
     __shared__ float4 s_stage[DT_X * DT_Y];   // skew_store_tile
     const SlotParams& sp = batch[blockIdx.z];
+    if (sp.skip) return;   // before the barriers' init and the first TMA load
     const Const& k = v.k;
     const CfgConst& kc = sp.cfg;
     const int N = k.N, N2 = k.N2;
@@ -1347,6 +1352,7 @@ int launch_build_detect_table(const View& v, const CfgConst& c, float4* tab, cud
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SPIRAL_THREADS) k_spiral(View v, const SlotParams* __restrict__ batch) {
     const SlotParams& sp = batch[blockIdx.x];
+    if (sp.skip) return;
     const Const& k = v.k;
     const CfgConst& kc = sp.cfg;
     const int N = k.N;
@@ -1404,6 +1410,7 @@ __global__ void __launch_bounds__(THREADS) k_spiral_pipe(View v, const SlotParam
     const int L = v.levels;
     float2* xch = reinterpret_cast<float2*>(s_raw + (size_t)((L + 4) & ~3) * sizeof(int));  // [DIST + 1][THREADS]
     const SlotParams& sp = batch[blockIdx.x];
+    if (sp.skip) return;
     const Const& k = v.k;
     const int N = k.N;
     const int tid = threadIdx.x;
@@ -1775,6 +1782,9 @@ __device__ __forceinline__ void skew_irregular_thread(const View& v, const SlotP
 
 template <int MAXT, int MIN_CTAS = 1>
 __global__ void __launch_bounds__(MAXT, MIN_CTAS) k_spiral_skew(View v, const SlotParams* __restrict__ batch) {
+    // a skipped scan, tested first through the read-only path (a plain test after the shared-memory carve-up makes ptxas
+    // spill more in every instantiation; this placement spills less in three of the four)
+    if (__ldg(&batch[blockIdx.x].skip)) return;
     extern __shared__ __align__(16) unsigned char s_raw[];
     const SkewView& w = v.skew;
     // [ring: SKEW_RING levels x irr_chunks uint4][xch: SKEW_XCH_DEPTH x lanes float2][nb: irr_max*9 float2][dd: irr_max float]
@@ -2394,6 +2404,13 @@ __global__ void __launch_bounds__(POSE_THREADS) k_stage_poses(PoseTables t, Coun
         c.last[p.slot] = u;
     }
     if (b & POSE_LAST_COUNT) p.n_points = c.last[p.slot];
+    if (b & POSE_MASK) {
+        // a skipped scan runs on 0 points: the per-point kernels find nothing to do, the others test skip at entry
+        const int skip = c.mask[p.slot] == 0;
+        p.skip = skip;
+        if (skip) p.n_points = 0;
+        c.last[p.slot] = p.n_points;
+    }
     if (b & POSE_POSITION) {
         const double2 q = t.position[p.slot];
         p.px = q.x;
@@ -2444,14 +2461,15 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_resolve(double res, PoseT
     if (in.moved) in.moved[k] = moved;
 }
 
-// Point counts from device memory (gg_set_point_counts_from_device): record j stores the caller's count of its slot.
-// Values are stored as given; k_stage_poses applies the capacity rule when a scan uses them.
-__global__ void __launch_bounds__(POSE_THREADS) k_store_counts(CountTables c, const SlotParams* __restrict__ batch, int count,
+// Point counts and scan masks from device memory (gg_set_point_counts_from_device, gg_set_scan_masks_from_device):
+// record j stores the caller's value of its slot into its slot's entry of `table`.  Values are stored as given;
+// k_stage_poses applies the capacity rule (counts) or tests for 0 (masks) when a scan uses them.
+__global__ void __launch_bounds__(POSE_THREADS) k_store_counts(int32_t* __restrict__ table, const SlotParams* __restrict__ batch, int count,
                                                                const int32_t* __restrict__ dev_n) {
     const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
     if (j >= count) return;
     const SlotParams& p = batch[j];
-    c.stored[p.slot] = dev_n[p.pos];
+    table[p.slot] = dev_n[p.pos];
 }
 
 // Part counts from device memory (gg_set_part_counts_from_device): record j stores the caller's part counts of its slot,
@@ -2489,8 +2507,11 @@ __global__ void __launch_bounds__(POSE_THREADS) k_store_configs(ConfigTables t, 
 __global__ void __launch_bounds__(POSE_THREADS) k_stage_parts(CountTables c, SlotParams* __restrict__ batch, const int* __restrict__ bits, int count,
                                                               PartRounds r) {
     const int j = blockIdx.x * POSE_THREADS + threadIdx.x;
-    if (j >= count || !(bits[j] & POSE_PART_COUNTS)) return;
+    if (j >= count) return;
+    const int b = bits[j];
     SlotParams& p = batch[j];
+    const bool skip = (b & POSE_MASK) && p.skip;   // k_stage_poses ran before: no part of a skipped scan is unpacked
+    if (!(b & POSE_PART_COUNTS) && !skip) return;
     const int32_t* stored = c.parts + (size_t)p.slot * GG_MAX_CLOUD_PARTS;
     int first = 0;   // <= the scan's capacity <= max_points: no overflow
 #pragma unroll 1
@@ -2499,7 +2520,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_stage_parts(CountTables c, Slo
         SlotParams& sp = r.params[q][j];
         const int cap = sp.n_points;
         int u = 0;
-        if (cap > 0) {
+        if (cap > 0 && !skip) {
             const int v = stored[q];
             u = (v >= 0 && v <= cap) ? v : 0;
         }
@@ -2976,8 +2997,8 @@ int launch_store_configs(const View& v, const ConfigTables& t, SlotParams* batch
     return 2;
 }
 
-int launch_store_counts(const CountTables& c, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof) {
-    GG_LAUNCH(K_STORE_COUNTS, k_store_counts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(c, batch, count, dev_n));
+int launch_store_counts(int32_t* table, const SlotParams* batch, int count, const int32_t* dev_n, cudaStream_t st, Profiler* prof) {
+    GG_LAUNCH(K_STORE_COUNTS, k_store_counts<<<cdiv(count, POSE_THREADS), POSE_THREADS, 0, st>>>(table, batch, count, dev_n));
     return 1;
 }
 

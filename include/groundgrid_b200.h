@@ -89,10 +89,15 @@ typedef struct gg_handle_s* gg_handle;
  *             GG_SCAN_DEVICE_PART_COUNTS: gg_run_merged_cloud_msgs_to_device only (every other call rejects it with
  *             GG_E_ARG): each part's n_points is its capacity and the part runs on the slot's stored part count
  *             (gg_set_part_counts_from_device);
+ *             GG_SCAN_DEVICE_MASK: the scan runs only if the slot's stored scan mask is nonzero, and is skipped --
+ *             map, inputs and outputs untouched -- if it is 0 (gg_set_scan_masks_from_device).  A roll is not a scan: to
+ *             hold a slot's roll as well, give it a non-finite xy in gg_update_poses_from_device (dev_moved = -1, map and
+ *             position untouched);
  *             the other bits are reserved and ignored (pass 0)                */
 #define GG_SCAN_DEVICE_POSE 1
 #define GG_SCAN_DEVICE_COUNT 2
 #define GG_SCAN_DEVICE_PART_COUNTS 4
+#define GG_SCAN_DEVICE_MASK 8
 typedef struct gg_scan_desc {
     int slot;
     int flags;
@@ -239,6 +244,42 @@ int gg_update_poses_from_device(gg_handle h, int count, const int* slots, const 
  * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
  * _wait) first. */
 int gg_set_point_counts_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_n_points, void* stream);
+
+/* ---- scan masks from caller GPU memory ----
+ * Which slots' next scans run, read from DEVICE memory, for batches whose sensors do not all deliver every step
+ * (LiDARs at different rates on one handle, dropped frames, a simulator's finished episodes).  In the reference a node
+ * that receives no cloud does nothing: filter_cloud never runs and the map keeps its state.  A scan of 0 points is not
+ * that: it still resets the per-scan layers, sets the centre cell and decays every confidence beyond sqrt(12) m by
+ * C / occupied_cells_decrease_factor, at the full cost of the spiral.
+ *   dev_mask : int32 [count], 4-byte aligned, on the handle's device; dev_mask[k] becomes the stored scan mask of
+ *              slots[k]: nonzero = scan, 0 = skip.
+ *   stream   : the contract of gg_set_point_counts_from_device: the work starts after everything already enqueued on
+ *              `stream` and on the stream groups of the slots, nothing waits on the host except the flow control of the
+ *              parameter staging ring, and `stream` may free or refill dev_mask right after the call.
+ * A scan whose gg_scan_desc sets GG_SCAN_DEVICE_MASK reads the latest stored mask of its slot in the slot's stream order;
+ * every later flagged scan reuses it until the next call stores another.  The flag is honoured by gg_run_scans_device,
+ * gg_run_scans_to_device, gg_run_cloud_msgs_to_device and gg_run_merged_cloud_msgs_to_device, together with
+ * GG_SCAN_DEVICE_POSE, GG_SCAN_DEVICE_COUNT, GG_SCAN_DEVICE_PART_COUNTS and any stop_after.  The calls whose labels land on
+ * the host -- gg_run_scans and gg_filter_cloud_batch[_begin] -- reject it with GG_E_ARG, and a flagged scan of a slot with
+ * no stored mask since its gg_init_map is GG_E_STATE, with nothing enqueued.
+ *   - a scanned slot (mask nonzero) ends up bit-identical, in every output and layer, to the same call without the flag;
+ *   - a skipped slot (mask 0) keeps every layer (GG_FLAG_FULL_LAYERS layers included), its map position and its stored
+ *     device scan pose, count and part counts bit-identical to before the call.  Its cloud or payload is never read, its
+ *     labels, index and cloud destinations are not written, and dev_counts[k] is written 0.  Its last scan becomes an
+ *     empty one: gg_get_output, gg_last_scan_points, gg_point_info_to_device, gg_eval_counts_to_device and
+ *     gg_eval_accumulate see 0 points, so tallies and point info cover only the scans that ran.
+ * The host cannot see the mask, so after a flagged scan the slot's last-scan count is device-owned, with every rule of
+ * GG_SCAN_DEVICE_COUNT (the host calls that need it wait for the slot's stream group), and the layer "points" names what
+ * the call's stop_after makes it name, scanned or not.  gg_init_map forgets the stored mask; gg_init_maps_from_device and
+ * gg_restore_maps_from_device keep it.  Slots bound to a step plan are accepted: the plan's flagged scans read the
+ * stored mask at replay time.
+ * count == 0 returns GG_OK and enqueues nothing.  Rejected with nothing enqueued:
+ *   GG_E_ARG   null handle, slots or dev_mask; count > n_slots; a slot out of range or repeated; dev_mask not 4-byte
+ *              aligned or overlapping the handle's layers
+ *   GG_E_STATE a slot whose map is not initialised
+ * As for every call: a gg_filter_cloud_batch_begin batch that touches the same slots needs a gg_synchronize (or its
+ * _wait) first. */
+int gg_set_scan_masks_from_device(gg_handle h, int count, const int* slots, const int32_t* dev_mask, void* stream);
 
 /* ---- map resets from caller GPU memory ----
  * GroundGrid::initGroundGrid (src/GroundGrid.cpp:50-80) for the slots a DEVICE mask picks, at DEVICE odometry poses,
@@ -1039,6 +1080,19 @@ typedef struct gg_step_snapshots {
 int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                        const gg_device_resets* resets, const gg_device_configs* configs,
                                        const gg_step_snapshots* snaps, const gg_step_readouts* readouts, gg_step_plan* out);
+/* A step plan whose scans run only where a device mask says so.  The step is that of gg_step_plan_create_with_snapshots
+ * with one more stage, gg_set_scan_masks_from_device(dev_scan_mask) over the plan's slots, just before the counts (step
+ * 4); every replay is bit-identical to that call sequence on the buffers' contents at replay time.  dev_scan_mask (DEVICE
+ * int32 [count], 4-byte aligned) only stores the masks: the scans that read them are those of desc->scans whose flags set
+ * GG_SCAN_DEVICE_MASK.  dev_scan_mask NULL is exactly gg_step_plan_create_with_snapshots; flagged scans then read the
+ * masks stored by standalone gg_set_scan_masks_from_device calls, also ones made after the plan's creation.  Validation:
+ * what gg_step_plan_create_with_snapshots validates and what gg_set_scan_masks_from_device validates, with the same codes;
+ * a rejected plan leaves no plan, no bound slot, and the slots' state and gg_kernel_launches unchanged.  The stage adds
+ * one kernel per stream group. */
+int gg_step_plan_create_with_scan_masks(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
+                                        const gg_device_resets* resets, const gg_device_configs* configs,
+                                        const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
+                                        const int32_t* dev_scan_mask, gg_step_plan* out);
 
 /* Streams.  Slots are bound to the handle's streams in contiguous groups (GG_STREAMS env,
  * default 4, capped by n_slots; 1 when the caller supplied a stream) and everything that
