@@ -241,7 +241,7 @@ class MapRestore(C.Structure):
 
 
 class StepSnapshots(C.Structure):
-    """gg_step_snapshots: a step plan's restore (step 3) and save (step 8) stages (gg_step_plan_create_with_snapshots)."""
+    """gg_step_snapshots: a step plan's restore (stage 3) and save (stage 9) stages (gg_step_plan_create_with_snapshots)."""
 
     _fields_ = [
         ("restore", MapRestore),
@@ -281,7 +281,7 @@ class StepParts(C.Structure):
 
 
 class StepReadouts(C.Structure):
-    """gg_step_readouts: the read-out calls of a step plan's step 4 (gg_step_plan_create_with_readouts); zero = not run."""
+    """gg_step_readouts: the read-out calls of a step plan's stage 8 (gg_step_plan_create_with_readouts); zero = not run."""
 
     _fields_ = [
         ("n_layer_names", C.c_int),
@@ -1440,7 +1440,7 @@ class GroundGridB200:
           scan_mask : CUDA int32 [count] or None: which scans run, read at every replay.  The step then stores it with
                      set_scan_masks_from_device just before the counts, and every scan is flagged device_masks
                      (gg_step_plan_create_with_scan_masks)
-        Read-outs: with any of these the step ends with a step 4 of read-out calls (gg_step_plan_create_with_readouts),
+        Read-outs: with any of these the step has a stage of read-out calls after the scan (gg_step_plan_create_with_readouts),
         whose results land in plan.readouts (PlanReadouts) at every replay:
           layers       : layer names, as get_layers_to_device
           layer_images : layer names, as layer_images_to_device
@@ -1558,32 +1558,12 @@ class GroundGridB200:
                 saved = torch.zeros((count, rb), dtype=torch.uint8, device=dev) if save is True else save
                 snap.save = dptr(saved, torch.uint8, (count, rb), "save")
                 snap.save_mask = dptr(save_mask, torch.int32, (count,), "save_mask")
-        if scan_mask is not None:
-            cc = None if configs is None else DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"),
-                                                            dptr(config_mask, torch.int32, (count,), "config_mask"))
-            _check(self._l.gg_step_plan_create_with_scan_masks(self._h, C.byref(d), None if sp is None else C.byref(sp),
-                                                               None if r is None else C.byref(r), None if cc is None else C.byref(cc),
-                                                               None if snap is None else C.byref(snap), None if ro_c is None else C.byref(ro_c),
-                                                               dptr(scan_mask, torch.int32, (count,), "scan_mask"), C.byref(p)))
-        elif snap is not None:
-            cc = None if configs is None else DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"),
-                                                            dptr(config_mask, torch.int32, (count,), "config_mask"))
-            _check(self._l.gg_step_plan_create_with_snapshots(self._h, C.byref(d), None if sp is None else C.byref(sp),
-                                                              None if r is None else C.byref(r), None if cc is None else C.byref(cc),
-                                                              C.byref(snap), None if ro_c is None else C.byref(ro_c), C.byref(p)))
-        elif configs is not None:
-            cc = DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"), dptr(config_mask, torch.int32, (count,), "config_mask"))
-            _check(self._l.gg_step_plan_create_with_configs(self._h, C.byref(d), None if sp is None else C.byref(sp), None if r is None else C.byref(r),
-                                                            C.byref(cc), None if ro_c is None else C.byref(ro_c), C.byref(p)))
-        elif sp is not None:
-            _check(self._l.gg_step_plan_create_with_parts(self._h, C.byref(d), C.byref(sp), None if r is None else C.byref(r),
-                                                          None if ro_c is None else C.byref(ro_c), C.byref(p)))
-        elif ro_c is not None:
-            _check(self._l.gg_step_plan_create_with_readouts(self._h, C.byref(d), None if r is None else C.byref(r), C.byref(ro_c), C.byref(p)))
-        elif r is None:
-            _check(self._l.gg_step_plan_create(self._h, C.byref(d), C.byref(p)))
-        else:
-            _check(self._l.gg_step_plan_create_with_resets(self._h, C.byref(d), C.byref(r), C.byref(p)))
+        cc = None if configs is None else DeviceConfigs(dptr(configs, torch.uint8, (count, C.sizeof(Config)), "configs"),
+                                                        dptr(config_mask, torch.int32, (count,), "config_mask"))
+        _check(self._l.gg_step_plan_create_with_scan_masks(self._h, C.byref(d), None if sp is None else C.byref(sp),
+                                                           None if r is None else C.byref(r), None if cc is None else C.byref(cc),
+                                                           None if snap is None else C.byref(snap), None if ro_c is None else C.byref(ro_c),
+                                                           dptr(scan_mask, torch.int32, (count,), "scan_mask"), C.byref(p)))
         plan = StepPlan(self, p, out, mv, keep, ro)
         plan.restore_status, plan.saved = rstatus, saved
         return plan

@@ -13,6 +13,7 @@
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <initializer_list>
 #include <mutex>
 #include <string>
@@ -2985,17 +2986,99 @@ void free_plan(gg_step_plan p) {
     delete p;
 }
 
+// A plan's step as a gg_step_plan_create[_with_*] call gives it: desc, and each optional stage's argument or NULL.
+struct StepSpec {
+    const gg_step_desc* desc;
+    const gg_step_parts* parts = nullptr;
+    const gg_device_resets* resets = nullptr;
+    const gg_device_configs* configs = nullptr;
+    const gg_step_snapshots* snaps = nullptr;
+    const gg_step_readouts* readouts = nullptr;
+    const int32_t* scan_mask = nullptr;
+};
+
+// The calls a plan's step can record; step_stages gives their order.
+enum class Stage { CONFIGS, RESETS, RESTORE, SCAN_MASKS, COUNTS, PART_COUNTS, POSES, SCAN, LAYERS, IMAGES, TERRAIN, SAMPLES, POINT_INFO, EVAL, SAVE };
+
+// The stages of the step on slots `sl`, in the order of the header's list: for each stage given, issue(kind) says whether
+// to make its standalone call on `root` (record_step issues them all; record_plan counts them and prepare_recording looks
+// for the image read-out, issuing none).  A stage counts as given when any of its fields is set; its call then checks
+// them as it always does.  Returns the first error of a call.
+int step_stages(gg_handle h, const StepSpec& step, const int* sl, cudaStream_t root, const std::function<bool(Stage)>& issue) {
+    const gg_step_desc& d = *step.desc;
+    const int n = d.count;
+    const gg_device_poses& q = d.poses;
+    const gg_step_parts* pt = step.parts;
+    const gg_step_snapshots sn = step.snaps ? *step.snaps : gg_step_snapshots{};
+    const gg_map_restore& r = sn.restore;
+    const gg_step_readouts o = step.readouts ? *step.readouts : gg_step_readouts{};
+    auto on = [&](Stage kind, bool given) { return given && issue(kind); };
+    int rc;
+    if (on(Stage::CONFIGS, step.configs) && (rc = gg_set_slot_configs_from_device(h, n, sl, step.configs, root))) return rc;
+    if (on(Stage::RESETS, step.resets) && (rc = gg_init_maps_from_device(h, n, sl, step.resets, root))) return rc;
+    if (on(Stage::RESTORE, r.pool || r.n_pool || r.index || r.status) && (rc = gg_restore_maps_from_device(h, n, sl, &r, root))) return rc;
+    if (on(Stage::SCAN_MASKS, step.scan_mask) && (rc = gg_set_scan_masks_from_device(h, n, sl, step.scan_mask, root))) return rc;
+    if (on(Stage::COUNTS, d.dev_n_points) && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
+    if (on(Stage::PART_COUNTS, pt && pt->dev_part_counts) && (rc = gg_set_part_counts_from_device(h, n, sl, pt->parts_per_slot, pt->dev_part_counts, root)))
+        return rc;
+    if (on(Stage::POSES, q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, n, sl, &q, d.dev_moved, root)))
+        return rc;
+    if (on(Stage::SCAN, true)) {
+        rc = pt ? gg_run_merged_cloud_msgs_to_device(h, n, d.scans, pt->n_parts, pt->parts, d.outs, d.select, d.dev_counts, root)
+             : d.dev_points ? gg_run_scans_to_device(h, n, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root)
+                            : gg_run_cloud_msgs_to_device(h, n, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
+        if (rc) return rc;
+        // the payload records k_stage_transforms patches (the part rounds remember their own: PlanRecorder::Block::part)
+        for (PlanRecorder::Block& b : h->rec->blk)
+            if (!pt && b.per_call) b.scan = b.next - b.per_call;
+    }
+    if (on(Stage::LAYERS, o.n_layer_names || o.layer_names || o.layers) &&
+        (rc = gg_get_layers_to_device(h, n, sl, o.n_layer_names, o.layer_names, o.layers, root)))
+        return rc;
+    if (on(Stage::IMAGES, o.n_image_names || o.image_names || o.images || o.image_ranges) &&
+        (rc = gg_layer_images_to_device(h, n, sl, o.n_image_names, o.image_names, o.images, o.image_ranges, root)))
+        return rc;
+    if (on(Stage::TERRAIN, o.terrain_images) && (rc = gg_terrain_images_to_device(h, n, sl, o.terrain_images, root))) return rc;
+    if (on(Stage::SAMPLES, o.n_sample_names || o.sample_names || o.samples) &&
+        (rc = gg_sample_layers_to_device(h, n, sl, o.samples, o.n_sample_names, o.sample_names, o.sample_mode, root)))
+        return rc;
+    if (on(Stage::POINT_INFO, o.point_info) && (rc = gg_point_info_to_device(h, n, sl, o.point_info, root))) return rc;
+    if (on(Stage::EVAL, o.eval_counts) && (rc = gg_eval_counts_to_device(h, n, sl, o.eval_counts, root))) return rc;
+    if (on(Stage::SAVE, sn.save || sn.save_mask) && (rc = gg_save_maps_to_device(h, n, sl, sn.save, sn.save_mask, root))) return rc;
+    return GG_OK;
+}
+
+// A device transform entry of the step: scan `scan`'s payload (part -1), or part `part` of it; k counts the payloads,
+// or the parts over all scans.  dev is the device pointer, host the host transform it goes with.
+struct DeviceT {
+    int scan, part, k;
+    const double* dev;
+    const double* host;
+};
+
+// Every payload's entry of dev_T_map_from_frame, or every part's of dev_T_map_from_part; none when the plan has neither.
+std::vector<DeviceT> device_transforms(const StepSpec& step) {
+    const gg_step_desc& d = *step.desc;
+    const gg_step_parts* pt = step.parts;
+    std::vector<DeviceT> ts;
+    for (int i = 0, k = 0; pt && pt->dev_T_map_from_part && i < d.count; ++i)
+        for (int q = 0; q < pt->n_parts[i]; ++q, ++k) ts.push_back({i, q, k, pt->dev_T_map_from_part[k], pt->parts[k].msg.T_map_from_frame});
+    for (int i = 0; !pt && d.dev_T_map_from_frame && i < d.count; ++i) ts.push_back({i, -1, i, d.dev_T_map_from_frame[i], d.msgs[i].T_map_from_frame});
+    return ts;
+}
+
 // What gg_step_plan_create checks beyond the step's calls (those check their own arguments while the step is recorded).
-int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs) {
-    if (resets && !resets->xyz) return fail(GG_E_ARG, "resets without xyz");
-    if (configs && !configs->cfg) return fail(GG_E_ARG, "configs without cfg");
+int check_step_desc(gg_handle h, const StepSpec& step) {
+    const gg_step_desc& d = *step.desc;
+    if (step.resets && !step.resets->xyz) return fail(GG_E_ARG, "resets without xyz");
+    if (step.configs && !step.configs->cfg) return fail(GG_E_ARG, "configs without cfg");
     if (d.count <= 0) return fail(GG_E_ARG, "a step plan needs count > 0 scans, got %d", d.count);
     if (!d.scans) return fail(GG_E_ARG, "null scans");
     if (d.count > h->n_slots) return fail(GG_E_ARG, "count %d exceeds the number of slots %d", d.count, h->n_slots);
-    if (parts) {
+    if (step.parts) {
         if (d.dev_points || d.msgs || d.dev_T_map_from_frame || d.dev_n_points)
             return fail(GG_E_ARG, "a step plan with parts takes no dev_points, msgs, dev_T_map_from_frame or dev_n_points");
-        if (!parts->n_parts || !parts->parts) return fail(GG_E_ARG, "null n_parts or parts");
+        if (!step.parts->n_parts || !step.parts->parts) return fail(GG_E_ARG, "null n_parts or parts");
     } else {
         if (!d.dev_points == !d.msgs) return fail(GG_E_ARG, "a step plan takes exactly one of dev_points and msgs");
         if (d.dev_T_map_from_frame && !d.msgs) return fail(GG_E_ARG, "dev_T_map_from_frame needs msgs");
@@ -3005,76 +3088,27 @@ int check_step_desc(gg_handle h, const gg_step_desc& d, const gg_step_parts* par
         const int slot = d.scans[i].slot;
         if ((rc = check_slot(h, slot))) return rc;
         if (h->slot_plan[slot]) return fail(GG_E_STATE, "slot %d is already bound to a step plan", slot);
-        if (parts && (parts->n_parts[i] < 0 || parts->n_parts[i] > GG_MAX_CLOUD_PARTS))
-            return fail(GG_E_ARG, "scan %d: %d parts, not in [0, %d]", i, parts->n_parts[i], GG_MAX_CLOUD_PARTS);
+        if (step.parts && (step.parts->n_parts[i] < 0 || step.parts->n_parts[i] > GG_MAX_CLOUD_PARTS))
+            return fail(GG_E_ARG, "scan %d: %d parts, not in [0, %d]", i, step.parts->n_parts[i], GG_MAX_CLOUD_PARTS);
     }
-    // the device transforms: per payload (msgs) or per part, each with its host transform
-    std::vector<std::pair<const double*, const double*>> dev_host;
-    if (parts && parts->dev_T_map_from_part) {
-        for (int i = 0, at = 0; i < d.count; at += parts->n_parts[i++])
-            for (int q = 0; q < parts->n_parts[i]; ++q) dev_host.push_back({parts->dev_T_map_from_part[at + q], parts->parts[at + q].msg.T_map_from_frame});
-    } else if (!parts && d.dev_T_map_from_frame) {
-        for (int k = 0; k < d.count; ++k) dev_host.push_back({d.dev_T_map_from_frame[k], d.msgs[k].T_map_from_frame});
-    }
-    const char* what = parts ? "part" : "scan";   // k below counts the parts over all scans, or the scans
-    const char* name = parts ? "dev_T_map_from_part" : "dev_T_map_from_frame";
+    const char* what = step.parts ? "part" : "scan";
+    const char* name = step.parts ? "dev_T_map_from_part" : "dev_T_map_from_frame";
     std::vector<ByteRange> ts;   // every transform counts as an output: none may overlap another
-    for (size_t k = 0; k < dev_host.size(); ++k) {
-        const uintptr_t t = reinterpret_cast<uintptr_t>(dev_host[k].first);
-        if (!t) continue;
-        if (t % alignof(double)) return fail(GG_E_ARG, "%s %zu: %s is not 8-byte aligned", what, k, name);
-        if (dev_host[k].second) return fail(GG_E_ARG, "%s %zu: both a device and a host T_map_from_frame", what, k);
-        ts.push_back({t, t + 12 * sizeof(double), (int)k, true});
+    for (const DeviceT& t : device_transforms(step)) {
+        const uintptr_t a = reinterpret_cast<uintptr_t>(t.dev);
+        if (!a) continue;
+        if (a % alignof(double)) return fail(GG_E_ARG, "%s %d: %s is not 8-byte aligned", what, t.k, name);
+        if (t.host) return fail(GG_E_ARG, "%s %d: both a device and a host T_map_from_frame", what, t.k);
+        ts.push_back({a, a + 12 * sizeof(double), t.k, true});
     }
     const auto bad = find_overlap(ts);
     if (bad.first) return fail(GG_E_ARG, "the %s entries of %s %d and %s %d overlap", name, what, bad.first->set, what, bad.second->set);
     return GG_OK;
 }
 
-// Which calls of step 4 a plan's read-outs give (gg_step_plan_create_with_readouts): a call runs when any of its
-// fields is set, and then checks them as it always does.
-struct ReadoutCalls {
-    bool layers = false, images = false, terrain = false, samples = false, point_info = false, eval = false;
-    explicit ReadoutCalls(const gg_step_readouts* o) {
-        if (!o) return;
-        layers = o->n_layer_names || o->layer_names || o->layers;
-        images = o->n_image_names || o->image_names || o->images || o->image_ranges;
-        terrain = o->terrain_images != nullptr;
-        samples = o->n_sample_names || o->sample_names || o->samples;
-        point_info = o->point_info != nullptr;
-        eval = o->eval_counts != nullptr;
-    }
-    int count() const { return layers + images + terrain + samples + point_info + eval; }
-};
-
-// Which snapshot stages a plan's step records (gg_step_plan_create_with_snapshots): the restore when any field of
-// snaps->restore is set, the save when save or save_mask is; each call then checks its arguments as it always does.
-struct SnapshotCalls {
-    bool restore = false, save = false;
-    explicit SnapshotCalls(const gg_step_snapshots* s) {
-        if (!s) return;
-        restore = s->restore.pool || s->restore.n_pool || s->restore.index || s->restore.status;
-        save = s->save || s->save_mask;
-    }
-};
-
-// The calls a plan's step records: the configurations, resets, restore, scan masks, counts (or part counts) and poses when
-// given, the scans, the read-outs, and the save when given.
-int step_calls(const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-               const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const int32_t* scan_mask) {
-    const gg_device_poses& q = d.poses;
-    const SnapshotCalls sc(snaps);
-    return (configs != nullptr) + (resets != nullptr) + sc.restore + (scan_mask != nullptr) + (d.dev_n_points != nullptr) + (parts && parts->dev_part_counts) +
-           (q.xy || q.T_base_from_map || q.origin || q.base_z) + 1 + ReadoutCalls(readouts).count() + sc.save;
-}
-
-// The step of plan p, recorded on the capture root `root` (gg_step_plan_create_with_scan_masks): per branch the restore of
-// its records and, where a payload takes a device transform, the transform staging; then the step's calls, the
-// configurations, the resets, the restore and the scan masks (when given) first, then the read-outs, and the save (when
-// given) last.
-int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const int32_t* scan_mask, const std::vector<int>& slots,
-                const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
+// The step of plan p, recorded on the capture root `root`: per branch the restore of its records and, where a payload
+// takes a device transform, the transform staging; then the step's stages.
+int record_step(gg_handle h, const StepSpec& step, const std::vector<char>& T_group, cudaStream_t root, cudaEvent_t fork, gg_step_plan p) {
     PlanRecorder& r = *h->rec;
     GG_CUDA(cudaEventRecord(fork, root));
     for (int g : p->groups) {
@@ -3086,55 +3120,22 @@ int record_step(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         if (T_group[g])
             h->launches += gg::launch_stage_transforms(reinterpret_cast<gg::UnpackDesc*>(p->work + b.at + l.unpack), p->dev_T + b.first, b.calls * b.per_call, st);
     }
-    int rc;
-    const int n = d.count;
-    const int* sl = slots.data();
-    const gg_device_poses& q = d.poses;
-    if (configs && (rc = gg_set_slot_configs_from_device(h, n, sl, configs, root))) return rc;
-    if (resets && (rc = gg_init_maps_from_device(h, n, sl, resets, root))) return rc;
-    const SnapshotCalls sc(snaps);
-    if (sc.restore && (rc = gg_restore_maps_from_device(h, n, sl, &snaps->restore, root))) return rc;
-    if (scan_mask && (rc = gg_set_scan_masks_from_device(h, n, sl, scan_mask, root))) return rc;
-    if (d.dev_n_points && (rc = gg_set_point_counts_from_device(h, n, sl, d.dev_n_points, root))) return rc;
-    if (parts && parts->dev_part_counts && (rc = gg_set_part_counts_from_device(h, n, sl, parts->parts_per_slot, parts->dev_part_counts, root)))
-        return rc;
-    if ((q.xy || q.T_base_from_map || q.origin || q.base_z) && (rc = gg_update_poses_from_device(h, n, sl, &q, d.dev_moved, root))) return rc;
-    if (parts) {
-        // the part rounds remember their own records (PlanRecorder::Block::part)
-        rc = gg_run_merged_cloud_msgs_to_device(h, n, d.scans, parts->n_parts, parts->parts, d.outs, d.select, d.dev_counts, root);
-        if (rc) return rc;
-    } else {
-        rc = d.dev_points ? gg_run_scans_to_device(h, n, d.scans, d.dev_points, d.outs, d.select, d.dev_counts, root)
-                          : gg_run_cloud_msgs_to_device(h, n, d.scans, d.msgs, d.outs, d.select, d.dev_counts, root);
-        if (rc) return rc;
-        for (int g : p->groups) r.blk[g].scan = r.blk[g].next - r.blk[g].per_call;   // the payload records k_stage_transforms patches
-    }
-    const ReadoutCalls c(readouts);
-    const gg_step_readouts o = readouts ? *readouts : gg_step_readouts{};
-    if (c.layers && (rc = gg_get_layers_to_device(h, n, sl, o.n_layer_names, o.layer_names, o.layers, root))) return rc;
-    if (c.images && (rc = gg_layer_images_to_device(h, n, sl, o.n_image_names, o.image_names, o.images, o.image_ranges, root))) return rc;
-    if (c.terrain && (rc = gg_terrain_images_to_device(h, n, sl, o.terrain_images, root))) return rc;
-    if (c.samples && (rc = gg_sample_layers_to_device(h, n, sl, o.samples, o.n_sample_names, o.sample_names, o.sample_mode, root))) return rc;
-    if (c.point_info && (rc = gg_point_info_to_device(h, n, sl, o.point_info, root))) return rc;
-    if (c.eval && (rc = gg_eval_counts_to_device(h, n, sl, o.eval_counts, root))) return rc;
-    if (sc.save && (rc = gg_save_maps_to_device(h, n, sl, snaps->save, snaps->save_mask, root))) return rc;
-    return GG_OK;
+    return step_stages(h, step, p->slots.data(), root, [](Stage) { return true; });
 }
 
 // Everything the recorded kernels address that the step's calls would allocate on first use, and the spiral's shared
 // memory opt-in: a recording may not allocate, and the View it records must not change afterwards.
-int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_configs* configs, const gg_step_readouts* readouts) {
+int prepare_recording(gg_handle h, const StepSpec& step, const std::vector<int>& slots) {
     // the tables of the poses, counts, part counts and scan masks whether or not the step records those calls (record_plan seeds the
     // positions), and the output cloud
     unsigned need = T_POSES | T_STORED_COUNTS | T_LAST_COUNTS | T_PART_COUNTS | T_SCAN_MASKS | T_OUT_CLOUD;
-    if (ReadoutCalls(readouts).images) need |= T_IMAGE_RANGES;
+    step_stages(h, step, slots.data(), nullptr, [&](Stage kind) {
+        if (kind == Stage::IMAGES) need |= T_IMAGE_RANGES;
+        return false;
+    });
     int rc;
     if ((rc = ensure_tables(h, need))) return rc;
-    if (configs) {
-        std::vector<int> slots(d.count);
-        for (int i = 0; i < d.count; ++i) slots[i] = d.scans[i].slot;
-        if ((rc = ensure_config_tables(h, d.count, slots.data()))) return rc;
-    }
+    if (step.configs && (rc = ensure_config_tables(h, (int)slots.size(), slots.data()))) return rc;
     if (gg::prepare_scan_pipeline(h->view)) return fail(GG_E_CUDA, "spiral shared-memory opt-in: %s", cudaGetErrorString(cudaGetLastError()));
     return GG_OK;
 }
@@ -3142,33 +3143,33 @@ int prepare_recording(gg_handle h, const gg_step_desc& d, const gg_device_config
 // gg_step_plan_create after check_step_desc and prepare_recording: lays out the record blocks, seeds the positions,
 // records the step into p->graph, and leaves the slots' state as it found it (seeded positions aside) with the state a
 // step leaves in p->after.
-int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, const gg_device_resets* resets, const gg_device_configs* configs,
-                const gg_step_snapshots* snaps, const gg_step_readouts* readouts, const int32_t* scan_mask, gg_step_plan p) {
-    const int count = d.count, calls = step_calls(d, parts, resets, configs, snaps, readouts, scan_mask);
-    std::vector<int>& slots = p->slots;
-    slots.resize(count);
-    for (int i = 0; i < count; ++i) slots[i] = d.scans[i].slot;
-    // with parts: index in parts->parts of each scan's first part
-    std::vector<int> base(count, 0);
-    for (int i = 1; parts && i < count; ++i) base[i] = base[i - 1] + parts->n_parts[i - 1];
-    PlanRecorder rec;
+int record_plan(gg_handle h, const StepSpec& step, gg_step_plan p) {
+    const int count = step.desc->count;
+    const std::vector<int>& slots = p->slots;
+    int calls = 0;
+    step_stages(h, step, slots.data(), nullptr, [&](Stage) {
+        ++calls;
+        return false;
+    });
+    // per group its scans and the part rounds of its merged scans (an entry each), and each scan's row in its group
+    int per_call[kStreams] = {}, rounds[kStreams] = {};
+    std::vector<int> row(count);
+    for (int i = 0; i < count; ++i) {
+        const int g = stream_index(h, slots[i]);
+        row[i] = per_call[g]++;
+        if (step.parts) rounds[g] = std::max(rounds[g], step.parts->n_parts[i]);
+    }
+    const std::vector<DeviceT> ts = device_transforms(step);
     std::vector<char> T_group(kStreams, 0);
+    for (const DeviceT& t : ts)
+        if (t.dev) T_group[stream_index(h, slots[t.scan])] = 1;
+    PlanRecorder rec;
     size_t at = 0;
     for (int g = 0; g < h->n_streams; ++g) {
-        int c = 0, rounds = 0;   // the group's scans, and the part rounds of its merged scans (one entry each at most)
-        for (int i = 0; i < count; ++i)
-            if (stream_index(h, slots[i]) == g) {
-                ++c;
-                if (d.dev_T_map_from_frame && d.dev_T_map_from_frame[i]) T_group[g] = 1;
-                if (!parts) continue;
-                rounds = std::max(rounds, parts->n_parts[i]);
-                for (int q = 0; parts->dev_T_map_from_part && q < parts->n_parts[i]; ++q)
-                    if (parts->dev_T_map_from_part[base[i] + q]) T_group[g] = 1;
-            }
-        if (c == 0) continue;
+        if (per_call[g] == 0) continue;
         PlanRecorder::Block& b = rec.blk[g];
-        b.per_call = c;
-        b.calls = calls + rounds;
+        b.per_call = per_call[g];
+        b.calls = calls + rounds[g];
         b.first = rec.records;
         rec.records += b.calls * b.per_call;
         b.at = at;
@@ -3179,8 +3180,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->pristine), at));
     GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->work), at));
     rec.work = p->work;
-    const bool dev_T = d.dev_T_map_from_frame || (parts && parts->dev_T_map_from_part);
-    if (dev_T) GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->dev_T), (size_t)rec.records * sizeof(double*)));
+    if (!ts.empty()) GG_CUDA(cudaMalloc(reinterpret_cast<void**>(&p->dev_T), (size_t)rec.records * sizeof(double*)));
 
     // the slots' stream groups are idle from here on: nothing in flight reads or writes what is seeded below
     for (int g : p->groups) GG_CUDA(cudaStreamSynchronize(h->streams[g]));
@@ -3203,7 +3203,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     // with configurations, the slots become device-configured here (seeded, as a standalone call seeds them), so the
     // recorded call has nothing to seed; a rejected plan takes the seed launches back with the state
     const uint64_t seed_launches = h->launches;
-    for (int j = 0; configs && j < count; ++j) {
+    for (int j = 0; step.configs && j < count; ++j) {
         SlotState& s = h->slots[slots[j]];
         if (s.device_config) continue;
         if (int rc = seed_device_config(h, slots[j])) {
@@ -3229,7 +3229,7 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
         const uint64_t launches = h->launches;
         h->prof = nullptr;
         h->rec = &rec;
-        rc = record_step(h, d, parts, resets, configs, snaps, readouts, scan_mask, slots, T_group, root, fork, p);
+        rc = record_step(h, step, T_group, root, fork, p);
         h->rec = nullptr;
         h->prof = prof;
         p->kernels = (int)(h->launches - launches);
@@ -3258,22 +3258,16 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     }
     for (int j = 0; j < count; ++j) {
         h->slots[slots[j]].device_position = true;
-        if (configs) h->slots[slots[j]].device_config = true;
+        if (step.configs) h->slots[slots[j]].device_config = true;
     }
 
     // the records as recorded, the caller transforms of the payload records (row j of the scan entry, or of part round q's
     // entry, is the group's j-th scan), and the executable graph
     std::vector<const double*> T_rec(rec.records, nullptr);
-    for (int g : p->groups) {
-        const PlanRecorder::Block& b = rec.blk[g];
-        int j = 0;
-        for (int i = 0; i < count; ++i) {
-            if (stream_index(h, slots[i]) != g) continue;
-            if (!parts && d.dev_T_map_from_frame) T_rec[b.first + b.scan + j] = d.dev_T_map_from_frame[i];
-            for (int q = 0; parts && parts->dev_T_map_from_part && q < parts->n_parts[i]; ++q)
-                if (b.part[q] >= 0) T_rec[b.first + b.part[q] + j] = parts->dev_T_map_from_part[base[i] + q];
-            ++j;
-        }
+    for (const DeviceT& t : ts) {
+        const PlanRecorder::Block& b = rec.blk[stream_index(h, slots[t.scan])];
+        const int entry = t.part < 0 ? b.scan : b.part[t.part];
+        if (entry >= 0) T_rec[b.first + entry + row[t.scan]] = t.dev;
     }
     GG_CUDA(cudaMemcpy(p->pristine, rec.host.data(), at, cudaMemcpyHostToDevice));
     if (p->dev_T) GG_CUDA(cudaMemcpy(p->dev_T, T_rec.data(), T_rec.size() * sizeof(double*), cudaMemcpyHostToDevice));
@@ -3281,48 +3275,19 @@ int record_plan(gg_handle h, const gg_step_desc& d, const gg_step_parts* parts, 
     std::memcpy(&p->view, &h->view, sizeof(p->view));   // bytewise: gg_step_plan_launch compares it bytewise
     return GG_OK;
 }
-}  // namespace
 
-int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out) { return gg_step_plan_create_with_resets(h, desc, nullptr, out); }
-
-int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out) {
-    return gg_step_plan_create_with_readouts(h, desc, resets, nullptr, out);
-}
-
-int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, const gg_step_readouts* readouts,
-                                      gg_step_plan* out) {
-    return gg_step_plan_create_with_parts(h, desc, nullptr, resets, readouts, out);
-}
-
-int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
-                                   const gg_step_readouts* readouts, gg_step_plan* out) {
-    return gg_step_plan_create_with_configs(h, desc, parts, resets, nullptr, readouts, out);
-}
-
-int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
-                                     const gg_device_configs* configs, const gg_step_readouts* readouts, gg_step_plan* out) {
-    return gg_step_plan_create_with_snapshots(h, desc, parts, resets, configs, nullptr, readouts, out);
-}
-
-int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
-                                       const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
-                                       gg_step_plan* out) {
-    return gg_step_plan_create_with_scan_masks(h, desc, parts, resets, configs, snaps, readouts, nullptr, out);
-}
-
-int gg_step_plan_create_with_scan_masks(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
-                                        const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
-                                        const int32_t* dev_scan_mask, gg_step_plan* out) {
+// Every gg_step_plan_create[_with_*] entry point: checks, prepares, records and binds the plan of `step`.
+int create_plan(gg_handle h, const StepSpec& step, gg_step_plan* out) {
     if (!out) return fail(GG_E_ARG, "null out pointer");
     *out = nullptr;
-    if (!h || !desc) return fail(GG_E_ARG, "null argument");
+    if (!h || !step.desc) return fail(GG_E_ARG, "null argument");
     int rc;
-    if ((rc = check_step_desc(h, *desc, parts, resets, configs))) return rc;
+    if ((rc = check_step_desc(h, step))) return rc;
     GG_CUDA(cudaSetDevice(h->device));
-    if ((rc = prepare_recording(h, *desc, configs, readouts))) return rc;
     gg_step_plan p = new gg_step_plan_s();
     p->h = h;
-    if ((rc = record_plan(h, *desc, parts, resets, configs, snaps, readouts, dev_scan_mask, p))) {
+    for (int i = 0; i < step.desc->count; ++i) p->slots.push_back(step.desc->scans[i].slot);
+    if ((rc = prepare_recording(h, step, p->slots)) || (rc = record_plan(h, step, p))) {
         free_plan(p);
         return rc;
     }
@@ -3330,6 +3295,40 @@ int gg_step_plan_create_with_scan_masks(gg_handle h, const gg_step_desc* desc, c
     h->plans.push_back(p);
     *out = p;
     return GG_OK;
+}
+}  // namespace
+
+int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out) { return create_plan(h, {desc}, out); }
+
+int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out) {
+    return create_plan(h, {desc, nullptr, resets}, out);
+}
+
+int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, const gg_step_readouts* readouts,
+                                      gg_step_plan* out) {
+    return create_plan(h, {desc, nullptr, resets, nullptr, nullptr, readouts}, out);
+}
+
+int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                   const gg_step_readouts* readouts, gg_step_plan* out) {
+    return create_plan(h, {desc, parts, resets, nullptr, nullptr, readouts}, out);
+}
+
+int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                     const gg_device_configs* configs, const gg_step_readouts* readouts, gg_step_plan* out) {
+    return create_plan(h, {desc, parts, resets, configs, nullptr, readouts}, out);
+}
+
+int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                       const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
+                                       gg_step_plan* out) {
+    return create_plan(h, {desc, parts, resets, configs, snaps, readouts}, out);
+}
+
+int gg_step_plan_create_with_scan_masks(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts, const gg_device_resets* resets,
+                                        const gg_device_configs* configs, const gg_step_snapshots* snaps, const gg_step_readouts* readouts,
+                                        const int32_t* dev_scan_mask, gg_step_plan* out) {
+    return create_plan(h, {desc, parts, resets, configs, snaps, readouts, dev_scan_mask}, out);
 }
 
 int gg_step_plan_launch(gg_step_plan p, void* stream) {

@@ -609,11 +609,24 @@ int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scan
  * For callers that keep every per-step input on the GPU and run their step as a CUDA graph (simulators stepping many
  * robots, replay services, GPU perception stacks).  A plan is a fixed batch of `count` distinct slots and a fixed set of
  * caller DEVICE buffers; the host issues the launches, copies and fences of a step once, at gg_step_plan_create, and a
- * replay issues none of them.  Its step is, by definition, this call sequence on those slots and buffers:
- *   1. if dev_n_points: gg_set_point_counts_from_device(dev_n_points);
- *   2. if any pointer of `poses` is given: gg_update_poses_from_device(poses, dev_moved);
- *   3. gg_run_scans_to_device over dev_points, or gg_run_cloud_msgs_to_device over msgs, with scans, outs, select and
- *      dev_counts (stop_after 0).
+ * replay issues none of them.  Its step is, by definition, this sequence of stages, each a call over the plan's slots in
+ * desc->scans order on those buffers, and each only when it is given.  gg_step_plan_create gives stages 5 to 7; the
+ * gg_step_plan_create_with_* variants add the arguments of the others:
+ *   1. configurations: gg_set_slot_configs_from_device(configs), if configs is given;
+ *   2. resets: gg_init_maps_from_device(resets), if resets is given;
+ *   3. restore: gg_restore_maps_from_device(&snaps->restore), if any field of snaps->restore is set;
+ *   4. scan masks: gg_set_scan_masks_from_device(dev_scan_mask), if dev_scan_mask is given;
+ *   5. counts: gg_set_point_counts_from_device(dev_n_points), if dev_n_points is given; with parts, the part counts
+ *      instead: gg_set_part_counts_from_device(parts->parts_per_slot, parts->dev_part_counts), if dev_part_counts is
+ *      given;
+ *   6. poses: gg_update_poses_from_device(poses, dev_moved), if any pointer of `poses` is given;
+ *   7. the scan, always: gg_run_scans_to_device over dev_points, or gg_run_cloud_msgs_to_device over msgs, with scans,
+ *      outs, select and dev_counts (stop_after 0); with parts, gg_run_merged_cloud_msgs_to_device(scans, parts->n_parts,
+ *      parts->parts, outs, select, dev_counts);
+ *   8. the read-outs, in this order, each call when any of its fields of gg_step_readouts is set:
+ *      gg_get_layers_to_device, gg_layer_images_to_device, gg_terrain_images_to_device, gg_sample_layers_to_device,
+ *      gg_point_info_to_device, gg_eval_counts_to_device;
+ *   9. save: gg_save_maps_to_device(snaps->save, snaps->save_mask), if either is set.
  * Every replay is bit-identical to that sequence run with the buffers' contents at replay time: labels, index, cloud,
  * dev_counts, dev_moved, every layer, the map position, gg_get_output, point info, tallies and gg_last_scan_points.  The
  * flags GG_SCAN_DEVICE_POSE and GG_SCAN_DEVICE_COUNT mean what they mean for those calls; the buffers' ADDRESSES are
@@ -630,7 +643,7 @@ int gg_run_cloud_msgs_to_device(gg_handle h, int count, const gg_scan_desc* scan
  * position or change the configuration the plan's records carry by value.  gg_get_map_position waits for the slot's
  * stream group and returns the device position; the slot stays device-owned.  Every other call behaves as on any slot
  * whose position is device-owned.
- * gg_step_plan_create validates what the three calls validate, with the same codes, and also rejects (GG_E_ARG) a null
+ * gg_step_plan_create validates what its calls validate, with the same codes, and also rejects (GG_E_ARG) a null
  * handle, desc or out, count <= 0, both or neither of dev_points / msgs, dev_T_map_from_frame without msgs, an entry of
  * it that is misaligned, overlaps another or goes with a non-NULL msgs[k].T_map_from_frame; GG_E_STATE: a slot bound to
  * another plan.  It waits for the slots' stream groups, allocates what the recorded kernels address, and does not run
@@ -655,20 +668,20 @@ typedef struct gg_step_desc {
     const gg_point* const* dev_points;          /* host [count] of device clouds, or NULL ... */
     const gg_cloud_msg* msgs;                   /* ... or host [count] of payloads (exactly one of the two) */
     const double* const* dev_T_map_from_frame;  /* NULL or host [count] of device pointers / NULL entries (msgs only) */
-    const int32_t* dev_n_points;                /* device [count] or NULL: step 1 */
-    gg_device_poses poses;                      /* step 2; all four NULL: no step 2 */
+    const int32_t* dev_n_points;                /* device [count] or NULL: stage 5 */
+    gg_device_poses poses;                      /* stage 6; all four NULL: no stage 6 */
     int32_t* dev_moved;                         /* as in gg_update_poses_from_device */
     const gg_scan_outputs* outs;                /* as in gg_run_scans_to_device */
     unsigned select;
     int32_t* dev_counts;
 } gg_step_desc;
 int gg_step_plan_create(gg_handle h, const gg_step_desc* desc, gg_step_plan* out);
-/* A step plan whose step starts with a step 0: gg_init_maps_from_device(resets) over the plan's slots in desc->scans
- * order, then steps 1-3 as above.  Every replay is bit-identical to that four-call sequence run with the buffers'
- * contents at replay time (resets->xyz and resets->mask are read at replay time, so the mask may change every step).
- * resets NULL is exactly gg_step_plan_create.  Validation: what gg_step_plan_create validates, what
- * gg_init_maps_from_device validates, and GG_E_ARG for resets without xyz.  The plan adds one kernel per stream group.
- * gg_step_plan_create_with_readouts (below, after gg_sample_layers_to_device) adds a step 4 of read-outs. */
+/* A step plan with the resets stage (stage 2 above): gg_init_maps_from_device(resets).  Every replay is bit-identical to
+ * the stage sequence run with the buffers' contents at replay time (resets->xyz and resets->mask are read at replay
+ * time, so the mask may change every step).  resets NULL is exactly gg_step_plan_create.  Validation: what
+ * gg_step_plan_create validates, what gg_init_maps_from_device validates, and GG_E_ARG for resets without xyz.  The
+ * stage adds one kernel per stream group.  gg_step_plan_create_with_readouts (below, after gg_sample_layers_to_device)
+ * adds the read-outs (stage 8). */
 int gg_step_plan_create_with_resets(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets, gg_step_plan* out);
 int gg_step_plan_launch(gg_step_plan plan, void* stream);
 int gg_step_plan_kernels(gg_step_plan plan);   /* kernels per replay */
@@ -741,15 +754,12 @@ int gg_set_part_counts_from_device(gg_handle h, int count, const int* slots, int
                                    void* stream);
 
 /* A step plan whose step is a merged scan (a multi-LiDAR rig in a CUDA graph).  Scan k of desc->scans owns the next
- * n_parts[k] entries of `parts`.  The step is, by definition, this sequence over the plan's slots in desc->scans order:
- *   0. gg_init_maps_from_device(resets), if resets is given;
- *   1. gg_set_part_counts_from_device(parts_per_slot, dev_part_counts), if dev_part_counts is given;
- *   2. gg_update_poses_from_device(desc->poses, desc->dev_moved), if any pose pointer is given;
- *   3. gg_run_merged_cloud_msgs_to_device(desc->scans, n_parts, parts, desc->outs, desc->select, desc->dev_counts);
- *      part p with a non-NULL dev_T_map_from_part entry is transformed with the 12 doubles found there AT REPLAY TIME,
- *      bit-identical to passing them as its host T_map_from_frame (which must then be NULL);
- *   4. the read-outs, as in gg_step_plan_create_with_readouts.
- * Every replay is bit-identical to that sequence run on the buffers' contents at replay time.  desc->dev_points,
+ * n_parts[k] entries of `parts`.  The scan stage (stage 7 in the list at gg_step_plan_create) is
+ * gg_run_merged_cloud_msgs_to_device(desc->scans, n_parts, parts, desc->outs, desc->select, desc->dev_counts), and the
+ * counts stage (5) is gg_set_part_counts_from_device(parts_per_slot, dev_part_counts), if dev_part_counts is given.  Part
+ * p with a non-NULL dev_T_map_from_part entry is transformed with the 12 doubles found there AT REPLAY TIME,
+ * bit-identical to passing them as its host T_map_from_frame (which must then be NULL).
+ * Every replay is bit-identical to the stage sequence run on the buffers' contents at replay time.  desc->dev_points,
  * desc->msgs, desc->dev_T_map_from_frame and desc->dev_n_points must be NULL (GG_E_ARG).  parts NULL is exactly
  * gg_step_plan_create_with_readouts.  Everything else is what the recorded calls and gg_step_plan_create validate, with
  * the same codes, plus GG_E_ARG for null n_parts or parts, an n_parts[k] outside [0, GG_MAX_CLOUD_PARTS], and a
@@ -762,7 +772,7 @@ typedef struct gg_step_parts {
                                                   at fixed addresses; n_points = capacity for flagged scans */
     const double* const* dev_T_map_from_part;  /* NULL or host [sum n_parts] of DEVICE pointers (12 doubles, 8-byte
                                                   aligned, pairwise disjoint) or NULL entries */
-    const int32_t* dev_part_counts;            /* DEVICE [count][parts_per_slot] or NULL: step 1 */
+    const int32_t* dev_part_counts;            /* DEVICE [count][parts_per_slot] or NULL: stage 5 */
     int parts_per_slot;
 } gg_step_parts;
 /* gg_step_plan_create_with_parts is declared after gg_step_plan_create_with_readouts, below. */
@@ -1004,16 +1014,10 @@ int gg_sample_layers_to_device(gg_handle h, int count, const int* slots, const g
                                int mode, void* stream);
 
 /* ---- step plan read-outs: what a replayed step writes into caller memory besides its scan outputs ----
- * A plan created with read-outs has a step 4 after step 3 (gg_step_plan_create): these calls, in this order, over the
- * plan's slots in desc->scans order, each only when one of its fields is set (nonzero / non-NULL):
- *   1. gg_get_layers_to_device(n_layer_names, layer_names, layers)
- *   2. gg_layer_images_to_device(n_image_names, image_names, images, image_ranges)
- *   3. gg_terrain_images_to_device(terrain_images)
- *   4. gg_sample_layers_to_device(samples, n_sample_names, sample_names, sample_mode)
- *   5. gg_point_info_to_device(point_info)
- *   6. gg_eval_counts_to_device(eval_counts)
- * Every replay is bit-identical to the plan's step followed by that call sequence, run with the buffers' contents at
- * replay time.  What gg_step_plan_create_with_readouts reads, and when:
+ * A plan created with read-outs has the read-out stage (stage 8 in the list at gg_step_plan_create): the calls listed
+ * there, each only when one of its fields is set (nonzero / non-NULL).  A call's fields are its row of gg_step_readouts
+ * below, and are its arguments of the same names.  Every replay is bit-identical to the stage sequence run with the
+ * buffers' contents at replay time.  What gg_step_plan_create_with_readouts reads, and when:
  *   - the host arrays (layer_names, image_names, sample_names, samples[count], point_info[count]) and sample_mode are
  *     read at creation and may be freed afterwards;
  *   - every DEVICE address (layers, images, image_ranges, terrain_images, samples[k].data / dst / cell,
@@ -1039,55 +1043,49 @@ typedef struct gg_step_readouts {
 } gg_step_readouts;
 int gg_step_plan_create_with_readouts(gg_handle h, const gg_step_desc* desc, const gg_device_resets* resets,
                                       const gg_step_readouts* readouts, gg_step_plan* out);
-/* A step plan whose step 3 is a merged scan: see gg_step_parts (after gg_run_merged_cloud_msgs_to_device). */
+/* A step plan whose scan stage (7) is a merged scan: see gg_step_parts (after gg_run_merged_cloud_msgs_to_device). */
 int gg_step_plan_create_with_parts(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                    const gg_device_resets* resets, const gg_step_readouts* readouts, gg_step_plan* out);
-/* A step plan whose step starts with the slots' configurations: gg_set_slot_configs_from_device(configs) over the plan's
- * slots in desc->scans order, then steps 0-4 as in gg_step_plan_create_with_parts (parts may be NULL: then
- * desc->dev_points / msgs as in gg_step_plan_create_with_readouts).  Every replay is bit-identical to that call sequence
- * run on the buffers' contents at replay time: configs->cfg and configs->mask are read at replay time, so both may change
- * every step.  configs NULL is exactly gg_step_plan_create_with_parts.  With configs the plan's slots become
- * device-configured at creation (seeded with their current configurations, as a first standalone call seeds them).
- * Bound slots: a plan's records of a slot that is device-configured at creation read the slot's configuration at every
- * replay, with or without configs, so a standalone gg_set_slot_configs_from_device on such a bound slot is accepted and
- * reaches the plan's next replay; on a slot that was host-configured at creation it is GG_E_STATE.  gg_set_slot_config and
- * gg_set_config stay refused on bound slots.  Validation: what gg_step_plan_create_with_parts validates, what
- * gg_set_slot_configs_from_device validates, and GG_E_ARG for configs without cfg.  A rejected plan leaves no plan, no
- * bound slot, no device-configured slot, and the slots' state and gg_kernel_launches unchanged.  The config stage adds
- * two kernels per stream group. */
+/* A step plan with the configuration stage (stage 1 in the list at gg_step_plan_create):
+ * gg_set_slot_configs_from_device(configs) (parts may be NULL: then desc->dev_points / msgs as in
+ * gg_step_plan_create_with_readouts).  Every replay is bit-identical to the stage sequence run on the buffers' contents
+ * at replay time: configs->cfg and configs->mask are read at replay time, so both may change every step.  configs NULL
+ * is exactly gg_step_plan_create_with_parts.  With configs the plan's slots become device-configured at creation
+ * (seeded with their current configurations, as a first standalone call seeds them).  Bound slots: a plan's records of a
+ * slot that is device-configured at creation read the slot's configuration at every replay, with or without configs, so
+ * a standalone gg_set_slot_configs_from_device on such a bound slot is accepted and reaches the plan's next replay; on
+ * a slot that was host-configured at creation it is GG_E_STATE.  gg_set_slot_config and gg_set_config stay refused on
+ * bound slots.  Validation: what gg_step_plan_create_with_parts validates, what gg_set_slot_configs_from_device
+ * validates, and GG_E_ARG for configs without cfg.  A rejected plan leaves no plan, no bound slot, no device-configured
+ * slot, and the slots' state and gg_kernel_launches unchanged.  The config stage adds two kernels per stream group. */
 int gg_step_plan_create_with_configs(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                      const gg_device_resets* resets, const gg_device_configs* configs,
                                      const gg_step_readouts* readouts, gg_step_plan* out);
-/* A step plan that also restores and saves map snapshots (gg_restore_maps_from_device, gg_save_maps_to_device).  The step
- * is, by definition, this call sequence over the plan's slots in desc->scans order, each stage only when it is given:
- *   1. gg_set_slot_configs_from_device(configs);
- *   2. gg_init_maps_from_device(resets);
- *   3. gg_restore_maps_from_device(&snaps->restore), when any field of snaps->restore is set;
- *   4. the counts (or part counts), 5. the poses and 6. the scan, as in gg_step_plan_create_with_configs;
- *   7. the read-outs;
- *   8. gg_save_maps_to_device(snaps->save, snaps->save_mask), when either is set.
- * Every replay is bit-identical to that sequence run on the buffers' contents at replay time: the pool, the index, the
- * save mask and the slots' planes are read, and the status and the saved records written, at replay time.  A restore and
- * a save on the same pool in one plan are allowed; the stage order defines them.  snaps NULL is exactly
+/* A step plan that also restores and saves map snapshots: the restore stage (stage 3 in the list at
+ * gg_step_plan_create), gg_restore_maps_from_device(&snaps->restore), when any field of snaps->restore is set, and the
+ * save stage (9), gg_save_maps_to_device(snaps->save, snaps->save_mask), when either is set.  Every replay is
+ * bit-identical to the stage sequence run on the buffers' contents at replay time: the pool, the index, the save mask
+ * and the slots' planes are read, and the status and the saved records written, at replay time.  A restore and a save
+ * on the same pool in one plan are allowed; the stage order defines them.  snaps NULL is exactly
  * gg_step_plan_create_with_configs.  Validation: what gg_step_plan_create_with_configs validates and what the two calls
  * validate, with the same codes.  A rejected plan leaves no plan, no bound slot, and the slots' state and
  * gg_kernel_launches unchanged.  Each snapshot stage adds one kernel per stream group. */
 typedef struct gg_step_snapshots {
-    gg_map_restore restore;      /* step 3 */
-    void* save;                  /* step 8: DEVICE [count][gg_map_snapshot_bytes] or NULL */
+    gg_map_restore restore;      /* stage 3 */
+    void* save;                  /* stage 9: DEVICE [count][gg_map_snapshot_bytes] or NULL */
     const int32_t* save_mask;    /* DEVICE [count] or NULL */
 } gg_step_snapshots;
 int gg_step_plan_create_with_snapshots(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                        const gg_device_resets* resets, const gg_device_configs* configs,
                                        const gg_step_snapshots* snaps, const gg_step_readouts* readouts, gg_step_plan* out);
-/* A step plan whose scans run only where a device mask says so.  The step is that of gg_step_plan_create_with_snapshots
- * with one more stage, gg_set_scan_masks_from_device(dev_scan_mask) over the plan's slots, just before the counts (step
- * 4); every replay is bit-identical to that call sequence on the buffers' contents at replay time.  dev_scan_mask (DEVICE
- * int32 [count], 4-byte aligned) only stores the masks: the scans that read them are those of desc->scans whose flags set
- * GG_SCAN_DEVICE_MASK.  dev_scan_mask NULL is exactly gg_step_plan_create_with_snapshots; flagged scans then read the
- * masks stored by standalone gg_set_scan_masks_from_device calls, also ones made after the plan's creation.  Validation:
- * what gg_step_plan_create_with_snapshots validates and what gg_set_scan_masks_from_device validates, with the same codes;
- * a rejected plan leaves no plan, no bound slot, and the slots' state and gg_kernel_launches unchanged.  The stage adds
+/* A step plan whose scans run only where a device mask says so: the scan-mask stage (stage 4 in the list at
+ * gg_step_plan_create), gg_set_scan_masks_from_device(dev_scan_mask); every replay is bit-identical to the stage
+ * sequence on the buffers' contents at replay time.  dev_scan_mask (DEVICE int32 [count], 4-byte aligned) only stores
+ * the masks: the scans that read them are those of desc->scans whose flags set GG_SCAN_DEVICE_MASK.  dev_scan_mask NULL
+ * is exactly gg_step_plan_create_with_snapshots; flagged scans then read the masks stored by standalone
+ * gg_set_scan_masks_from_device calls, also ones made after the plan's creation.  Validation: what
+ * gg_step_plan_create_with_snapshots validates and what gg_set_scan_masks_from_device validates, with the same codes; a
+ * rejected plan leaves no plan, no bound slot, and the slots' state and gg_kernel_launches unchanged.  The stage adds
  * one kernel per stream group. */
 int gg_step_plan_create_with_scan_masks(gg_handle h, const gg_step_desc* desc, const gg_step_parts* parts,
                                         const gg_device_resets* resets, const gg_device_configs* configs,

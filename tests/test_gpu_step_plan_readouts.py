@@ -240,24 +240,23 @@ def test_readouts_with_resets(monkeypatch):
 
 
 class Lib:
-    """The library with gg_step_plan_create[_with_resets] sent through gg_step_plan_create_with_readouts(readouts), or
-    with gg_step_plan_create_with_readouts's read-outs edited by `edit` first."""
+    """The library with gg_step_plan_create_with_scan_masks's read-outs replaced by `readouts`, or edited by `edit` first.
+    `calls` counts the calls it intercepted."""
 
     def __init__(self, L, readouts=None, edit=None):
         self._L, self._r, self._edit = L, readouts, edit
+        self.calls = 0
 
     def __getattr__(self, name):
         return getattr(self._L, name)
 
-    def gg_step_plan_create(self, h, d, p):
-        return self._L.gg_step_plan_create_with_readouts(h, d, None, self._r, p)
-
-    def gg_step_plan_create_with_resets(self, h, d, r, p):
-        return self._L.gg_step_plan_create_with_readouts(h, d, r, self._r, p)
-
-    def gg_step_plan_create_with_readouts(self, h, d, r, ro, p):
-        self._edit(ro._obj)
-        return self._L.gg_step_plan_create_with_readouts(h, d, r, ro, p)
+    def gg_step_plan_create_with_scan_masks(self, h, d, sp, r, cc, snap, ro, mask, p):
+        self.calls += 1
+        if self._edit is None:
+            ro = self._r
+        else:
+            self._edit(ro._obj)
+        return self._L.gg_step_plan_create_with_scan_masks(h, d, sp, r, cc, snap, ro, mask, p)
 
 
 @pytest.mark.parametrize("resets", [False, True])
@@ -275,13 +274,14 @@ def test_plans_without_readouts_are_unchanged(monkeypatch, resets):
         if resets:
             extra = dict(reset_xyz=torch.zeros((B, 3), dtype=torch.float64, device="cuda"), reset_mask=torch.zeros(B, dtype=torch.int32, device="cuda"))
         L = g._l
-        g._l = Lib(L, variant)
+        g._l = shim = Lib(L, variant)
         try:
             plan = inp.plan(g, "all") if not resets else g.step_plan(inp.slots, clouds=inp.buf, counts=inp.counts, xy=inp.xy, T_base_from_map=inp.T,
                                                                      pose_origins=inp.origins, pose_base_z=inp.base_z, moved=True, labels=True,
                                                                      select="all", index=True, **extra)
         finally:
             g._l = L
+        assert shim.calls == 1, f"variant {variant}: the plan was not created through the shim"
         ref = inp.plan(twin, "all") if not resets else twin.step_plan(inp.slots, clouds=inp.buf, counts=inp.counts, xy=inp.xy, T_base_from_map=inp.T,
                                                                       pose_origins=inp.origins, pose_base_z=inp.base_z, moved=True, labels=True,
                                                                       select="all", index=True, **extra)
@@ -425,13 +425,15 @@ def test_rejections(monkeypatch):
         pos_before = [h.position(slot=s).tobytes() for s in inp.slots]
         counts_before = [h.last_scan_points(slot=s) for s in inp.slots]
         L = h._l
+        shim = None
         if edit is not None:
-            h._l = Lib(L, edit=edit)
+            h._l = shim = Lib(L, edit=edit)
         try:
             with pytest.raises(capi.GroundGridError) as e:
                 plan(h, **kw)
         finally:
             h._l = L
+        assert shim is None or shim.calls == 1, f"{name}: the edited read-outs did not reach the C call"
         assert e.value.code == want, f"{name}: {e.value}"
         assert h.kernel_launches == before, f"{name}: launches"
         assert [h.position(slot=s).tobytes() for s in inp.slots] == pos_before, f"{name}: positions"
